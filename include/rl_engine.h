@@ -50,8 +50,8 @@ enum { RL_MEM_HOST = 0, RL_MEM_DEVICE = 1,
  * overflow): the call (or the next rl_sync) also reports the error; the byte is never a silent 0 = allowed */
 #define RL_VERDICT_ERROR 0xFFu
 #define RL_MAX_COUNTERS_PER_REQUEST 16 /* counters one request may name (general form); the matcher refuses more */
-/* test aid: narrow the in-kernel grouping tag so that distinct keys collide and the
- * collision path (salted re-insertion) is exercised */
+/* test aid: the in-kernel row grouping table gives every row one of only four home slots, so that
+ * distinct rows collide and its linear probing is exercised to full length */
 #define RL_FLAG_DEBUG_WEAK_TAGS 1u
 /* Record calls with RL_MEM_DEVICE / RL_MEM_HOST_ASYNC buffers are software-pipelined over three internal
  * streams: probe+count of call s+2 and scan+scatter of call s+1 overlap the replay of call s.  Results are

@@ -11,12 +11,12 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
-
-#include <functional>
 
 #include "rl_kernels.cuh"
 #include "rl_shard.cuh"
@@ -49,10 +49,17 @@ struct HostGroup {
     }
 };
 
+// Device memory owned by its holder: freed when the holder goes away.
 template <class T>
 struct DevBuf {
     T* p = nullptr;
     size_t n = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
     cudaError_t reserve(size_t want) {
         if (want <= n) return cudaSuccess;
         if (p) cudaFree(p);
@@ -62,26 +69,16 @@ struct DevBuf {
         if (r == cudaSuccess) n = want;
         return r;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        n = 0;
-    }
 };
 
 }  // namespace
 
-// A second copy of the per-batch workspace: with RL_FLAG_PIPELINE the partition kernels of
+// The per-batch workspace.  With RL_FLAG_PIPELINE there is one per call in flight: the partition kernels of
 // batch s+1 run (on their own stream) while k_main of batch s is still replaying.
 struct WorkSet {
     DevBuf<uint32_t> tile_loc, region_total, part_idx, part_row, row_of, chain_status,
         chain_wcnt, chain_w, small;  // small: [0] blocks-done counter of the probe, [1] item count, [2] ticket, [3] exit counter
     DevBuf<uint4> items;
-    void release() {
-        tile_loc.release(); region_total.release(); part_idx.release(); part_row.release();
-        row_of.release(); chain_status.release(); chain_wcnt.release();
-        chain_w.release(); small.release(); items.release();
-    }
 };
 
 struct rl_engine {
@@ -90,7 +87,7 @@ struct rl_engine {
     uint32_t cells = 1, log2P = 0, log2R = 0, row_bytes = 32;
     uint64_t capacity = 0;
     uint32_t max_batch = 0, max_counters = 0;
-    uint8_t* d_rows = nullptr;
+    DevBuf<uint8_t> d_rows;
 
     // registry
     std::vector<HostLimit> limits;
@@ -111,18 +108,16 @@ struct rl_engine {
     uint32_t limits_cap = 0, ns_cap = 0;
 
     // workspace
-    DevBuf<uint32_t> d_tile_loc, d_region_total, d_part_idx, d_part_row, d_row_of, d_misc;  // misc: err, flags, scan_ctr, changed, ...
+    DevBuf<uint32_t> d_misc;  // misc: err, flags, changed, exchange error detail (MISC_*)
     DevBuf<RlAccess> d_acc;
     DevBuf<uint64_t> d_delta, d_now;
     DevBuf<uint32_t> d_fl_prev, d_fl_next;
-    DevBuf<uint4> d_items;
     DevBuf<unsigned long long> d_kstats;
     DevBuf<uint4> d_trace;     // RL_FLAG_TRACE: event ring
     DevBuf<uint32_t> d_hot;    // [RL_HOT_SLOTS] hot rows + [RL_HOT_CAND] candidates + [1] candidate count
     bool hot_rows = false;     // RL_HOT=1 enables the hot-row partitions (k_hot); see DESIGN.md §3.4 for why it is opt-in
     DevBuf<uint32_t> d_misc2;  // [0] trace write position
     uint32_t trace_seq = 0;
-    DevBuf<uint32_t> d_chain_status, d_chain_wcnt, d_chain_w;
     DevBuf<uint8_t*> d_log_row;
     DevBuf<ulonglong2> d_log_state;
     // staging for RL_MEM_HOST calls
@@ -140,12 +135,10 @@ struct rl_engine {
 
     rl_stats stats{};
     std::string last_error = "";
-    // rl_profile_begin/end
-    // RL_FLAG_PIPELINE
-    bool pipeline = false;
+    bool pipeline = false;                 // RL_FLAG_PIPELINE
     bool kernel_stats = false;  // RL_FLAG_KERNEL_STATS
     static constexpr int kSets = RL_SETS;  // workspace sets = calls in flight (probe | scan+scatter | replay)
-    WorkSet wsx[kSets - 1];                // sets 1.. (set 0 = the engine's own members)
+    WorkSet ws[kSets];                     // sets 1.. are allocated with RL_FLAG_PIPELINE only
     cudaStream_t sq = nullptr;       // scan + scatter stream
     cudaStream_t sp = nullptr, sm = nullptr;  // partition / replay streams
     cudaEvent_t ev_in = nullptr, ev_probe[kSets] = {}, ev_part[kSets] = {}, ev_main[kSets] = {};  // ev_probe: replay done, before a post_main hook
@@ -176,7 +169,7 @@ struct rl_engine {
 
 namespace {
 
-enum { MISC_ERR = 0, MISC_FLAGS = 1, MISC_SCANCTR = 2, MISC_CHANGED = 3, MISC_NITEMS = 4, MISC_TICKET = 5, MISC_EXITCTR = 6, MISC_N = 8 };
+enum { MISC_ERR = 0, MISC_FLAGS = 1, MISC_CHANGED = 3, MISC_XCHG = 7, MISC_N = 8 };
 
 int fail(rl_engine* e, int status, const char* fmt, ...) {
     char buf[512];
@@ -215,7 +208,7 @@ uint32_t log2_ceil(uint64_t x) {
 
 RlDev make_dev(rl_engine* e) {
     RlDev D;
-    D.rows = e->d_rows;
+    D.rows = e->d_rows.p;
     D.log2P = e->log2P;
     D.log2R = e->log2R;
     D.desc = e->d_desc.p;
@@ -345,8 +338,8 @@ int check_device_error(rl_engine* e) {
         case RL_DEV_TOO_MANY_COUNTERS:
             return fail(e, RL_FATAL, "a request has more than %d counters", RL_MAX_CTRS_PER_REQ);
         case RL_DEV_EXCHANGE: {
-            const uint32_t d = e->h_misc[7];
-            RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + 7, 0, sizeof(uint32_t), e->stream));
+            const uint32_t d = e->h_misc[MISC_XCHG];
+            RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_XCHG, 0, sizeof(uint32_t), e->stream));
             const char* what = (d >> 28) == 1 ? "records of source rank" : (d >> 28) == 2 ? "verdicts of owner rank" : "inbox larger than max_batch, rank";
             return fail(e, RL_FATAL, "peer exchange failed at step %u: %s %u did not arrive within %.0f s (or a block fill was out of range)",
                         d & 0xFFFFFu, what, (d >> 20) & 0xFFu, (double)RL_XCHG_TIMEOUT_NS * 1e-9);
@@ -380,6 +373,7 @@ struct Outs {
 
 RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, int lc, int set = 0, uint32_t n_hint = 0,
                    bool hot_ok = true) {
+    const WorkSet& w = e->ws[set];
     RlBatch B;
     B.nhot = (hot_ok && e->hot_rows) ? RL_HOT_SLOTS : 0;
     B.n_acc = n_acc;
@@ -388,14 +382,14 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     B.omap_prefix = nullptr;
     B.omap_n = 0;
     B.omap_stride = 0;
-    B.tile_loc = e->d_tile_loc.p;
-    B.region_total = e->d_region_total.p;
-    B.part_idx = e->d_part_idx.p;
-    B.row_of = e->d_row_of.p;
-    B.part_row = e->d_part_row.p;
-    B.scan_ctr = e->d_misc.p + MISC_SCANCTR;
-    B.ticket = e->d_misc.p + MISC_TICKET;
-    B.exit_ctr = e->d_misc.p + MISC_EXITCTR;
+    B.tile_loc = w.tile_loc.p;
+    B.region_total = w.region_total.p;
+    B.part_idx = w.part_idx.p;
+    B.row_of = w.row_of.p;
+    B.part_row = w.part_row.p;
+    B.scan_ctr = w.small.p + 0;
+    B.ticket = w.small.p + 2;
+    B.exit_ctr = w.small.p + 3;
     uint32_t tile = ceil_div(n_acc, kMaxTiles);
     tile = std::max<uint32_t>(512, ((tile + 255) / 256) * 256);
     B.tile = tile;
@@ -414,11 +408,11 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     B.fl_next = e->d_fl_next.p;
     B.phase = RL_PHASE_COMMIT;
     B.load_counters = lc;
-    B.items = e->d_items.p;
-    B.n_items = e->d_misc.p + MISC_NITEMS;
-    B.chain_status = e->d_chain_status.p;
-    B.chain_wcnt = e->d_chain_wcnt.p;
-    B.chain_w = e->d_chain_w.p;
+    B.items = w.items.p;
+    B.n_items = w.small.p + 1;
+    B.chain_status = w.chain_status.p;
+    B.chain_wcnt = w.chain_wcnt.p;
+    B.chain_w = w.chain_w.p;
     B.chunk = e->chunk;
     // a region is split into chained chunks only when it is far heavier than the average one
     // partition granularity: about one k_main chunk per partition, never finer than the table's regions
@@ -433,74 +427,56 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     B.heavy_len = e->heavy_mult ? std::max<uint32_t>(2 * e->chunk, e->heavy_mult * ceil_div(n_size, B.nparts)) : 0xFFFFFFFFu;
     B.log_row = nullptr;
     B.log_state = nullptr;
-    if (set >= 1) {
-        WorkSet& w = e->wsx[set - 1];
-        B.tile_loc = w.tile_loc.p;
-        B.region_total = w.region_total.p;
-        B.part_idx = w.part_idx.p;
-        B.row_of = w.row_of.p;
-        B.part_row = w.part_row.p;
-        B.scan_ctr = w.small.p + 0;
-        B.items = w.items.p;
-        B.n_items = w.small.p + 1;
-        B.ticket = w.small.p + 2;
-        B.exit_ctr = w.small.p + 3;
-        B.chain_status = w.chain_status.p;
-        B.chain_wcnt = w.chain_wcnt.p;
-        B.chain_w = w.chain_w.p;
-    }
     return B;
 }
 
-template <int CELLS, class Src>
-int launch_front_cells(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st) {
-    const uint32_t P1 = B.nparts + B.nhot + 1;
-    const size_t smem = ((size_t)RL_PART_WARPS * P1 + P1 + 1) * sizeof(uint32_t);
-    static int smem_limit[64] = {};  // per instantiation and device: raised as engines with more regions appear
-    const int dv = e->device & 63;
-    // (k_front also has ~8 KB of static shared memory: opt in well before the 48 KB default is reached)
-    if (smem > 32 * 1024 && (int)smem > smem_limit[dv]) {
-        const uint32_t maxP1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;
-        const int max_smem = (int)(((size_t)RL_PART_WARPS * maxP1 + maxP1 + 1) * sizeof(uint32_t));
-        RL_CUDA(e, cudaFuncSetAttribute(k_front<CELLS, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-        smem_limit[dv] = max_smem;
+// Calls f(std::integral_constant<int, CELLS>{}) for the engine's row geometry: 1, 3 or 7 cells per row.
+template <class F>
+auto with_cells(const rl_engine* e, F&& f) {
+    switch (e->cells) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        default: return f(std::integral_constant<int, 7>{});
     }
-    k_front<CELLS, Src><<<B.num_tiles, RL_PART_THREADS, smem, st>>>(D, B, src);
-    RL_LAUNCH_CHECK(e);
-    return RL_OK;
 }
 
 // probe + stable partition by table region (one launch)
 template <class Src>
 int launch_front(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st = nullptr) {
     if (!st) st = e->stream;
-    switch (e->cells) {
-        case 1: return launch_front_cells<1, Src>(e, D, B, src, st);
-        case 3: return launch_front_cells<3, Src>(e, D, B, src, st);
-        default: return launch_front_cells<7, Src>(e, D, B, src, st);
-    }
+    const uint32_t P1 = B.nparts + B.nhot + 1;
+    const size_t smem = ((size_t)RL_PART_WARPS * P1 + P1 + 1) * sizeof(uint32_t);
+    return with_cells(e, [&](auto c) -> int {
+        auto kern = k_front<decltype(c)::value, Src>;
+        static int smem_limit[64] = {};  // per instantiation and device: raised as engines with more regions appear
+        const int dv = e->device & 63;
+        // (k_front also has ~8 KB of static shared memory: opt in well before the 48 KB default is reached)
+        if (smem > 32 * 1024 && (int)smem > smem_limit[dv]) {
+            const uint32_t maxP1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;
+            const int max_smem = (int)(((size_t)RL_PART_WARPS * maxP1 + maxP1 + 1) * sizeof(uint32_t));
+            RL_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+            smem_limit[dv] = max_smem;
+        }
+        kern<<<B.num_tiles, RL_PART_THREADS, smem, st>>>(D, B, src);
+        RL_LAUNCH_CHECK(e);
+        return RL_OK;
+    });
 }
 
 template <int GEO, int CELLS, class Src, int MODE, bool LC, int CH>
 int launch_main_ch(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st) {
-    using Smem = RlMainSmem<CELLS, CH>;
     auto kern = k_main<GEO, CELLS, Src, MODE, CH, LC>;
     static bool attr_set[64] = {};  // per instantiation and device (function attributes are per device)
-    static uint32_t resident[64] = {};
     const int dv = e->device & 63;
     if (!attr_set[dv]) {
         RL_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)rl_main_smem_bytes<CELLS, CH>(RL_MAX_TILES)));
-        int per_sm = 0;
-        RL_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CH, sizeof(Smem)));
-        resident[dv] = (uint32_t)std::max(per_sm, 1) * (e->main_grid_cap / 16);  // CTAs that fit at once (one wave)
         attr_set[dv] = true;
     }
     // upper bound of the work-item count: one per partition + one per chunk of a heavy partition; CTAs take
     // items from a ticket, so a smaller grid only means that some CTAs take several
     // (capping the grid at one resident wave was tried: the CTAs that then take a second item make the kernel last
     // two chunk latencies instead of one)
-    (void)resident;
     const uint32_t grid = std::min<uint32_t>(B.nparts + ceil_div(B.n_acc, CH), e->main_grid_cap);
     kern<<<grid, CH, rl_main_smem_bytes<CELLS, CH>(B.num_tiles), st>>>(D, B, src, e->weak_slots);
     return RL_OK;
@@ -598,11 +574,11 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
             B.phase = RL_PHASE_SPEC;
             r = launch_main<AccSrc, 0>(e, D, B, src);
             if (r) return r;
-            switch (e->cells) {
-                case 1: k_restore<1><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, 1, B.log_row, B.log_state); break;
-                case 3: k_restore<3><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, 3, B.log_row, B.log_state); break;
-                default: k_restore<7><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, e->max_cells_used <= 4 ? 4 : 7, B.log_row, B.log_state); break;
-            }
+            with_cells(e, [&](auto c) {
+                constexpr int C = decltype(c)::value;
+                const uint32_t act = C == 7 && e->max_cells_used <= 4 ? 4 : C;
+                k_restore<C><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, act, B.log_row, B.log_state);
+            });
             RL_LAUNCH_CHECK(e);
             k_fl_step<<<ceil_div(n_req, 256), 256, 0, e->stream>>>(n_req, B.fl_prev, B.fl_next,
                                                                     e->d_misc.p + MISC_CHANGED);
@@ -633,86 +609,73 @@ int run_record_pipeline(rl_engine* e, uint32_t n, const rl_record* d_recs, int m
                         bool may_pipeline = false, const PipeHooks* hooks = nullptr, uint32_t n_hint = 0,
                         uint64_t compact_now = 0) {
     RlDev D = make_dev(e);
-    if (hooks && !(may_pipeline && e->pipeline && !e->any_multi_ns))
-        return fail(e, RL_FATAL, "sharded steps need RL_FLAG_PIPELINE and single-row namespaces");
-    if (may_pipeline && e->pipeline && !e->any_multi_ns) {
-        // Two-stage software pipeline over successive calls: the front (probe + partition, `sp`) of
-        // batch s+1 (and s+2) overlaps the replay of batch s (`sm`).  The front only reads row headers
-        // and claims empty rows; the replay only touches the cells of rows found by ITS front, and
-        // replays stay in call order on `sm`, so the table sees the batches in order.
-        const int k = (int)(e->pipe_seq % rl_engine::kSets);
-        RlBatch B = make_batch(e, n, n, o, lc, k, n_hint);
-        RecordSrc src{d_recs, nullptr, 0, 0, compact_now ? 1u : 0u, compact_now};
-        if (hooks) {
-            // the inbox is filled by the peers' kernels and handed over through step flags, not through
-            // anything on the caller's stream
-            src = hooks->src;
-            B.n_dev = hooks->n_dev;
-            if (hooks->patch_batch) hooks->patch_batch(B);
-        } else {
-            RL_CUDA(e, cudaEventRecord(e->ev_in, e->stream));  // inputs: whatever the caller enqueued so far
-            RL_CUDA(e, cudaStreamWaitEvent(e->sp, e->ev_in, 0));
-        }
-        if (e->pipe_seq >= (uint64_t)rl_engine::kSets)
-            RL_CUDA(e, cudaStreamWaitEvent(e->sp, e->ev_main[k], 0));  // workspace set k is free again
-        int r = RL_OK;
-        if (hooks && hooks->pre_probe && (r = hooks->pre_probe(e->sp, k))) return r;
-        r = launch_front(e, D, B, src, e->sp);
-        if (r) return r;
-        RL_CUDA(e, cudaEventRecord(e->ev_part[k], e->sp));
-        RL_CUDA(e, cudaStreamWaitEvent(e->sm, e->ev_part[k], 0));
-        r = mode == 2 ? launch_main<RecordSrc, 2>(e, D, B, src, e->sm) : launch_main<RecordSrc, 0>(e, D, B, src, e->sm);
-        if (r) return r;
-        // per-namespace metrics (rl_ns_metrics_enable): one reduction kernel right behind the replay, same stream
-        if (e->ns_hook && !hooks && mode == 0 && o.limited &&
-            (r = e->ns_hook(e, e->sm, n, d_recs, compact_now ? 16 : 32, o.limited, o.first)))
-            return r;
-        if (hooks && hooks->post_main) {
-            // the hook (a sharded step's verdict return) runs on its own stream: the replay of the next call does
-            // not wait for it, only the reuse of this workspace set does
-            RL_CUDA(e, cudaEventRecord(e->ev_probe[k], e->sm));
-            RL_CUDA(e, cudaStreamWaitEvent(e->sq, e->ev_probe[k], 0));
-            if ((r = hooks->post_main(e->sq, k))) return r;
-            RL_CUDA(e, cudaEventRecord(e->ev_main[k], e->sq));
-        } else {
-            RL_CUDA(e, cudaEventRecord(e->ev_main[k], e->sm));
-        }
-        e->pipe_seq++;
-        e->pipe_pending = true;
-        return RL_OK;
-    }
-    {
-        int r = pipe_fence(e);
-        if (r) return r;
-    }
-    if (!e->any_multi_ns) {
-        RlBatch B = make_batch(e, n, n, o, lc);
-        RecordSrc src{d_recs, nullptr, 0, 0, compact_now ? 1u : 0u, compact_now};
-        int r = launch_front(e, D, B, src);
-        if (r) return r;
-        r = mode == 2 ? launch_main<RecordSrc, 2>(e, D, B, src) : launch_main<RecordSrc, 0>(e, D, B, src);
-        if (r == RL_OK && e->ns_hook && mode == 0 && o.limited)
-            r = e->ns_hook(e, e->stream, n, d_recs, compact_now ? 16 : 32, o.limited, o.first);
+    const bool pipelined = may_pipeline && e->pipeline && !e->any_multi_ns;
+    if (hooks && !pipelined) return fail(e, RL_FATAL, "sharded steps need RL_FLAG_PIPELINE and single-row namespaces");
+    int r = pipelined ? RL_OK : pipe_fence(e);
+    if (r) return r;
+    if (e->any_multi_ns) {
+        if (compact_now) return fail(e, RL_FATAL, "16-byte records need single-row namespaces (use the 32-byte form)");
+        // some namespace spans several rows: materialise accesses (stride = max limits per ns)
+        const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
+        if (stride > RL_MAX_CTRS_PER_REQ)
+            return fail(e, RL_FATAL, "a namespace has more than %d limits", RL_MAX_CTRS_PER_REQ);
+        const uint64_t n_acc = (uint64_t)n * stride;
+        if (n_acc > e->d_acc.n)
+            return fail(e, RL_FATAL, "batch of %u records x %u limits exceeds max_counters=%u", n, stride, e->max_counters);
+        RlResolveOut O{e->d_acc.p, e->d_delta.p, e->d_now.p, o.limited, o.first};
+        k_resolve_records<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, n, d_recs, stride, O, mode == 0);
+        RL_LAUNCH_CHECK(e);
+        if ((r = check_resolve_error(e))) return r;
+        r = run_acc_pipeline(e, (uint32_t)n_acc, n, e->d_delta.p, e->d_now.p, mode, lc, o);
+        if (r == RL_OK && e->ns_hook && mode == 0 && o.limited) r = e->ns_hook(e, e->stream, n, d_recs, 32, o.limited, o.first);
         return r;
     }
-    if (compact_now) return fail(e, RL_FATAL, "16-byte records need single-row namespaces (use the 32-byte form)");
-    // some namespace spans several rows: materialise accesses (stride = max limits per ns)
-    const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
-    if (stride > RL_MAX_CTRS_PER_REQ)
-        return fail(e, RL_FATAL, "a namespace has more than %d limits", RL_MAX_CTRS_PER_REQ);
-    const uint64_t n_acc = (uint64_t)n * stride;
-    if (n_acc > e->d_acc.n)
-        return fail(e, RL_FATAL, "batch of %u records x %u limits exceeds max_counters=%u", n, stride, e->max_counters);
-    RlResolveOut O{e->d_acc.p, e->d_delta.p, e->d_now.p, o.limited, o.first};
-    k_resolve_records<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, n, d_recs, stride, O, mode == 0);
-    RL_LAUNCH_CHECK(e);
-    {
-        int r = check_resolve_error(e);
-        if (r) return r;
+    // Pipelined, this is a two-stage software pipeline over successive calls: the front (probe + partition,
+    // `sp`) of batch s+1 (and s+2) overlaps the replay of batch s (`sm`).  The front only reads row headers
+    // and claims empty rows; the replay only touches the cells of rows found by ITS front, and replays stay
+    // in call order on `sm`, so the table sees the batches in order.  Otherwise both run on the caller's stream.
+    const int k = pipelined ? (int)(e->pipe_seq % rl_engine::kSets) : 0;
+    const cudaStream_t sf = pipelined ? e->sp : e->stream, sr = pipelined ? e->sm : e->stream;  // front, replay
+    RlBatch B = make_batch(e, n, n, o, lc, k, n_hint);
+    RecordSrc src{d_recs, nullptr, 0, 0, compact_now ? 1u : 0u, compact_now};
+    if (hooks) {
+        // the inbox is filled by the peers' kernels and handed over through step flags, not through
+        // anything on the caller's stream
+        src = hooks->src;
+        B.n_dev = hooks->n_dev;
+        if (hooks->patch_batch) hooks->patch_batch(B);
+    } else if (pipelined) {
+        RL_CUDA(e, cudaEventRecord(e->ev_in, e->stream));  // inputs: whatever the caller enqueued so far
+        RL_CUDA(e, cudaStreamWaitEvent(e->sp, e->ev_in, 0));
     }
-    int r = run_acc_pipeline(e, (uint32_t)n_acc, n, e->d_delta.p, e->d_now.p, mode, lc, o);
-    if (r == RL_OK && e->ns_hook && mode == 0 && o.limited) r = e->ns_hook(e, e->stream, n, d_recs, 32, o.limited, o.first);
-    return r;
+    if (pipelined && e->pipe_seq >= (uint64_t)rl_engine::kSets)
+        RL_CUDA(e, cudaStreamWaitEvent(e->sp, e->ev_main[k], 0));  // workspace set k is free again
+    if (hooks && hooks->pre_probe && (r = hooks->pre_probe(e->sp, k))) return r;
+    if ((r = launch_front(e, D, B, src, sf))) return r;
+    if (pipelined) {
+        RL_CUDA(e, cudaEventRecord(e->ev_part[k], e->sp));
+        RL_CUDA(e, cudaStreamWaitEvent(e->sm, e->ev_part[k], 0));
+    }
+    r = mode == 2 ? launch_main<RecordSrc, 2>(e, D, B, src, sr) : launch_main<RecordSrc, 0>(e, D, B, src, sr);
+    if (r) return r;
+    // per-namespace metrics (rl_ns_metrics_enable): one reduction kernel right behind the replay, same stream
+    if (e->ns_hook && !hooks && mode == 0 && o.limited &&
+        (r = e->ns_hook(e, sr, n, d_recs, compact_now ? 16 : 32, o.limited, o.first)))
+        return r;
+    if (!pipelined) return RL_OK;
+    if (hooks && hooks->post_main) {
+        // the hook (a sharded step's verdict return) runs on its own stream: the replay of the next call does
+        // not wait for it, only the reuse of this workspace set does
+        RL_CUDA(e, cudaEventRecord(e->ev_probe[k], e->sm));
+        RL_CUDA(e, cudaStreamWaitEvent(e->sq, e->ev_probe[k], 0));
+        if ((r = hooks->post_main(e->sq, k))) return r;
+        RL_CUDA(e, cudaEventRecord(e->ev_main[k], e->sq));
+    } else {
+        RL_CUDA(e, cudaEventRecord(e->ev_main[k], e->sm));
+    }
+    e->pipe_seq++;
+    e->pipe_pending = true;
+    return RL_OK;
 }
 
 int ensure_ready(rl_engine* e, uint64_t n, bool fence = true) {
@@ -750,21 +713,37 @@ int preload_main(rl_engine* e) {
     return RL_OK;
 }
 int preload_record_kernels(rl_engine* e) {
-    cudaFuncAttributes fa;
     int r = upload_tables(e);  // max_cells_used selects the k_main instantiation
     if (r) return r;
-    switch (e->cells) {
-        case 1:
-            RL_CUDA(e, cudaFuncGetAttributes(&fa, k_front<1, RecordSrc>));
-            return preload_main<1, 1>(e);
-        case 3:
-            RL_CUDA(e, cudaFuncGetAttributes(&fa, k_front<3, RecordSrc>));
-            return preload_main<3, 3>(e);
-        default:
-            RL_CUDA(e, cudaFuncGetAttributes(&fa, k_front<7, RecordSrc>));
-            if ((r = preload_main<7, 4>(e))) return r;
-            return preload_main<7, 7>(e);
-    }
+    return with_cells(e, [&](auto c) -> int {
+        constexpr int C = decltype(c)::value;
+        cudaFuncAttributes fa;
+        RL_CUDA(e, cudaFuncGetAttributes(&fa, k_front<C, RecordSrc>));
+        if (C != 7) return preload_main<C, C>(e);
+        if ((r = preload_main<7, 4>(e))) return r;
+        return preload_main<7, 7>(e);
+    });
+}
+
+// Allocates one workspace set for batches of up to max_counters accesses.
+int alloc_workset(rl_engine* e, WorkSet& w) {
+    const uint32_t P1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;  // cold partitions + hot slots + the no-row bucket
+    const size_t maxA = e->max_counters;
+    const size_t bufA = maxA + maxA / 128 + 256 * 1024 + 1024;  // part_idx/part_row: every tile's slice is a whole tile
+    const size_t max_items = (size_t)(1u << e->log2P) + maxA / 128 + 2;
+    RL_CUDA(e, w.tile_loc.reserve((size_t)(kMaxTiles + 1) * (P1 + 1)));
+    RL_CUDA(e, w.region_total.reserve(P1 + 1));
+    RL_CUDA(e, cudaMemsetAsync(w.region_total.p, 0, (P1 + 1) * sizeof(uint32_t), e->stream));
+    RL_CUDA(e, w.part_idx.reserve(bufA));
+    RL_CUDA(e, w.part_row.reserve(bufA));
+    RL_CUDA(e, w.row_of.reserve(maxA));
+    RL_CUDA(e, w.items.reserve(max_items));
+    RL_CUDA(e, w.chain_status.reserve(max_items));
+    RL_CUDA(e, w.chain_wcnt.reserve(max_items));
+    RL_CUDA(e, w.chain_w.reserve(max_items * 256));
+    RL_CUDA(e, w.small.reserve(8));
+    RL_CUDA(e, cudaMemsetAsync(w.small.p, 0, 8 * sizeof(uint32_t), e->stream));
+    return RL_OK;
 }
 
 }  // namespace
@@ -830,39 +809,24 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     if (cfg->flags & 1u) e->weak_slots = 1;  // RL_FLAG_DEBUG_WEAK_TAGS: four home slots in the grouping table
 
     const size_t bytes = (size_t)e->capacity * e->row_bytes;
-    RL_CUDA(e, cudaMalloc((void**)&e->d_rows, bytes));
-    RL_CUDA(e, cudaMemsetAsync(e->d_rows, 0, bytes, e->stream));
+    RL_CUDA(e, e->d_rows.reserve(bytes));
+    RL_CUDA(e, cudaMemsetAsync(e->d_rows.p, 0, bytes, e->stream));
 
-    const uint32_t P1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;  // cold partitions + hot slots + the no-row bucket
-    const size_t maxA = e->max_counters;
-    const size_t bufA = maxA + maxA / 128 + 256 * 1024 + 1024;  // part_idx/part_row: every tile's slice is a whole tile
-    RL_CUDA(e, e->d_tile_loc.reserve((size_t)(kMaxTiles + 1) * (P1 + 1)));
-    RL_CUDA(e, e->d_region_total.reserve(P1 + 1));
-    RL_CUDA(e, cudaMemsetAsync(e->d_region_total.p, 0, (P1 + 1) * sizeof(uint32_t), e->stream));
-    RL_CUDA(e, e->d_part_idx.reserve(bufA));
-    RL_CUDA(e, e->d_row_of.reserve(maxA));
-    RL_CUDA(e, e->d_part_row.reserve(bufA));
+    int r = alloc_workset(e, e->ws[0]);
+    if (r) return r;
     RL_CUDA(e, e->d_misc.reserve(MISC_N));
     RL_CUDA(e, cudaMemsetAsync(e->d_misc.p, 0, MISC_N * sizeof(uint32_t), e->stream));
     RL_CUDA(e, cudaMallocHost((void**)&e->h_misc, MISC_N * sizeof(uint32_t)));
-    RL_CUDA(e, e->d_acc.reserve(maxA));
+    RL_CUDA(e, e->d_acc.reserve(e->max_counters));
     RL_CUDA(e, e->d_kstats.reserve(32));
     RL_CUDA(e, cudaMemsetAsync(e->d_kstats.p, 0, 32 * sizeof(unsigned long long), e->stream));
-    RL_CUDA(e, e->d_items.reserve((size_t)(1u << e->log2P) + maxA / 128 + 2));
-    {
-        const size_t max_items = (size_t)(1u << e->log2P) + maxA / 128 + 2;
-        RL_CUDA(e, e->d_chain_status.reserve(max_items));
-        RL_CUDA(e, e->d_chain_wcnt.reserve(max_items));
-        RL_CUDA(e, e->d_chain_w.reserve(max_items * 256));
-    }
     RL_CUDA(e, e->d_delta.reserve(e->max_batch));
     RL_CUDA(e, e->d_now.reserve(e->max_batch));
     e->kernel_stats = (cfg->flags & RL_FLAG_KERNEL_STATS) != 0;
     e->hot_rows = (cfg->flags & RL_FLAG_HOT_ROWS) != 0;
     if (const char* v = getenv("RL_HOT")) e->hot_rows = atoi(v) != 0;
     RL_CUDA(e, e->d_hot.reserve(RL_HOT_SLOTS + RL_HOT_CAND + 4));
-    RL_CUDA(e, cudaMemsetAsync(e->d_hot.p, 0xFF, (RL_HOT_SLOTS + RL_HOT_CAND) * sizeof(uint32_t), e->stream));
-    RL_CUDA(e, cudaMemsetAsync(e->d_hot.p + RL_HOT_SLOTS + RL_HOT_CAND, 0, 4 * sizeof(uint32_t), e->stream));
+    if ((r = rl_internal_reset_hot_rows(e))) return r;
     RL_CUDA(e, e->d_misc2.reserve(4));
     RL_CUDA(e, cudaMemsetAsync(e->d_misc2.p, 0, 4 * sizeof(uint32_t), e->stream));
     if (cfg->flags & RL_FLAG_TRACE) {
@@ -880,22 +844,7 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
             RL_CUDA(e, cudaEventCreateWithFlags(&e->ev_probe[k], cudaEventDisableTiming));
             RL_CUDA(e, cudaEventCreateWithFlags(&e->ev_part[k], cudaEventDisableTiming));
             RL_CUDA(e, cudaEventCreateWithFlags(&e->ev_main[k], cudaEventDisableTiming));
-        }
-        const size_t max_items = (size_t)(1u << e->log2P) + maxA / 128 + 2;
-        for (int wi = 0; wi < rl_engine::kSets - 1; wi++) {
-        WorkSet& w = e->wsx[wi];
-        RL_CUDA(e, w.tile_loc.reserve((size_t)(kMaxTiles + 1) * (P1 + 1)));
-        RL_CUDA(e, w.region_total.reserve(P1 + 1));
-        RL_CUDA(e, cudaMemsetAsync(w.region_total.p, 0, (P1 + 1) * sizeof(uint32_t), e->stream));
-        RL_CUDA(e, w.part_idx.reserve(bufA));
-        RL_CUDA(e, w.part_row.reserve(bufA));
-        RL_CUDA(e, w.row_of.reserve(maxA));
-        RL_CUDA(e, w.items.reserve(max_items));
-        RL_CUDA(e, w.chain_status.reserve(max_items));
-        RL_CUDA(e, w.chain_wcnt.reserve(max_items));
-        RL_CUDA(e, w.chain_w.reserve(max_items * 256));
-        RL_CUDA(e, w.small.reserve(8));
-        RL_CUDA(e, cudaMemsetAsync(w.small.p, 0, 8 * sizeof(uint32_t), e->stream));
+            if (k > 0 && (r = alloc_workset(e, e->ws[k]))) return r;  // set 0 is allocated above
         }
     }
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -908,72 +857,25 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
 void rl_engine_destroy(rl_engine* e) {
     if (!e) return;
     cudaSetDevice(e->device);
-    if (e->sp) cudaStreamSynchronize(e->sp);
-    if (e->sm) cudaStreamSynchronize(e->sm);
+    for (cudaStream_t st : {e->sp, e->sm, e->sq, e->stream})
+        if (st) cudaStreamSynchronize(st);
+    // the maintenance state goes first, once its kernels (on e->stream and the replay stream) are done
     if (e->ext && e->ext_free) {
-        if (e->stream) cudaStreamSynchronize(e->stream);
         e->ext_free(e->ext);
         e->ext = nullptr;
     }
-    for (int k = 0; k < rl_engine::kRing; k++) {
-        e->ring_recs[k].release();
-        e->ring_lim[k].release();
-        e->ring_first[k].release();
-        if (e->ev_slot[k]) cudaEventDestroy(e->ev_slot[k]);
-    }
-    if (e->stream) cudaStreamSynchronize(e->stream);
-    for (int k = 0; k < rl_engine::kSets - 1; k++) e->wsx[k].release();
-    if (e->sq) cudaStreamSynchronize(e->sq);
+    for (cudaEvent_t ev : e->ev_slot)
+        if (ev) cudaEventDestroy(ev);
     if (e->ev_in) cudaEventDestroy(e->ev_in);
     for (int k = 0; k < rl_engine::kSets; k++) {
         if (e->ev_probe[k]) cudaEventDestroy(e->ev_probe[k]);
         if (e->ev_part[k]) cudaEventDestroy(e->ev_part[k]);
         if (e->ev_main[k]) cudaEventDestroy(e->ev_main[k]);
     }
-    if (e->sq) cudaStreamDestroy(e->sq);
-    if (e->sp) cudaStreamDestroy(e->sp);
-    if (e->sm) cudaStreamDestroy(e->sm);
-    if (e->d_rows) cudaFree(e->d_rows);
-    e->d_desc.release();
-    e->d_limits.release();
-    e->d_ns.release();
-    e->d_ns_limit_ids.release();
-    e->d_group_ns.release();
-    e->d_tile_loc.release();
-    e->d_region_total.release();
-    e->d_part_idx.release();
-    e->d_row_of.release();
-    e->d_part_row.release();
-    e->d_misc.release();
-    e->d_acc.release();
-    e->d_delta.release();
-    e->d_now.release();
-    e->d_fl_prev.release();
-    e->d_fl_next.release();
-    e->d_items.release();
-    e->d_kstats.release();
-    e->d_trace.release();
-    e->d_hot.release();
-    e->d_misc2.release();
-    e->d_chain_status.release();
-    e->d_chain_wcnt.release();
-    e->d_chain_w.release();
-    e->d_log_row.release();
-    e->d_log_state.release();
-    e->d_in_recs.release();
-    e->d_in_off.release();
-    e->d_in_ctrs.release();
-    e->d_in_delta.release();
-    e->d_in_now.release();
-    e->d_out_limited.release();
-    e->d_out_first.release();
-    e->d_out_rem.release();
-    e->d_out_ttl.release();
-    e->d_bucket.release();
-    e->d_bucket_counts.release();
+    for (cudaStream_t st : {e->sq, e->sp, e->sm, e->own_stream})
+        if (st) cudaStreamDestroy(st);
     if (e->h_misc) cudaFreeHost(e->h_misc);
-    if (e->own_stream) cudaStreamDestroy(e->own_stream);
-    delete e;
+    delete e;  // frees the device buffers, on the device made current above
 }
 
 int rl_engine_set_stream(rl_engine* e, void* cuda_stream) {
@@ -1164,14 +1066,11 @@ static int reset_selected(rl_engine* e, const std::vector<uint8_t>& sel) {
     RL_CUDA(e, cudaMemcpyAsync(d_sel.p, sel.data(), sel.size(), cudaMemcpyHostToDevice, e->stream));
     RlDev D = make_dev(e);
     const uint32_t blocks = ceil_div(e->capacity, 256);
-    switch (e->cells) {
-        case 1: k_reset<1><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 0, 0, d_sel.p, nullptr); break;
-        case 3: k_reset<3><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 0, 0, d_sel.p, nullptr); break;
-        default: k_reset<7><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 0, 0, d_sel.p, nullptr); break;
-    }
+    with_cells(e, [&](auto c) {
+        k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 0, 0, d_sel.p, nullptr);
+    });
     RL_LAUNCH_CHECK(e);
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    d_sel.release();
     return RL_OK;
 }
 
@@ -1209,17 +1108,11 @@ int rl_limits_delete(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
 
 int rl_clear(rl_engine* e) {
     if (!e) return RL_FATAL;
-    RL_CUDA(e, cudaSetDevice(e->device));
     // in_memory.rs:197-201 — only simple_limits is cleared
-    std::vector<uint8_t> sel(std::max<size_t>(e->limits.size(), 1), 0);
-    bool any = false;
+    std::vector<uint32_t> ids;
     for (size_t id = 0; id < e->limits.size(); id++)
-        if (e->limits[id].defined && !e->limits[id].qualified) {
-            sel[id] = 1;
-            any = true;
-            e->limits[id].simple_present = false;
-        }
-    return any ? reset_selected(e, sel) : RL_OK;
+        if (e->limits[id].defined && !e->limits[id].qualified) ids.push_back((uint32_t)id);
+    return rl_delete_counters(e, ids.data(), (uint32_t)ids.size());
 }
 
 int rl_sweep(rl_engine* e, uint64_t now_us, uint64_t* out_invalidated) {
@@ -1234,16 +1127,13 @@ int rl_sweep(rl_engine* e, uint64_t now_us, uint64_t* out_invalidated) {
     RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
     RlDev D = make_dev(e);
     const uint32_t blocks = ceil_div(e->capacity, 256);
-    switch (e->cells) {
-        case 1: k_reset<1><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 1, now_us, nullptr, d_cnt.p); break;
-        case 3: k_reset<3><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 1, now_us, nullptr, d_cnt.p); break;
-        default: k_reset<7><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 1, now_us, nullptr, d_cnt.p); break;
-    }
+    with_cells(e, [&](auto c) {
+        k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 1, now_us, nullptr, d_cnt.p);
+    });
     RL_LAUNCH_CHECK(e);
     unsigned long long cnt = 0;
     RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    d_cnt.release();
     if (out_invalidated) *out_invalidated = cnt;
     return RL_OK;
 }
@@ -1275,11 +1165,9 @@ static int scan_table(rl_engine* e, int mode, uint64_t now_us, const std::vector
     RlDev D = make_dev(e);
     RlScanOut O{d_lid.p, d_lo.p, d_hi.p, d_a.p, d_b.p, d_cnt.p, dcap};
     const uint32_t blocks = ceil_div(e->capacity, 256);
-    switch (e->cells) {
-        case 1: k_scan<1><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O); break;
-        case 3: k_scan<3><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O); break;
-        default: k_scan<7><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O); break;
-    }
+    with_cells(e, [&](auto c) {
+        k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O);
+    });
     RL_LAUNCH_CHECK(e);
     unsigned long long cnt = 0;
     RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
@@ -1294,13 +1182,6 @@ static int scan_table(rl_engine* e, int mode, uint64_t now_us, const std::vector
         RL_CUDA(e, cudaMemcpy(a.data(), d_a.p, got * 8, cudaMemcpyDeviceToHost));
         RL_CUDA(e, cudaMemcpy(b.data(), d_b.p, got * 8, cudaMemcpyDeviceToHost));
     }
-    d_lid.release();
-    d_lo.release();
-    d_hi.release();
-    d_a.release();
-    d_b.release();
-    d_cnt.release();
-    d_sel.release();
     // host fix-up of unqualified counters: present iff simple_present (in_memory.rs:14,38-44)
     uint64_t w = 0, total = 0;
     std::vector<uint8_t> seen(e->limits.size() + 1, 0);
@@ -1358,147 +1239,127 @@ int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_
 }
 
 // ---------------------------------------------------------------------------------------
-static int stage_outs(rl_engine* e, uint64_t n, uint64_t n_ctr_out, bool want_first, bool want_lc, Outs& dev) {
-    RL_CUDA(e, e->d_out_limited.reserve(e->max_batch));
-    dev.limited = e->d_out_limited.p;
-    if (want_first) {
-        RL_CUDA(e, e->d_out_first.reserve(e->max_batch));
-        dev.first = e->d_out_first.p;
+// Staging of the decision calls.  A call first normalises `mem`: RL_MEM_HOST_ASYNC stays only where the call can
+// take it (async_ok) and is RL_MEM_HOST everywhere else, as rl_engine.h promises.
+static int normalise_mem(rl_engine* e, int& mem, bool async_ok) {
+    if (mem == RL_MEM_HOST_ASYNC && !async_ok) mem = RL_MEM_HOST;
+    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE && mem != RL_MEM_HOST_ASYNC)
+        return fail(e, RL_FATAL, "mem must be RL_MEM_HOST, RL_MEM_DEVICE or RL_MEM_HOST_ASYNC (got %d)", mem);
+    return RL_OK;
+}
+
+// A record call's input on the device: the caller's buffer (RL_MEM_DEVICE), the next ring slot (RL_MEM_HOST_ASYNC)
+// or the staging buffer (RL_MEM_HOST).  rec_bytes: 32 (rl_record) or 16 (rl_record16).
+static int stage_records(rl_engine* e, int mem, uint64_t n, const void* recs, size_t rec_bytes, const rl_record*& d_recs) {
+    d_recs = static_cast<const rl_record*>(recs);
+    if (mem == RL_MEM_DEVICE) return RL_OK;
+    DevBuf<rl_record>* buf = &e->d_in_recs;
+    if (mem == RL_MEM_HOST_ASYNC) {
+        // H2D on the caller's stream (which carries nothing else of ours), kernels on the pipeline
+        // streams, D2H behind the replay: the copies of one call overlap the kernels of its neighbours.
+        const int slot = (int)(e->ring_seq % rl_engine::kRing);
+        buf = &e->ring_recs[slot];
+        if (e->ring_seq >= (uint64_t)rl_engine::kRing)
+            RL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_slot[slot], 0));  // slot drained (its D2H done)
     }
-    if (want_lc) {
-        RL_CUDA(e, e->d_out_rem.reserve(std::max<uint64_t>(n_ctr_out, e->max_counters)));
-        RL_CUDA(e, e->d_out_ttl.reserve(std::max<uint64_t>(n_ctr_out, e->max_counters)));
+    RL_CUDA(e, buf->reserve(e->max_batch));
+    RL_CUDA(e, cudaMemcpyAsync(buf->p, recs, n * rec_bytes, cudaMemcpyHostToDevice, e->stream));
+    d_recs = buf->p;
+    return RL_OK;
+}
+
+// Where the kernels write a call's outputs: the caller's buffers (RL_MEM_DEVICE), the current ring slot
+// (RL_MEM_HOST_ASYNC) or the staging buffers (RL_MEM_HOST; n_ctr remaining/ttl slots).  `user` holds the
+// caller's pointers, null where an output is not wanted.
+static int bind_outs(rl_engine* e, int mem, const Outs& user, uint64_t n_ctr, Outs& dev) {
+    dev = user;
+    if (mem == RL_MEM_DEVICE) return RL_OK;
+    const int slot = (int)(e->ring_seq % rl_engine::kRing);
+    DevBuf<uint8_t>& lim = mem == RL_MEM_HOST_ASYNC ? e->ring_lim[slot] : e->d_out_limited;
+    DevBuf<uint32_t>& first = mem == RL_MEM_HOST_ASYNC ? e->ring_first[slot] : e->d_out_first;
+    RL_CUDA(e, lim.reserve(e->max_batch));
+    dev.limited = lim.p;
+    if (user.first) {
+        RL_CUDA(e, first.reserve(e->max_batch));
+        dev.first = first.p;
+    }
+    if (user.rem || user.ttl) {  // RL_MEM_HOST only
+        RL_CUDA(e, e->d_out_rem.reserve(std::max<uint64_t>(n_ctr, e->max_counters)));
+        RL_CUDA(e, e->d_out_ttl.reserve(std::max<uint64_t>(n_ctr, e->max_counters)));
         dev.rem = e->d_out_rem.p;
         dev.ttl = e->d_out_ttl.p;
     }
-    (void)n;
+    return RL_OK;
+}
+
+// Copies a host-memory call's outputs back to the caller.  RL_MEM_HOST: on the engine's stream, then the device
+// error is checked.  RL_MEM_HOST_ASYNC: enqueued only, and the ring slot moves on.
+static int copy_back(rl_engine* e, int mem, uint64_t n, uint64_t n_ctr, const Outs& dev, const Outs& user) {
+    if (mem == RL_MEM_DEVICE) return RL_OK;
+    // The verdicts of an RL_MEM_HOST_ASYNC call leave on the replay stream itself, right behind their k_main.
+    // A dedicated copy stream parked on "replay done" looked cleaner, but streams share hardware queues:
+    // whenever it landed on the queue of the stream carrying the next H2D, that copy waited for the replay
+    // too and the whole pipeline serialised (the end-to-end rate fell to a fraction, one run in three).
+    const cudaStream_t sd = mem == RL_MEM_HOST_ASYNC ? e->sm : e->stream;
+    if (user.limited) RL_CUDA(e, cudaMemcpyAsync(user.limited, dev.limited, n, cudaMemcpyDeviceToHost, sd));
+    if (user.first) RL_CUDA(e, cudaMemcpyAsync(user.first, dev.first, n * 4, cudaMemcpyDeviceToHost, sd));
+    if (user.rem && n_ctr) RL_CUDA(e, cudaMemcpyAsync(user.rem, dev.rem, n_ctr * 8, cudaMemcpyDeviceToHost, sd));
+    if (user.ttl && n_ctr) RL_CUDA(e, cudaMemcpyAsync(user.ttl, dev.ttl, n_ctr * 8, cudaMemcpyDeviceToHost, sd));
+    if (mem == RL_MEM_HOST) return check_device_error(e);
+    const int slot = (int)(e->ring_seq % rl_engine::kRing);
+    RL_CUDA(e, cudaEventRecord(e->ev_slot[slot], sd));
+    e->d2h_pending = true;
+    e->d2h_last = slot;
+    e->ring_seq++;
     return RL_OK;
 }
 
 int rl_check_and_update_records(rl_engine* e, uint64_t n, const rl_record* recs, int load_counters, int mem,
                                 uint8_t* out_limited, uint32_t* out_first_limited, uint64_t* out_remaining,
                                 uint64_t* out_ttl_us, uint32_t out_stride) {
-    const bool host_async = (mem == RL_MEM_HOST_ASYNC) && e && e->pipeline && !e->any_multi_ns &&
-                            !(load_counters && (out_remaining || out_ttl_us));
-    if (mem == RL_MEM_HOST_ASYNC && !host_async) mem = RL_MEM_HOST;  // not available: plain synchronous call
-    int r = ensure_ready(e, n, mem == RL_MEM_HOST);
+    const bool lc = load_counters && (out_remaining || out_ttl_us);
+    int r = normalise_mem(e, mem, e && e->pipeline && !e->any_multi_ns && !lc);
     if (r) return r;
+    if ((r = ensure_ready(e, n, mem == RL_MEM_HOST))) return r;
     if (n == 0) return RL_OK;
     if (!recs || !out_limited) return fail(e, RL_FATAL, "null recs/out_limited");
-    const bool lc = load_counters && (out_remaining || out_ttl_us);
     if (lc && out_stride < e->max_ns_limits)
         return fail(e, RL_FATAL, "out_stride %u < limits per namespace %u", out_stride, e->max_ns_limits);
     e->stats.batches++;
     e->stats.requests += n;
     e->trace_seq = (uint32_t)e->stats.batches;
-    if (mem == RL_MEM_DEVICE) {
-        Outs o;
-        o.limited = out_limited;
-        o.first = out_first_limited;
-        o.rem = lc ? out_remaining : nullptr;
-        o.ttl = lc ? out_ttl_us : nullptr;
-        o.stride = out_stride;
-        return run_record_pipeline(e, (uint32_t)n, recs, 0, load_counters ? 1 : 0, o, true);
-    }
-    if (host_async) {
-        // H2D on the caller's stream (which carries nothing else of ours), kernels on the pipeline
-        // streams, D2H behind the replay: the copies of one call overlap the kernels of its neighbours.
-        const int slot = (int)(e->ring_seq % rl_engine::kRing);
-        RL_CUDA(e, e->ring_recs[slot].reserve(e->max_batch));
-        RL_CUDA(e, e->ring_lim[slot].reserve(e->max_batch));
-        if (out_first_limited) RL_CUDA(e, e->ring_first[slot].reserve(e->max_batch));
-        if (e->ring_seq >= (uint64_t)rl_engine::kRing)
-            RL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_slot[slot], 0));  // slot drained (its D2H done)
-        RL_CUDA(e, cudaMemcpyAsync(e->ring_recs[slot].p, recs, n * sizeof(rl_record), cudaMemcpyHostToDevice, e->stream));
-        Outs o;
-        o.limited = e->ring_lim[slot].p;
-        o.first = out_first_limited ? e->ring_first[slot].p : nullptr;
-        o.stride = out_stride;
-        if ((r = run_record_pipeline(e, (uint32_t)n, e->ring_recs[slot].p, 0, load_counters ? 1 : 0, o, true))) return r;
-        // The verdicts leave on the replay stream itself, right behind their k_main.  A dedicated copy
-        // stream parked on "replay done" looked cleaner, but streams share hardware queues: whenever
-        // it landed on the queue of the stream carrying the next H2D, that copy waited for the replay
-        // too and the whole pipeline serialised (the end-to-end rate fell to a fraction, one run in three).
-        cudaStream_t sd = e->sm;
-        RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, sd));
-        if (out_first_limited)
-            RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, sd));
-        RL_CUDA(e, cudaEventRecord(e->ev_slot[slot], sd));
-        e->d2h_pending = true;
-        e->d2h_last = slot;
-        e->ring_seq++;
-        return RL_OK;
-    }
-    RL_CUDA(e, e->d_in_recs.reserve(e->max_batch));
-    RL_CUDA(e, cudaMemcpyAsync(e->d_in_recs.p, recs, n * sizeof(rl_record), cudaMemcpyHostToDevice, e->stream));
-    Outs o;
+    const Outs user{out_limited, out_first_limited, lc ? out_remaining : nullptr, lc ? out_ttl_us : nullptr, nullptr,
+                    out_stride};
     const uint64_t nout = lc ? n * out_stride : 0;
-    if ((r = stage_outs(e, n, nout, out_first_limited != nullptr, lc, o))) return r;
-    o.stride = out_stride;
-    if (lc) {
+    const rl_record* d_recs;
+    Outs o;
+    if ((r = stage_records(e, mem, n, recs, sizeof(rl_record), d_recs)) || (r = bind_outs(e, mem, user, nout, o))) return r;
+    if (lc && mem == RL_MEM_HOST) {
         // slots of limits a namespace does not have stay 0
         RL_CUDA(e, cudaMemsetAsync(o.rem, 0, nout * 8, e->stream));
         RL_CUDA(e, cudaMemsetAsync(o.ttl, 0, nout * 8, e->stream));
     }
-    if ((r = run_record_pipeline(e, (uint32_t)n, e->d_in_recs.p, 0, load_counters ? 1 : 0, o))) return r;
-    RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, e->stream));
-    if (out_first_limited)
-        RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, e->stream));
-    if (lc && out_remaining) RL_CUDA(e, cudaMemcpyAsync(out_remaining, o.rem, nout * 8, cudaMemcpyDeviceToHost, e->stream));
-    if (lc && out_ttl_us) RL_CUDA(e, cudaMemcpyAsync(out_ttl_us, o.ttl, nout * 8, cudaMemcpyDeviceToHost, e->stream));
-    return check_device_error(e);
+    if ((r = run_record_pipeline(e, (uint32_t)n, d_recs, 0, load_counters ? 1 : 0, o, mem != RL_MEM_HOST))) return r;
+    return copy_back(e, mem, n, nout, o, user);
 }
 
 int rl_check_and_update_compact(rl_engine* e, uint64_t n, const rl_record16* recs, uint64_t now_us, int mem,
                                 uint8_t* out_limited, uint32_t* out_first_limited) {
-    const bool host_async = (mem == RL_MEM_HOST_ASYNC) && e && e->pipeline && !e->any_multi_ns;
-    if (mem == RL_MEM_HOST_ASYNC && !host_async) mem = RL_MEM_HOST;
-    int r = ensure_ready(e, n, mem == RL_MEM_HOST);
+    int r = normalise_mem(e, mem, e && e->pipeline && !e->any_multi_ns);
     if (r) return r;
+    if ((r = ensure_ready(e, n, mem == RL_MEM_HOST))) return r;
     if (n == 0) return RL_OK;
     if (!recs || !out_limited) return fail(e, RL_FATAL, "null recs/out_limited");
     if (now_us == 0) return fail(e, RL_FATAL, "now_us must be >= 1");
     e->stats.batches++;
     e->stats.requests += n;
     e->trace_seq = (uint32_t)e->stats.batches;
-    const rl_record* as32 = reinterpret_cast<const rl_record*>(recs);  // RecordSrc::compact reads 16-byte strides
-    if (mem == RL_MEM_DEVICE) {
-        Outs o;
-        o.limited = out_limited;
-        o.first = out_first_limited;
-        return run_record_pipeline(e, (uint32_t)n, as32, 0, 0, o, true, nullptr, 0, now_us);
-    }
-    if (host_async) {
-        const int slot = (int)(e->ring_seq % rl_engine::kRing);
-        RL_CUDA(e, e->ring_recs[slot].reserve(e->max_batch));
-        RL_CUDA(e, e->ring_lim[slot].reserve(e->max_batch));
-        if (out_first_limited) RL_CUDA(e, e->ring_first[slot].reserve(e->max_batch));
-        if (e->ring_seq >= (uint64_t)rl_engine::kRing)
-            RL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_slot[slot], 0));
-        RL_CUDA(e, cudaMemcpyAsync(e->ring_recs[slot].p, recs, n * sizeof(rl_record16), cudaMemcpyHostToDevice, e->stream));
-        Outs o;
-        o.limited = e->ring_lim[slot].p;
-        o.first = out_first_limited ? e->ring_first[slot].p : nullptr;
-        if ((r = run_record_pipeline(e, (uint32_t)n, e->ring_recs[slot].p, 0, 0, o, true, nullptr, 0, now_us))) return r;
-        cudaStream_t sd = e->sm;
-        RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, sd));
-        if (out_first_limited)
-            RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, sd));
-        RL_CUDA(e, cudaEventRecord(e->ev_slot[slot], sd));
-        e->d2h_pending = true;
-        e->d2h_last = slot;
-        e->ring_seq++;
-        return RL_OK;
-    }
-    RL_CUDA(e, e->d_in_recs.reserve(e->max_batch));
-    RL_CUDA(e, cudaMemcpyAsync(e->d_in_recs.p, recs, n * sizeof(rl_record16), cudaMemcpyHostToDevice, e->stream));
+    const Outs user{out_limited, out_first_limited};
+    const rl_record* d_recs;  // RecordSrc::compact reads 16-byte strides
     Outs o;
-    if ((r = stage_outs(e, n, 0, out_first_limited != nullptr, false, o))) return r;
-    if ((r = run_record_pipeline(e, (uint32_t)n, e->d_in_recs.p, 0, 0, o, false, nullptr, 0, now_us))) return r;
-    RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, e->stream));
-    if (out_first_limited)
-        RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, e->stream));
-    return check_device_error(e);
+    if ((r = stage_records(e, mem, n, recs, sizeof(rl_record16), d_recs)) || (r = bind_outs(e, mem, user, 0, o))) return r;
+    if ((r = run_record_pipeline(e, (uint32_t)n, d_recs, 0, 0, o, mem != RL_MEM_HOST, nullptr, 0, now_us))) return r;
+    return copy_back(e, mem, n, 0, o, user);
 }
 
 // Brings a CSR batch onto the device (or aliases it) and returns the total counter count.
@@ -1513,35 +1374,28 @@ struct CsrDev {
 static int stage_csr(rl_engine* e, uint64_t n, const uint32_t* off, const rl_counter* ctrs, const uint64_t* delta,
                      const uint64_t* now, int mem, CsrDev& d) {
     if (!off || !delta || !now) return fail(e, RL_FATAL, "null CSR arrays");
+    d = CsrDev{off, ctrs, delta, now, 0};
     if (mem == RL_MEM_DEVICE) {
         uint32_t last = 0;
         RL_CUDA(e, cudaMemcpyAsync(&last, off + n, 4, cudaMemcpyDeviceToHost, e->stream));
         RL_CUDA(e, cudaStreamSynchronize(e->stream));
-        d.off = off;
-        d.ctrs = ctrs;
-        d.delta = delta;
-        d.now = now;
         d.total = last;
     } else {
         d.total = off[n];
-        if (d.total > e->max_counters)
-            return fail(e, RL_FATAL, "batch has %llu counters > max_counters=%u", (unsigned long long)d.total, e->max_counters);
-        RL_CUDA(e, e->d_in_off.reserve(e->max_batch + 1));
-        RL_CUDA(e, e->d_in_ctrs.reserve(e->max_counters));
-        RL_CUDA(e, e->d_in_delta.reserve(e->max_batch));
-        RL_CUDA(e, e->d_in_now.reserve(e->max_batch));
-        RL_CUDA(e, cudaMemcpyAsync(e->d_in_off.p, off, (n + 1) * 4, cudaMemcpyHostToDevice, e->stream));
-        if (d.total)
-            RL_CUDA(e, cudaMemcpyAsync(e->d_in_ctrs.p, ctrs, d.total * sizeof(rl_counter), cudaMemcpyHostToDevice, e->stream));
-        RL_CUDA(e, cudaMemcpyAsync(e->d_in_delta.p, delta, n * 8, cudaMemcpyHostToDevice, e->stream));
-        RL_CUDA(e, cudaMemcpyAsync(e->d_in_now.p, now, n * 8, cudaMemcpyHostToDevice, e->stream));
-        d.off = e->d_in_off.p;
-        d.ctrs = e->d_in_ctrs.p;
-        d.delta = e->d_in_delta.p;
-        d.now = e->d_in_now.p;
     }
     if (d.total > e->max_counters)
         return fail(e, RL_FATAL, "batch has %llu counters > max_counters=%u", (unsigned long long)d.total, e->max_counters);
+    if (mem == RL_MEM_DEVICE) return RL_OK;
+    RL_CUDA(e, e->d_in_off.reserve(e->max_batch + 1));
+    RL_CUDA(e, e->d_in_ctrs.reserve(e->max_counters));
+    RL_CUDA(e, e->d_in_delta.reserve(e->max_batch));
+    RL_CUDA(e, e->d_in_now.reserve(e->max_batch));
+    RL_CUDA(e, cudaMemcpyAsync(e->d_in_off.p, off, (n + 1) * 4, cudaMemcpyHostToDevice, e->stream));
+    if (d.total)
+        RL_CUDA(e, cudaMemcpyAsync(e->d_in_ctrs.p, ctrs, d.total * sizeof(rl_counter), cudaMemcpyHostToDevice, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(e->d_in_delta.p, delta, n * 8, cudaMemcpyHostToDevice, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(e->d_in_now.p, now, n * 8, cudaMemcpyHostToDevice, e->stream));
+    d = CsrDev{e->d_in_off.p, e->d_in_ctrs.p, e->d_in_delta.p, e->d_in_now.p, d.total};
     return RL_OK;
 }
 
@@ -1549,8 +1403,9 @@ int rl_check_and_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off,
                               const uint64_t* delta, const uint64_t* now_us, int load_counters, int mem,
                               uint8_t* out_limited, uint32_t* out_first_limited, uint64_t* out_remaining,
                               uint64_t* out_ttl_us) {
-    int r = ensure_ready(e, n);
+    int r = normalise_mem(e, mem, false);
     if (r) return r;
+    if ((r = ensure_ready(e, n))) return r;
     if (n == 0) return RL_OK;
     if (!out_limited) return fail(e, RL_FATAL, "null out_limited");
     CsrDev c;
@@ -1558,15 +1413,9 @@ int rl_check_and_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off,
     const bool lc = load_counters && (out_remaining || out_ttl_us);
     e->stats.batches++;
     e->stats.requests += n;
+    const Outs user{out_limited, out_first_limited, lc ? out_remaining : nullptr, lc ? out_ttl_us : nullptr};
     Outs o;
-    if (mem == RL_MEM_DEVICE) {
-        o.limited = out_limited;
-        o.first = out_first_limited;
-        o.rem = lc ? out_remaining : nullptr;
-        o.ttl = lc ? out_ttl_us : nullptr;
-    } else {
-        if ((r = stage_outs(e, n, c.total, out_first_limited != nullptr, lc, o))) return r;
-    }
+    if ((r = bind_outs(e, mem, user, c.total, o))) return r;
     o.off = c.off;
     RlDev D = make_dev(e);
     RlResolveOut O{e->d_acc.p, nullptr, nullptr, o.limited, o.first};
@@ -1576,23 +1425,14 @@ int rl_check_and_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off,
     if (c.total) {
         if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 0, load_counters ? 1 : 0, o))) return r;
     }
-    if (mem == RL_MEM_HOST) {
-        RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, e->stream));
-        if (out_first_limited)
-            RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, e->stream));
-        if (lc && out_remaining && c.total)
-            RL_CUDA(e, cudaMemcpyAsync(out_remaining, o.rem, c.total * 8, cudaMemcpyDeviceToHost, e->stream));
-        if (lc && out_ttl_us && c.total)
-            RL_CUDA(e, cudaMemcpyAsync(out_ttl_us, o.ttl, c.total * 8, cudaMemcpyDeviceToHost, e->stream));
-        return check_device_error(e);
-    }
-    return RL_OK;
+    return copy_back(e, mem, n, c.total, o, user);
 }
 
 int rl_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off, const rl_counter* ctrs, const uint64_t* delta,
                     const uint64_t* now_us, int mem) {
-    int r = ensure_ready(e, n);
+    int r = normalise_mem(e, mem, false);
     if (r) return r;
+    if ((r = ensure_ready(e, n))) return r;
     if (n == 0) return RL_OK;
     CsrDev c;
     if ((r = stage_csr(e, n, ctr_off, ctrs, delta, now_us, mem, c))) return r;
@@ -1606,94 +1446,64 @@ int rl_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off, const rl_
     RL_LAUNCH_CHECK(e);
     if ((r = check_resolve_error(e))) return r;
     if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 2, 0, o))) return r;
-    if (mem == RL_MEM_HOST) return check_device_error(e);
-    return RL_OK;
+    return copy_back(e, mem, n, 0, o, o);
 }
 
 int rl_update_records(rl_engine* e, uint64_t n, const rl_record* recs, int mem) {
-    int r = ensure_ready(e, n, mem != RL_MEM_DEVICE);
+    int r = normalise_mem(e, mem, false);
     if (r) return r;
+    if ((r = ensure_ready(e, n, mem != RL_MEM_DEVICE))) return r;
     if (n == 0) return RL_OK;
     if (!recs) return fail(e, RL_FATAL, "null recs");
     e->stats.batches++;
     e->stats.requests += n;
-    const rl_record* d_recs = recs;
-    if (mem == RL_MEM_HOST) {
-        RL_CUDA(e, e->d_in_recs.reserve(e->max_batch));
-        RL_CUDA(e, cudaMemcpyAsync(e->d_in_recs.p, recs, n * sizeof(rl_record), cudaMemcpyHostToDevice, e->stream));
-        d_recs = e->d_in_recs.p;
-    }
+    const rl_record* d_recs;
+    if ((r = stage_records(e, mem, n, recs, sizeof(rl_record), d_recs))) return r;
     Outs o;
     if ((r = run_record_pipeline(e, (uint32_t)n, d_recs, 2, 0, o, mem == RL_MEM_DEVICE))) return r;
-    if (mem == RL_MEM_HOST) return check_device_error(e);
-    return RL_OK;
+    return copy_back(e, mem, n, 0, o, o);
 }
 
 int rl_is_within_limits_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off, const rl_counter* ctrs,
                               const uint64_t* delta, const uint64_t* now_us, int mem, uint8_t* out_limited,
                               uint32_t* out_first_limited) {
-    int r = ensure_ready(e, n);
+    int r = normalise_mem(e, mem, false);
     if (r) return r;
+    if ((r = ensure_ready(e, n))) return r;
     if (n == 0) return RL_OK;
     if (!out_limited) return fail(e, RL_FATAL, "null out_limited");
     CsrDev c;
     if ((r = stage_csr(e, n, ctr_off, ctrs, delta, now_us, mem, c))) return r;
+    const Outs user{out_limited, out_first_limited};
     Outs o;
-    if (mem == RL_MEM_DEVICE) {
-        o.limited = out_limited;
-        o.first = out_first_limited;
-    } else if ((r = stage_outs(e, n, 0, out_first_limited != nullptr, false, o))) {
-        return r;
-    }
+    if ((r = bind_outs(e, mem, user, 0, o))) return r;
     RlDev D = make_dev(e);
-    const uint32_t blocks = ceil_div(n, 128);
-    switch (e->cells) {
-        case 1: k_query_csr<1><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, c.delta, c.now, o.limited, o.first); break;
-        case 3: k_query_csr<3><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, c.delta, c.now, o.limited, o.first); break;
-        default: k_query_csr<7><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, c.delta, c.now, o.limited, o.first); break;
-    }
+    with_cells(e, [&](auto cl) {
+        k_query_csr<decltype(cl)::value><<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, c.delta,
+                                                                                   c.now, o.limited, o.first);
+    });
     RL_LAUNCH_CHECK(e);
-    if (mem == RL_MEM_HOST) {
-        RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, e->stream));
-        if (out_first_limited)
-            RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, e->stream));
-        return check_device_error(e);
-    }
-    return RL_OK;
+    return copy_back(e, mem, n, 0, o, user);
 }
 
 int rl_is_within_limits_records(rl_engine* e, uint64_t n, const rl_record* recs, int mem, uint8_t* out_limited,
                                 uint32_t* out_first_limited) {
-    int r = ensure_ready(e, n);
+    int r = normalise_mem(e, mem, false);
     if (r) return r;
+    if ((r = ensure_ready(e, n))) return r;
     if (n == 0) return RL_OK;
     if (!recs || !out_limited) return fail(e, RL_FATAL, "null recs/out_limited");
-    const rl_record* d_recs = recs;
+    const Outs user{out_limited, out_first_limited};
+    const rl_record* d_recs;
     Outs o;
-    if (mem == RL_MEM_DEVICE) {
-        o.limited = out_limited;
-        o.first = out_first_limited;
-    } else {
-        RL_CUDA(e, e->d_in_recs.reserve(e->max_batch));
-        RL_CUDA(e, cudaMemcpyAsync(e->d_in_recs.p, recs, n * sizeof(rl_record), cudaMemcpyHostToDevice, e->stream));
-        d_recs = e->d_in_recs.p;
-        if ((r = stage_outs(e, n, 0, out_first_limited != nullptr, false, o))) return r;
-    }
+    if ((r = stage_records(e, mem, n, recs, sizeof(rl_record), d_recs)) || (r = bind_outs(e, mem, user, 0, o))) return r;
     RlDev D = make_dev(e);
-    const uint32_t blocks = ceil_div(n, 128);
-    switch (e->cells) {
-        case 1: k_query_records<1><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, d_recs, o.limited, o.first); break;
-        case 3: k_query_records<3><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, d_recs, o.limited, o.first); break;
-        default: k_query_records<7><<<blocks, 128, 0, e->stream>>>(D, (uint32_t)n, d_recs, o.limited, o.first); break;
-    }
+    with_cells(e, [&](auto c) {
+        k_query_records<decltype(c)::value><<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, d_recs, o.limited,
+                                                                                     o.first);
+    });
     RL_LAUNCH_CHECK(e);
-    if (mem == RL_MEM_HOST) {
-        RL_CUDA(e, cudaMemcpyAsync(out_limited, o.limited, n, cudaMemcpyDeviceToHost, e->stream));
-        if (out_first_limited)
-            RL_CUDA(e, cudaMemcpyAsync(out_first_limited, o.first, n * 4, cudaMemcpyDeviceToHost, e->stream));
-        return check_device_error(e);
-    }
-    return RL_OK;
+    return copy_back(e, mem, n, 0, o, user);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1802,7 +1612,7 @@ int rl_internal_view(rl_engine* e, RlTableView* out) {
     if (r) return r;
     r = upload_tables(e);
     if (r) return r;
-    out->rows = e->d_rows;
+    out->rows = e->d_rows.p;
     out->cells = e->cells;
     out->log2P = e->log2P;
     out->log2R = e->log2R;

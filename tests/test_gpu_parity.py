@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 from limitador_b200 import Engine, EngineError
+from limitador_b200 import engine as engine_module
 from limitador_b200 import streams
 from limitador_b200.engine import LIMIT_DESC_DTYPE, NONE, RECORD_DTYPE, COUNTER_DTYPE
 from tests import helpers as H
@@ -149,6 +150,29 @@ def test_update_and_is_within_limits_batches():
     lim, fl = e.is_within_limits_records(recs)
     wl, wf, _, _ = o.batch_records(1, recs)
     assert lim.tolist() == wl.tolist() and fl.tolist() == wf.tolist()
+
+
+@pytest.mark.parametrize("flags", [0, 2])
+def test_host_async_mem_acts_as_host_where_a_call_cannot_take_it(flags, monkeypatch):
+    """RL_MEM_HOST_ASYNC behaves like RL_MEM_HOST outside the record check calls (rl_engine.h): the query calls
+    and the CSR check write their outputs to host memory before they return."""
+    descs = H.mixed_limits(n_ns=12, seed=9)
+    e_host = engine_with_limits(descs, 3, regions=4, flags=flags)
+    e_async = engine_with_limits(descs, 3, regions=4, flags=flags)
+    for b in range(3):
+        off, ctrs, delta, now = H.random_csr_stream(descs, 1500, 700 + b, n_keys=4)
+        recs = H.random_records(descs, 1500, 800 + b, n_keys=4)
+        want = [e_host.check_and_update_batch(off, ctrs, delta, now, True),
+                e_host.is_within_limits_batch(off, ctrs, delta, now), e_host.is_within_limits_records(recs)]
+        with monkeypatch.context() as m:
+            m.setattr(engine_module, "MEM_HOST", engine_module.MEM_HOST_ASYNC)  # what the Engine methods pass as mem
+            got = [e_async.check_and_update_batch(off, ctrs, delta, now, True),
+                   e_async.is_within_limits_batch(off, ctrs, delta, now), e_async.is_within_limits_records(recs)]
+        for w, g in zip(want, got):
+            for k in range(len(w)):
+                assert g[k].tolist() == w[k].tolist(), f"output {k} differs in batch {b}"
+        assert int(want[0][0].sum()) > 0  # some request was limited: the outputs differ from their initial values
+    assert_tables_equal(e_async, e_host, descs)
 
 
 def test_hot_key_spanning_many_chunks():
