@@ -265,6 +265,34 @@ int rl_dump_table(rl_engine *e, uint64_t cap, uint32_t *out_limit_id, uint64_t *
                   uint64_t *out_key_hi, uint64_t *out_value, uint64_t *out_expiry_us,
                   uint64_t *out_count);
 
+/* ---- Counter snapshots: restart, resize or re-shard an engine without losing counters -----------------------------
+ * A snapshot is the five arrays rl_dump_table returns.  Export it from one engine and import it into another (one with
+ * another capacity, cells_per_row or region count, or another rank of a sharded store): the counters go on exactly
+ * where they were.  Limit ids are the caller's: the target must register the same limits under the same ids
+ * (rl_limits_get lists them) before the import.  No reference function: the reference keeps counters across restarts
+ * only in its disk store (limitador/src/storage/disk/rocksdb_storage.rs). */
+/* Every present counter of the selected namespaces (ns_ids == NULL: all), as rl_dump_table reports them.
+ * now_us == 0: the exact state.  now_us > 0: qualified counters with 0 < expiry <= now_us are left out, i.e. the
+ * state rl_sweep(now_us) would leave.  mem = RL_MEM_HOST or RL_MEM_DEVICE for the five outputs; unordered (the
+ * counters of one row are adjacent), at most cap written, *out_count = number found (may exceed cap).  Does not
+ * change the table. */
+int rl_counters_export(rl_engine *e, const uint32_t *ns_ids, uint32_t n_ns, uint64_t now_us, uint64_t cap, int mem,
+                       uint32_t *out_limit_id, uint64_t *out_key_lo, uint64_t *out_key_hi,
+                       uint64_t *out_value, uint64_t *out_expiry_us, uint64_t *out_count);
+/* Set n counters to exactly (value, expiry_us).  A present counter is replaced; other counters are untouched (import
+ * into a fresh engine for a clone).  limit_id is resolved against THIS engine's registry, so the target may have
+ * another capacity, cells_per_row, region count or row-group assignment.  The key is ignored for unqualified limits,
+ * whose counters become present (as after add_counter).  Refused with RL_FATAL before any counter changes: unknown
+ * limit id, key_hi >= 2^32, a qualified counter with expiry 0, the same counter twice.  A full region: RL_TRANSIENT,
+ * and again no counter changes (a refused call leaves the table as it was, rows included).  rl_last_error names the
+ * first refused entry.  Serialise with the request path (as
+ * rl_compact). */
+int rl_counters_import(rl_engine *e, uint64_t n, const uint32_t *limit_id, const uint64_t *key_lo,
+                       const uint64_t *key_hi, const uint64_t *value, const uint64_t *expiry_us, int mem);
+/* Every registered limit, ascending id (what a snapshot must be restored against).  At most cap written,
+ * *out_n = number registered. */
+int rl_limits_get(rl_engine *e, uint32_t cap, rl_limit_desc *out, uint32_t *out_n);
+
 /* Measurement aid (bench.py roofline leg): between begin and end the engine brackets every
  * launch of its dominant kernel (k_main) with CUDA events on the launching stream;
  * end() synchronises and returns the summed device time and the launch count. */

@@ -42,3 +42,14 @@ __device__ __forceinline__ unsigned long long rlm_ld64(const void* p) { return _
 #else
 inline unsigned long long rlm_ld64(const void* p) { return *reinterpret_cast<const unsigned long long*>(p); }
 #endif
+
+// atomic OR of a 32-bit word; returns the old value
+#if !defined(RL_SHIM) && !defined(RL_SIMT)
+__device__ __forceinline__ unsigned rlm_or(unsigned* p, unsigned v) { return atomicOr(p, v); }
+#else
+inline unsigned rlm_or(unsigned* p, unsigned v) {
+    const unsigned o = *p;
+    *p = o | v;
+    return o;
+}
+#endif

@@ -1163,7 +1163,7 @@ static int scan_table(rl_engine* e, int mode, uint64_t now_us, const std::vector
     if (!ns_sel.empty())
         RL_CUDA(e, cudaMemcpyAsync(d_sel.p, ns_sel.data(), ns_sel.size(), cudaMemcpyHostToDevice, e->stream));
     RlDev D = make_dev(e);
-    RlScanOut O{d_lid.p, d_lo.p, d_hi.p, d_a.p, d_b.p, d_cnt.p, dcap};
+    RlScanOut O{d_lid.p, d_lo.p, d_hi.p, d_a.p, d_b.p, d_cnt.p, dcap, nullptr, nullptr};
     const uint32_t blocks = ceil_div(e->capacity, 256);
     with_cells(e, [&](auto c) {
         k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O);
@@ -1236,6 +1236,117 @@ int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_
     }
     return scan_table(e, 1, now_us, ns_sel, cap, out_limit_id, out_key_lo, out_key_hi, out_remaining, out_ttl_us,
                       out_count);
+}
+
+int rl_counters_export(rl_engine* e, const uint32_t* ns_ids, uint32_t n_ns, uint64_t now_us, uint64_t cap, int mem,
+                       uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_value,
+                       uint64_t* out_expiry_us, uint64_t* out_count) {
+    if (!e) return RL_FATAL;
+    RL_CUDA(e, cudaSetDevice(e->device));
+    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE)
+        return fail(e, RL_FATAL, "rl_counters_export: mem must be RL_MEM_HOST or RL_MEM_DEVICE (got %d)", mem);
+    if (cap && (!out_limit_id || !out_key_lo || !out_key_hi || !out_value || !out_expiry_us))
+        return fail(e, RL_FATAL, "rl_counters_export: cap > 0 needs all five output arrays");
+    if (n_ns && !ns_ids) return fail(e, RL_FATAL, "rl_counters_export: n_ns > 0 with ns_ids == NULL");
+    int r = pipe_fence(e);
+    if (r) return r;
+    r = upload_tables(e);
+    if (r) return r;
+    // the namespace selection (empty = every namespace) and the limits whose counters exist
+    std::vector<uint8_t> ns_sel;
+    if (ns_ids) {
+        ns_sel.assign(std::max<size_t>(e->ns_limits.size(), 1), 0);
+        for (uint32_t i = 0; i < n_ns; i++)
+            if (ns_ids[i] < ns_sel.size()) ns_sel[ns_ids[i]] = 1;
+    }
+    const uint32_t L = e->limits_cap;
+    std::vector<uint8_t> flags(2 * (size_t)L, 0);  // present [L] | seen [L]
+    for (size_t l = 0; l < e->limits.size(); l++)
+        flags[l] = e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
+    DevBuf<uint8_t> d_sel, d_flags;
+    DevBuf<unsigned long long> d_cnt;
+    RL_CUDA(e, d_sel.reserve(std::max<size_t>(ns_sel.size(), 1)));
+    RL_CUDA(e, d_flags.reserve(flags.size()));
+    RL_CUDA(e, d_cnt.reserve(1));
+    // outputs: the caller's device arrays, or staging no larger than the table's cells
+    DevBuf<uint32_t> s_lid;
+    DevBuf<uint64_t> s_lo, s_hi, s_val, s_exp;
+    uint64_t dcap = cap;
+    RlScanOut O{out_limit_id, out_key_lo, out_key_hi, out_value, out_expiry_us, d_cnt.p, cap, d_flags.p, d_flags.p + L};
+    if (mem == RL_MEM_HOST) {
+        dcap = std::min<uint64_t>(cap, e->capacity * e->cells);
+        const size_t n = std::max<uint64_t>(dcap, 1);
+        RL_CUDA(e, s_lid.reserve(n));
+        RL_CUDA(e, s_lo.reserve(n));
+        RL_CUDA(e, s_hi.reserve(n));
+        RL_CUDA(e, s_val.reserve(n));
+        RL_CUDA(e, s_exp.reserve(n));
+        O = RlScanOut{s_lid.p, s_lo.p, s_hi.p, s_val.p, s_exp.p, d_cnt.p, dcap, d_flags.p, d_flags.p + L};
+    }
+    RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
+    if (!ns_sel.empty()) RL_CUDA(e, cudaMemcpyAsync(d_sel.p, ns_sel.data(), ns_sel.size(), cudaMemcpyHostToDevice, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(d_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, e->stream));
+    RlDev D = make_dev(e);
+    const uint32_t blocks = ceil_div(e->capacity, 256);
+    const uint8_t* sel = ns_sel.empty() ? nullptr : d_sel.p;
+    with_cells(e, [&](auto c) {
+        k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 2, now_us, sel, e->d_group_ns.p, O);
+    });
+    RL_LAUNCH_CHECK(e);
+    unsigned long long cnt = 0;
+    RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(flags.data() + L, d_flags.p + L, L, cudaMemcpyDeviceToHost, e->stream));
+    RL_CUDA(e, cudaStreamSynchronize(e->stream));
+    // present unqualified limits of the selected namespaces whose row was never touched: (l, 0, 0, 0, 0), appended
+    std::vector<uint32_t> extra;
+    for (size_t l = 0; l < e->limits.size(); l++) {
+        const HostLimit& h = e->limits[l];
+        if (h.defined && !h.qualified && h.simple_present && !flags[L + l] && (ns_sel.empty() || ns_sel[h.ns]))
+            extra.push_back((uint32_t)l);
+    }
+    const uint64_t fit = cnt < cap ? std::min<uint64_t>(extra.size(), cap - cnt) : 0;
+    if (mem == RL_MEM_HOST) {
+        const uint64_t got = std::min<uint64_t>(cnt, dcap);
+        if (got) {
+            RL_CUDA(e, cudaMemcpy(out_limit_id, s_lid.p, got * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+            RL_CUDA(e, cudaMemcpy(out_key_lo, s_lo.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+            RL_CUDA(e, cudaMemcpy(out_key_hi, s_hi.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+            RL_CUDA(e, cudaMemcpy(out_value, s_val.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+            RL_CUDA(e, cudaMemcpy(out_expiry_us, s_exp.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        }
+        for (uint64_t k = 0; k < fit; k++) {
+            out_limit_id[cnt + k] = extra[k];
+            out_key_lo[cnt + k] = out_key_hi[cnt + k] = out_value[cnt + k] = out_expiry_us[cnt + k] = 0;
+        }
+    } else if (fit) {
+        const std::vector<uint64_t> zero(fit, 0);
+        RL_CUDA(e, cudaMemcpy(out_limit_id + cnt, extra.data(), fit * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        for (uint64_t* o : {out_key_lo, out_key_hi, out_value, out_expiry_us})
+            RL_CUDA(e, cudaMemcpy(o + cnt, zero.data(), fit * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    }
+    if (out_count) *out_count = cnt + extra.size();
+    return RL_OK;
+}
+
+int rl_limits_get(rl_engine* e, uint32_t cap, rl_limit_desc* out, uint32_t* out_n) {
+    if (!e) return RL_FATAL;
+    if (cap && !out) return fail(e, RL_FATAL, "rl_limits_get: cap > 0 with out == NULL");
+    uint32_t n = 0;
+    for (size_t id = 0; id < e->limits.size(); id++) {
+        const HostLimit& l = e->limits[id];
+        if (!l.defined) continue;
+        if (n < cap) {
+            out[n].limit_id = (uint32_t)id;
+            out[n].ns_id = l.ns;
+            out[n].varset_id = l.varset;
+            out[n].qualified = l.qualified;
+            out[n].max_value = l.max_value;
+            out[n].window_us = l.window_us;
+        }
+        n++;
+    }
+    if (out_n) *out_n = n;
+    return RL_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1620,6 +1731,7 @@ int rl_internal_view(rl_engine* e, RlTableView* out) {
     out->capacity = e->capacity;
     out->ns_cap = e->ns_cap;
     out->limits_cap = e->limits_cap;
+    out->limits = e->d_limits.p;
     out->stream = e->stream;
     out->device = e->device;
     return RL_OK;
@@ -1638,4 +1750,8 @@ int rl_internal_reset_hot_rows(rl_engine* e) {
     RL_CUDA(e, cudaMemsetAsync(e->d_hot.p, 0xFF, (RL_HOT_SLOTS + RL_HOT_CAND) * sizeof(uint32_t), e->stream));
     RL_CUDA(e, cudaMemsetAsync(e->d_hot.p + RL_HOT_SLOTS + RL_HOT_CAND, 0, 4 * sizeof(uint32_t), e->stream));
     return RL_OK;
+}
+void rl_internal_mark_present(rl_engine* e, const uint8_t* flags, uint32_t n) {
+    for (uint32_t l = 0; l < n && l < e->limits.size(); l++)
+        if (flags[l] && e->limits[l].defined && !e->limits[l].qualified) e->limits[l].simple_present = true;
 }

@@ -11,6 +11,7 @@ struct RlTableView {
     uint32_t cells, log2P, log2R, row_bytes;
     uint64_t capacity;  // rows
     uint32_t ns_cap, limits_cap;
+    const RlLimitDev* limits;  // [limits_cap] device limit table: group (0 = not registered), cell, qualified
     cudaStream_t stream;
     int device;
 };
@@ -29,3 +30,5 @@ void** rl_internal_ext(rl_engine* e, void (*ext_free)(void*));  // slot for rl_m
 void rl_internal_set_ns_hook(rl_engine* e, rl_ns_hook_fn fn);
 // forget the hot-row table (rows move when a region is rebuilt); enqueued on the engine's stream
 int rl_internal_reset_hot_rows(rl_engine* e);
+// the unqualified limits l with flags[l] != 0 (l < n) have a counter again (as after add_counter): host registry only
+void rl_internal_mark_present(rl_engine* e, const uint8_t* flags, uint32_t n);

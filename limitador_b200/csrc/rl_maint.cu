@@ -262,4 +262,88 @@ int rl_compact(rl_engine* e, uint32_t min_tombstone_pct, rl_compact_stats* out) 
     return RL_OK;
 }
 
+int rl_counters_import(rl_engine* e, uint64_t n, const uint32_t* limit_id, const uint64_t* key_lo, const uint64_t* key_hi,
+                       const uint64_t* value, const uint64_t* expiry_us, int mem) {
+    RlTableView v;
+    int r = rl_internal_view(e, &v);
+    if (r) return r;
+    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE)
+        return rl_internal_fail(e, RL_FATAL, "rl_counters_import: mem must be RL_MEM_HOST or RL_MEM_DEVICE");
+    if (n && (!limit_id || !key_lo || !key_hi || !value || !expiry_us))
+        return rl_internal_fail(e, RL_FATAL, "rl_counters_import: n > 0 needs all five input arrays");
+    if (n >= (1ull << 48)) return rl_internal_fail(e, RL_FATAL, "rl_counters_import: n must stay below 2^48");
+    if (n == 0) return RL_OK;
+    // inputs on the device: the caller's arrays, or staged for the call
+    Scratch<uint32_t> s_lid;
+    Scratch<uint64_t> s_words;  // key_lo | key_hi | value | expiry, n each
+    RlImportIn I{limit_id, key_lo, key_hi, value, expiry_us, n};
+    if (mem == RL_MEM_HOST) {
+        RLM_CUDA(e, s_lid.alloc(n));
+        RLM_CUDA(e, s_words.alloc(4 * n));
+        RLM_CUDA(e, cudaMemcpyAsync(s_lid.p, limit_id, n * sizeof(uint32_t), cudaMemcpyHostToDevice, v.stream));
+        const uint64_t* src[4] = {key_lo, key_hi, value, expiry_us};
+        for (int k = 0; k < 4; k++)
+            RLM_CUDA(e, cudaMemcpyAsync(s_words.p + k * n, src[k], n * sizeof(uint64_t), cudaMemcpyHostToDevice, v.stream));
+        I = RlImportIn{s_lid.p, s_words.p, s_words.p + n, s_words.p + 2 * n, s_words.p + 3 * n, n};
+    }
+    const RlImportTab T{v.rows, v.row_bytes, v.log2P, v.log2R, v.limits, v.limits_cap};
+    Scratch<unsigned long long> d_err, d_row_of;
+    Scratch<uint8_t> d_unq;
+    Scratch<unsigned> d_mask;  // per-row cell mask of this call
+    RLM_CUDA(e, d_err.alloc(1));
+    RLM_CUDA(e, d_unq.alloc(v.limits_cap));
+    RLM_CUDA(e, cudaMemsetAsync(d_err.p, 0xFF, sizeof(unsigned long long), v.stream));
+    RLM_CUDA(e, cudaMemsetAsync(d_unq.p, 0, v.limits_cap, v.stream));
+    const uint32_t threads = 256;
+    const uint32_t blocks = (uint32_t)((n + threads - 1) / threads);
+    unsigned long long err = ~0ull;
+    auto report = [&](const char* pass) {
+        const uint64_t idx = err >> 8;
+        const uint32_t why = (uint32_t)(err & 0xFF);
+        static const char* const reason[] = {"", "limit id not registered in this engine", "qualified counter with key_hi >= 2^32",
+                                             "qualified counter with expiry 0", "the same counter appears twice",
+                                             "its table region is full"};
+        char b[256];
+        snprintf(b, sizeof b, "rl_counters_import: entry %llu refused (%s) in the %s pass; no counter changed",
+                 (unsigned long long)idx, why <= RLM_IMP_TABLE_FULL ? reason[why] : "?", pass);
+        return rl_internal_fail(e, why == RLM_IMP_TABLE_FULL ? RL_TRANSIENT : RL_FATAL, b);
+    };
+    // pass 1: every entry names a registered limit and a valid key / expiry
+    k_import_resolve<<<blocks, threads, 0, v.stream>>>(T, I, d_err.p, d_unq.p);
+    RLM_CUDA(e, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    RLM_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
+    RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+    if (err != ~0ull) return report("resolve");
+    // pass 2: find or claim the rows; duplicates and full regions are found before any cell is written
+    RLM_CUDA(e, d_row_of.alloc(n));
+    if (d_mask.alloc(v.capacity) != cudaSuccess) {
+        cudaGetLastError();
+        return rl_internal_fail(e, RL_TRANSIENT, "rl_counters_import: no device memory for the per-row cell mask");
+    }
+    RLM_CUDA(e, cudaMemsetAsync(d_mask.p, 0, v.capacity * sizeof(unsigned), v.stream));
+    RLM_CUDA(e, cudaMemsetAsync(d_row_of.p, 0, n * sizeof(unsigned long long), v.stream));
+    k_import_claim<<<blocks, threads, 0, v.stream>>>(T, I, d_row_of.p, d_mask.p, d_err.p);
+    RLM_CUDA(e, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    RLM_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
+    RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+    if (err != ~0ull) {  // give back the rows this call claimed: the table is byte-identical to before the call
+        k_import_release<<<blocks, threads, 0, v.stream>>>(T, n, d_row_of.p);
+        RLM_CUDA(e, cudaGetLastError());
+        rl_internal_launched(e, 1);
+        RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+        return report("claim");
+    }
+    // pass 3: the cells
+    k_import_write<<<blocks, threads, 0, v.stream>>>(T, I, d_row_of.p);
+    RLM_CUDA(e, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    std::vector<uint8_t> unq(v.limits_cap);
+    RLM_CUDA(e, cudaMemcpyAsync(unq.data(), d_unq.p, unq.size(), cudaMemcpyDeviceToHost, v.stream));
+    RLM_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged inputs are freed
+    rl_internal_mark_present(e, unq.data(), v.limits_cap);
+    return RL_OK;
+}
+
 }  // extern "C"

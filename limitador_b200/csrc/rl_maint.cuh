@@ -9,6 +9,9 @@
 //                       (rl_kernels.cuh rl_probe: home = low hash bits, linear probing inside the region, 128-bit
 //                       CAS on the header).  No reference analog (moka evicts, in_memory.rs:205-212); observable
 //                       state is unchanged: rl_dump_table before == after.
+//   k_import_resolve /  counter import (rl_counters_import): set counters to exported (value, expiry) pairs in three
+//   k_import_claim /    passes — check every entry, find or claim every row by rl_probe's rule, then write the cells —
+//   k_import_write      so that a refused call has written no cell (DESIGN.md §9f).
 //
 // Written so that the SAME source runs under tests/emu/cuda_shim.h (one CUDA thread after the other on the host):
 // grid-stride / one-item-per-thread kernels, global atomics only; warp-aggregated fast paths sit inside
@@ -179,4 +182,158 @@ __global__ void k_compact_reinsert(uint8_t* rows, const uint8_t* __restrict__ sc
         return;
     }
     atomicAdd(&counts[2], 1ull);  // cannot happen: the region held this row before
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Counter import.  The entries are the five arrays rl_dump_table returns; every error is one word, (index << 8) |
+// reason, lowered with atomicMin so that the host learns the first bad index (~0 = no error).
+enum : uint32_t {
+    RLM_IMP_UNKNOWN_LIMIT = 1,  // limit id not registered in this engine
+    RLM_IMP_KEY_RANGE = 2,      // qualified counter with key_hi >= 2^32
+    RLM_IMP_NO_EXPIRY = 3,      // qualified counter with expiry 0 (that is an absent counter)
+    RLM_IMP_DUPLICATE = 4,      // the same counter twice in one call
+    RLM_IMP_TABLE_FULL = 5,     // the row's region has no free row
+};
+
+struct RlImportIn {
+    const uint32_t* limit_id;
+    const uint64_t* key_lo;
+    const uint64_t* key_hi;
+    const uint64_t* value;
+    const uint64_t* expiry;
+    uint64_t n;
+};
+
+struct RlImportTab {
+    uint8_t* rows;
+    uint32_t row_bytes, log2P, log2R;
+    const RlLimitDev* limits;  // [limits_cap], group 0 = not registered
+    uint32_t limits_cap;
+};
+
+// Entry i -> row header (key_lo, hdr_hi = group << 32 | key_hi; key 0 for unqualified limits) and cell, or a reason.
+__device__ __forceinline__ uint32_t rlm_import_entry(const RlImportTab& T, const RlImportIn& I, uint64_t i, uint64_t& klo,
+                                                     uint64_t& hhi, uint32_t& cell, bool& qualified) {
+    const uint32_t lid = I.limit_id[i];
+    if (lid >= T.limits_cap) return RLM_IMP_UNKNOWN_LIMIT;
+    const RlLimitDev l = T.limits[lid];
+    if (l.group == 0) return RLM_IMP_UNKNOWN_LIMIT;
+    qualified = l.qualified != 0;
+    cell = l.cell;
+    klo = 0;
+    hhi = (uint64_t)l.group << 32;
+    if (qualified) {
+        const uint64_t khi = I.key_hi[i];
+        if (khi >> 32) return RLM_IMP_KEY_RANGE;
+        if (I.expiry[i] == 0) return RLM_IMP_NO_EXPIRY;
+        klo = I.key_lo[i];
+        hhi |= khi;
+    }
+    return 0;
+}
+
+// Pass 1: check every entry; unq[limit] = 1 for the unqualified limits named (they become present on success).
+__global__ void k_import_resolve(RlImportTab T, RlImportIn I, unsigned long long* err, uint8_t* unq) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= I.n) return;
+    uint64_t klo, hhi;
+    uint32_t cell;
+    bool q = false;
+    const uint32_t why = rlm_import_entry(T, I, i, klo, hhi, cell, q);
+    if (why) {
+        atomicMin(err, ((unsigned long long)i << 8) | why);
+        return;
+    }
+    if (!q) unq[I.limit_id[i]] = 1;
+}
+
+// row_of[] words: the row index, plus whether this call claimed the row and what the row was before
+#define RLM_ROW_CLAIMED (1ull << 63)
+#define RLM_ROW_WAS_TOMB (1ull << 62)
+#define RLM_ROW_INDEX(w) ((w) & ((1ull << 62) - 1))
+#define RLM_ROW_NONE 0xFFFFFFFFFFFFFFFFull  // the region is full
+
+// rl_probe (rl_kernels.cuh) with create: linear probing inside the key's region from its home row, the first tombstone
+// passed is reused once the key is known to be absent, rows are claimed with a 128-bit CAS on the header.
+__device__ __forceinline__ uint64_t rlm_claim_row(const RlImportTab& T, uint64_t h, uint64_t klo, uint64_t hhi) {
+    const uint32_t R = 1u << T.log2R;
+    const uint64_t base = (T.log2P ? (h >> (64 - T.log2P)) : 0ull) << T.log2R;
+    const uint32_t idx = (uint32_t)h & (R - 1);
+    int64_t tomb = -1;
+    uint32_t restarts = 0;
+    for (uint32_t i = 0; i < R;) {
+        const uint64_t r = base + ((idx + i) & (R - 1));
+        const ulonglong2 cur = rlm_ld(T.rows + r * T.row_bytes);
+        if (cur.x == klo && cur.y == hhi) return r;
+        if (cur.x == 0 && cur.y == 0) {
+            const uint64_t target = tomb >= 0 ? (uint64_t)tomb : r;
+            const ulonglong2 expect = make_ulonglong2(0ull, tomb >= 0 ? RLM_TOMB_HI : 0ull);
+            const ulonglong2 old = rlm_cas128(T.rows + target * T.row_bytes, expect, make_ulonglong2(klo, hhi));
+            if (old.x == expect.x && old.y == expect.y) return target | RLM_ROW_CLAIMED | (tomb >= 0 ? RLM_ROW_WAS_TOMB : 0ull);
+            if (++restarts > 4 * R) break;  // another thread took the row first: rescan
+            tomb = -1;
+            i = 0;
+            continue;
+        }
+        if (cur.y == RLM_TOMB_HI && tomb < 0) tomb = (int64_t)r;
+        i++;
+    }
+    if (tomb >= 0) {
+        const ulonglong2 old = rlm_cas128(T.rows + (uint64_t)tomb * T.row_bytes, make_ulonglong2(0ull, RLM_TOMB_HI),
+                                          make_ulonglong2(klo, hhi));
+        if (old.x == 0 && old.y == RLM_TOMB_HI) return (uint64_t)tomb | RLM_ROW_CLAIMED | RLM_ROW_WAS_TOMB;
+        if (old.x == klo && old.y == hhi) return (uint64_t)tomb;
+    }
+    return RLM_ROW_NONE;
+}
+
+// Pass 2: find or claim every entry's row (row_of[i], zeroed for the call) and mark its cell in cellmask[row] (zeroed
+// too); a cell marked twice is a duplicate.  Claimed rows keep the cells they had (all zero) until pass 3, which runs
+// only if this pass reported nothing.  Device path: the lanes of a warp that name the same row probe once.
+__global__ void k_import_claim(RlImportTab T, RlImportIn I, unsigned long long* row_of, unsigned* cellmask,
+                               unsigned long long* err) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint64_t klo = 0, hhi = 0;
+    uint32_t cell = 0;
+    bool q = false;
+    const bool valid = i < I.n && rlm_import_entry(T, I, i, klo, hhi, cell, q) == 0;
+    uint64_t row = RLM_ROW_NONE;
+#ifndef RL_SHIM
+    // every lane of the warp reaches this point (blockDim is a multiple of 32, no thread returned)
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned vmask = __ballot_sync(0xFFFFFFFFu, valid);
+    const unsigned grp = __match_any_sync(0xFFFFFFFFu, klo) & __match_any_sync(0xFFFFFFFFu, hhi) & (valid ? vmask : ~vmask);
+    const unsigned leader = (unsigned)(__ffs(grp) - 1);
+    if (valid && lane == leader) row = rlm_claim_row(T, rl_row_hash(klo, hhi), klo, hhi);
+    const unsigned r_lo = __shfl_sync(0xFFFFFFFFu, (unsigned)(row & 0xFFFFFFFFull), (int)leader);
+    const unsigned r_hi = __shfl_sync(0xFFFFFFFFu, (unsigned)(row >> 32), (int)leader);
+    row = ((uint64_t)r_hi << 32) | r_lo;
+    if (lane != leader && row != RLM_ROW_NONE) row &= ~(RLM_ROW_CLAIMED | RLM_ROW_WAS_TOMB);  // the leader claimed it
+#else
+    if (valid) row = rlm_claim_row(T, rl_row_hash(klo, hhi), klo, hhi);
+#endif
+    if (!valid) return;
+    if (row == RLM_ROW_NONE) {
+        atomicMin(err, ((unsigned long long)i << 8) | RLM_IMP_TABLE_FULL);
+        return;
+    }
+    row_of[i] = row;
+    const unsigned old = rlm_or(&cellmask[RLM_ROW_INDEX(row)], 1u << cell);
+    if (old >> cell & 1u) atomicMin(err, ((unsigned long long)i << 8) | RLM_IMP_DUPLICATE);
+}
+
+// After a refused pass 2: every row the call claimed gets its old header back (empty or tombstone; its cells were never
+// written).  A row that was empty before the call lies on no older key's probe chain, so the table is as it was.
+__global__ void k_import_release(RlImportTab T, uint64_t n, const unsigned long long* __restrict__ row_of) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !(row_of[i] & RLM_ROW_CLAIMED)) return;
+    rlm_st(T.rows + RLM_ROW_INDEX(row_of[i]) * T.row_bytes, 0ull, (row_of[i] & RLM_ROW_WAS_TOMB) ? RLM_TOMB_HI : 0ull);
+}
+
+// Pass 3: (value, expiry) into every entry's cell.
+__global__ void k_import_write(RlImportTab T, RlImportIn I, const unsigned long long* __restrict__ row_of) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= I.n) return;
+    const uint32_t cell = T.limits[I.limit_id[i]].cell;
+    rlm_st(T.rows + RLM_ROW_INDEX(row_of[i]) * T.row_bytes + 16 + 16 * cell, I.value[i], I.expiry[i]);
 }

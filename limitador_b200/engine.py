@@ -54,7 +54,10 @@ ABI_SYMBOLS = [
     "rl_shard_slab", "rl_shard_slab_bytes", "rl_shard_send", "rl_shard_decide", "rl_shard_collect", "rl_shard_step",
     "rl_shard_flush", "rl_shard_debug", "rl_trace_dump", "rl_check_and_update_compact", "rl_shard_fence",
     "rl_compact", "rl_ns_metrics_enable", "rl_ns_metrics_accumulate", "rl_ns_metrics_read",
+    "rl_counters_export", "rl_counters_import", "rl_limits_get",
 ]
+
+SNAPSHOT_VERSION = 1  # format of Engine.save_counters files
 
 
 class RlConfig(C.Structure):
@@ -127,6 +130,9 @@ def load_library(path: str | None = None):
     L.rl_ns_metrics_accumulate.argtypes = [vp, u64, vp, u32, vp, vp, i32]
     L.rl_ns_metrics_read.argtypes = [vp, u32, vp, vp, vp, u32, vp, vp, i32]
     L.rl_dump_table.argtypes = [vp, u64, vp, vp, vp, vp, vp, vp]
+    L.rl_counters_export.argtypes = [vp, vp, u32, u64, u64, i32, vp, vp, vp, vp, vp, vp]
+    L.rl_counters_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, i32]
+    L.rl_limits_get.argtypes = [vp, u32, vp, vp]
     L.rl_bucket_by_owner.argtypes = [vp, u64, vp, u32, vp, vp, vp]
     L.rl_unpermute_u8.argtypes = [vp, u64, vp, vp, vp]
     L.rl_bucket_by_owner_padded.argtypes = [vp, u64, vp, u32, u32, vp, vp, vp]
@@ -443,6 +449,88 @@ class Engine:
         """Sorted list of (limit_id, key_lo, key_hi, value, expiry_us) for every present counter."""
         lid, lo, hi, val, exp = self.dump_arrays()
         return sorted(zip(lid.tolist(), lo.tolist(), hi.tolist(), val.tolist(), exp.tolist()))
+
+    # -- snapshots: restart, resize or re-shard without losing counters --
+    def limits_get(self) -> np.ndarray:
+        """Every registered limit (LIMIT_DESC_DTYPE), ascending id."""
+        n = C.c_uint32(0)
+        self._check(self._lib.rl_limits_get(self._h, 0, None, C.byref(n)))
+        out = np.zeros(n.value, dtype=LIMIT_DESC_DTYPE)
+        self._check(self._lib.rl_limits_get(self._h, len(out), _p(out), C.byref(n)))
+        return out
+
+    def export_counters(self, now_us: int = 0, ns_ids=None, device: bool = False):
+        """rl_counters_export -> (limit_id, key_lo, key_hi, value, expiry_us).  numpy arrays (uint32, then uint64), or
+        with device=True torch tensors on the engine's GPU (int32 / int64 holding the same bits), written there by the
+        scan itself.  ns_ids=None: every namespace.  now_us > 0 leaves out the qualified counters rl_sweep(now_us)
+        would drop."""
+        ids = None if ns_ids is None else np.ascontiguousarray(ns_ids, dtype=np.uint32)
+        n_ids = 0 if ids is None else len(ids)
+        cnt, cap = C.c_uint64(0), 0
+        while True:  # count, then fetch (again if the table grew in between)
+            if device:
+                import torch
+                dev = torch.device("cuda", self.device)
+                arrs = [torch.empty(max(cap, 1), dtype=torch.int32, device=dev)] + [
+                    torch.empty(max(cap, 1), dtype=torch.int64, device=dev) for _ in range(4)]
+                ptrs = [C.c_void_p(a.data_ptr()) for a in arrs]
+            else:
+                arrs = [np.zeros(cap, dtype=np.uint32)] + [np.zeros(cap, dtype=np.uint64) for _ in range(4)]
+                ptrs = [_p(a) for a in arrs]
+            self._check(self._lib.rl_counters_export(self._h, _p(ids), n_ids, now_us, cap,
+                                                     MEM_DEVICE if device else MEM_HOST, *ptrs, C.byref(cnt)))
+            if cnt.value <= cap:
+                return tuple(a[:cnt.value] for a in arrs)
+            cap = int(cnt.value)
+
+    def import_counters(self, limit_id, key_lo, key_hi, value, expiry_us):
+        """rl_counters_import: set each counter to exactly (value, expiry_us), all or nothing.  numpy arrays, or torch
+        CUDA tensors on the engine's GPU (4- and 8-byte integers as export_counters(device=True) returns them)."""
+        cols = (limit_id, key_lo, key_hi, value, expiry_us)
+        n = len(limit_id)
+        if any(len(c) != n for c in cols):
+            raise ValueError("import_counters: the five arrays must have the same length")
+        if all(hasattr(c, "is_cuda") and c.is_cuda for c in cols):
+            import torch
+            cols = [c.contiguous() for c in cols]
+            if cols[0].element_size() != 4 or any(c.element_size() != 8 for c in cols[1:]):
+                raise ValueError("import_counters: limit_id must be a 4-byte and the other columns 8-byte tensors")
+            torch.cuda.current_stream(cols[0].device).synchronize()  # the engine's stream reads them next
+            ptrs, mem = [C.c_void_p(c.data_ptr()) for c in cols], MEM_DEVICE
+        elif any(hasattr(c, "is_cuda") and c.is_cuda for c in cols):
+            raise ValueError("import_counters: either all five columns are CUDA tensors or none is")
+        else:
+            cols = [np.ascontiguousarray(cols[0], dtype=np.uint32)] + [np.ascontiguousarray(c, dtype=np.uint64) for c in cols[1:]]
+            ptrs, mem = [_p(c) for c in cols], MEM_HOST
+        self._check(self._lib.rl_counters_import(self._h, n, *ptrs, mem))
+
+    def save_counters(self, path: str, now_us: int = 0):
+        """Write the limits (rl_limits_get) and every counter (export_counters(now_us)) to one .npz file at `path`;
+        the counters sorted by (limit_id, key) so that the same table always gives the same file."""
+        limits = self.limits_get()
+        lid, lo, hi, val, exp = self.export_counters(now_us)
+        order = np.lexsort((hi, lo, lid))
+        with open(path, "wb") as f:
+            np.savez(f, version=np.uint32(SNAPSHOT_VERSION), limits=limits, limit_id=lid[order], key_lo=lo[order],
+                     key_hi=hi[order], value=val[order], expiry_us=exp[order])
+
+    def load_counters(self, path: str):
+        """Import a save_counters file.  Limit ids are interned by the caller: this engine must have registered the same
+        limits under the same ids (the same configuration, registered in the same order) before the call.  Refused
+        before any counter changes if a limit of the file is registered here with another namespace, window or
+        qualified flag (a limit's identity, limit.rs:177-214; max_value may differ, as after update_limit)."""
+        with np.load(path) as z:
+            if int(z["version"]) != SNAPSHOT_VERSION:
+                raise ValueError(f"{path}: snapshot format {int(z['version'])}, this build reads {SNAPSHOT_VERSION}")
+            limits = z["limits"]
+            cols = [z[k] for k in ("limit_id", "key_lo", "key_hi", "value", "expiry_us")]
+        mine = {int(d["limit_id"]): d for d in self.limits_get()}
+        used = set(np.unique(cols[0]).tolist())
+        bad = sorted(int(d["limit_id"]) for d in limits if int(d["limit_id"]) in used and int(d["limit_id"]) in mine
+                     and any(int(d[k]) != int(mine[int(d["limit_id"])][k]) for k in ("ns_id", "window_us", "qualified")))
+        if bad:
+            raise ValueError(f"{path}: limits {bad} are registered here with another namespace, window or qualified flag")
+        self.import_counters(*cols)
 
 
 def owner_of(ns_id: int, world: int) -> int:

@@ -139,6 +139,14 @@ def owner_of(ns_id: int, world: int) -> int:
     return int(_eng.load_library().rl_owner_of(int(ns_id), int(world)))
 
 
+def namespaces_owned(ns_ids, rank: int, world: int) -> np.ndarray:
+    """The namespaces of `ns_ids` that `rank` owns in a store of `world` ranks (uint32, ascending).  Re-sharding a
+    store to a new world size: every old rank exports, for each new rank r, its counters of namespaces_owned(all, r,
+    new_world) (Engine.export_counters(ns_ids=...)), and new rank r imports what every old rank exported for it."""
+    ids = sorted({int(n) for n in np.asarray(ns_ids).ravel().tolist()})
+    return np.array([n for n in ids if owner_of(n, world) == rank], dtype=np.uint32)
+
+
 def observed_block_max(recs, owner_lut, world: int) -> int:
     """Largest number of records one step of `recs` ([steps, batch, 4] int64 = rl_record) sends to one owner.
     `owner_lut[ns_id]` = owner rank (a tensor on the records' device)."""
