@@ -49,7 +49,9 @@ enum { RL_MEM_HOST = 0, RL_MEM_DEVICE = 1,
 /* out_limited[i] of a request that could NOT be evaluated (malformed key, full table region, exchange block
  * overflow): the call (or the next rl_sync) also reports the error; the byte is never a silent 0 = allowed */
 #define RL_VERDICT_ERROR 0xFFu
-#define RL_MAX_COUNTERS_PER_REQUEST 16 /* counters one request may name (general form); the matcher refuses more */
+#define RL_MAX_COUNTERS_PER_REQUEST 16 /* counters one request may name (general form) on a default engine; the matcher
+                                          refuses more unless its cap is raised */
+#define RL_MAX_COUNTERS_PER_REQUEST_WIDE 64 /* the most rl_config.max_counters_per_request may ask for */
 /* test aid: the in-kernel row grouping table gives every row one of only four home slots, so that
  * distinct rows collide and its linear probing is exercised to full length */
 #define RL_FLAG_DEBUG_WEAK_TAGS 1u
@@ -80,7 +82,12 @@ typedef struct rl_config {
     uint32_t max_counters;   /* max total counters per CSR call (0 = 4 * max_batch) */
     uint32_t regions;        /* 0 = auto; power of two */
     uint32_t flags;          /* RL_FLAG_* */
-    uint32_t _pad;
+    uint32_t max_counters_per_request; /* counters one request may name, and limits one namespace may have on the record
+                                          path: 0 or 16 = RL_MAX_COUNTERS_PER_REQUEST (a 17-counter request is refused
+                                          before the table is touched); 17..64 = a wide engine; anything else is refused
+                                          by rl_engine_create.  Declares a maximum, it does not choose a code path: a
+                                          batch runs the wide kernels only if it holds a request of more than 16
+                                          counters (DESIGN.md §9g), so narrow traffic costs the same on a wide engine */
 } rl_config;
 
 /* A limit as the storage sees it (limit.rs:177-214: identity excludes max_value/name).
@@ -146,6 +153,8 @@ typedef struct rl_stats {
 
 int rl_engine_create(const rl_config *cfg, rl_engine **out);
 void rl_engine_destroy(rl_engine *e);
+/* The engine's max_counters_per_request (16 for a default engine, and for e == NULL). */
+uint32_t rl_engine_max_counters_per_request(rl_engine *e);
 /* Message of the last non-OK status on this engine (never NULL). */
 const char *rl_last_error(rl_engine *e);
 /* Use the caller's CUDA stream (a cudaStream_t) for all subsequent work; NULL = the
@@ -185,7 +194,7 @@ int rl_check_and_update_records(rl_engine *e, uint64_t n, const rl_record *recs,
 /* The record form over 16-byte records, all stamped now_us (single-row namespaces only, no load_counters). */
 int rl_check_and_update_compact(rl_engine *e, uint64_t n, const rl_record16 *recs, uint64_t now_us, int mem,
                                 uint8_t *out_limited, uint32_t *out_first_limited);
-/* General form: request i owns ctrs[ctr_off[i] .. ctr_off[i+1]) (at most 16), counters are
+/* General form: request i owns ctrs[ctr_off[i] .. ctr_off[i+1]) (at most max_counters_per_request), counters are
  * processed unqualified-first then in the given order (in_memory.rs:105,121);
  * out_remaining/out_ttl_us are indexed like ctrs.  An empty counter list is "not limited"
  * (lib.rs:434-440). */
@@ -196,7 +205,7 @@ int rl_check_and_update_batch(rl_engine *e, uint64_t n, const uint32_t *ctr_off,
 
 /* CounterStorage::is_within_limits (in_memory.rs:20-35) folded over a request's counters
  * as RateLimiter::is_rate_limited does (lib.rs:362-409): read-only, given order, first
- * counter over its limit wins. */
+ * counter over its limit wins.  Any number of counters per request, on every engine. */
 int rl_is_within_limits_batch(rl_engine *e, uint64_t n, const uint32_t *ctr_off, const rl_counter *ctrs,
                               const uint64_t *delta, const uint64_t *now_us, int mem,
                               uint8_t *out_limited, uint32_t *out_first_limited);
@@ -378,6 +387,7 @@ int rl_shard_debug(rl_shard *s, uint32_t *out);
 typedef struct rl_front rl_front;
 int rl_front_create(rl_engine *e, uint32_t max_batch, uint32_t max_delay_us, rl_front **out);
 void rl_front_destroy(rl_front *f);
+/* m: up to the engine's max_counters_per_request (the matched counters of one request) */
 int rl_front_check_and_update(rl_front *f, const rl_counter *ctrs, uint32_t m, uint64_t delta, uint64_t now_us,
                               int load_counters, uint8_t *out_limited, uint32_t *out_first_limited,
                               uint64_t *out_remaining, uint64_t *out_ttl_us, uint64_t *out_seq);

@@ -75,10 +75,11 @@ int rl_matcher_add_limit_ex(rl_matcher *m, const char *ns, uint64_t max_value, u
                             uint32_t n_var, const char *name /* nullable */, int keep_existing,
                             rl_limit_desc *out_desc, int *out_existed /* nullable */);
 int rl_matcher_delete_limit(rl_matcher *m, uint32_t limit_id);
-/* Counters one request may produce before matching fails (default RL_MAX_COUNTERS_PER_REQUEST = what the engine takes
- * per request, so that an oversized request is refused here, before anything is enqueued).  A caller that only matches
- * — the matcher benchmark on the reference's "50 limits per namespace" scenarios, limitador/benches/bench.rs:65-90 — may
- * raise it; such requests cannot be shipped to the engine. */
+/* Counters one request may produce before matching fails (default RL_MAX_COUNTERS_PER_REQUEST = what a default engine
+ * takes per request, so that an oversized request is refused here, before anything is enqueued).  A caller whose engine
+ * was created with a larger rl_config.max_counters_per_request (up to 64) raises it to match: the reference's "50
+ * limits per namespace" scenarios (limitador/benches/bench.rs:65-90) then run end to end.  Raised past the engine's
+ * maximum, requests over the latter match but cannot be shipped to the engine. */
 int rl_matcher_set_counter_cap(rl_matcher *m, uint32_t cap);
 /* RL_OK and *out_ns_id, or RL_FATAL if no limit was ever added for the namespace (no limits => allow,
  * lib.rs:434-440: the caller skips the engine). */
@@ -127,7 +128,9 @@ int rl_matcher_response_headers_batch(rl_matcher *m, uint64_t n, const uint32_t 
  * the matcher is read-shared) and then through the front's queue (include/rl_engine.h: rl_front_check_and_update), i.e.
  * RateLimiter::check_rate_limited_and_update (lib.rs:425-464) end to end.  out_ctrs (nullable, capacity
  * RL_MAX_COUNTERS_PER_REQUEST) / *out_n_ctrs (nullable) receive the counters that applied; out_remaining / out_ttl_us
- * are indexed like them.  A namespace without limits, or a context no limit applies to, is "not limited" without
+ * are indexed like them.  This helper matches at most RL_MAX_COUNTERS_PER_REQUEST counters whatever the engine's
+ * max_counters_per_request: a wider request is matched by the caller (rl_matcher_counters) and shipped with
+ * rl_front_check_and_update, which takes up to the engine's maximum.  A namespace without limits, or a context no limit applies to, is "not limited" without
  * touching the store (lib.rs:434-440). */
 int rl_front_check_and_update_bindings(rl_front *f, rl_matcher *m, const char *ns, const rl_binding *binds, uint32_t n_binds,
                                        uint64_t delta, uint64_t now_us, int load_counters, uint8_t *out_limited,

@@ -27,7 +27,7 @@ SCENARIOS = [(10, 50, 10, 0), (1, 1, 1, 1), (10, 10, 10, 10), (10, 50, 10, 10)] 
 
 def build(n_ns, n_lim, n_cond, n_var):
     m = MT.Matcher()
-    m.set_counter_cap(max(16, n_lim))  # matching only: the engine itself takes at most 16 counters per request
+    m.set_counter_cap(max(16, n_lim))  # a default engine takes 16 counters per request; tools/reference_scenarios.py decides these on a wide one
     conds = [f"cond_{i} == '1'" for i in range(n_cond)]
     vars_ = [f"var_{j}" for j in range(n_var)]
     for ns in range(n_ns):

@@ -21,6 +21,7 @@
 #define RL_NONE_U32 0xFFFFFFFFu
 #define RL_MAX_CELLS 7          // cells per row: 16-B header + 7 x 16-B cells = 128 B
 #define RL_MAX_CTRS_PER_REQ 16  // positions are packed in nibbles
+#define RL_MAX_CTRS_PER_REQ_WIDE 64  // wide encoding: six-bit positions, original index kept apart (RlAccess)
 #define RL_TOMB_HI 0xFFFFFFFFFFFFFFFFull
 
 // device error codes (sticky max in RlBatchCtl::err)
@@ -68,6 +69,11 @@ struct RlNsDev {
 //            request has other accesses too (multi-row request)
 //   posorig= nibble k: position of that cell in the request's processing order
 //            (unqualified first, in_memory.rs:105,121); nibble 8+k... see helpers below
+// Two encodings of posorig, chosen per batch (template parameter WIDE of the functions that read it):
+//   narrow (requests of <= 16 counters): nibble k = processing position of cell k, nibble 8+k = its original index;
+//   wide   (<= 64 counters): bits 6k..6k+5 = processing position of cell k, no original index.  The wide walkers
+//          write remaining / ttl at the position, and the resolve writes perm[position] = original index, so one
+//          scatter puts them in the caller's order afterwards (DESIGN.md §9g).
 struct RlAccess {
     uint64_t key_lo;
     uint64_t hdr_hi;
@@ -81,6 +87,15 @@ RL_HD bool rl_cells_multi(uint32_t cells) { return (cells >> 31) != 0; }
 RL_HD uint32_t rl_cells_at(uint32_t cells, uint32_t k) { return (cells >> (4 * k)) & 0xFu; }
 RL_HD uint32_t rl_pos_at(uint64_t posorig, uint32_t k) { return (uint32_t)(posorig >> (4 * k)) & 0xFu; }
 RL_HD uint32_t rl_orig_at(uint64_t posorig, uint32_t k) { return (uint32_t)(posorig >> (32 + 4 * k)) & 0xFu; }
+// processing position of the k-th cell, and the index its remaining / ttl outputs are written at
+template <bool WIDE>
+RL_HD uint32_t rl_pos_of(uint64_t posorig, uint32_t k) {
+    return WIDE ? ((uint32_t)(posorig >> (6 * k)) & 0x3Fu) : rl_pos_at(posorig, k);
+}
+template <bool WIDE>
+RL_HD uint32_t rl_out_of(uint64_t posorig, uint32_t k) {
+    return WIDE ? rl_pos_of<true>(posorig, k) : rl_orig_at(posorig, k);
+}
 
 // 64-bit mixer (splitmix64 / murmur3 finaliser constants).
 RL_HD uint64_t rl_mix64(uint64_t x) {
@@ -132,8 +147,9 @@ RL_HD void rl_cell_update(RlRow<CELLS>& row, uint32_t c, uint64_t delta, uint64_
 // (in_memory.rs:72-156).  Returns the processing-order position of the first limited
 // counter, or RL_NONE_U32 (= Authorization::Ok, all counters incremented).
 //   desc        : RlCellDesc[RL_MAX_CELLS+1] of the row group
-//   rem/ttl     : per-request output base (indexed by original counter index), nullable
-template <int CELLS>
+//   rem/ttl     : per-request output base (indexed by rl_out_of: the original counter index, or the
+//                 processing position for WIDE), nullable
+template <int CELLS, bool WIDE = false>
 RL_HD uint32_t rl_walk_check_single(RlRow<CELLS>& row, uint32_t& dirty, const RlCellDesc* desc,
                                     uint32_t cells, uint64_t posorig, uint64_t delta, uint64_t now,
                                     bool load_counters, uint64_t* rem, uint64_t* ttl) {
@@ -151,12 +167,12 @@ RL_HD uint32_t rl_walk_check_single(RlRow<CELLS>& row, uint32_t& dirty, const Rl
         const uint64_t sum = v + delta;  // wraps like a release build
         const bool over = sum > d.max_value;
         if (load_counters) {
-            const uint32_t oi = rl_orig_at(posorig, k);
+            const uint32_t oi = rl_out_of<WIDE>(posorig, k);
             if (rem) rem[oi] = over ? 0 : d.max_value - sum;  // checked_sub, :88-89
             if (ttl) ttl[oi] = rl_ttl(row.expiry[c], now);    // pre-update ttl, :114-116,:134-136
         }
         if (over && first == RL_NONE_U32) {
-            first = rl_pos_at(posorig, k);
+            first = rl_pos_of<WIDE>(posorig, k);
             if (!load_counters) return first;  // early return, :110-112,:130-132
         }
     }
@@ -176,7 +192,7 @@ RL_HD uint32_t rl_walk_check_single(RlRow<CELLS>& row, uint32_t& dirty, const Rl
 //   * !load_counters: counters at positions <= fl_in are looked up (created if absent);
 //     later ones are never reached (early return).
 //   * fl_in == NONE: every counter is incremented.
-template <int CELLS>
+template <int CELLS, bool WIDE = false>
 RL_HD uint32_t rl_walk_check_multi(RlRow<CELLS>& row, uint32_t& dirty, const RlCellDesc* desc,
                                    uint32_t cells, uint64_t posorig, uint64_t delta, uint64_t now,
                                    bool load_counters, uint32_t fl_in, uint64_t* rem, uint64_t* ttl) {
@@ -185,7 +201,7 @@ RL_HD uint32_t rl_walk_check_multi(RlRow<CELLS>& row, uint32_t& dirty, const RlC
     for (uint32_t k = 0; k < n; k++) {
         const uint32_t c = rl_cells_at(cells, k);
         const RlCellDesc d = desc[c];
-        const uint32_t pos = rl_pos_at(posorig, k);
+        const uint32_t pos = rl_pos_of<WIDE>(posorig, k);
         const bool reached = load_counters || fl_in == RL_NONE_U32 || pos <= fl_in;
         if (reached && d.qualified && row.expiry[c] == 0) {
             row.value[c] = 0;
@@ -197,7 +213,7 @@ RL_HD uint32_t rl_walk_check_multi(RlRow<CELLS>& row, uint32_t& dirty, const RlC
         const uint64_t sum = v + delta;
         const bool over = sum > d.max_value;
         if (load_counters) {
-            const uint32_t oi = rl_orig_at(posorig, k);
+            const uint32_t oi = rl_out_of<WIDE>(posorig, k);
             if (rem) rem[oi] = over ? 0 : d.max_value - sum;
             if (ttl) ttl[oi] = rl_ttl(row.expiry[c], now);
         }
@@ -238,13 +254,13 @@ RL_HD void rl_walk_update(RlRow<CELLS>& row, uint32_t& dirty, const RlCellDesc* 
 //   * otherwise request pos is applied alone with the sequential rule.
 // Every step is exact, so the replay equals one-at-a-time execution; saturated hot keys
 // (all denied) and hot keys far from their limit (all allowed) finish in one step.
-template <int CELLS>
+template <int CELLS, bool WIDE = false>
 RL_HD bool rl_eval_deny_noeffect(const RlRow<CELLS>& S, const RlCellDesc* desc, uint32_t cells, uint64_t posorig,
                                  uint64_t delta, uint64_t now, bool load_counters) {
     RlRow<CELLS> tmp = S;
     uint32_t dirty = 0;
     const uint32_t fl =
-        rl_walk_check_single<CELLS>(tmp, dirty, desc, cells, posorig, delta, now, load_counters, nullptr, nullptr);
+        rl_walk_check_single<CELLS, WIDE>(tmp, dirty, desc, cells, posorig, delta, now, load_counters, nullptr, nullptr);
     return fl != RL_NONE_U32 && dirty == 0;
 }
 
@@ -282,18 +298,26 @@ RL_HD void rl_advance_run(RlRow<CELLS>& S, uint32_t cells, uint64_t dprev) {
 // processing order: unqualified counters first, then qualified, each in the given order
 // (in_memory.rs:105,121).  Writes at most m accesses to acc[0..m) (unused ones get
 // hdr_hi = 0) and returns the number of accesses, or a negative RL_DEV_* code.
+// WIDE: up to max_ctrs (<= 64) counters in the wide position encoding, and perm[position] = original index
+// for position < m (the output scatter's map); narrow: up to 16, perm and max_ctrs unused.
 struct RlCtrIn {
     uint32_t limit_id;
     uint64_t key_lo, key_hi;
 };
 
-template <class GetCtr>
+template <bool WIDE> struct RlUsedMask { typedef uint32_t T; };
+template <> struct RlUsedMask<true> { typedef uint64_t T; };
+
+template <bool WIDE = false, class GetCtr>
 RL_HD int rl_resolve_request(uint32_t req, uint32_t m, GetCtr get, const RlLimitDev* limits,
-                             uint32_t limits_cap, bool unqualified_first, RlAccess* acc) {
-    if (m > RL_MAX_CTRS_PER_REQ) return -(int)RL_DEV_TOO_MANY_COUNTERS;
-    uint32_t grp[RL_MAX_CTRS_PER_REQ], cel[RL_MAX_CTRS_PER_REQ];
-    uint64_t klo[RL_MAX_CTRS_PER_REQ], khi[RL_MAX_CTRS_PER_REQ];
-    uint8_t order[RL_MAX_CTRS_PER_REQ];
+                             uint32_t limits_cap, bool unqualified_first, RlAccess* acc, uint8_t* perm = nullptr,
+                             uint32_t max_ctrs = RL_MAX_CTRS_PER_REQ_WIDE) {
+    constexpr uint32_t MAXC = WIDE ? RL_MAX_CTRS_PER_REQ_WIDE : RL_MAX_CTRS_PER_REQ;
+    typedef typename RlUsedMask<WIDE>::T Used;
+    if (m > MAXC || (WIDE && m > max_ctrs)) return -(int)RL_DEV_TOO_MANY_COUNTERS;
+    uint32_t grp[MAXC], cel[MAXC];
+    uint64_t klo[MAXC], khi[MAXC];
+    uint8_t order[MAXC];
     uint32_t npos = 0;
     // pass 0: unqualified, pass 1: qualified (single pass in given order if !unqualified_first)
     for (int pass = 0; pass < 2; pass++) {
@@ -311,11 +335,13 @@ RL_HD int rl_resolve_request(uint32_t req, uint32_t m, GetCtr get, const RlLimit
             order[npos++] = (uint8_t)j;
         }
     }
-    uint32_t used = 0;  // bitmask of counters already assigned to an access
+    Used used = 0;  // bitmask of counters already assigned to an access
     uint32_t nacc = 0;
+    if (WIDE)
+        for (uint32_t p = 0; p < npos; p++) perm[p] = order[p];
     for (uint32_t p = 0; p < npos; p++) {
         const uint32_t j = order[p];
-        if (used & (1u << j)) continue;
+        if (used & ((Used)1 << j)) continue;
         RlAccess a;
         a.key_lo = klo[j];
         a.hdr_hi = ((uint64_t)grp[j] << 32) | khi[j];
@@ -324,13 +350,17 @@ RL_HD int rl_resolve_request(uint32_t req, uint32_t m, GetCtr get, const RlLimit
         uint64_t posorig = 0;
         for (uint32_t q = p; q < npos; q++) {
             const uint32_t jj = order[q];
-            if (used & (1u << jj)) continue;
+            if (used & ((Used)1 << jj)) continue;
             if (grp[jj] != grp[j] || klo[jj] != klo[j] || khi[jj] != khi[j]) continue;
             if (cnt >= RL_MAX_CELLS) return -(int)RL_DEV_GROUP_SPLIT;
             cells |= cel[jj] << (4 * cnt);
-            posorig |= (uint64_t)q << (4 * cnt);
-            posorig |= (uint64_t)jj << (32 + 4 * cnt);
-            used |= 1u << jj;
+            if (WIDE) {
+                posorig |= (uint64_t)q << (6 * cnt);
+            } else {
+                posorig |= (uint64_t)q << (4 * cnt);
+                posorig |= (uint64_t)jj << (32 + 4 * cnt);
+            }
+            used |= (Used)1 << jj;
             cnt++;
         }
         a.cells = cells | (cnt << 28);

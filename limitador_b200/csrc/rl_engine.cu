@@ -87,6 +87,7 @@ struct rl_engine {
     uint32_t cells = 1, log2P = 0, log2R = 0, row_bytes = 32;
     uint64_t capacity = 0;
     uint32_t max_batch = 0, max_counters = 0;
+    uint32_t max_ctrs_req = RL_MAX_CTRS_PER_REQ;  // rl_config.max_counters_per_request (16: narrow encoding only)
     DevBuf<uint8_t> d_rows;
 
     // registry
@@ -110,6 +111,10 @@ struct rl_engine {
     // workspace
     DevBuf<uint32_t> d_misc;  // misc: err, flags, changed, exchange error detail (MISC_*)
     DevBuf<RlAccess> d_acc;
+    // wide batches (max_ctrs_req > 16): perm[slot] = original index of the counter at that position (resolve);
+    // remaining / ttl in processing order (k_main with load_counters), before k_wide_scatter
+    DevBuf<uint8_t> d_perm;
+    DevBuf<uint64_t> d_wide_rem, d_wide_ttl;
     DevBuf<uint64_t> d_delta, d_now;
     DevBuf<uint32_t> d_fl_prev, d_fl_next;
     DevBuf<unsigned long long> d_kstats;
@@ -336,7 +341,7 @@ int check_device_error(rl_engine* e) {
         case RL_DEV_KEY_RANGE:
             return fail(e, RL_FATAL, "key_hi bits 32..55 must be zero (counter identity is a 96-bit digest)");
         case RL_DEV_TOO_MANY_COUNTERS:
-            return fail(e, RL_FATAL, "a request has more than %d counters", RL_MAX_CTRS_PER_REQ);
+            return fail(e, RL_FATAL, "a request has more than %u counters", e->max_ctrs_req);
         case RL_DEV_EXCHANGE: {
             const uint32_t d = e->h_misc[MISC_XCHG];
             RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_XCHG, 0, sizeof(uint32_t), e->stream));
@@ -350,7 +355,7 @@ int check_device_error(rl_engine* e) {
 }
 
 // A resolve kernel (request -> accesses) found a request the engine cannot take (unknown limit, more than
-// RL_MAX_COUNTERS_PER_REQUEST counters, key out of range): refuse the WHOLE call before anything touches the
+// max_counters_per_request counters, key out of range): refuse the WHOLE call before anything touches the
 // table, so that the caller can fix the batch and retry without double counting (ADVICE r1).
 int check_resolve_error(rl_engine* e) {
     RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
@@ -484,13 +489,18 @@ int launch_main_ch(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& sr
 
 template <int GEO, int CELLS, class Src, int MODE, bool LC>
 int launch_main_cells(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st) {
-    if (B.nhot && B.phase == RL_PHASE_COMMIT) {
-        // the hot rows' partitions: one CTA per hot slot (most exit at once), ahead of the cold partitions
-        k_hot<GEO, CELLS, Src, MODE, LC><<<B.nhot, RL_HOT_THREADS, 0, st>>>(D, B, src);
-        RL_LAUNCH_CHECK(e);
+    if constexpr (Src::kWide) {
+        // wide batches get no hot rows (run_acc_pipeline) and run 128-access chunks only
+        return launch_main_ch<GEO, CELLS, Src, MODE, LC, 128>(e, D, B, src, st);
+    } else {
+        if (B.nhot && B.phase == RL_PHASE_COMMIT) {
+            // the hot rows' partitions: one CTA per hot slot (most exit at once), ahead of the cold partitions
+            k_hot<GEO, CELLS, Src, MODE, LC><<<B.nhot, RL_HOT_THREADS, 0, st>>>(D, B, src);
+            RL_LAUNCH_CHECK(e);
+        }
+        return e->chunk == 128 ? launch_main_ch<GEO, CELLS, Src, MODE, LC, 128>(e, D, B, src, st)
+                               : launch_main_ch<GEO, CELLS, Src, MODE, LC, 256>(e, D, B, src, st);
     }
-    return e->chunk == 128 ? launch_main_ch<GEO, CELLS, Src, MODE, LC, 128>(e, D, B, src, st)
-                           : launch_main_ch<GEO, CELLS, Src, MODE, LC, 256>(e, D, B, src, st);
 }
 
 template <class Src, int MODE>
@@ -532,18 +542,31 @@ int pipe_fence(rl_engine* e) {
 }
 
 // Runs partition + main for accesses that may contain multi-row requests (AccSrc).
-// mode: 0 check_and_update, 2 update.
+// mode: 0 check_and_update, 2 update.  wide: the accesses were resolved with the wide position encoding
+// (k_resolve_*_wide); check_and_update then runs the wide k_main, whose remaining / ttl go to scratch in processing
+// order (slot = off[req] + position, or req * acc_stride + position for records) and are scattered into `o` at the
+// end.  update_counters never reads positions: its k_main is the same for both encodings.
 int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_t* d_delta, const uint64_t* d_now,
-                     int mode, int lc, const Outs& o) {
+                     int mode, int lc, const Outs& o, bool wide = false, uint32_t acc_stride = 0) {
     RlDev D = make_dev(e);
+    const bool scatter = wide && mode == 0 && lc && (o.rem || o.ttl);
+    Outs ob = o;  // where k_main writes
+    if (scatter) {
+        RL_CUDA(e, e->d_wide_rem.reserve(e->max_counters));
+        RL_CUDA(e, e->d_wide_ttl.reserve(e->max_counters));
+        if (o.rem) ob.rem = e->d_wide_rem.p;
+        if (o.ttl) ob.ttl = e->d_wide_ttl.p;
+        if (!o.off) ob.stride = acc_stride;
+    }
     // check_and_update in the general form may hold coupled (multi-row) requests, replayed in phases: partitions
     // stay sequential and no row gets a partition of its own
-    RlBatch B = make_batch(e, n_acc, n_req, o, lc, 0, 0, mode != 0);
+    RlBatch B = make_batch(e, n_acc, n_req, ob, lc, 0, 0, mode != 0);
     if (mode == 0) B.heavy_len = 0xFFFFFFFFu;
     AccSrc src{e->d_acc.p, d_delta, d_now};
     int r = launch_front(e, D, B, src);
     if (r) return r;
     if (mode == 2) return launch_main<AccSrc, 2>(e, D, B, src);
+    auto main0 = [&]() { return wide ? launch_main<AccSrcWide, 0>(e, D, B, AccSrcWide{src}) : launch_main<AccSrc, 0>(e, D, B, src); };
     // does the batch contain coupled (multi-row) requests?
     RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -564,7 +587,7 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
         B.log_state = e->d_log_state.p;
         RL_CUDA(e, cudaMemsetAsync(B.log_row, 0, (size_t)buf_len * sizeof(uint8_t*), e->stream));
         B.phase = RL_PHASE_SNAPSHOT;
-        r = launch_main<AccSrc, 0>(e, D, B, src);
+        r = main0();
         if (r) return r;
         // Fixed-point iteration over the requests' first-limited positions (DESIGN.md §3.4):
         // each speculative round replays the batch from the committed table state.
@@ -572,7 +595,7 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
             if (round > n_req + 2) return fail(e, RL_FATAL, "fixed-point iteration did not converge");
             RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_CHANGED, 0, sizeof(uint32_t), e->stream));
             B.phase = RL_PHASE_SPEC;
-            r = launch_main<AccSrc, 0>(e, D, B, src);
+            r = main0();
             if (r) return r;
             with_cells(e, [&](auto c) {
                 constexpr int C = decltype(c)::value;
@@ -591,7 +614,11 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
         }
     }
     B.phase = RL_PHASE_COMMIT;
-    return launch_main<AccSrc, 0>(e, D, B, src);
+    if ((r = main0()) || !scatter) return r;
+    k_wide_scatter<<<ceil_div(n_req, 128), 128, 0, e->stream>>>(n_req, o.off, acc_stride, o.stride, e->d_perm.p, ob.rem,
+                                                                 ob.ttl, o.rem, o.ttl);
+    RL_LAUNCH_CHECK(e);
+    return RL_OK;
 }
 
 // Hooks of the sharded step (rl_shard_*): the owner's inbox is a segmented record source whose size is
@@ -617,16 +644,22 @@ int run_record_pipeline(rl_engine* e, uint32_t n, const rl_record* d_recs, int m
         if (compact_now) return fail(e, RL_FATAL, "16-byte records need single-row namespaces (use the 32-byte form)");
         // some namespace spans several rows: materialise accesses (stride = max limits per ns)
         const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
-        if (stride > RL_MAX_CTRS_PER_REQ)
-            return fail(e, RL_FATAL, "a namespace has more than %d limits", RL_MAX_CTRS_PER_REQ);
+        if (stride > e->max_ctrs_req)
+            return fail(e, RL_FATAL, "a namespace has more than %u limits", e->max_ctrs_req);
         const uint64_t n_acc = (uint64_t)n * stride;
         if (n_acc > e->d_acc.n)
             return fail(e, RL_FATAL, "batch of %u records x %u limits exceeds max_counters=%u", n, stride, e->max_counters);
         RlResolveOut O{e->d_acc.p, e->d_delta.p, e->d_now.p, o.limited, o.first};
-        k_resolve_records<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, n, d_recs, stride, O, mode == 0);
+        // the namespace with the most limits sets the stride, and with it the encoding of the whole batch
+        const bool wide = stride > RL_MAX_CTRS_PER_REQ;
+        if (wide)
+            k_resolve_records_wide<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, n, d_recs, stride, O, mode == 0, e->d_perm.p,
+                                                                             e->max_ctrs_req);
+        else
+            k_resolve_records<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, n, d_recs, stride, O, mode == 0);
         RL_LAUNCH_CHECK(e);
         if ((r = check_resolve_error(e))) return r;
-        r = run_acc_pipeline(e, (uint32_t)n_acc, n, e->d_delta.p, e->d_now.p, mode, lc, o);
+        r = run_acc_pipeline(e, (uint32_t)n_acc, n, e->d_delta.p, e->d_now.p, mode, lc, o, wide, stride);
         if (r == RL_OK && e->ns_hook && mode == 0 && o.limited) r = e->ns_hook(e, e->stream, n, d_recs, 32, o.limited, o.first);
         return r;
     }
@@ -757,6 +790,8 @@ uint32_t rl_owner_of(uint32_t ns_id, uint32_t world) {
 
 const char* rl_last_error(rl_engine* e) { return e ? e->last_error.c_str() : "null engine"; }
 
+uint32_t rl_engine_max_counters_per_request(rl_engine* e) { return e ? e->max_ctrs_req : RL_MAX_COUNTERS_PER_REQUEST; }
+
 int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     if (!cfg || !out) return RL_FATAL;
     *out = nullptr;
@@ -770,6 +805,13 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     rl_engine* e = new rl_engine();
     *out = e;  // returned even on failure so the caller can read rl_last_error, then destroy
     e->device = cfg->device;
+    {
+        const uint32_t w = cfg->max_counters_per_request;
+        if (w != 0 && (w < RL_MAX_COUNTERS_PER_REQUEST || w > RL_MAX_COUNTERS_PER_REQUEST_WIDE))
+            return fail(e, RL_FATAL, "max_counters_per_request=%u: must be 0 (= %d) or %d..%d", w, RL_MAX_COUNTERS_PER_REQUEST,
+                        RL_MAX_COUNTERS_PER_REQUEST, RL_MAX_COUNTERS_PER_REQUEST_WIDE);
+        if (w) e->max_ctrs_req = w;
+    }
     RL_CUDA(e, cudaSetDevice(e->device));
     cudaDeviceProp prop;
     RL_CUDA(e, cudaGetDeviceProperties(&prop, e->device));
@@ -818,6 +860,7 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     RL_CUDA(e, cudaMemsetAsync(e->d_misc.p, 0, MISC_N * sizeof(uint32_t), e->stream));
     RL_CUDA(e, cudaMallocHost((void**)&e->h_misc, MISC_N * sizeof(uint32_t)));
     RL_CUDA(e, e->d_acc.reserve(e->max_counters));
+    if (e->max_ctrs_req > RL_MAX_CTRS_PER_REQ) RL_CUDA(e, e->d_perm.reserve(e->max_counters));
     RL_CUDA(e, e->d_kstats.reserve(32));
     RL_CUDA(e, cudaMemsetAsync(e->d_kstats.p, 0, 32 * sizeof(unsigned long long), e->stream));
     RL_CUDA(e, e->d_delta.reserve(e->max_batch));
@@ -1510,6 +1553,30 @@ static int stage_csr(rl_engine* e, uint64_t n, const uint32_t* off, const rl_cou
     return RL_OK;
 }
 
+// The general form's resolve.  k_resolve_csr takes requests of up to 16 counters and reports a longer one as
+// RL_DEV_TOO_MANY_COUNTERS.  On an engine created for more (max_counters_per_request > 16) that report is what
+// selects the wide path: the batch is resolved again with the wide encoding and `wide` is set.  A batch without such
+// a request runs exactly the kernels of a default engine.
+static int resolve_csr(rl_engine* e, uint64_t n, const CsrDev& c, const RlResolveOut& O, int write_defaults, bool& wide) {
+    RlDev D = make_dev(e);
+    wide = false;
+    k_resolve_csr<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, write_defaults);
+    RL_LAUNCH_CHECK(e);
+    if (e->max_ctrs_req > RL_MAX_CTRS_PER_REQ) {
+        RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+        RL_CUDA(e, cudaStreamSynchronize(e->stream));
+        if (e->h_misc[MISC_ERR] == RL_DEV_TOO_MANY_COUNTERS) {
+            // every other refusal has a lower code (the error word is a sticky max): the wide pass finds it again
+            RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_ERR, 0, 2 * sizeof(uint32_t), e->stream));  // error + flags
+            k_resolve_csr_wide<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, write_defaults,
+                                                                        e->d_perm.p, e->max_ctrs_req);
+            RL_LAUNCH_CHECK(e);
+            wide = true;
+        }
+    }
+    return check_resolve_error(e);
+}
+
 int rl_check_and_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off, const rl_counter* ctrs,
                               const uint64_t* delta, const uint64_t* now_us, int load_counters, int mem,
                               uint8_t* out_limited, uint32_t* out_first_limited, uint64_t* out_remaining,
@@ -1528,13 +1595,12 @@ int rl_check_and_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off,
     Outs o;
     if ((r = bind_outs(e, mem, user, c.total, o))) return r;
     o.off = c.off;
-    RlDev D = make_dev(e);
     RlResolveOut O{e->d_acc.p, nullptr, nullptr, o.limited, o.first};
-    k_resolve_csr<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, 1);
-    RL_LAUNCH_CHECK(e);
-    if ((r = check_resolve_error(e))) return r;
+    bool wide;
+    if ((r = resolve_csr(e, n, c, O, 1, wide))) return r;
     if (c.total) {
-        if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 0, load_counters ? 1 : 0, o))) return r;
+        if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 0, load_counters ? 1 : 0, o, wide)))
+            return r;
     }
     return copy_back(e, mem, n, c.total, o, user);
 }
@@ -1551,12 +1617,10 @@ int rl_update_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off, const rl_
     e->stats.requests += n;
     if (c.total == 0) return RL_OK;
     Outs o;
-    RlDev D = make_dev(e);
     RlResolveOut O{e->d_acc.p, nullptr, nullptr, nullptr, nullptr};
-    k_resolve_csr<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, 0);
-    RL_LAUNCH_CHECK(e);
-    if ((r = check_resolve_error(e))) return r;
-    if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 2, 0, o))) return r;
+    bool wide;
+    if ((r = resolve_csr(e, n, c, O, 0, wide))) return r;
+    if ((r = run_acc_pipeline(e, (uint32_t)c.total, (uint32_t)n, c.delta, c.now, 2, 0, o, wide))) return r;
     return copy_back(e, mem, n, 0, o, o);
 }
 

@@ -271,6 +271,7 @@ struct RlReq {       // what the replay needs of an access
 struct RecordSrc {
     static constexpr bool kAccessIsRequest = true;
     static constexpr bool kCanBeMulti = false;  // every namespace maps to one row
+    static constexpr bool kWide = false;        // posorig encoding (rl_core.h)
     const rl_record* recs;
     const uint32_t* seg_prefix;  // [nseg+1] exclusive prefix of the block fills (device), or nullptr
     uint32_t nseg;
@@ -349,6 +350,7 @@ struct RecordSrc {
 struct AccSrc {
     static constexpr bool kAccessIsRequest = false;
     static constexpr bool kCanBeMulti = true;
+    static constexpr bool kWide = false;
     const RlAccess* acc;
     const uint64_t* delta;  // per request
     const uint64_t* now;    // per request
@@ -372,6 +374,11 @@ struct AccSrc {
         q.delta = delta[q.req];
         q.now = now[q.req];
     }
+};
+// Accesses of a batch with a request of more than 16 counters: resolved with the wide position encoding
+// (rl_core.h, DESIGN.md §9g), whose remaining / ttl outputs go to scratch in processing order.
+struct AccSrcWide : AccSrc {
+    static constexpr bool kWide = true;
 };
 
 // ---------------------------------------------------------------------------------------
@@ -758,7 +765,7 @@ struct RlMyLimits {
 //          first limited counter (in_memory.rs:110-112,130-132,141-143)
 //   b_ok : every touched cell is live at `now` and stays within its limit after adding
 //          `dsum` (this request's delta plus those of the run before it)
-template <int CELLS>
+template <int CELLS, bool WIDE = false>
 __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const unsigned long long* se,
                                            const RlMyLimits& L, uint32_t cells, uint64_t posorig, uint64_t delta,
                                            uint64_t dsum, uint64_t now, bool lc, bool check_limit, bool& a_ok,
@@ -774,7 +781,7 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
             const bool reached = lc || fl == RL_NONE_U32;  // !lc: the walk returns at the first limited counter
             if (reached && ((L.qmask >> k) & 1u) && e == 0) absent_reached = true;
             const uint64_t vv = (e <= now) ? 0 : v;
-            if (reached && fl == RL_NONE_U32 && vv + delta > L.mx[k]) fl = rl_pos_at(posorig, k);
+            if (reached && fl == RL_NONE_U32 && vv + delta > L.mx[k]) fl = rl_pos_of<WIDE>(posorig, k);
             if (e <= now) live_all = false;
             if (v + dsum > L.mx[k]) within_all = false;
         }
@@ -813,7 +820,7 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
 // memory) — the default path (single-row request, load_counters off).  Same arithmetic as
 // rl_walk_check_single / rl_walk_update (rl_core.h), without a private copy of the row.
 //   in_memory.rs:122-127 (insert on lookup), :110-112,130-132 (early return), :146-153 (update)
-template <int CELLS>
+template <int CELLS, bool WIDE = false>
 __device__ __forceinline__ uint32_t rl_apply_check_smem(unsigned long long* sv, unsigned long long* se,
                                                         const RlMyLimits& L, const RlCellDesc* gdesc, uint32_t cells,
                                                         uint64_t posorig, uint64_t delta, uint64_t now,
@@ -833,7 +840,7 @@ __device__ __forceinline__ uint32_t rl_apply_check_smem(unsigned long long* sv, 
                 dirty |= 1u << c;
             }
             const uint64_t vv = (e <= now) ? 0 : v;
-            if (vv + delta > L.mx[k]) fl = rl_pos_at(posorig, k);
+            if (vv + delta > L.mx[k]) fl = rl_pos_of<WIDE>(posorig, k);
         }
     }
     if (fl != RL_NONE_U32) return fl;
@@ -882,7 +889,7 @@ __device__ __forceinline__ void rl_apply_update_smem(unsigned long long* sv, uns
 //   ord/cnt  my stream-order ordinal inside the group and the group's size
 //   peers    the lanes of my warp that belong to my group (leader = lowest of them; solo = I am alone)
 // Returns the number of rounds the CTA ran.
-template <int CELLS, int MODE, bool LC>
+template <int CELLS, int MODE, bool LC, bool WIDE = false>
 __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool write_out, unsigned long long* gsv,
                                                      unsigned long long* gse, uint32_t* gmin, uint32_t gstride,
                                                      uint32_t* gdirty, const RlReq& acc, const RlMyLimits& L,
@@ -904,7 +911,7 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
             if (!multi) {
                 const uint64_t dsum = (uint64_t)(ord - pos + 1) * delta;
                 // update_counters never tests the limit: a run only needs live cells
-                rl_eval_ab<CELLS>(gsv, gse, L, acc.cells, acc.posorig, delta, dsum, now, lc, MODE == 0, aok, bok, fl);
+                rl_eval_ab<CELLS, WIDE>(gsv, gse, L, acc.cells, acc.posorig, delta, dsum, now, lc, MODE == 0, aok, bok, fl);
                 if (MODE == 2) aok = false;
                 bok = bok && like_rep;
             }
@@ -950,7 +957,7 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
                 if (ord < mA) {
                     mine = true;
                     if (lc && write_out) {  // remaining / ttl of every counter
-                        fl = rl_walk_check_single<CELLS>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, true, rem, ttl);
+                        fl = rl_walk_check_single<CELLS, WIDE>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, true, rem, ttl);
                         dirty = 0;
                     }
                 }
@@ -962,7 +969,7 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
                     store = (ord == mB - 1);
                     if (MODE == 0 && lc && write_out) {
                         rl_advance_run<CELLS>(loc, acc.cells, (uint64_t)(ord - pos) * delta);
-                        fl = rl_walk_check_single<CELLS>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, lc, rem, ttl);
+                        fl = rl_walk_check_single<CELLS, WIDE>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, lc, rem, ttl);
                         fast_store = false;
                     } else if (store) {
                         // the run's last member is the sole writer of S (nobody reads it until
@@ -989,7 +996,7 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
                             rl_apply_update_smem<CELLS>(gsv, gse, gdesc, acc.cells,
                                                         delta, now, dirty);
                         else
-                            fl = rl_apply_check_smem<CELLS>(gsv, gse, L, gdesc,
+                            fl = rl_apply_check_smem<CELLS, WIDE>(gsv, gse, L, gdesc,
                                                             acc.cells, acc.posorig, delta, now, dirty);
                     } else {
                         if (!lc) {
@@ -1002,11 +1009,11 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
                         if (MODE == 2) {
                             rl_walk_update<CELLS>(loc, dirty, desc, acc.cells, delta, now);
                         } else if (!multi) {
-                            fl = rl_walk_check_single<CELLS>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, lc, rem, ttl);
+                            fl = rl_walk_check_single<CELLS, WIDE>(loc, dirty, desc, acc.cells, acc.posorig, delta, now, lc, rem, ttl);
                         } else {
                             const uint32_t fl_in = B.fl_prev[acc.req];
-                            const uint32_t local = rl_walk_check_multi<CELLS>(loc, dirty, desc, acc.cells, acc.posorig,
-                                                                             delta, now, lc, fl_in, rem, ttl);
+                            const uint32_t local = rl_walk_check_multi<CELLS, WIDE>(loc, dirty, desc, acc.cells, acc.posorig,
+                                                                                   delta, now, lc, fl_in, rem, ttl);
                             if (!write_out && local != RL_NONE_U32) atomicMin(&B.fl_next[acc.req], local);
                             fl = fl_in;
                         }
@@ -1024,7 +1031,7 @@ __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool writ
                             // the access holding position fl names the limit
 #pragma unroll
                             for (int k = 0; k < CELLS; k++)
-                                if ((uint32_t)k < ncell && rl_pos_at(acc.posorig, k) == fl)
+                                if ((uint32_t)k < ncell && rl_pos_of<WIDE>(acc.posorig, k) == fl)
                                     B.out_first_limited[acc.req] = desc[rl_cells_at(acc.cells, k)].limit_id;
                         }
                     }
@@ -1294,7 +1301,7 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             bool done = !valid || snapshot;
             uint32_t pos = 0;
             for (int attempt = 0;; attempt++) {
-            const uint32_t nrounds = rl_replay_rounds<CELLS, MODE, LC>(
+            const uint32_t nrounds = rl_replay_rounds<CELLS, MODE, LC, Src::kWide>(
                 B, write_out, &sm.s_val[gid * CELLS], &sm.s_exp[gid * CELLS], &sm.g_min[0][0][gid], CH, &sm.g_dirty[gid], acc, L,
                 desc, gdesc, multi, like_rep, valid, peers, solo, leader, lane, ord, cnt, done, pos);
             if (tid == 0) {
@@ -1760,8 +1767,15 @@ struct RlResolveOut {
     uint32_t* out_first_limited;  // nullable
 };
 
-__global__ void k_resolve_csr(RlDev D, uint32_t n, const uint32_t* __restrict__ off,
-                              const rl_counter* __restrict__ ctrs, RlResolveOut O, int write_defaults) {
+// The general form's body, instantiated narrow (k_resolve_csr: up to 16 counters) and wide (k_resolve_csr_wide: up
+// to max_ctrs <= 64, perm[slot] = original index of the counter processed at that slot's position).  The narrow
+// kernels report a longer request as RL_DEV_TOO_MANY_COUNTERS; on an engine created for more, that report selects
+// the wide kernels (rl_engine.cu).
+template <bool WIDE>
+__device__ __forceinline__ void rl_resolve_csr(const RlDev& D, uint32_t n, const uint32_t* __restrict__ off,
+                                               const rl_counter* __restrict__ ctrs, const RlResolveOut& O,
+                                               int write_defaults, uint8_t* perm, uint32_t max_ctrs) {
+    constexpr uint32_t MAXC = WIDE ? RL_MAX_CTRS_PER_REQ_WIDE : RL_MAX_CTRS_PER_REQ;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t o0 = off[i], m = off[i + 1] - o0;
@@ -1780,11 +1794,11 @@ __global__ void k_resolve_csr(RlDev D, uint32_t n, const uint32_t* __restrict__ 
         r.key_hi = c.key_hi;
         return r;
     };
-    RlAccess tmp[RL_MAX_CTRS_PER_REQ];
-    const int nacc = rl_resolve_request(i, m, get, D.limits, D.limits_cap, true, tmp);
+    RlAccess tmp[MAXC];
+    const int nacc = rl_resolve_request<WIDE>(i, m, get, D.limits, D.limits_cap, true, tmp, WIDE ? perm + o0 : nullptr, max_ctrs);
     if (nacc < 0) {
         rl_set_err(D, (uint32_t)(-nacc));
-        for (uint32_t x = 0; x < m && x < RL_MAX_CTRS_PER_REQ; x++) {
+        for (uint32_t x = 0; x < m && x < MAXC; x++) {
             RlAccess z;
             z.key_lo = 0;
             z.hdr_hi = 0;
@@ -1793,8 +1807,8 @@ __global__ void k_resolve_csr(RlDev D, uint32_t n, const uint32_t* __restrict__ 
             z.posorig = 0;
             O.acc[o0 + x] = z;
         }
-        // slots beyond RL_MAX_CTRS_PER_REQ (too-many-counters error) are cleared too
-        for (uint32_t x = RL_MAX_CTRS_PER_REQ; x < m; x++) {
+        // slots beyond MAXC (too-many-counters error) are cleared too
+        for (uint32_t x = MAXC; x < m; x++) {
             RlAccess z;
             z.key_lo = 0;
             z.hdr_hi = 0;
@@ -1808,6 +1822,16 @@ __global__ void k_resolve_csr(RlDev D, uint32_t n, const uint32_t* __restrict__ 
     }
     for (uint32_t x = 0; x < m; x++) O.acc[o0 + x] = tmp[x];
     if (nacc > 1) atomicOr(D.flags, 1u);
+}
+
+__global__ void k_resolve_csr(RlDev D, uint32_t n, const uint32_t* __restrict__ off,
+                              const rl_counter* __restrict__ ctrs, RlResolveOut O, int write_defaults) {
+    rl_resolve_csr<false>(D, n, off, ctrs, O, write_defaults, nullptr, 0);
+}
+__global__ void k_resolve_csr_wide(RlDev D, uint32_t n, const uint32_t* __restrict__ off,
+                                   const rl_counter* __restrict__ ctrs, RlResolveOut O, int write_defaults,
+                                   uint8_t* perm, uint32_t max_ctrs) {
+    rl_resolve_csr<true>(D, n, off, ctrs, O, write_defaults, perm, max_ctrs);
 }
 
 // Records whose namespaces span several rows: slot base = i * stride.
@@ -1856,6 +1880,76 @@ __global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restri
     }
     for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = (x < m) ? tmp[x] : z;
     if (nacc > 1) atomicOr(D.flags, 1u);
+}
+
+// The wide form of k_resolve_records (kept apart so that the narrow kernel's code stays as it was).  perm[slot] =
+// original index of the counter processed at that slot's position, 0xFF for a slot without a counter.
+__global__ void k_resolve_records_wide(RlDev D, uint32_t n, const rl_record* __restrict__ recs, uint32_t stride,
+                                       RlResolveOut O, int write_defaults, uint8_t* perm, uint32_t max_ctrs) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const rl_record rec = recs[i];
+    O.delta[i] = rec.hits_addend;
+    O.now[i] = rec.now_us;
+    uint32_t m = 0, lim_off = 0;
+    if (rec.ns_id < D.ns_cap) {
+        const RlNsDev ns = D.ns[rec.ns_id];
+        m = ns.lim_cnt;
+        lim_off = ns.lim_off;
+    }
+    const size_t o0 = (size_t)i * stride;
+    RlAccess z;
+    z.key_lo = 0;
+    z.hdr_hi = 0;
+    z.req = i;
+    z.cells = 0;
+    z.posorig = 0;
+    for (uint32_t x = 0; x < stride; x++) perm[o0 + x] = 0xFFu;  // the resolve overwrites the first m
+    if (m == 0) {
+        for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
+        if (write_defaults) {
+            O.out_limited[i] = 0;
+            if (O.out_first_limited) O.out_first_limited[i] = RL_NONE_U32;
+        }
+        return;
+    }
+    auto get = [&](uint32_t j) {
+        RlCtrIn r;
+        r.limit_id = D.ns_limit_ids[lim_off + j];
+        r.key_lo = rec.key_lo;
+        r.key_hi = rec.key_hi & RL_RECORD_KEY_HI_MASK;
+        return r;
+    };
+    RlAccess tmp[RL_MAX_CTRS_PER_REQ_WIDE];
+    const int nacc = rl_resolve_request<true>(i, m, get, D.limits, D.limits_cap, true, tmp, perm + o0, max_ctrs);
+    if (nacc < 0) {
+        rl_set_err(D, (uint32_t)(-nacc));
+        for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
+        if (write_defaults) O.out_limited[i] = 0;
+        return;
+    }
+    for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = (x < m) ? tmp[x] : z;
+    if (nacc > 1) atomicOr(D.flags, 1u);
+}
+
+// Wide batches with load_counters: k_main wrote remaining / ttl at the request's base slot + processing position;
+// put them where the caller expects them, at the original index (perm, written by the wide resolve).
+//   CSR (off != nullptr): slots off[i] .. off[i+1], caller's index off[i] + original index
+//   records             : slots i*in_stride .., caller's index i*out_stride + original index (0xFF: no counter)
+__global__ void k_wide_scatter(uint32_t n, const uint32_t* __restrict__ off, uint32_t in_stride, uint32_t out_stride,
+                               const uint8_t* __restrict__ perm, const uint64_t* __restrict__ rem_in,
+                               const uint64_t* __restrict__ ttl_in, uint64_t* rem, uint64_t* ttl) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const size_t b_in = off ? (size_t)off[i] : (size_t)i * in_stride;
+    const uint32_t m = off ? off[i + 1] - off[i] : in_stride;
+    const size_t b_out = off ? (size_t)off[i] : (size_t)i * out_stride;
+    for (uint32_t p = 0; p < m; p++) {
+        const uint32_t j = perm[b_in + p];
+        if (j == 0xFFu) continue;
+        if (rem) rem[b_out + j] = rem_in[b_in + p];
+        if (ttl) ttl[b_out + j] = ttl_in[b_in + p];
+    }
 }
 
 // Undo a speculative round: put every logged row back to its state at batch start.

@@ -522,6 +522,13 @@ int rl_matcher_set_counter_cap(rl_matcher* m, uint32_t cap) {
     return RL_OK;
 }
 
+// The cap in force (0 for m == NULL).  Library-internal: the RLS service sizes its counter buffers by it.
+uint32_t rl_matcher_counter_cap(rl_matcher* m) {
+    if (!m) return 0;
+    std::shared_lock<std::shared_mutex> lock(m->mu);
+    return m->counter_cap;
+}
+
 int rl_matcher_delete_limit(rl_matcher* m, uint32_t limit_id) {
     if (!m) return RL_FATAL;
     std::unique_lock<std::shared_mutex> lock(m->mu);

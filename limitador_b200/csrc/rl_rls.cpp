@@ -24,6 +24,11 @@
 
 #include "rl_rls.h"
 
+extern "C" uint32_t rl_matcher_counter_cap(rl_matcher* m);  // rl_match.cpp (library-internal)
+// Weak: the wire surface is also linked without the engine (the sanitizer build of tests/san); there every service
+// plans with the default engine's maximum.
+extern "C" __attribute__((weak)) uint32_t rl_engine_max_counters_per_request(rl_engine* e);
+
 namespace {
 
 // ---- protobuf wire format (proto3) -----------------------------------------------------------------------------
@@ -487,7 +492,11 @@ void plan_range(rl_rls* s, const uint64_t* off, uint32_t w) {
     const uint64_t k_req = W.req_of.size();
     W.ctr_off.assign(k_req + 1, 0);
     W.status.assign(k_req, 0);
-    W.ctrs.ensure((k_req + 1) * (size_t)RL_MAX_COUNTERS_PER_REQUEST);
+    // room per request: the matcher's cap, but not more than the engine takes (a service without an engine: 16)
+    const uint32_t engine_max = (s->engine && rl_engine_max_counters_per_request)
+                                    ? rl_engine_max_counters_per_request(s->engine) : RL_MAX_COUNTERS_PER_REQUEST;
+    const uint32_t per_req = std::min(rl_matcher_counter_cap(s->m), engine_max);
+    W.ctrs.ensure((k_req + 1) * (size_t)per_req);
     if (rl_matcher_counters_batch_ns(s->m, k_req, W.ns.data(), W.bind_off.data(), W.binds.data(), W.ctr_off.data(), W.ctrs.data(),
                                      W.ctrs.size(), W.status.data()) != RL_OK) {
         for (const uint64_t i : W.req_of) s->plan[i].kind = REQ_UNSUPPORTED;  // (the matcher's cap was raised past the engine's)

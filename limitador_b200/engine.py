@@ -44,6 +44,7 @@ LIMIT_DESC_DTYPE = np.dtype(
 # every symbol include/rl_engine.h declares (tests check the library exports them all)
 ABI_SYMBOLS = [
     "rl_engine_create", "rl_engine_destroy", "rl_last_error", "rl_engine_set_stream", "rl_engine_stream",
+    "rl_engine_max_counters_per_request",
     "rl_sync", "rl_get_stats", "rl_limits_set", "rl_limits_delete", "rl_check_and_update_records",
     "rl_check_and_update_batch", "rl_is_within_limits_batch", "rl_is_within_limits_records",
     "rl_update_batch", "rl_update_records", "rl_get_counters", "rl_delete_counters", "rl_clear",
@@ -64,7 +65,7 @@ class RlConfig(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32), ("device", C.c_int32), ("capacity_rows", C.c_uint64),
         ("cells_per_row", C.c_uint32), ("max_batch", C.c_uint32), ("max_counters", C.c_uint32),
-        ("regions", C.c_uint32), ("flags", C.c_uint32), ("_pad", C.c_uint32),
+        ("regions", C.c_uint32), ("flags", C.c_uint32), ("max_counters_per_request", C.c_uint32),
     ]
 
 
@@ -106,6 +107,8 @@ def load_library(path: str | None = None):
     L.rl_engine_destroy.restype = None
     L.rl_last_error.argtypes = [vp]
     L.rl_last_error.restype = C.c_char_p
+    L.rl_engine_max_counters_per_request.argtypes = [vp]
+    L.rl_engine_max_counters_per_request.restype = u32
     L.rl_engine_set_stream.argtypes = [vp, vp]
     L.rl_engine_stream.argtypes = [vp]
     L.rl_engine_stream.restype = vp
@@ -184,11 +187,14 @@ class Engine:
     """One GPU-resident counter table (one per process / per GPU)."""
 
     def __init__(self, capacity_rows: int, cells_per_row: int = 1, max_batch: int = 65536,
-                 max_counters: int = 0, regions: int = 0, device: int = 0, flags: int = 0):
+                 max_counters: int = 0, regions: int = 0, device: int = 0, flags: int = 0,
+                 max_counters_per_request: int = 0):
+        """max_counters_per_request: counters one request may name (and limits one namespace may have on the
+        record path); 0 = 16, up to 64.  Batches without a longer request run the same kernels either way."""
         self._lib = load_library()
         self._h = C.c_void_p()
         cfg = RlConfig(C.sizeof(RlConfig), device, capacity_rows, cells_per_row, max_batch, max_counters,
-                       regions, flags, 0)
+                       regions, flags, max_counters_per_request)
         st = self._lib.rl_engine_create(C.byref(cfg), C.byref(self._h))
         if st != RL_OK:
             msg = "rl_engine_create failed (no CUDA device? limitador_b200 has no CPU fallback)"
@@ -200,6 +206,7 @@ class Engine:
         self.cells_per_row = cells_per_row
         self.max_batch = max_batch
         self.device = device
+        self.max_counters_per_request = int(self._lib.rl_engine_max_counters_per_request(self._h))
 
     # -- lifecycle --
     def close(self):

@@ -136,7 +136,8 @@ class Matcher:
         return desc[0], bool(existed.value)
 
     def set_counter_cap(self, cap: int):
-        """Counters one request may produce (default 16 = what the engine takes); raise it only to match without the engine."""
+        """Counters one request may produce (default 16 = what a default engine takes); raise it to the engine's
+        max_counters_per_request (up to 64) to ship wider requests, or past it to match without the engine."""
         self._check(self._lib.rl_matcher_set_counter_cap(self._h, cap))
 
     def delete_limit(self, limit_id: int):
