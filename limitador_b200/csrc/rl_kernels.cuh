@@ -1767,6 +1767,17 @@ struct RlResolveOut {
     uint32_t* out_first_limited;  // nullable
 };
 
+// An access slot of request req without a counter (hdr_hi = 0: no row).
+__device__ __forceinline__ RlAccess rl_no_access(uint32_t req) {
+    RlAccess z;
+    z.key_lo = 0;
+    z.hdr_hi = 0;
+    z.req = req;
+    z.cells = 0;
+    z.posorig = 0;
+    return z;
+}
+
 // The general form's body, instantiated narrow (k_resolve_csr: up to 16 counters) and wide (k_resolve_csr_wide: up
 // to max_ctrs <= 64, perm[slot] = original index of the counter processed at that slot's position).  The narrow
 // kernels report a longer request as RL_DEV_TOO_MANY_COUNTERS; on an engine created for more, that report selects
@@ -1798,25 +1809,7 @@ __device__ __forceinline__ void rl_resolve_csr(const RlDev& D, uint32_t n, const
     const int nacc = rl_resolve_request<WIDE>(i, m, get, D.limits, D.limits_cap, true, tmp, WIDE ? perm + o0 : nullptr, max_ctrs);
     if (nacc < 0) {
         rl_set_err(D, (uint32_t)(-nacc));
-        for (uint32_t x = 0; x < m && x < MAXC; x++) {
-            RlAccess z;
-            z.key_lo = 0;
-            z.hdr_hi = 0;
-            z.req = i;
-            z.cells = 0;
-            z.posorig = 0;
-            O.acc[o0 + x] = z;
-        }
-        // slots beyond MAXC (too-many-counters error) are cleared too
-        for (uint32_t x = MAXC; x < m; x++) {
-            RlAccess z;
-            z.key_lo = 0;
-            z.hdr_hi = 0;
-            z.req = i;
-            z.cells = 0;
-            z.posorig = 0;
-            O.acc[o0 + x] = z;
-        }
+        for (uint32_t x = 0; x < m; x++) O.acc[o0 + x] = rl_no_access(i);  // beyond MAXC too (too many counters)
         if (write_defaults) O.out_limited[i] = 0;
         return;
     }
@@ -1834,9 +1827,13 @@ __global__ void k_resolve_csr_wide(RlDev D, uint32_t n, const uint32_t* __restri
     rl_resolve_csr<true>(D, n, off, ctrs, O, write_defaults, perm, max_ctrs);
 }
 
-// Records whose namespaces span several rows: slot base = i * stride.
-__global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restrict__ recs, uint32_t stride,
-                                  RlResolveOut O, int write_defaults) {
+// Records whose namespaces span several rows: slot base = i * stride.  The body of k_resolve_records (narrow) and
+// k_resolve_records_wide (wide: perm as in rl_resolve_csr, 0xFF for a slot without a counter).
+template <bool WIDE>
+__device__ __forceinline__ void rl_resolve_records(const RlDev& D, uint32_t n, const rl_record* __restrict__ recs,
+                                                   uint32_t stride, const RlResolveOut& O, int write_defaults,
+                                                   uint8_t* perm, uint32_t max_ctrs) {
+    constexpr uint32_t MAXC = WIDE ? RL_MAX_CTRS_PER_REQ_WIDE : RL_MAX_CTRS_PER_REQ;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const rl_record rec = recs[i];
@@ -1849,12 +1846,9 @@ __global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restri
         lim_off = ns.lim_off;
     }
     const size_t o0 = (size_t)i * stride;
-    RlAccess z;
-    z.key_lo = 0;
-    z.hdr_hi = 0;
-    z.req = i;
-    z.cells = 0;
-    z.posorig = 0;
+    const RlAccess z = rl_no_access(i);
+    if (WIDE)
+        for (uint32_t x = 0; x < stride; x++) perm[o0 + x] = 0xFFu;  // the resolve overwrites the first m
     if (m == 0) {
         for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
         if (write_defaults) {
@@ -1870,8 +1864,8 @@ __global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restri
         r.key_hi = rec.key_hi & RL_RECORD_KEY_HI_MASK;
         return r;
     };
-    RlAccess tmp[RL_MAX_CTRS_PER_REQ];
-    const int nacc = rl_resolve_request(i, m, get, D.limits, D.limits_cap, true, tmp);
+    RlAccess tmp[MAXC];
+    const int nacc = rl_resolve_request<WIDE>(i, m, get, D.limits, D.limits_cap, true, tmp, WIDE ? perm + o0 : nullptr, max_ctrs);
     if (nacc < 0) {
         rl_set_err(D, (uint32_t)(-nacc));
         for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
@@ -1882,54 +1876,13 @@ __global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restri
     if (nacc > 1) atomicOr(D.flags, 1u);
 }
 
-// The wide form of k_resolve_records (kept apart so that the narrow kernel's code stays as it was).  perm[slot] =
-// original index of the counter processed at that slot's position, 0xFF for a slot without a counter.
+__global__ void k_resolve_records(RlDev D, uint32_t n, const rl_record* __restrict__ recs, uint32_t stride,
+                                  RlResolveOut O, int write_defaults) {
+    rl_resolve_records<false>(D, n, recs, stride, O, write_defaults, nullptr, RL_MAX_CTRS_PER_REQ_WIDE);
+}
 __global__ void k_resolve_records_wide(RlDev D, uint32_t n, const rl_record* __restrict__ recs, uint32_t stride,
                                        RlResolveOut O, int write_defaults, uint8_t* perm, uint32_t max_ctrs) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const rl_record rec = recs[i];
-    O.delta[i] = rec.hits_addend;
-    O.now[i] = rec.now_us;
-    uint32_t m = 0, lim_off = 0;
-    if (rec.ns_id < D.ns_cap) {
-        const RlNsDev ns = D.ns[rec.ns_id];
-        m = ns.lim_cnt;
-        lim_off = ns.lim_off;
-    }
-    const size_t o0 = (size_t)i * stride;
-    RlAccess z;
-    z.key_lo = 0;
-    z.hdr_hi = 0;
-    z.req = i;
-    z.cells = 0;
-    z.posorig = 0;
-    for (uint32_t x = 0; x < stride; x++) perm[o0 + x] = 0xFFu;  // the resolve overwrites the first m
-    if (m == 0) {
-        for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
-        if (write_defaults) {
-            O.out_limited[i] = 0;
-            if (O.out_first_limited) O.out_first_limited[i] = RL_NONE_U32;
-        }
-        return;
-    }
-    auto get = [&](uint32_t j) {
-        RlCtrIn r;
-        r.limit_id = D.ns_limit_ids[lim_off + j];
-        r.key_lo = rec.key_lo;
-        r.key_hi = rec.key_hi & RL_RECORD_KEY_HI_MASK;
-        return r;
-    };
-    RlAccess tmp[RL_MAX_CTRS_PER_REQ_WIDE];
-    const int nacc = rl_resolve_request<true>(i, m, get, D.limits, D.limits_cap, true, tmp, perm + o0, max_ctrs);
-    if (nacc < 0) {
-        rl_set_err(D, (uint32_t)(-nacc));
-        for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = z;
-        if (write_defaults) O.out_limited[i] = 0;
-        return;
-    }
-    for (uint32_t x = 0; x < stride; x++) O.acc[o0 + x] = (x < m) ? tmp[x] : z;
-    if (nacc > 1) atomicOr(D.flags, 1u);
+    rl_resolve_records<true>(D, n, recs, stride, O, write_defaults, perm, max_ctrs);
 }
 
 // Wide batches with load_counters: k_main wrote remaining / ttl at the request's base slot + processing position;

@@ -3,7 +3,8 @@
 // resolution into row accesses, per-row stream-order replay, and the fixed-point rounds
 // for multi-row requests — so the algorithm can be checked against the oracle on a
 // machine without a GPU.  GPU-only mechanics (partition, smem grouping, CAS inserts) are
-// covered by the -m gpu tests.
+// covered by the -m gpu tests.  Both position encodings of rl_core.h run through the one
+// driver: narrow (up to 16 counters per request) and wide (up to 64).
 #include <cstdint>
 #include <cstring>
 #include <map>
@@ -24,24 +25,18 @@ struct emu {
     std::map<std::pair<uint64_t, uint64_t>, RlRow<RL_MAX_CELLS>> table;
 };
 
-extern "C" {
-
-emu* emu_create(int cells) {
-    emu* e = new emu();
-    e->cells = cells;
-    return e;
-}
-void emu_destroy(emu* e) { delete e; }
-
-void emu_set_tables(emu* e, const RlLimitDev* limits, uint32_t n_limits, const RlCellDesc* desc, uint32_t n_groups) {
-    e->limits.assign(limits, limits + n_limits);
-    e->desc.assign(desc, desc + (size_t)n_groups * 8);
-}
-
 // mode 0: check_and_update, 2: update.  Returns 0 or a positive RL_DEV_* code.
-int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_counter* ctrs, const uint64_t* delta,
-                  const uint64_t* now, int lc, uint8_t* out_limited, uint32_t* out_first, uint64_t* out_rem,
-                  uint64_t* out_ttl, int* rounds_out) {
+// WIDE: the walkers write remaining / ttl in processing order into scratch, and the resolve's permutation scatters
+// them into the caller's order, as k_wide_scatter does.
+template <bool WIDE>
+static int batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_counter* ctrs, const uint64_t* delta,
+                     const uint64_t* now, int lc, uint8_t* out_limited, uint32_t* out_first, uint64_t* out_rem_user,
+                     uint64_t* out_ttl_user, int* rounds_out) {
+    constexpr uint32_t MAXC = WIDE ? RL_MAX_CTRS_PER_REQ_WIDE : RL_MAX_CTRS_PER_REQ;
+    std::vector<uint64_t> scr_rem(WIDE ? off[n] + 1 : 0), scr_ttl(WIDE ? off[n] + 1 : 0);
+    std::vector<uint8_t> perm(WIDE ? off[n] + 1 : 0);
+    uint64_t* out_rem = WIDE ? (out_rem_user ? scr_rem.data() : nullptr) : out_rem_user;
+    uint64_t* out_ttl = WIDE ? (out_ttl_user ? scr_ttl.data() : nullptr) : out_ttl_user;
     std::vector<RlAccess> acc(off[n]);
     bool any_multi = false;
     for (uint32_t i = 0; i < n; i++) {
@@ -58,8 +53,9 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
             r.key_hi = ctrs[o0 + j].key_hi;
             return r;
         };
-        RlAccess tmp[RL_MAX_CTRS_PER_REQ];
-        const int nacc = rl_resolve_request(i, m, get, e->limits.data(), (uint32_t)e->limits.size(), true, tmp);
+        RlAccess tmp[MAXC];
+        const int nacc = rl_resolve_request<WIDE>(i, m, get, e->limits.data(), (uint32_t)e->limits.size(), true, tmp,
+                                                  WIDE ? perm.data() + o0 : nullptr);
         if (nacc < 0) return -nacc;
         for (uint32_t x = 0; x < m; x++) acc[o0 + x] = tmp[x];
         if (nacc > 1) any_multi = true;
@@ -71,6 +67,11 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
 
     std::vector<uint32_t> fl_prev(n, RL_NONE_U32), fl_next(n, RL_NONE_U32);
     auto pass = [&](bool commit) {
+        // where the walkers write request req's remaining / ttl: only in the committing pass
+        auto lc_out = [&](uint32_t req) {
+            const bool on = lc && commit;
+            return std::make_pair(on && out_rem ? out_rem + off[req] : nullptr, on && out_ttl ? out_ttl + off[req] : nullptr);
+        };
         for (auto& kv : by_row) {
             RlRow<RL_MAX_CELLS> st;
             auto it = e->table.find(kv.first);
@@ -102,7 +103,7 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
                     return;
                 }
                 for (uint32_t k = 0; k < rl_cells_n(A.cells); k++)
-                    if (rl_pos_at(A.posorig, k) == fl) out_first[req] = desc[rl_cells_at(A.cells, k)].limit_id;
+                    if (rl_pos_of<WIDE>(A.posorig, k) == fl) out_first[req] = desc[rl_cells_at(A.cells, k)].limit_id;
             };
             while (pos < n) {
                 uint32_t mA = n, mB = n;
@@ -112,7 +113,7 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
                     bool aok = false, bok = false;
                     if (!multi) {
                         if (mode == 0) {
-                            aok = rl_eval_deny_noeffect<RL_MAX_CELLS>(st, desc, A.cells, A.posorig, delta[A.req], now[A.req], lc != 0);
+                            aok = rl_eval_deny_noeffect<RL_MAX_CELLS, WIDE>(st, desc, A.cells, A.posorig, delta[A.req], now[A.req], lc != 0);
                             bok = uniform && rl_eval_allow_run<RL_MAX_CELLS>(st, desc, A.cells, P[i] - pbase, now[A.req]);
                         } else {
                             bok = uniform && rl_eval_update_run<RL_MAX_CELLS>(st, A.cells, now[A.req]);
@@ -128,10 +129,9 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
                         const RlAccess& A = acc[mem[i]];
                         RlRow<RL_MAX_CELLS> loc = st;
                         uint32_t dd = 0;
-                        uint64_t* rem = (lc && commit && out_rem) ? out_rem + off[A.req] : nullptr;
-                        uint64_t* ttl = (lc && commit && out_ttl) ? out_ttl + off[A.req] : nullptr;
-                        const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS>(loc, dd, desc, A.cells, A.posorig, delta[A.req],
-                                                                               now[A.req], lc != 0, rem, ttl);
+                        const auto [rem, ttl] = lc_out(A.req);
+                        const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS, WIDE>(loc, dd, desc, A.cells, A.posorig, delta[A.req],
+                                                                                     now[A.req], lc != 0, rem, ttl);
                         if (commit) outputs(A, fl);
                     }
                 } else if (mB > pos) {
@@ -142,10 +142,9 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
                         uint32_t dd = 0;
                         rl_advance_run<RL_MAX_CELLS>(loc, A.cells, (P[i] - delta[A.req]) - pbase);
                         if (mode == 0) {
-                            uint64_t* rem = (lc && commit && out_rem) ? out_rem + off[A.req] : nullptr;
-                            uint64_t* ttl = (lc && commit && out_ttl) ? out_ttl + off[A.req] : nullptr;
-                            const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS>(loc, dd, desc, A.cells, A.posorig,
-                                                                                   delta[A.req], now[A.req], lc != 0, rem, ttl);
+                            const auto [rem, ttl] = lc_out(A.req);
+                            const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS, WIDE>(loc, dd, desc, A.cells, A.posorig,
+                                                                                         delta[A.req], now[A.req], lc != 0, rem, ttl);
                             if (commit) outputs(A, fl);
                         } else {
                             rl_walk_update<RL_MAX_CELLS>(loc, dd, desc, A.cells, delta[A.req], now[A.req]);
@@ -160,16 +159,15 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
                     if (mode == 2) {
                         rl_walk_update<RL_MAX_CELLS>(st, dd, desc, A.cells, delta[req], now[req]);
                     } else {
-                        uint64_t* rem = (lc && commit && out_rem) ? out_rem + off[req] : nullptr;
-                        uint64_t* ttl = (lc && commit && out_ttl) ? out_ttl + off[req] : nullptr;
+                        const auto [rem, ttl] = lc_out(req);
                         if (!rl_cells_multi(A.cells)) {
-                            const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS>(st, dd, desc, A.cells, A.posorig, delta[req],
-                                                                                   now[req], lc != 0, rem, ttl);
+                            const uint32_t fl = rl_walk_check_single<RL_MAX_CELLS, WIDE>(st, dd, desc, A.cells, A.posorig, delta[req],
+                                                                                         now[req], lc != 0, rem, ttl);
                             if (commit) outputs(A, fl);
                         } else {
                             const uint32_t fl_in = fl_prev[req];
-                            const uint32_t local = rl_walk_check_multi<RL_MAX_CELLS>(st, dd, desc, A.cells, A.posorig, delta[req],
-                                                                                    now[req], lc != 0, fl_in, rem, ttl);
+                            const uint32_t local = rl_walk_check_multi<RL_MAX_CELLS, WIDE>(st, dd, desc, A.cells, A.posorig, delta[req],
+                                                                                          now[req], lc != 0, fl_in, rem, ttl);
                             if (!commit) {
                                 if (local < fl_next[req]) fl_next[req] = local;
                             } else {
@@ -202,8 +200,53 @@ int emu_batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const emu_c
         }
     }
     pass(true);
+    if (WIDE && lc)
+        for (uint32_t i = 0; i < n; i++)
+            for (uint32_t p = off[i]; p < off[i + 1]; p++) {
+                if (out_rem_user) out_rem_user[off[i] + perm[p]] = scr_rem[p];
+                if (out_ttl_user) out_ttl_user[off[i] + perm[p]] = scr_ttl[p];
+            }
     if (rounds_out) *rounds_out = rounds;
     return 0;
+}
+
+extern "C" {
+
+emu* emu_create(int cells) {
+    emu* e = new emu();
+    e->cells = cells;
+    return e;
+}
+void emu_destroy(emu* e) { delete e; }
+
+void emu_set_tables(emu* e, const RlLimitDev* limits, uint32_t n_limits, const RlCellDesc* desc, uint32_t n_groups) {
+    e->limits.assign(limits, limits + n_limits);
+    e->desc.assign(desc, desc + (size_t)n_groups * 8);
+}
+
+// batch_csr in the narrow (wide = 0) or the wide position encoding.
+int emu_batch_csr(emu* e, int wide, int mode, uint32_t n, const uint32_t* off, const emu_counter* ctrs,
+                  const uint64_t* delta, const uint64_t* now, int lc, uint8_t* out_limited, uint32_t* out_first,
+                  uint64_t* out_rem, uint64_t* out_ttl, int* rounds_out) {
+    return (wide ? batch_csr<true> : batch_csr<false>)(e, mode, n, off, ctrs, delta, now, lc, out_limited, out_first,
+                                                       out_rem, out_ttl, rounds_out);
+}
+
+// rl_resolve_request alone, for request index `req` of m counters: out_acc[0..m) and (wide) out_perm[0..m).  Returns the
+// number of accesses or a negative RL_DEV_* code.
+int emu_resolve(emu* e, int wide, uint32_t req, uint32_t m, const emu_counter* ctrs, uint32_t max_ctrs,
+                RlAccess* out_acc, uint8_t* out_perm) {
+    auto get = [&](uint32_t j) {
+        RlCtrIn r;
+        r.limit_id = ctrs[j].limit_id;
+        r.key_lo = ctrs[j].key_lo;
+        r.key_hi = ctrs[j].key_hi;
+        return r;
+    };
+    if (wide)
+        return rl_resolve_request<true>(req, m, get, e->limits.data(), (uint32_t)e->limits.size(), true, out_acc, out_perm,
+                                        max_ctrs);
+    return rl_resolve_request(req, m, get, e->limits.data(), (uint32_t)e->limits.size(), true, out_acc);
 }
 
 // every present cell -> (limit_id, key_lo, key_hi, value, expiry); unqualified cells always

@@ -1,7 +1,7 @@
-// emu_maint.cpp — TEST-ONLY host driver of the maintenance and CRDT kernels (limitador_b200/csrc/rl_maint.cuh,
-// rl_crdt.cuh) under tests/emu/cuda_shim.h: the SAME kernel source the GPU runs, one CUDA thread after the other in a
-// shuffled order.  Not shipped, not a fallback.  The launch geometry and the call sequences follow rl_maint.cu /
-// rl_crdt.cu; the table helpers restate rl_kernels.cuh's rl_probe so that a rebuilt region is checked by the rule the
+// emu_maint.cpp — TEST-ONLY host driver of the maintenance, counter-import and CRDT kernels
+// (limitador_b200/csrc/rl_maint.cuh, rl_crdt.cuh) under tests/emu/cuda_shim.h: the SAME kernel source the GPU runs, one
+// CUDA thread after the other in a shuffled order.  Not shipped, not a fallback.  The launch geometry and the call
+// sequences follow rl_maint.cu / rl_crdt.cu; the table helpers restate rl_kernels.cuh's rl_probe so that a rebuilt region is checked by the rule the
 // hot path looks rows up with.
 // Built twice: plain (cuda_shim.h: one thread after the other, the kernels' `#ifndef RL_SHIM` fast paths compiled out) and
 // with -DEMU_SIMT (cuda_simt.h: the threads of a block as fibers, warp intrinsics as rendezvous — the DEVICE branches run).
@@ -149,6 +149,34 @@ void emu_table_compact(emu_table* t, uint32_t min_tombstone_pct, unsigned long l
     stats[4] = counts[0];
     stats[5] = chosen ? tomb_chosen + counts[1] : 0;
     stats[6] = counts[2];
+}
+
+// rl_counters_import (rl_maint.cu), same launch geometry and pass sequence.  rows: the table (capacity =
+// 2^(log2P + log2R) rows of 16 * (1 + cells) bytes), changed in place; limits: RlLimitDev[limits_cap].  Returns the
+// error word ((index << 8) | reason, ~0 = imported); unq_out[limits_cap] = the unqualified limits the call makes present.
+unsigned long long emu_import(uint8_t* rows, uint32_t cells, uint32_t log2P, uint32_t log2R, const RlLimitDev* limits,
+                              uint32_t limits_cap, uint64_t n, const uint32_t* limit_id, const uint64_t* key_lo,
+                              const uint64_t* key_hi, const uint64_t* value, const uint64_t* expiry_us,
+                              uint8_t* unq_out) {
+    const RlImportTab T{rows, 16u * (1 + cells), log2P, log2R, limits, limits_cap};
+    const RlImportIn I{limit_id, key_lo, key_hi, value, expiry_us, n};
+    const uint64_t capacity = 1ull << (log2P + log2R);
+    unsigned long long err = ~0ull;
+    std::vector<uint8_t> unq(limits_cap, 0);
+    const uint32_t threads = 256, blocks = (uint32_t)((n + threads - 1) / threads);
+    if (n == 0) return err;
+    shim_launch(blocks, threads, [&] { k_import_resolve(T, I, &err, unq.data()); });
+    if (err != ~0ull) return err;
+    std::vector<unsigned long long> row_of(n, 0);
+    std::vector<unsigned> mask(capacity, 0);
+    shim_launch(blocks, threads, [&] { k_import_claim(T, I, row_of.data(), mask.data(), &err); });
+    if (err != ~0ull) {
+        shim_launch(blocks, threads, [&] { k_import_release(T, n, row_of.data()); });
+        return err;
+    }
+    shim_launch(blocks, threads, [&] { k_import_write(T, I, row_of.data()); });
+    for (uint32_t l = 0; l < limits_cap; l++) unq_out[l] = unq[l];
+    return err;
 }
 
 // ---- the replicated counter value ------------------------------------------------------------------------------------

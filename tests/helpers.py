@@ -3,6 +3,7 @@ engine's row-group logic, the host emulator binding and random stream builders."
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 import subprocess
 
@@ -13,6 +14,7 @@ from limitador_b200.engine import COUNTER_DTYPE, LIMIT_DESC_DTYPE, NONE, RECORD_
 from limitador_b200.limiter import Authorization
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
 T0 = 1_700_000_000_000_000
 
 LIMITDEV_DTYPE = np.dtype([("group", "<u4"), ("cell", "<u4"), ("ns_id", "<u4"), ("qualified", "<u4")])
@@ -52,43 +54,61 @@ def assign_tables(descs: np.ndarray, cells: int):
     return limits, desc, len(groups)
 
 
-_emu = None
+def host_lib(src, name, defines=()):
+    """tests/emu/<src> compiled for the host into tests/emu/<name> (with -D<defines>).  It is rebuilt when it is older than
+    any source in tests/emu/, any .h / .cuh in limitador_b200/csrc/ or any header in include/: everything it can
+    include."""
+    so = os.path.join(HERE, "emu", name)
+    dirs = {os.path.join(HERE, "emu"): (".cpp", ".h"), os.path.join(ROOT, "limitador_b200", "csrc"): (".h", ".cuh"),
+            os.path.join(ROOT, "include"): (".h",)}
+    deps = [os.path.join(d, f) for d, ext in dirs.items() for f in os.listdir(d) if f.endswith(ext)]
+    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(d) for d in deps):
+        tmp = f"{so}.{os.getpid()}.so"  # a process that has the old library loaded keeps its copy
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", *[f"-D{d}" for d in defines], "-o", tmp,
+                               os.path.join(HERE, "emu", src)])
+        os.replace(tmp, so)
+    return C.CDLL(so)
 
 
+@functools.cache
 def emu_lib():
-    global _emu
-    if _emu is None:
-        src = os.path.join(HERE, "emu", "emu.cpp")
-        so = os.path.join(HERE, "emu", "librl_emu.so")
-        core = os.path.join(os.path.dirname(HERE), "limitador_b200", "csrc", "rl_core.h")
-        if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(core)):
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", so, src])
-        L = C.CDLL(so)
-        vp = C.c_void_p
-        L.emu_create.restype = vp
-        L.emu_create.argtypes = [C.c_int]
-        L.emu_destroy.argtypes = [vp]
-        L.emu_set_tables.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
-        L.emu_batch_csr.argtypes = [vp, C.c_int, C.c_uint32, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
-        L.emu_dump.restype = C.c_uint64
-        L.emu_dump.argtypes = [vp, C.c_uint64, vp, vp, vp, vp, vp]
-        _emu = L
-    return _emu
+    L = host_lib("emu.cpp", "librl_emu.so")
+    vp = C.c_void_p
+    L.emu_create.restype = vp
+    L.emu_create.argtypes = [C.c_int]
+    L.emu_destroy.argtypes = [vp]
+    L.emu_set_tables.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
+    L.emu_batch_csr.argtypes = [vp, C.c_int, C.c_int, C.c_uint32, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    L.emu_resolve.argtypes = [vp, C.c_int, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, vp]
+    L.emu_resolve.restype = C.c_int
+    L.emu_dump.restype = C.c_uint64
+    L.emu_dump.argtypes = [vp, C.c_uint64, vp, vp, vp, vp, vp]
+    return L
 
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-class Emu:
-    """Sequential host run of the kernels' algorithm (tests/emu/emu.cpp)."""
+ACCESS_DTYPE = np.dtype([("key_lo", "<u8"), ("hdr_hi", "<u8"), ("req", "<u4"), ("cells", "<u4"), ("posorig", "<u8")])
+assert ACCESS_DTYPE.itemsize == 32
 
-    def __init__(self, descs: np.ndarray, cells: int):
+
+class Emu:
+    """Sequential host run of the kernels' algorithm (tests/emu/emu.cpp), in the narrow position encoding or, with
+    wide=True, the wide one (requests of up to 64 counters)."""
+
+    def __init__(self, descs: np.ndarray, cells: int, wide: bool = False):
         self.L = emu_lib()
+        self.wide = wide
         self.h = self.L.emu_create(cells)
         limits, desc, ngroups = assign_tables(descs, cells)
         self.L.emu_set_tables(self.h, _p(limits), len(limits), _p(desc), ngroups)
         self.rounds = 0
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.L.emu_destroy(self.h)
 
     def batch_csr(self, mode, off, ctrs, delta, now_us, load_counters=False):
         off = np.ascontiguousarray(off, dtype=np.uint32)
@@ -101,11 +121,22 @@ class Emu:
         rem = np.zeros(len(ctrs), dtype=np.uint64)
         ttl = np.zeros(len(ctrs), dtype=np.uint64)
         rounds = C.c_int(0)
-        r = self.L.emu_batch_csr(self.h, mode, n, _p(off), _p(ctrs), _p(delta), _p(now_us), int(load_counters),
-                                 _p(lim), _p(fl), _p(rem), _p(ttl), C.byref(rounds))
+        r = self.L.emu_batch_csr(self.h, int(self.wide), mode, n, _p(off), _p(ctrs), _p(delta), _p(now_us),
+                                 int(load_counters), _p(lim), _p(fl), _p(rem), _p(ttl), C.byref(rounds))
         assert r == 0, f"emu error {r}"
         self.rounds = rounds.value
         return lim, fl, rem, ttl
+
+    def resolve(self, ctrs, req=0, max_ctrs=64, wide=None):
+        """rl_resolve_request alone on one request (in the emulator's encoding unless `wide` says otherwise): the number
+        of accesses or a negative RL_DEV_* code, the accesses and (wide) the permutation."""
+        wide = self.wide if wide is None else wide
+        ctrs = np.ascontiguousarray(ctrs, dtype=COUNTER_DTYPE)
+        m = len(ctrs)
+        acc = np.zeros(max(m, 1), dtype=ACCESS_DTYPE)
+        perm = np.full(max(m, 1), 0xFF, dtype=np.uint8)
+        r = self.L.emu_resolve(self.h, int(wide), req, m, _p(ctrs), max_ctrs, _p(acc), _p(perm))
+        return r, acc, perm
 
     def dump(self):
         cap = 1 << 20
@@ -116,6 +147,27 @@ class Emu:
         exp = np.zeros(cap, dtype=np.uint64)
         c = self.L.emu_dump(self.h, cap, _p(lid), _p(lo), _p(hi), _p(val), _p(exp))
         return sorted(zip(lid[:c].tolist(), lo[:c].tolist(), hi[:c].tolist(), val[:c].tolist(), exp[:c].tolist()))
+
+
+def emu_vs_oracle(descs, cells, batches, load_counters, mode=0, wide=False):
+    """Run `batches` (CSR tuples) through the emulator and the oracle and compare them bit for bit: verdicts,
+    first-limited ids and (load_counters) remaining / ttl for check_and_update (mode 0), the table after every batch.
+    Returns the emulator's fixed-point rounds per batch."""
+    emu = Emu(descs, cells, wide)
+    orc = oracle_with_limits(descs)
+    rounds = []
+    for off, ctrs, delta, now in batches:
+        e = emu.batch_csr(mode, off, ctrs, delta, now, load_counters)
+        o = orc.batch_csr(mode, off, ctrs, delta, now, load_counters)
+        rounds.append(emu.rounds)
+        if mode == 0:
+            assert e[0].tolist() == o[0].tolist(), "verdicts differ"
+            assert e[1].tolist() == o[1].tolist(), "first-limited limit differs"
+            if load_counters:
+                assert e[2].tolist() == o[2].tolist(), "remaining differs"
+                assert e[3].tolist() == o[3].tolist(), "ttl differs"
+        assert normalise_dump(emu.dump(), descs) == normalise_dump(orc.dump(), descs), "table differs"
+    return rounds
 
 
 def normalise_dump(dump, descs):
@@ -249,6 +301,56 @@ def random_csr_stream(descs, n, seed, n_keys=5, monotone=True, subset=True):
             delta, now)
 
 
+def wide_limits(seed, sizes=(20, 33, 64, 3), small=True):
+    """Namespaces of `sizes` limits, qualified (three variable sets) and unqualified interleaved in registration order,
+    with small maxima so that the limits bite."""
+    rng = np.random.default_rng(seed)
+    descs, lid = [], 0
+    for ns, size in enumerate(sizes):
+        for _ in range(size):
+            q = 1 if rng.random() < 0.7 else 0
+            varset = int(rng.integers(1, 4)) if q else 0
+            mx = int(rng.choice([0, 1, 2, 3, 5, 8, 20, 1 << 40])) if small else (1 << 62)
+            win = int(rng.choice([1, 2, 10, 60, 3600])) * 1_000_000
+            descs.append((lid, ns, varset, q, mx, win))
+            lid += 1
+    return np.array(descs, dtype=LIMIT_DESC_DTYPE)
+
+
+def wide_stream(descs, n, seed, n_keys=3, monotone=True, min_ctrs=17):
+    """Requests naming at least min_ctrs of their namespace's limits where it has that many (all of a smaller one),
+    in shuffled order half of the time; per-variable-set keys from a tiny key space."""
+    rng = np.random.default_rng(seed)
+    by_ns = {}
+    for d in descs:
+        by_ns.setdefault(int(d["ns_id"]), []).append(d)
+    nss = sorted(by_ns)
+    off, ctrs = [0], []
+    delta = np.zeros(n, dtype=np.uint64)
+    now = np.zeros(n, dtype=np.uint64)
+    t = T0
+    for i in range(n):
+        lims = by_ns[int(rng.choice(nss))]
+        lo_k = min(min_ctrs, len(lims))
+        k = int(rng.integers(lo_k, len(lims) + 1))
+        pick = sorted(rng.choice(len(lims), size=k, replace=False).tolist())
+        if rng.random() < 0.5:
+            rng.shuffle(pick)
+        vkeys = {}
+        for j in pick:
+            d = lims[j]
+            vs = int(d["varset_id"]) if d["qualified"] else 0
+            if vs not in vkeys:
+                vkeys[vs] = (int(rng.integers(1, n_keys + 1)), int(rng.integers(0, 2)))
+            lo, hi = vkeys[vs] if d["qualified"] else (0, 0)
+            ctrs.append((int(d["limit_id"]), 0, lo, hi))
+        off.append(len(ctrs))
+        delta[i] = int(rng.choice([1, 1, 1, 2, 3, 7]))
+        t += int(rng.choice([0, 0, 1, 1000, 400_000, 1_500_000]))
+        now[i] = t if monotone else max(1, t - int(rng.choice([0, 0, 2_000_000])))
+    return np.array(off, dtype=np.uint32), np.array(ctrs, dtype=COUNTER_DTYPE), delta, now
+
+
 def random_records(descs, n, seed, n_keys=5, monotone=True):
     rng = np.random.default_rng(seed)
     nss = sorted({int(d["ns_id"]) for d in descs}) + [int(descs["ns_id"].max()) + 3]  # + a namespace without limits
@@ -265,54 +367,45 @@ def random_records(descs, n, seed, n_keys=5, monotone=True):
     return r
 
 
-_emu_maint = {}
-
-
+@functools.cache
 def emu_maint_lib(simt: bool = False):
-    """tests/emu/emu_maint.cpp: the maintenance / CRDT kernels (rl_maint.cuh, rl_crdt.cuh) compiled for the host — under
-    tests/emu/cuda_shim.h (one CUDA thread after the other; the kernels' warp-aggregated branches compiled out), or with
-    simt=True under tests/emu/cuda_simt.h (fibers + warp rendezvous: the device branches themselves run)."""
-    if simt not in _emu_maint:
-        src = os.path.join(HERE, "emu", "emu_maint.cpp")
-        so = os.path.join(HERE, "emu", "librl_emu_simt.so" if simt else "librl_emu_maint.so")
-        csrc = os.path.join(os.path.dirname(HERE), "limitador_b200", "csrc")
-        deps = [src, os.path.join(HERE, "emu", "cuda_simt.h" if simt else "cuda_shim.h")] + [
-            os.path.join(csrc, f) for f in ("rl_core.h", "rl_devmem.cuh", "rl_maint.cuh", "rl_crdt.cuh")]
-        deps.append(os.path.join(os.path.dirname(HERE), "include", "rl_crdt.h"))
-        if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(d) for d in deps):
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", *(["-DEMU_SIMT"] if simt else []), "-o", so, src])
-        L = C.CDLL(so)
-        vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
-        L.emu_seed.argtypes = [u64]
-        L.emu_ns_metrics.argtypes = [vp, u32, u32, vp, vp, u32, u32, vp]
-        L.emu_ns_metrics.restype = None
-        L.emu_table_create.restype = vp
-        L.emu_table_create.argtypes = [u32, u32, u32]
-        L.emu_table_destroy.argtypes = [vp]
-        L.emu_table_raw.restype = vp
-        L.emu_table_raw.argtypes = [vp]
-        L.emu_table_bytes.restype = u64
-        L.emu_table_bytes.argtypes = [vp]
-        for f in (L.emu_table_put, L.emu_table_get):
-            f.restype = C.c_int64
-            f.argtypes = [vp, u64, u64, vp]
-        L.emu_table_tombstone.restype = C.c_int64
-        L.emu_table_tombstone.argtypes = [vp, u64, u64]
-        L.emu_table_compact.argtypes = [vp, u32, vp, vp]
-        L.emu_table_compact.restype = None
-        L.emu_crdt_create.restype = vp
-        L.emu_crdt_create.argtypes = [u64, u32, u32]
-        L.emu_crdt_destroy.argtypes = [vp]
-        L.emu_crdt_inc.argtypes = [vp, u32, vp, vp, vp, vp, u64]
-        L.emu_crdt_inc.restype = u32
-        L.emu_crdt_merge.argtypes = [vp, u32, vp, vp, vp, u64, u64]
-        L.emu_crdt_merge.restype = u32
-        L.emu_crdt_read.argtypes = [vp, u32, vp, u64, vp, vp]
-        L.emu_crdt_read.restype = u32
-        L.emu_crdt_scan.argtypes = [vp, C.c_int, u64, u64, vp, vp, vp, vp]
-        L.emu_crdt_scan.restype = u64
-        _emu_maint[simt] = L
-    return _emu_maint[simt]
+    """tests/emu/emu_maint.cpp: the maintenance, counter-import and CRDT kernels (rl_maint.cuh, rl_crdt.cuh) compiled for
+    the host — under tests/emu/cuda_shim.h (one CUDA thread after the other; the kernels' warp-aggregated branches
+    compiled out), or with simt=True under tests/emu/cuda_simt.h (fibers + warp rendezvous: the device branches
+    themselves run)."""
+    L = host_lib("emu_maint.cpp", "librl_emu_simt.so" if simt else "librl_emu_maint.so", ["EMU_SIMT"] if simt else [])
+    vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
+    L.emu_seed.argtypes = [u64]
+    L.emu_ns_metrics.argtypes = [vp, u32, u32, vp, vp, u32, u32, vp]
+    L.emu_ns_metrics.restype = None
+    L.emu_table_create.restype = vp
+    L.emu_table_create.argtypes = [u32, u32, u32]
+    L.emu_table_destroy.argtypes = [vp]
+    L.emu_table_raw.restype = vp
+    L.emu_table_raw.argtypes = [vp]
+    L.emu_table_bytes.restype = u64
+    L.emu_table_bytes.argtypes = [vp]
+    for f in (L.emu_table_put, L.emu_table_get):
+        f.restype = C.c_int64
+        f.argtypes = [vp, u64, u64, vp]
+    L.emu_table_tombstone.restype = C.c_int64
+    L.emu_table_tombstone.argtypes = [vp, u64, u64]
+    L.emu_table_compact.argtypes = [vp, u32, vp, vp]
+    L.emu_table_compact.restype = None
+    L.emu_crdt_create.restype = vp
+    L.emu_crdt_create.argtypes = [u64, u32, u32]
+    L.emu_crdt_destroy.argtypes = [vp]
+    L.emu_crdt_inc.argtypes = [vp, u32, vp, vp, vp, vp, u64]
+    L.emu_crdt_inc.restype = u32
+    L.emu_crdt_merge.argtypes = [vp, u32, vp, vp, vp, u64, u64]
+    L.emu_crdt_merge.restype = u32
+    L.emu_crdt_read.argtypes = [vp, u32, vp, u64, vp, vp]
+    L.emu_crdt_read.restype = u32
+    L.emu_crdt_scan.argtypes = [vp, C.c_int, u64, u64, vp, vp, vp, vp]
+    L.emu_crdt_scan.restype = u64
+    L.emu_import.restype = u64
+    L.emu_import.argtypes = [vp, u32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp, vp]
+    return L
 
 
 class EmuCrdt:

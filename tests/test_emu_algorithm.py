@@ -7,30 +7,13 @@ import pytest
 from tests import helpers as H
 
 
-def run_both(descs, cells, batches, load_counters):
-    emu = H.Emu(descs, cells)
-    orc = H.oracle_with_limits(descs)
-    rounds = []
-    for off, ctrs, delta, now in batches:
-        e = emu.batch_csr(0, off, ctrs, delta, now, load_counters)
-        o = orc.batch_csr(0, off, ctrs, delta, now, load_counters)
-        rounds.append(emu.rounds)
-        assert e[0].tolist() == o[0].tolist(), "verdicts differ"
-        assert e[1].tolist() == o[1].tolist(), "first-limited limit differs"
-        if load_counters:
-            assert e[2].tolist() == o[2].tolist(), "remaining differs"
-            assert e[3].tolist() == o[3].tolist(), "ttl differs"
-        assert H.normalise_dump(emu.dump(), descs) == H.normalise_dump(orc.dump(), descs), "table differs"
-    return rounds
-
-
 @pytest.mark.parametrize("cells", [1, 3, 7])
 @pytest.mark.parametrize("load_counters", [False, True])
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_random_streams_match_oracle(cells, load_counters, seed):
     descs = H.mixed_limits(n_ns=12, seed=seed)
     batches = [H.random_csr_stream(descs, 300, seed * 100 + b, n_keys=3, monotone=(b % 2 == 0)) for b in range(6)]
-    rounds = run_both(descs, cells, batches, load_counters)
+    rounds = H.emu_vs_oracle(descs, cells, batches, load_counters)
     assert max(rounds) >= 1  # the mixed table always has multi-row requests
 
 
@@ -57,7 +40,7 @@ def test_long_dependency_chain_converges():
         ctrs[2 * i + 1] = (1, 0, 1 + (i + 1) // 2, 0)  # row B_k shared by requests 2k-1, 2k
     delta = np.ones(n, dtype=np.uint64)
     now = np.full(n, H.T0, dtype=np.uint64)
-    rounds = run_both(descs, 1, [(off, ctrs, delta, now)], False)
+    rounds = H.emu_vs_oracle(descs, 1, [(off, ctrs, delta, now)], False)
     assert rounds[0] > 2
 
 
@@ -68,4 +51,4 @@ def test_wide_key_space_streams_match_oracle(cells, load_counters, seed):
     rehash bug with."""
     descs = H.mixed_limits(n_ns=12, seed=seed)
     batches = [H.random_csr_stream(descs, 2500, seed * 100 + b, n_keys=120, monotone=bool(b & 1)) for b in range(4)]
-    run_both(descs, cells, batches, load_counters)
+    H.emu_vs_oracle(descs, cells, batches, load_counters)

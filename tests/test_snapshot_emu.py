@@ -8,44 +8,17 @@ shuffled order — and their warp-aggregated probe under tests/emu/cuda_simt.h:
 oracle_restore applies the same import to the CPU oracle through the oracle's own public calls (the GPU tests continue
 a stream on it after an import); it is pinned here by a small known-answer test.
 The GPU runs of rl_counters_export / rl_counters_import are in tests/test_zz4_snapshot_gpu.py."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
-
 import numpy as np
 import pytest
 
 from limitador_b200.engine import LIMIT_DESC_DTYPE
 from oracle import binding as ob
+from tests import helpers as H
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 TOMB = 0xFFFFFFFFFFFFFFFF
 M64 = (1 << 64) - 1
 LIMIT_DEV = np.dtype([("group", "<u4"), ("cell", "<u4"), ("ns_id", "<u4"), ("qualified", "<u4")])
 UNKNOWN_LIMIT, KEY_RANGE, NO_EXPIRY, DUPLICATE, TABLE_FULL = 1, 2, 3, 4, 5
-
-_libs = {}
-_dir = tempfile.mkdtemp(prefix="rl_emu_snapshot_")
-
-
-def lib(simt):
-    if simt not in _libs:
-        so = os.path.join(_dir, "simt.so" if simt else "plain.so")
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", *(["-DEMU_SIMT"] if simt else []),
-                               "-o", so, os.path.join(HERE, "emu", "emu_snapshot.cpp")])
-        L = C.CDLL(so)
-        vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
-        L.emu_seed.argtypes = [u64]
-        L.emu_import.restype = u64
-        L.emu_import.argtypes = [vp, u32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp, vp]
-        _libs[simt] = L
-    return _libs[simt]
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
 
 def mix64(x):
     x ^= x >> 33
@@ -107,8 +80,9 @@ class Table:
     def import_(self, simt, limits, lid, klo, khi, val, exp):
         cols = [np.ascontiguousarray(lid, dtype=np.uint32)] + [np.ascontiguousarray(c, dtype=np.uint64) for c in (klo, khi, val, exp)]
         unq = np.zeros(len(limits), dtype=np.uint8)
-        err = lib(simt).emu_import(_p(self.w), self.cells, self.log2P, self.log2R, _p(limits), len(limits), len(cols[0]),
-                                   *[_p(c) for c in cols], _p(unq))
+        L = H.emu_maint_lib(simt)
+        err = L.emu_import(H._p(self.w), self.cells, self.log2P, self.log2R, H._p(limits), len(limits), len(cols[0]),
+                           *[H._p(c) for c in cols], H._p(unq))
         return (None if err == M64 else (err >> 8, err & 0xFF)), unq
 
 
@@ -159,7 +133,7 @@ def cols(a):
 @pytest.mark.parametrize("cells,log2P,log2R,prefill,seed", [(1, 2, 7, False, 1), (3, 3, 6, True, 2), (7, 0, 9, True, 3),
                                                             (4, 4, 5, True, 4)])
 def test_imported_counters_sit_where_the_hot_path_probes(cells, log2P, log2R, prefill, simt, seed):
-    lib(simt).emu_seed(seed)
+    H.emu_maint_lib(simt).emu_seed(seed)
     rng = np.random.default_rng(seed)
     limits = make_limits(cells, 4, rng)
     t = Table(cells, log2P, log2R)

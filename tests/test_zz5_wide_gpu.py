@@ -12,7 +12,6 @@ from limitador_b200 import matcher as MT
 from limitador_b200 import rls as R
 from tests import helpers as H
 from tests.test_rls import T0, CpuHarness, _req
-from tests.test_wide_emu import wide_limits, wide_stream
 
 pytestmark = pytest.mark.gpu
 SCENARIOS = [(10, 50, 10, 0), (1, 1, 1, 1), (10, 10, 10, 10), (10, 50, 10, 10)]  # limitador/benches/bench.rs:65-90
@@ -110,27 +109,27 @@ def test_reference_scenarios_three_calls_match_oracle(scn, small):
 @pytest.mark.parametrize("device", [False, True], ids=["host", "device"])
 @pytest.mark.parametrize("cells", [1, 3, 7])
 def test_random_wide_csr_streams_match_oracle(device, cells):
-    descs = wide_limits(cells)
+    descs = H.wide_limits(cells)
     e = _wide_engine(descs, cells)
     o = H.oracle_with_limits(descs)
     for b in range(4):
         lc = b % 2 == 1
-        off, ctrs, delta, now = wide_stream(descs, 500, 50 + b, n_keys=4, monotone=(b != 2), min_ctrs=1 if b == 3 else 17)
+        off, ctrs, delta, now = H.wide_stream(descs, 500, 50 + b, n_keys=4, monotone=(b != 2), min_ctrs=1 if b == 3 else 17)
         want = o.batch_csr(0, off, ctrs, delta, now, lc)
         got = _csr_device(e, off, ctrs, delta, now, lc) if device else e.check_and_update_batch(off, ctrs, delta, now, lc)
         _same(got, want, 4 if lc else 2)
         _tables(e, o, descs)
-    off, ctrs, delta, now = wide_stream(descs, 300, 99)
+    off, ctrs, delta, now = H.wide_stream(descs, 300, 99)
     e.update_batch(off, ctrs, delta, now)
     o.batch_csr(2, off, ctrs, delta, now)
     _tables(e, o, descs)
 
 
 def test_mixed_narrow_and_wide_batch_matches_oracle():
-    descs = wide_limits(5)
+    descs = H.wide_limits(5)
     e = _wide_engine(descs, 3)
     o = H.oracle_with_limits(descs)
-    off, ctrs, delta, now = wide_stream(descs, 2000, 77, min_ctrs=1)
+    off, ctrs, delta, now = H.wide_stream(descs, 2000, 77, min_ctrs=1)
     sizes = np.diff(off)
     assert sizes.max() > 16 and sizes.min() <= 16
     _same(e.check_and_update_batch(off, ctrs, delta, now, True), o.batch_csr(0, off, ctrs, delta, now, True), 4)
@@ -139,7 +138,7 @@ def test_mixed_narrow_and_wide_batch_matches_oracle():
 
 @pytest.mark.parametrize("cells", [3, 7])
 def test_records_of_wide_namespaces_with_load_counters(cells):
-    descs = wide_limits(cells + 20, sizes=(20, 64, 33, 2, 5))
+    descs = H.wide_limits(cells + 20, sizes=(20, 64, 33, 2, 5))
     e = _wide_engine(descs, cells)
     o = H.oracle_with_limits(descs)
     for b in range(4):
@@ -200,11 +199,11 @@ def test_engine_creation_refuses_a_maximum_out_of_range(bad):
 
 
 def test_is_within_limits_takes_any_number_of_counters_on_a_default_engine():
-    descs = wide_limits(3, sizes=(50,))
+    descs = H.wide_limits(3, sizes=(50,))
     e = Engine(capacity_rows=1 << 12, cells_per_row=7, max_batch=4096, max_counters=4096 * 50)
     e.limits_set(descs)
     o = H.oracle_with_limits(descs)
-    off, ctrs, delta, now = wide_stream(descs, 400, 5, min_ctrs=50)
+    off, ctrs, delta, now = H.wide_stream(descs, 400, 5, min_ctrs=50)
     assert int(np.diff(off).min()) == 50
     _same(e.is_within_limits_batch(off, ctrs, delta, now), o.batch_csr(1, off, ctrs, delta, now), 2)
 
@@ -249,11 +248,11 @@ def test_rls_should_rate_limit_over_a_50_limit_namespace_equals_the_cpu_mirror()
 
 
 def test_front_check_and_update_with_50_counters():
-    descs = wide_limits(9, sizes=(50,))
+    descs = H.wide_limits(9, sizes=(50,))
     e = _wide_engine(descs, 7)
     o = H.oracle_with_limits(descs)
     f = E.Front(e, max_batch=64, max_delay_us=0)
-    off, ctrs, delta, now = wide_stream(descs, 60, 8, min_ctrs=50)
+    off, ctrs, delta, now = H.wide_stream(descs, 60, 8, min_ctrs=50)
     for i in range(len(delta)):
         c = ctrs[off[i]:off[i + 1]]
         lim, first, _, rem, ttl = f.check_and_update(c, int(delta[i]), int(now[i]), load_counters=True)
