@@ -23,6 +23,7 @@ struct emu {
     std::vector<RlLimitDev> limits;
     std::vector<RlCellDesc> desc;  // [groups][8]
     std::map<std::pair<uint64_t, uint64_t>, RlRow<RL_MAX_CELLS>> table;
+    uint64_t steps = 0;  // replay steps (one run or one request alone each) of the last batch's committing pass
 };
 
 // mode 0: check_and_update, 2: update.  Returns 0 or a positive RL_DEV_* code.
@@ -66,6 +67,7 @@ static int batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const em
         if (acc[a].hdr_hi != 0) by_row[{acc[a].key_lo, acc[a].hdr_hi}].push_back(a);
 
     std::vector<uint32_t> fl_prev(n, RL_NONE_U32), fl_next(n, RL_NONE_U32);
+    e->steps = 0;
     auto pass = [&](bool commit) {
         // where the walkers write request req's remaining / ttl: only in the committing pass
         auto lc_out = [&](uint32_t req) {
@@ -178,6 +180,7 @@ static int batch_csr(emu* e, int mode, uint32_t n, const uint32_t* off, const em
                 }
                 pbase = P[newpos - 1];
                 pos = newpos;
+                if (commit) e->steps++;
             }
             if (commit) e->table[kv.first] = st;  // physical row exists once probed (cells may be absent)
         }
@@ -231,6 +234,8 @@ int emu_batch_csr(emu* e, int wide, int mode, uint32_t n, const uint32_t* off, c
     return (wide ? batch_csr<true> : batch_csr<false>)(e, mode, n, off, ctrs, delta, now, lc, out_limited, out_first,
                                                        out_rem, out_ttl, rounds_out);
 }
+
+uint64_t emu_steps(emu* e) { return e->steps; }
 
 // rl_resolve_request alone, for request index `req` of m counters: out_acc[0..m) and (wide) out_perm[0..m).  Returns the
 // number of accesses or a negative RL_DEV_* code.

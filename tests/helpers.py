@@ -1,5 +1,7 @@
 """Shared test helpers: oracle-backed CounterStorage, table assignment mirroring the
-engine's row-group logic, the host emulator binding and random stream builders."""
+engine's row-group logic, the host emulator binding, random stream builders, the edge-domain
+streams and known answers of the counter arithmetic, and oracle_restore (an import applied to the
+CPU oracle)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -83,6 +85,8 @@ def emu_lib():
     L.emu_resolve.restype = C.c_int
     L.emu_dump.restype = C.c_uint64
     L.emu_dump.argtypes = [vp, C.c_uint64, vp, vp, vp, vp, vp]
+    L.emu_steps.restype = C.c_uint64
+    L.emu_steps.argtypes = [vp]
     return L
 
 
@@ -102,9 +106,14 @@ class Emu:
         self.L = emu_lib()
         self.wide = wide
         self.h = self.L.emu_create(cells)
-        limits, desc, ngroups = assign_tables(descs, cells)
+        self.cells = cells
+        self.set_limits(descs)
+        self.rounds = self.steps = 0
+
+    def set_limits(self, descs):
+        """The limits again, e.g. with another max_value (rl_limits_set on live ids); the counters stay."""
+        limits, desc, ngroups = assign_tables(descs, self.cells)
         self.L.emu_set_tables(self.h, _p(limits), len(limits), _p(desc), ngroups)
-        self.rounds = 0
 
     def __del__(self):
         if getattr(self, "h", None):
@@ -125,6 +134,7 @@ class Emu:
                                  int(load_counters), _p(lim), _p(fl), _p(rem), _p(ttl), C.byref(rounds))
         assert r == 0, f"emu error {r}"
         self.rounds = rounds.value
+        self.steps = int(self.L.emu_steps(self.h))  # replay steps: a closed-form run counts one
         return lim, fl, rem, ttl
 
     def resolve(self, ctrs, req=0, max_ctrs=64, wide=None):
@@ -235,10 +245,17 @@ class OracleStorage:
 
 
 # ---------------------------------------------------------------------------------------
-def mixed_limits(n_ns=6, seed=0):
+def _plain_limit(rng):
+    """max 0 / tiny / huge, 1 s .. 1 h windows"""
+    mx = int(rng.choice([0, 1, 2, 3, 5, 8, 20, 1 << 40]))
+    win = int(rng.choice([1, 2, 10, 60, 3600])) * 1_000_000
+    return mx, win
+
+
+def mixed_limits(n_ns=6, seed=0, draw=_plain_limit):
     """A limits table exercising every row shape: single qualified limit, several limits on
     one variable set (one row), two variable sets (two rows), unqualified + qualified,
-    unqualified only, max 0 / tiny / huge limits, 1 s .. 1 h windows."""
+    unqualified only; (max_value, window_us) from `draw`."""
     rng = np.random.default_rng(seed)
     descs = []
     lid = 0
@@ -254,8 +271,7 @@ def mixed_limits(n_ns=6, seed=0):
             "q3u2": [(1, 1), (0, 0), (1, 1), (2, 1), (0, 0)],
         }[shape]
         for varset, q in plan:
-            mx = int(rng.choice([0, 1, 2, 3, 5, 8, 20, 1 << 40]))
-            win = int(rng.choice([1, 2, 10, 60, 3600])) * 1_000_000
+            mx, win = draw(rng)
             descs.append((lid, ns, varset, q, mx, win))
             lid += 1
     return np.array(descs, dtype=LIMIT_DESC_DTYPE)
@@ -301,17 +317,16 @@ def random_csr_stream(descs, n, seed, n_keys=5, monotone=True, subset=True):
             delta, now)
 
 
-def wide_limits(seed, sizes=(20, 33, 64, 3), small=True):
+def wide_limits(seed, sizes=(20, 33, 64, 3), small=True, draw=_plain_limit):
     """Namespaces of `sizes` limits, qualified (three variable sets) and unqualified interleaved in registration order,
-    with small maxima so that the limits bite."""
+    with small maxima so that the limits bite (or all 2^62 with small=False); windows and maxima from `draw`."""
     rng = np.random.default_rng(seed)
     descs, lid = [], 0
     for ns, size in enumerate(sizes):
         for _ in range(size):
             q = 1 if rng.random() < 0.7 else 0
             varset = int(rng.integers(1, 4)) if q else 0
-            mx = int(rng.choice([0, 1, 2, 3, 5, 8, 20, 1 << 40])) if small else (1 << 62)
-            win = int(rng.choice([1, 2, 10, 60, 3600])) * 1_000_000
+            mx, win = draw(rng) if small else (1 << 62, int(rng.choice([1, 2, 10, 60, 3600])) * 1_000_000)
             descs.append((lid, ns, varset, q, mx, win))
             lid += 1
     return np.array(descs, dtype=LIMIT_DESC_DTYPE)
@@ -460,3 +475,409 @@ class EmuCrdt:
         n = self.L.emu_crdt_scan(self.h, 1, 0, cap, _p(k), None, _p(exp), _p(vals))
         v = vals[:n * self.actors].reshape(n, self.actors)
         return sorted((int(k["lo"][i]), int(k["hi"][i]), int(exp[i]), tuple(v[i].tolist())) for i in range(n))
+
+
+def oracle_restore(o, descs, limit_id, key_lo, key_hi, value, expiry_us):
+    """What rl_counters_import does, applied to the CPU oracle through its own public calls: set each counter to exactly
+    (value, expiry_us); a present counter is replaced, an unqualified one (key ignored) becomes present, other counters
+    are untouched.  descs: the limits the oracle was given (limit_id, ns_id, max_value, window_us, qualified).
+
+    The counters of every limit named are read back (dump), deleted (delete_counters) and created again with the
+    imported ones merged in: update_counter(delta = value, now = expiry - window) creates exactly (value, expiry)
+    (in_memory.rs:47-69), and limit_set again on an unqualified limit without a counter recreates the (0, EPOCH) default
+    (add_counter, in_memory.rs:38-44).  A limit id the oracle does not know raises before anything changes."""
+    by_id = {int(d["limit_id"]): d for d in descs}
+    new = {}
+    for l, lo, hi, v, x in zip(*[np.asarray(c).tolist() for c in (limit_id, key_lo, key_hi, value, expiry_us)]):
+        if l not in by_id:
+            raise ValueError(f"limit {l} is not registered")
+        new[(l, lo, hi) if by_id[l]["qualified"] else (l, 0, 0)] = (v, x)
+    touched = sorted({k[0] for k in new})
+    state = {(l, lo, hi): (v, x) for l, lo, hi, v, x in o.dump() if l in touched}
+    state.update(new)
+    for (l, lo, hi), (v, x) in state.items():
+        w = int(by_id[l]["window_us"])
+        if x < w and (by_id[l]["qualified"] or (v, x) != (0, 0)):
+            raise ValueError(f"counter {(l, lo, hi)}: expiry {x} is earlier than one window after the epoch")
+    o.delete_counters(touched)
+    for (l, lo, hi), (v, x) in sorted(state.items()):
+        d = by_id[l]
+        if not d["qualified"] and (v, x) == (0, 0):
+            o.limit_set(l, int(d["ns_id"]), int(d["max_value"]), int(d["window_us"]), False)
+        else:
+            o.update_counters(ob.counters([(l, lo, hi)]), v, x - int(d["window_us"]))
+
+
+# ---------------------------------------------------------------------------------------
+# The edges of the counter arithmetic: u64 wrap of value + delta, maxima up to 2^64-1, counters above their maximum,
+# clocks exactly on a counter's expiry.  The closed-form replay (DESIGN.md §3.3) is exact only if it wraps and bounds
+# exactly like n sequential adds; the streams below reach those values on purpose, and CountingSpec proves they did.
+M64 = (1 << 64) - 1
+EDGE_MAXIMA = [0, 1, (1 << 32) - 1, 1 << 32, (1 << 63) - 1, 1 << 63, (1 << 64) - 2, M64]
+EDGE_WINDOWS = [1, 2, 1_000_000, 60_000_000, 1 << 40]
+SMALL_DELTAS = [0, 1, 1, 2, 3, 7]
+CSR_BIG_DELTAS = [1 << 31, (1 << 32) - 1, 1 << 32, (1 << 32) + 1, 1 << 62, 3 << 62, 1 << 63, M64]
+RECORD_BIG_DELTAS = [1 << 31, (1 << 31) + 1, 3 << 30, (1 << 32) - 1]  # hits_addend is a u32
+
+
+def _pick(rng, pool):
+    return pool[int(rng.integers(len(pool)))]
+
+
+def _edge_limit(rng):
+    """Maxima at the u32 / i64 / u64 boundaries or small enough to bite; windows of 1 µs .. 2^40 µs."""
+    mx = _pick(rng, EDGE_MAXIMA) if rng.random() < 0.6 else _pick(rng, [1, 2, 3, 5, 8, 20])
+    return mx, _pick(rng, EDGE_WINDOWS)
+
+
+def edge_limits(seed, shape="mixed", n_ns=6, cells=7, sizes=(20, 33, 64, 3)):
+    """Limits with edge maxima and windows in the row shapes of mixed_limits ("mixed"), of one row per namespace
+    ("single": 1..cells limits on one variable set, every fourth namespace unqualified, maxima >= 2^63-1 in the
+    second of every four) or of wide_limits ("wide")."""
+    if shape == "mixed":
+        return mixed_limits(n_ns, seed, draw=_edge_limit)
+    if shape == "wide":
+        return wide_limits(seed, sizes, draw=_edge_limit)
+    rng = np.random.default_rng(seed)
+    descs, lid = [], 0
+    for ns in range(n_ns):
+        q = 0 if ns % 4 == 3 else 1
+        for _ in range(int(rng.integers(1, cells + 1))):
+            mx, win = _edge_limit(rng)
+            if ns % 4 == 1:  # only the top of the u64 range bites: long runs stay allowed
+                mx = _pick(rng, EDGE_MAXIMA[4:])
+            descs.append((lid, ns, q, q, mx, win))
+            lid += 1
+    return np.array(descs, dtype=LIMIT_DESC_DTYPE)
+
+
+def spec_with_limits(descs, cls=None):
+    from tests.spec_model import SpecStore
+    s = (cls or SpecStore)()
+    for d in descs:
+        s.limit_set(int(d["limit_id"]), int(d["ns_id"]), int(d["max_value"]), int(d["window_us"]), bool(d["qualified"]))
+    s.clock = T0
+    return s
+
+
+def _edge_requests(descs, n, rng, shadow, mode, records, n_keys, monotone, big, hits, min_ctrs):
+    """[(counters [(limit_id, key_lo, key_hi)], (key_lo, key_hi), delta, now)] — see edge_csr_stream.  `shadow` (a
+    SpecStore) follows the stream so that clocks can be aimed at the expiry of the counter a request reads."""
+    by_ns = {}
+    for d in descs:
+        by_ns.setdefault(int(d["ns_id"]), []).append(d)
+    nss = sorted(by_ns)
+    out, t, i = [], shadow.clock, 0
+    while len(out) < n:
+        ns = int(rng.choice(nss))
+        lims = by_ns[ns]
+        if records or rng.random() < 0.6:
+            pick = list(range(len(lims)))
+        else:
+            pick = sorted(rng.choice(len(lims), size=int(rng.integers(min(min_ctrs, len(lims)) or 1, len(lims) + 1)),
+                                     replace=False).tolist())
+            if rng.random() < 0.3:
+                rng.shuffle(pick)
+        key, vkeys, ctrs = (int(rng.integers(1, n_keys + 1)), int(rng.integers(0, 2))), {}, []
+        for j in pick:
+            d = lims[j]
+            vs = int(d["varset_id"]) if d["qualified"] else 0
+            if vs not in vkeys:
+                vkeys[vs] = key if records else (int(rng.integers(1, n_keys + 1)), int(rng.integers(0, 2)))
+            ctrs.append((int(d["limit_id"]), *(vkeys[vs] if d["qualified"] else (0, 0))))
+        # the clock: small steps, half a second +-1, or exactly expiry - 1 / expiry / expiry + 1 of the first counter
+        t += _pick(rng, [0, 0, 0, 1, 2, 1000, 499_999, 500_000, 500_001])
+        now = t if monotone or rng.random() < 0.7 else max(1, t - _pick(rng, [1, 2, 500_000, 1_000_000]))
+        lid0, lo0, hi0 = ctrs[0]
+        e = shadow.qualified.get((lid0, lo0, hi0)) if lims[pick[0]]["qualified"] else shadow.simple.get(lid0)
+        if e is not None and e[1] > 2 and rng.random() < 0.25:
+            now = e[1] + _pick(rng, [-1, 0, 0, 1])
+            if now > t and (monotone or rng.random() < 0.5):
+                t = now
+        # a run: the same request again and again with one large delta (a member that differs only above bit 32)
+        if rng.random() < 0.07:
+            length = int(rng.integers(8, 25))
+            d0 = _pick(rng, big) if hits is None else int(rng.integers(hits[0], hits[1] + 1))
+            odd = int(rng.integers(1, length)) if not records and rng.random() < 0.4 else -1
+            for k in range(length):
+                dk = d0 ^ (1 << int(rng.integers(33, 63))) if k == odd else d0
+                out.append((ctrs, key, dk, now + k // 3))
+            t = max(t, now + length // 3)
+        else:
+            if hits is not None:
+                delta = int(rng.integers(hits[0], hits[1] + 1))
+            else:
+                delta = _pick(rng, SMALL_DELTAS) if rng.random() < 0.6 else _pick(rng, big)
+            out.append((ctrs, key, delta, now))
+        for ctrs_k, _, d_k, now_k in out[i:]:
+            if mode == 0:
+                shadow.check_and_update(ctrs_k, d_k, False, now_k)
+            elif mode == 2:
+                shadow.update_counters(ctrs_k, d_k, now_k)
+        i = len(out)
+    shadow.clock = t
+    return out[:n]
+
+
+def edge_csr_stream(descs, n, seed, shadow=None, mode=0, n_keys=3, monotone=True, min_ctrs=1):
+    """CSR requests over `descs` (a namespace, all or a subset of its limits, per-variable-set keys from a tiny key
+    space) whose deltas mix 0 and small values with 2^31, 2^32-1, 2^32, 2^32+1, 2^62, 3*2^62, 2^63 and 2^64-1; runs of 8
+    to 24 equal large deltas on one key (now and then one member differing from the others only above bit 32); clocks
+    stepping by half a second +-1 and landing at expiry - 1, expiry and expiry + 1 of the counter a request reads, and
+    (monotone=False) going back across them.  `shadow` (spec_with_limits) is the state the clocks aim at: pass the same
+    one to every batch of a stream, with the batch's `mode` (0 check_and_update, 1 is_rate_limited, 2 update)."""
+    rng = np.random.default_rng(seed)
+    shadow = shadow or spec_with_limits(descs)
+    reqs = _edge_requests(descs, n, rng, shadow, mode, False, n_keys, monotone, CSR_BIG_DELTAS, None, min_ctrs)
+    off = np.cumsum([0] + [len(r[0]) for r in reqs]).astype(np.uint32)
+    ctrs = np.array([(c[0], 0, c[1], c[2]) for r in reqs for c in r[0]], dtype=COUNTER_DTYPE)
+    return (off, ctrs, np.array([r[2] for r in reqs], dtype=np.uint64), np.array([r[3] for r in reqs], dtype=np.uint64))
+
+
+def edge_records(descs, n, seed, shadow=None, mode=0, n_keys=3, monotone=True, hits=None):
+    """32-byte records with the clocks and runs of edge_csr_stream and hits_addend up to 2^32-1 (or, with hits=(lo, hi),
+    drawn from lo..hi: 1..255 for rl_record16); 1 in 20 names a namespace without limits."""
+    rng = np.random.default_rng(seed)
+    shadow = shadow or spec_with_limits(descs)
+    reqs = _edge_requests(descs, n, rng, shadow, mode, True, n_keys, monotone, RECORD_BIG_DELTAS, hits, 1)
+    r = np.zeros(n, dtype=RECORD_DTYPE)
+    ns_of = {int(d["limit_id"]): int(d["ns_id"]) for d in descs}
+    r["ns_id"] = [ns_of[q[0][0][0]] for q in reqs]
+    r["ns_id"][rng.random(n) < 0.05] = int(descs["ns_id"].max()) + 3
+    r["hits_addend"] = [q[2] for q in reqs]
+    r["key_lo"] = [q[1][0] for q in reqs]
+    r["key_hi"] = [q[1][1] for q in reqs]
+    r["now_us"] = [q[3] for q in reqs]
+    return r
+
+
+def edge_batches(descs, seed, n_batches, n, form="csr", monotone=None, **kw):
+    """One edge stream as batches: [(mode, batch)], mostly check_and_update (0), every third an update_counters batch
+    (2) that pushes counters past their maximum, now and then an is_rate_limited one (1).  Odd batches go back in
+    time unless `monotone` is given."""
+    shadow = spec_with_limits(descs)
+    rng = np.random.default_rng(seed)
+    gen = edge_csr_stream if form == "csr" else edge_records
+    out = []
+    for b in range(n_batches):
+        mode = 2 if b % 3 == 1 else (1 if rng.random() < 0.15 else 0)
+        mono = (b % 2 == 0) if monotone is None else monotone
+        out.append((mode, gen(descs, n, seed * 1000 + b, shadow=shadow, mode=mode, monotone=mono, **kw)))
+    return out
+
+
+def records_as_csr(descs, recs):
+    """The CSR form of 32-byte records: every limit of the namespace in registration order, keyed by the record's key
+    if qualified."""
+    by_ns = {}
+    for d in descs:
+        by_ns.setdefault(int(d["ns_id"]), []).append(d)
+    off, ctrs = [0], []
+    for r in recs:
+        for d in by_ns.get(int(r["ns_id"]), []):
+            q = int(d["qualified"])
+            ctrs.append((int(d["limit_id"]), 0, int(r["key_lo"]) if q else 0, int(r["key_hi"]) if q else 0))
+        off.append(len(ctrs))
+    return (np.array(off, dtype=np.uint32), np.array(ctrs, dtype=COUNTER_DTYPE),
+            recs["hits_addend"].astype(np.uint64), recs["now_us"].astype(np.uint64))
+
+
+def _counting_spec():
+    from tests.spec_model import SpecStore
+
+    class CountingSpec(SpecStore):
+        """spec_model.SpecStore that counts the edges its calls reach (self.n):
+          wrapped_sums     a counter read whose value_at + delta passes 2^64
+          expiry_reads     a present counter read with now == its expiry (reads as 0, inclusive bound)
+          stale_flips      ... of those, reads where the expired value would have given the other verdict
+          above_max_reads  a live counter read whose value is above its limit's maximum
+          long_runs        >= 8 consecutive allowed increments of one counter by one delta, no window reset, that
+                           add up to more than 2^32
+          wrapping_runs    >= 2 such increments whose total passes 2^64 from the value the run started at
+          denied_runs      >= 4 consecutive denied check_and_update calls on one counter
+        Runs end at the end of a batch (end_batch), at a window reset, an update_counters call or another delta."""
+
+        KINDS = ("wrapped_sums", "expiry_reads", "stale_flips", "above_max_reads", "long_runs", "wrapping_runs",
+                 "denied_runs")
+
+        def __init__(self):
+            super().__init__()
+            self.n = dict.fromkeys(self.KINDS, 0)
+            self._run = {}  # counter -> [allowed?, delta, length, total, start value]
+
+        def _key(self, lid, lo, hi):
+            return (lid, lo, hi) if self.limits[lid][3] else (lid, 0, 0)
+
+        def _entry(self, lid, lo, hi):
+            return self.qualified.get((lid, lo, hi)) if self.limits[lid][3] else self.simple.get(lid)
+
+        def _reads(self, ctrs, delta, now):
+            for lid, lo, hi in ctrs:
+                e, mx = self._entry(lid, lo, hi), self.limits[lid][1]
+                if e is None:
+                    continue
+                v = self.value_at(e, now)
+                self.n["wrapped_sums"] += v + delta > M64
+                self.n["above_max_reads"] += v > mx
+                if e[1] == now:
+                    self.n["expiry_reads"] += 1
+                    self.n["stale_flips"] += (((e[0] + delta) & M64) > mx) != (delta > mx)
+
+        def _end(self, k):
+            r = self._run.pop(k, None)
+            if r is None:
+                return
+            allowed, _, length, total, v0 = r
+            if allowed:
+                self.n["long_runs"] += length >= 8 and total > 1 << 32
+                self.n["wrapping_runs"] += length >= 2 and v0 + total > M64
+            else:
+                self.n["denied_runs"] += length >= 4
+
+        def end_batch(self):
+            for k in list(self._run):
+                self._end(k)
+
+        def check_and_update(self, ctrs, delta, load_counters, now):
+            self._reads(ctrs, delta, now)
+            before = {self._key(*c): (lambda e: None if e is None else list(e))(self._entry(*c)) for c in ctrs}
+            res = super().check_and_update(ctrs, delta, load_counters, now)
+            for k, e0 in before.items():
+                r = self._run.get(k)
+                if res[0]:
+                    if r is None or r[0]:
+                        self._end(k)
+                        self._run[k] = r = [False, None, 0, 0, 0]
+                    r[2] += 1
+                elif e0 is None or e0[1] <= now:  # created or reset: a run can only start after it
+                    self._end(k)
+                else:
+                    if r is None or not r[0] or r[1] != delta:
+                        self._end(k)
+                        self._run[k] = r = [True, delta, 0, 0, e0[0]]
+                    r[2] += 1
+                    r[3] += delta
+            return res
+
+        def is_rate_limited(self, ctrs, delta, now):
+            self._reads(ctrs, delta, now)
+            return super().is_rate_limited(ctrs, delta, now)
+
+        def update_counters(self, ctrs, delta, now):
+            self._reads(ctrs, delta, now)
+            for c in ctrs:
+                self._end(self._key(*c))
+            super().update_counters(ctrs, delta, now)
+
+    return CountingSpec
+
+
+def spec_batch(s, mode, off, ctrs, delta, now, lc):
+    """A CSR batch through a spec_model.SpecStore, request by request -> (limited, first limited id, remaining, ttl)
+    like Oracle.batch_csr."""
+    n = len(delta)
+    lim, fl = np.zeros(n, dtype=np.uint8), np.full(n, NONE, dtype=np.uint32)
+    rem, ttl = np.zeros(len(ctrs), dtype=np.uint64), np.zeros(len(ctrs), dtype=np.uint64)
+    for i in range(n):
+        cs = [(int(c["limit_id"]), int(c["key_lo"]), int(c["key_hi"])) for c in ctrs[off[i]:off[i + 1]]]
+        if not cs:
+            continue  # no limits apply: not limited (lib.rs:434-440)
+        if mode == 0:
+            limited, first, r, t = s.check_and_update(cs, int(delta[i]), lc, int(now[i]))
+            if lc:
+                rem[off[i]:off[i + 1]] = r
+                ttl[off[i]:off[i + 1]] = t
+        elif mode == 1:
+            limited, first = s.is_rate_limited(cs, int(delta[i]), int(now[i]))
+        else:
+            s.update_counters(cs, int(delta[i]), int(now[i]))
+            limited, first = False, NONE
+        lim[i], fl[i] = int(limited), first
+    if hasattr(s, "end_batch"):
+        s.end_batch()
+    return lim, fl, rem, ttl
+
+
+def edge_coverage(descs, batches, form="csr"):
+    """Replay [(mode, batch)] (edge_batches) through a counting spec_model -> its counts."""
+    s = spec_with_limits(descs, _counting_spec())
+    for mode, b in batches:
+        spec_batch(s, mode, *(b if form == "csr" else records_as_csr(descs, b)), False)
+    return s.n
+
+
+def counting_spec(descs):
+    return spec_with_limits(descs, _counting_spec())
+
+
+# ---------------------------------------------------------------------------------------
+# Known answers at the edges, the numbers written out (not taken from the oracle).  One qualified limit (id 0, max
+# "max", window "window") and one counter (key 7); "seed" (value, t) is an update_counters(delta = value, now = t) on
+# the missing counter, i.e. the state (value, t + window).  Steps: ("check", deltas, nows, verdicts, remaining, ttl),
+# ("state", (value, expiry)), ("get", now, [(remaining, ttl)]) for get_counters, ("max", new max_value).
+_S = 1_000_000
+_T = T0
+_D = 0x4000000100000003  # 2^62 + 2^32 + 3: bits above 32, so a 32-bit product k * D gets the run's sums wrong
+EDGE_KATS = {
+    # 2^62 + 3*2^62 wraps to 0 <= 2^63: allowed, and the value becomes 0; 3*2^62 > 2^63 then denies twice
+    "wrap_allows_then_denies": dict(max=1 << 63, window=60 * _S, seed=(1 << 62, _T), steps=[
+        ("check", [3 << 62] * 3, [_T + 1, _T + 2, _T + 3], [0, 1, 1], [1 << 63, 0, 0],
+         [60 * _S - 1, 60 * _S - 2, 60 * _S - 3]),
+        ("state", (0, _T + 60 * _S))]),
+    # ten allowed increments by D from 0 (k*D passes 2^32 at once and wraps past 2^64 at k = 4 and 8) under max
+    # 3*2^62 + 2^35; the eleventh, 3*2^62 + 11*2^32 + 33, is over it
+    "closed_form_run_wraps": dict(max=0xC000000800000000, window=60 * _S, seed=(0, _T), steps=[
+        ("check", [_D] * 11, [_T + k for k in range(1, 12)], [0] * 10 + [1],
+         [0x80000006FFFFFFFD, 0x40000005FFFFFFFA, 0x4FFFFFFF7, 0xC0000003FFFFFFF4, 0x80000002FFFFFFF1,
+          0x40000001FFFFFFEE, 0xFFFFFFEB, 0xBFFFFFFFFFFFFFE8, 0x7FFFFFFEFFFFFFE5, 0x3FFFFFFDFFFFFFE2, 0],
+         [60 * _S - k for k in range(1, 12)]),
+        ("state", (0x8000000A0000001E, _T + 60 * _S))]),
+    # expiry T + 1 s: at T + 1 s - 2 and - 1 the 50 still counts; at T + 1 s it reads as 0 and the third request opens
+    # a new window (1, T + 2 s); the fourth, at the same clock, adds to it
+    "exact_boundary_in_a_run": dict(max=100, window=_S, seed=(50, _T), steps=[
+        ("check", [1] * 4, [_T + _S - 2, _T + _S - 1, _T + _S, _T + _S], [0, 0, 0, 0], [49, 48, 99, 98],
+         [2, 1, 0, _S]),
+        ("state", (2, _T + 2 * _S))]),
+    # 15 > max 10: delta 0 is denied and changes nothing; get_counters' remaining wraps (10 - 15); max 20 allows it
+    "above_the_maximum": dict(max=10, window=60 * _S, seed=(15, _T), steps=[
+        ("check", [0], [_T + 1], [1], [0], [60 * _S - 1]),
+        ("state", (15, _T + 60 * _S)),
+        ("get", _T + 1, [(M64 - 4, 60 * _S - 1)]),
+        ("max", 20),
+        ("check", [0], [_T + 2], [0], [5], [60 * _S - 2]),
+        ("get", _T + 3, [(5, 60 * _S - 3)]),
+        ("state", (15, _T + 60 * _S))]),
+    # max 0, value 1: 1 + (2^64 - 1) wraps to 0 <= 0, allowed, and the value becomes 0
+    "max_zero_wraps_to_zero": dict(max=0, window=60 * _S, seed=(1, _T), steps=[
+        ("check", [M64], [_T + 1], [0], [0], [60 * _S - 1]),
+        ("state", (0, _T + 60 * _S))]),
+}
+
+
+def edge_kat_limits(kat, max_value=None):
+    mx = kat["max"] if max_value is None else max_value
+    return np.array([(0, 0, 1, 1, mx, kat["window"])], dtype=LIMIT_DESC_DTYPE)
+
+
+def run_edge_kat(kat, layer, batched, lc):
+    """One EDGE_KATS entry through `layer`: an object with seed(value, now) (update_counters), check(deltas, nows, lc)
+    -> (verdicts, remaining, ttl) on the KAT's counter, state() -> (value, expiry), get(now) -> [(remaining, ttl)] or
+    None where the layer has no get_counters, set_max(max_value).  The checks go as one call per step (batched) or one
+    call per request."""
+    layer.seed(*kat["seed"])
+    for step in kat["steps"]:
+        if step[0] == "check":
+            _, deltas, nows, want_lim, want_rem, want_ttl = step
+            calls = [(deltas, nows)] if batched else [([d], [t]) for d, t in zip(deltas, nows)]
+            got = [layer.check(d, t, lc) for d, t in calls]
+            assert [v for g in got for v in g[0]] == want_lim, "verdicts"
+            if lc:
+                assert [v for g in got for v in g[1]] == want_rem, "remaining"
+                assert [v for g in got for v in g[2]] == want_ttl, "ttl"
+        elif step[0] == "state":
+            assert layer.state() == step[1], "counter state"
+        elif step[0] == "get":
+            got = layer.get(step[1])
+            assert got is None or got == step[2], "get_counters"
+        else:
+            layer.set_max(step[1])

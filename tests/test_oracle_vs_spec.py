@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from tests import helpers as H
-from tests.spec_model import NONE, SpecStore
+from tests.spec_model import SpecStore
 from oracle import binding as ob
 
 
@@ -16,28 +16,6 @@ def both(descs, cap=16):
         o.limit_set(*args)
         s.limit_set(*args)
     return o, s
-
-
-def spec_batch(s, mode, off, ctrs, delta, now, lc):
-    n = len(delta)
-    lim, fl = np.zeros(n, dtype=np.uint8), np.full(n, NONE, dtype=np.uint32)
-    rem, ttl = np.zeros(len(ctrs), dtype=np.uint64), np.zeros(len(ctrs), dtype=np.uint64)
-    for i in range(n):
-        cs = [(int(c["limit_id"]), int(c["key_lo"]), int(c["key_hi"])) for c in ctrs[off[i]:off[i + 1]]]
-        if not cs:
-            continue  # no limits apply: not limited (lib.rs:434-440)
-        if mode == 0:
-            limited, first, r, t = s.check_and_update(cs, int(delta[i]), lc, int(now[i]))
-            if lc:
-                rem[off[i]:off[i + 1]] = r
-                ttl[off[i]:off[i + 1]] = t
-        elif mode == 1:
-            limited, first = s.is_rate_limited(cs, int(delta[i]), int(now[i]))
-        else:
-            s.update_counters(cs, int(delta[i]), int(now[i]))
-            limited, first = False, NONE
-        lim[i], fl[i] = int(limited), first
-    return lim, fl, rem, ttl
 
 
 @pytest.mark.parametrize("seed", range(8))
@@ -53,7 +31,7 @@ def test_oracle_equals_the_python_spec_on_random_streams(seed):
         mode = int(rng.choice([0, 0, 0, 1, 2]))
         lc = bool(rng.integers(0, 2)) and mode == 0
         got = o.batch_csr(mode, off, ctrs, delta, now, lc)
-        want = spec_batch(s, mode, off, ctrs, delta, now, lc)
+        want = H.spec_batch(s, mode, off, ctrs, delta, now, lc)
         assert np.array_equal(got[0], want[0]), f"verdicts, batch {b} mode {mode}"
         if mode != 2:
             assert np.array_equal(got[1], want[1]), f"first limited, batch {b} mode {mode}"
@@ -90,7 +68,7 @@ def test_clear_drops_only_unqualified_counters_in_both():
     o, s = both(descs)
     off, ctrs, delta, now = H.random_csr_stream(descs, 600, 77, n_keys=20)
     o.batch_csr(0, off, ctrs, delta, now)
-    spec_batch(s, 0, off, ctrs, delta, now, False)
+    H.spec_batch(s, 0, off, ctrs, delta, now, False)
     o.clear()
     s.clear()
     assert sorted(o.dump()) == s.dump()

@@ -5,8 +5,8 @@ shuffled order — and their warp-aggregated probe under tests/emu/cuda_simt.h:
     hot path's probing rule (rl_kernels.cuh rl_probe, restated here) finds it, and every other row byte-identical;
   * every refusal (duplicate, unknown limit, key_hi >= 2^32, qualified expiry 0, full region) leaves the table
     byte-identical.
-oracle_restore applies the same import to the CPU oracle through the oracle's own public calls (the GPU tests continue
-a stream on it after an import); it is pinned here by a small known-answer test.
+tests/helpers.py oracle_restore applies the same import to the CPU oracle through the oracle's own public calls (the GPU
+tests continue a stream on it after an import); it is pinned here by a small known-answer test.
 The GPU runs of rl_counters_export / rl_counters_import are in tests/test_zz4_snapshot_gpu.py."""
 import numpy as np
 import pytest
@@ -230,37 +230,6 @@ def test_a_refused_import_changes_no_counter(simt):
     assert (small.w == before).all(), "a refused import changed the table"
 
 
-def oracle_restore(o, descs, limit_id, key_lo, key_hi, value, expiry_us):
-    """What rl_counters_import does, applied to the CPU oracle through its own public calls: set each counter to exactly
-    (value, expiry_us); a present counter is replaced, an unqualified one (key ignored) becomes present, other counters
-    are untouched.  descs: the limits the oracle was given (limit_id, ns_id, max_value, window_us, qualified).
-
-    The counters of every limit named are read back (dump), deleted (delete_counters) and created again with the
-    imported ones merged in: update_counter(delta = value, now = expiry - window) creates exactly (value, expiry)
-    (in_memory.rs:47-69), and limit_set again on an unqualified limit without a counter recreates the (0, EPOCH) default
-    (add_counter, in_memory.rs:38-44).  A limit id the oracle does not know raises before anything changes."""
-    by_id = {int(d["limit_id"]): d for d in descs}
-    new = {}
-    for l, lo, hi, v, x in zip(*[np.asarray(c).tolist() for c in (limit_id, key_lo, key_hi, value, expiry_us)]):
-        if l not in by_id:
-            raise ValueError(f"limit {l} is not registered")
-        new[(l, lo, hi) if by_id[l]["qualified"] else (l, 0, 0)] = (v, x)
-    touched = sorted({k[0] for k in new})
-    state = {(l, lo, hi): (v, x) for l, lo, hi, v, x in o.dump() if l in touched}
-    state.update(new)
-    for (l, lo, hi), (v, x) in state.items():
-        w = int(by_id[l]["window_us"])
-        if x < w and (by_id[l]["qualified"] or (v, x) != (0, 0)):
-            raise ValueError(f"counter {(l, lo, hi)}: expiry {x} is earlier than one window after the epoch")
-    o.delete_counters(touched)
-    for (l, lo, hi), (v, x) in sorted(state.items()):
-        d = by_id[l]
-        if not d["qualified"] and (v, x) == (0, 0):
-            o.limit_set(l, int(d["ns_id"]), int(d["max_value"]), int(d["window_us"]), False)
-        else:
-            o.update_counters(ob.counters([(l, lo, hi)]), v, x - int(d["window_us"]))
-
-
 def test_oracle_restore_sets_counters_exactly():
     W, T = 1_000_000, 5_000_000
     descs = np.array([(0, 0, 0, 0, 10, W), (1, 0, 1, 1, 10, W), (2, 1, 0, 0, 5, 2 * W)], dtype=LIMIT_DESC_DTYPE)
@@ -271,7 +240,7 @@ def test_oracle_restore_sets_counters_exactly():
     o.update_counters(ob.counters([(1, 7, 0)]), 3, T)  # (3, T + W)
     o.update_counters(ob.counters([(1, 8, 1)]), 2, T)
     assert o.dump() == [(0, 0, 0, 0, 0), (1, 7, 0, 3, T + W), (1, 8, 1, 2, T + W)]
-    oracle_restore(o, descs, [1, 1, 0, 2], [7, 9, 55, 66], [0, 4, 0, 0], [6, 1, 4, 2], [T + 500, T + 900, T + 700, T + 2 * W])
+    H.oracle_restore(o, descs, [1, 1, 0, 2], [7, 9, 55, 66], [0, 4, 0, 0], [6, 1, 4, 2], [T + 500, T + 900, T + 700, T + 2 * W])
     # a present counter replaced (even with an earlier expiry), a new one added, unqualified ones set with their key
     # ignored, limit 2 present again, counter (1, 8, 1) untouched
     assert o.dump() == [(0, 0, 0, 4, T + 700), (1, 7, 0, 6, T + 500), (1, 8, 1, 2, T + W), (1, 9, 4, 1, T + 900),
@@ -280,9 +249,9 @@ def test_oracle_restore_sets_counters_exactly():
     assert o.check_and_update(ob.counters([(1, 7, 0)]), 5, False, T + 500)[0] is False  # expired: a new window
     # the (0, EPOCH) default of an unqualified limit is restored as such
     o.delete_counters([0])
-    oracle_restore(o, descs, [0], [0], [0], [0], [0])
+    H.oracle_restore(o, descs, [0], [0], [0], [0], [0])
     assert (0, 0, 0, 0, 0) in o.dump()
     before = o.dump()
     with pytest.raises(ValueError):
-        oracle_restore(o, descs, [0, 3], [0, 0], [0, 0], [9, 9], [T, T])  # limit 3 is not registered
+        H.oracle_restore(o, descs, [0, 3], [0, 0], [0, 0], [9, 9], [T, T])  # limit 3 is not registered
     assert o.dump() == before

@@ -9,7 +9,6 @@ import pytest
 from limitador_b200 import Engine, EngineError, exchange, streams
 from limitador_b200.engine import RL_FATAL, RL_TRANSIENT, Shard
 from tests import helpers as H
-from tests.test_snapshot_emu import oracle_restore
 
 pytestmark = pytest.mark.gpu
 S = 1_000_000
@@ -106,7 +105,7 @@ def test_import_over_live_counters_replaces_them():
     keep = np.arange(len(cols[0])) % 3 != 0  # two thirds of A's counters, many of which B holds too
     cols = [c[keep] for c in cols]
     b.import_counters(*cols)
-    oracle_restore(ob_, descs, *cols)
+    H.oracle_restore(ob_, descs, *cols)
     assert H.normalise_dump(b.dump(), descs) == H.normalise_dump(ob_.dump(), descs)
     for s in range(2):
         _same_csr(b, ob_, H.random_csr_stream(descs, 3000, seed=33 + s, n_keys=30))
