@@ -13,7 +13,7 @@
  *   envoy.config.core.v3.HeaderValue (key, value)
  *
  * A batch of n wire requests is served in three stages:
- *   plan    (CPU, `threads` workers): decode every request, build its CEL context
+ *   plan    (GPU in rl_rls_serve, CPU in rl_rls_plan): decode every request, build its CEL context
  *           (`descriptors[i]` = the i-th descriptor's entries as a map, last duplicate key wins — server.rs:121-127),
  *           run counters_that_apply (include/rl_match.h) and lay the counters out as the CSR that
  *           rl_check_and_update_batch / rl_is_within_limits_batch / rl_update_batch take.  Requests that never reach
@@ -22,8 +22,12 @@
  *   decide  (GPU): ONE engine call for the whole batch; array order is the stream order that defines the result.
  *   finish  (CPU): verdicts (+ remaining / ttl with draft-03 headers) -> RateLimitResponse bytes, the three
  *           X-RateLimit-* headers sorted by key (server.rs:45-57, lib.rs:235-275), per-namespace metrics.
- * rl_rls_serve runs the three stages through the engine given at creation.  plan / finish are exported on their own so
- * that the CPU stages can be driven (and tested) without a GPU; the product never decides on the CPU.
+ * rl_rls_serve runs the three stages through the engine given at creation: the plan runs on the engine's device
+ * (rl_rls_plan_device: one thread per request, the same decoder and digest as the CPU plan, the matcher as a device
+ * image uploaded when its limits change), the store call reads the counters where the plan left them, and only what
+ * the finish reads comes back to the host.  rl_rls_plan (the CPU plan on `threads` workers) and rl_rls_finish are
+ * exported on their own so that the CPU stages can be driven (and tested) without a GPU; the product never decides on
+ * the CPU.
  *
  * gRPC status per request (what tonic would put in grpc-status): 0 OK with a response body; 13 INTERNAL for a
  * message that does not decode (prost DecodeError); 14 UNAVAILABLE "Service unavailable" when the store call fails
@@ -82,8 +86,15 @@ int rl_rls_create(rl_matcher *m, rl_engine *engine, int header_mode, uint32_t th
 void rl_rls_destroy(rl_rls *s);
 const char *rl_rls_last_error(rl_rls *s);
 
-/* Stage 1.  Request i = buf[off[i] .. off[i+1]).  now_us = the batch's clock reading (0 = wall clock now). */
+/* Stage 1 on the CPU workers.  Request i = buf[off[i] .. off[i+1]).  now_us = the batch's clock reading (0 = wall
+ * clock now). */
 int rl_rls_plan(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+/* Stage 1 on the engine's device (needs a service created with an engine); afterwards rl_rls_plan_view and
+ * rl_rls_finish behave exactly as after rl_rls_plan, and every array equals rl_rls_plan's.  One difference, in a
+ * misconfiguration only: with the matcher's counter cap raised above the engine's max_counters_per_request, the CPU
+ * plan refuses whole worker ranges (which ones depends on the thread count), the device plan refuses exactly the
+ * requests with more counters than the engine takes (gRPC 14 UNAVAILABLE). */
+int rl_rls_plan_device(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
 /* The store call of the planned batch: n_store requests (a subset of the batch, in batch order) as CSR arrays owned by
  * the service, valid until the next plan.  store_index[i] (nullable out, n entries) = position of request i in the
  * store call or RL_RLS_NO_STORE. */
@@ -99,14 +110,16 @@ int rl_rls_finish(rl_rls *s, int store_status, const uint8_t *limited, const uin
  * (*out_code)[i] the overall_code.  Valid until the next plan. */
 int rl_rls_responses(rl_rls *s, const uint8_t **out_buf, const uint64_t **out_off, const uint8_t **out_grpc,
                      const uint8_t **out_code);
-/* plan -> the engine -> finish. */
+/* rl_rls_plan_device -> the engine (RL_MEM_DEVICE: one device->host read of the store request count before it) ->
+ * finish. */
 int rl_rls_serve(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
 
 /* Prometheus text exposition of authorized_calls / authorized_hits / limited_calls (sorted by label values) plus
  * `limitador_up 1`: lines `name{limitador_namespace="ns"[,limit_name="x"]} value` as
  * metrics_exporter_prometheus renders them (prometheus_metrics.rs:415-447).  *out_len = bytes needed incl. NUL. */
 int rl_rls_metrics_render(rl_rls *s, char *out, uint64_t cap, uint64_t *out_len);
-/* Stage timings of the last serve call in microseconds: plan, store call, finish. */
+/* Stage timings of the last serve call in microseconds: plan (the device plan, and taking its per-request outcomes in),
+ * store call (with the copies of its outputs), finish. */
 int rl_rls_last_timings(rl_rls *s, double *out_plan_us, double *out_store_us, double *out_finish_us);
 
 #ifdef __cplusplus

@@ -36,6 +36,7 @@ _UNITS = {
     "rl_engine.cu": "csrc",   # the kernels' headers live beside it: any change under csrc/ rebuilds it
     "rl_maint.cu": "csrc",
     "rl_crdt.cu": "csrc",
+    "rl_rls_dev.cu": "csrc",
     "rl_front.cu": "public",
     "rl_match.cpp": "public",
     "rl_rls.cpp": "public",

@@ -17,114 +17,13 @@
 #include <unordered_map>
 #include <vector>
 
+#include "rl_blake2b.h"
 #include "rl_match.h"
+#include "rl_match_image.h"
 
 namespace {
 
-// ---- BLAKE2b (RFC 7693), unkeyed, streaming ----------------------------------------------
-struct Blake2b {
-    uint64_t h[8];
-    uint64_t t = 0;
-    uint8_t buf[128];
-    size_t fill = 0;
-    size_t outlen;
-
-    static inline uint64_t rotr(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
-    static inline uint64_t load64(const uint8_t* p) {
-        uint64_t v;
-        memcpy(&v, p, 8);  // little-endian hosts only (x86-64, aarch64)
-        return v;
-    }
-    explicit Blake2b(size_t out) : outlen(out) {
-        static const uint64_t IV[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL,
-                                       0xa54ff53a5f1d36f1ULL, 0x510e527fade682d1ULL, 0x9b05688c2b3e6c1fULL,
-                                       0x1f83d9abfb41bd6bULL, 0x5be0cd19137e2179ULL};
-        memcpy(h, IV, sizeof h);
-        h[0] ^= 0x01010000ULL ^ (uint64_t)out;
-    }
-    void compress(const uint8_t* block, bool last) {
-        static const uint64_t IV[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL,
-                                       0xa54ff53a5f1d36f1ULL, 0x510e527fade682d1ULL, 0x9b05688c2b3e6c1fULL,
-                                       0x1f83d9abfb41bd6bULL, 0x5be0cd19137e2179ULL};
-        static const uint8_t S[12][16] = {
-            {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15}, {14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3},
-            {11, 8, 12, 0, 5, 2, 15, 13, 10, 14, 3, 6, 7, 1, 9, 4}, {7, 9, 3, 1, 13, 12, 11, 14, 2, 6, 5, 10, 4, 0, 15, 8},
-            {9, 0, 5, 7, 2, 4, 10, 15, 14, 1, 11, 12, 6, 8, 3, 13}, {2, 12, 6, 10, 0, 11, 8, 3, 4, 13, 7, 5, 15, 14, 1, 9},
-            {12, 5, 1, 15, 14, 13, 4, 10, 0, 7, 6, 3, 9, 2, 8, 11}, {13, 11, 7, 14, 12, 1, 3, 9, 5, 0, 15, 4, 8, 6, 2, 10},
-            {6, 15, 14, 9, 11, 3, 0, 8, 12, 2, 13, 7, 1, 4, 10, 5}, {10, 2, 8, 4, 7, 6, 1, 5, 15, 11, 9, 14, 3, 12, 13, 0},
-            {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15}, {14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3}};
-        uint64_t m[16], v[16];
-        for (int i = 0; i < 16; i++) m[i] = load64(block + 8 * i);
-        for (int i = 0; i < 8; i++) {
-            v[i] = h[i];
-            v[i + 8] = IV[i];
-        }
-        v[12] ^= t;  // message lengths stay far below 2^64: the high counter word is 0
-        if (last) v[14] = ~v[14];
-#define RL_B2_G(a, b, c, d, x, y)          \
-    v[a] = v[a] + v[b] + (x);              \
-    v[d] = rotr(v[d] ^ v[a], 32);          \
-    v[c] = v[c] + v[d];                    \
-    v[b] = rotr(v[b] ^ v[c], 24);          \
-    v[a] = v[a] + v[b] + (y);              \
-    v[d] = rotr(v[d] ^ v[a], 16);          \
-    v[c] = v[c] + v[d];                    \
-    v[b] = rotr(v[b] ^ v[c], 63);
-        for (int r = 0; r < 12; r++) {
-            const uint8_t* s = S[r];
-            RL_B2_G(0, 4, 8, 12, m[s[0]], m[s[1]])
-            RL_B2_G(1, 5, 9, 13, m[s[2]], m[s[3]])
-            RL_B2_G(2, 6, 10, 14, m[s[4]], m[s[5]])
-            RL_B2_G(3, 7, 11, 15, m[s[6]], m[s[7]])
-            RL_B2_G(0, 5, 10, 15, m[s[8]], m[s[9]])
-            RL_B2_G(1, 6, 11, 12, m[s[10]], m[s[11]])
-            RL_B2_G(2, 7, 8, 13, m[s[12]], m[s[13]])
-            RL_B2_G(3, 4, 9, 14, m[s[14]], m[s[15]])
-        }
-#undef RL_B2_G
-        for (int i = 0; i < 8; i++) h[i] ^= v[i] ^ v[i + 8];
-    }
-    void update(const void* data, size_t n) {
-        const uint8_t* p = (const uint8_t*)data;
-        while (n) {
-            if (fill == 128) {  // a full buffer is only compressed once more input follows it
-                t += 128;
-                compress(buf, false);
-                fill = 0;
-            }
-            const size_t k = std::min(n, (size_t)128 - fill);
-            memcpy(buf + fill, p, k);
-            fill += k;
-            p += k;
-            n -= k;
-        }
-    }
-    void final(uint8_t* out) {
-        t += fill;
-        memset(buf + fill, 0, 128 - fill);
-        compress(buf, true);
-        uint8_t full[64];
-        memcpy(full, h, 64);
-        memcpy(out, full, outlen);
-    }
-};
-
-struct KeyDigest {
-    Blake2b b{12};
-    void str(const char* s, size_t n) {
-        const uint32_t len = (uint32_t)n;
-        b.update(&len, 4);
-        b.update(s, n);
-    }
-    void finish(uint64_t& lo, uint64_t& hi) {
-        uint8_t d[12];
-        b.final(d);
-        uint32_t hi32;
-        memcpy(&lo, d, 8);
-        memcpy(&hi32, d + 8, 4);
-        hi = hi32;
-    }
-};
+using rl_b2::KeyDigest;  // rl_blake2b.h: the same digest as the device plan
 
 // ---- operand slots ------------------------------------------------------------------------
 struct SlotKey {
@@ -303,6 +202,7 @@ struct rl_matcher {
     std::vector<std::vector<uint32_t>> ns_limits;  // registration order
     std::map<std::string, uint32_t> by_identity;
     std::map<std::string, uint32_t> varsets;  // (namespace, variables) -> id, from 1
+    uint64_t generation = 1;                  // rl_matcher_generation: bumped by every change of the limits or the cap
 };
 
 namespace {
@@ -505,6 +405,7 @@ int rl_matcher_add_limit_ex(rl_matcher* m, const char* ns, uint64_t max_value, u
         m->ns_limits[L.ns_id].push_back(lid);
         m->limits.push_back(std::move(L));
     }
+    m->generation++;
     const MLimit& R = m->limits[lid];
     out_desc->limit_id = lid;
     out_desc->ns_id = R.ns_id;
@@ -519,6 +420,7 @@ int rl_matcher_set_counter_cap(rl_matcher* m, uint32_t cap) {
     if (!m || cap == 0) return RL_FATAL;
     std::unique_lock<std::shared_mutex> lock(m->mu);
     m->counter_cap = cap;
+    m->generation++;
     return RL_OK;
 }
 
@@ -534,6 +436,7 @@ int rl_matcher_delete_limit(rl_matcher* m, uint32_t limit_id) {
     std::unique_lock<std::shared_mutex> lock(m->mu);
     if (limit_id >= m->limits.size()) return mfail(m, "unknown limit_id %u", limit_id);
     m->limits[limit_id].deleted = true;
+    m->generation++;
     return RL_OK;
 }
 
@@ -746,6 +649,116 @@ int rl_matcher_response_headers_batch(rl_matcher* m, uint64_t n, const uint32_t*
     }
     *out_len = w;
     return fits ? RL_OK : mfail(m, "header text needs %llu bytes", (unsigned long long)w);
+}
+
+uint64_t rl_matcher_generation(rl_matcher* m) {
+    if (!m) return 0;
+    std::shared_lock<std::shared_mutex> lock(m->mu);
+    return m->generation;
+}
+
+int rl_matcher_image(rl_matcher* m, uint32_t* out, uint64_t cap_words, uint64_t* out_words, uint64_t* out_generation) {
+    if (!m || !out_words || (cap_words && !out)) return RL_FATAL;
+    std::shared_lock<std::shared_mutex> lock(m->mu);
+    std::vector<uint32_t> w(RL_IMG_HDR_WORDS, 0);
+    std::string arena;
+    auto put_str = [&](const std::string& x) {
+        const uint32_t o = (uint32_t)arena.size();
+        arena += x;
+        return o;
+    };
+    auto table_mask = [](size_t n) {
+        size_t cap = 16;
+        while (cap < 2 * n) cap *= 2;
+        return (uint32_t)(cap - 1);
+    };
+    // namespaces: id -> string, then the open-addressed table
+    const uint32_t n_ns = (uint32_t)m->ns_limits.size();
+    std::vector<const std::string*> ns_of(n_ns, nullptr);
+    for (const auto& kv : m->ns_ids) ns_of[kv.second] = &kv.first;
+    const uint32_t ns_mask = table_mask(n_ns);
+    w[RL_IMG_H_NS_TAB] = (uint32_t)w.size();
+    w.resize(w.size() + ns_mask + 1, RL_IMG_EMPTY);
+    w[RL_IMG_H_NS_STR] = (uint32_t)w.size();
+    for (uint32_t id = 0; id < n_ns; id++) {
+        const std::string& x = *ns_of[id];
+        w.push_back(put_str(x));
+        w.push_back((uint32_t)x.size());
+        uint32_t* tab = w.data() + w[RL_IMG_H_NS_TAB];
+        uint64_t p = rl_img_hash(RL_IMG_NS_SEED, (const uint8_t*)x.data(), (uint32_t)x.size()) & ns_mask;
+        while (tab[p] != RL_IMG_EMPTY) p = (p + 1) & ns_mask;
+        tab[p] = id;
+    }
+    // per namespace, its live limits in counter output order
+    w[RL_IMG_H_NS_LIM_OFF] = (uint32_t)w.size();
+    w.resize(w.size() + n_ns + 1, 0);
+    w[RL_IMG_H_NS_LIMS] = (uint32_t)w.size();
+    for (uint32_t id = 0; id < n_ns; id++) {
+        w[w[RL_IMG_H_NS_LIM_OFF] + id] = (uint32_t)(w.size() - w[RL_IMG_H_NS_LIMS]);
+        for (const uint32_t lid : m->ns_limits[id])
+            if (!m->limits[lid].deleted) w.push_back(lid);
+    }
+    w[w[RL_IMG_H_NS_LIM_OFF] + n_ns] = (uint32_t)(w.size() - w[RL_IMG_H_NS_LIMS]);
+    // slots
+    const uint32_t n_slots = (uint32_t)m->slots.keys.size();
+    const uint32_t slot_mask = table_mask(n_slots);
+    w[RL_IMG_H_SLOT_TAB] = (uint32_t)w.size();
+    w.resize(w.size() + slot_mask + 1, RL_IMG_EMPTY);
+    w[RL_IMG_H_SLOT_KEY] = (uint32_t)w.size();
+    for (uint32_t s = 0; s < n_slots; s++) {
+        const SlotKey& k = m->slots.keys[s];
+        w.push_back(k.desc);
+        w.push_back(put_str(k.key));
+        w.push_back((uint32_t)k.key.size());
+        uint32_t* tab = w.data() + w[RL_IMG_H_SLOT_TAB];
+        uint64_t p = rl_img_hash(k.desc, (const uint8_t*)k.key.data(), (uint32_t)k.key.size()) & slot_mask;
+        while (tab[p] != RL_IMG_EMPTY) p = (p + 1) & slot_mask;
+        tab[p] = s;
+    }
+    // limits, their predicates and variables
+    const uint32_t n_limits = (uint32_t)m->limits.size();
+    std::vector<uint32_t> preds, vars;
+    w[RL_IMG_H_LIMS] = (uint32_t)w.size();
+    for (uint32_t lid = 0; lid < n_limits; lid++) {
+        const MLimit& L = m->limits[lid];
+        w.push_back((uint32_t)(preds.size() / 4));
+        w.push_back((uint32_t)L.preds.size());
+        w.push_back((uint32_t)(vars.size() / 3));
+        w.push_back((uint32_t)L.var_slots.size());
+        w.push_back(L.varset_id);
+        for (const Pred& p : L.preds) {
+            preds.push_back(p.slot);
+            preds.push_back(p.neq ? 1u : 0u);
+            preds.push_back(put_str(p.lit));
+            preds.push_back((uint32_t)p.lit.size());
+        }
+        for (size_t j = 0; j < L.var_slots.size(); j++) {
+            vars.push_back(L.var_slots[j]);
+            vars.push_back(put_str(L.vars[j]));
+            vars.push_back((uint32_t)L.vars[j].size());
+        }
+    }
+    w[RL_IMG_H_PREDS] = (uint32_t)w.size();
+    w.insert(w.end(), preds.begin(), preds.end());
+    w[RL_IMG_H_VARS] = (uint32_t)w.size();
+    w.insert(w.end(), vars.begin(), vars.end());
+    w[RL_IMG_H_ARENA] = (uint32_t)w.size();
+    w[RL_IMG_H_ARENA_BYTES] = (uint32_t)arena.size();
+    const size_t arena_words = (arena.size() + 3) / 4;
+    w.resize(w.size() + arena_words, 0);
+    if (!arena.empty()) memcpy(w.data() + w[RL_IMG_H_ARENA], arena.data(), arena.size());
+    w[RL_IMG_H_MAGIC] = RL_IMG_MAGIC;
+    w[RL_IMG_H_N_NS] = n_ns;
+    w[RL_IMG_H_NS_MASK] = ns_mask;
+    w[RL_IMG_H_N_SLOTS] = n_slots;
+    w[RL_IMG_H_SLOT_MASK] = slot_mask;
+    w[RL_IMG_H_N_LIMITS] = n_limits;
+    w[RL_IMG_H_COUNTER_CAP] = m->counter_cap;
+    *out_words = w.size();
+    if (out_generation) *out_generation = m->generation;
+    if (w.size() > cap_words) return RL_FATAL;
+    memcpy(out, w.data(), w.size() * sizeof(uint32_t));
+    return RL_OK;
 }
 
 void rl_counter_key(const char* const* sources, const char* const* values, uint32_t n, uint64_t* key_lo, uint64_t* key_hi) {

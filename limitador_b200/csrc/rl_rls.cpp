@@ -4,9 +4,10 @@
 // Host-only code.  The reference serves one request per tonic task: prost decodes the message, a HashMap per
 // descriptor is built and bound as `descriptors` (envoy_rls/server.rs:121-139), counters_that_apply walks the CEL
 // ASTs, the store is called, the response is built (:183-205).  Here a batch of wire messages is decoded and
-// matched by a pool of workers (each request is independent), the counters are laid out as one CSR, the store is
-// called once for the whole batch, and the responses are encoded by the same pool.  No protobuf runtime: the four
-// message types on the path have a handful of fields, decoded and encoded by hand below.
+// matched — on the engine's device (rl_rls_dev.cu) in rl_rls_serve, by a pool of CPU workers in rl_rls_plan (each
+// request is independent) —, the counters are laid out as one CSR, the store is called once for the whole batch, and
+// the responses are encoded by the worker pool.  No protobuf runtime: the four message types on the path have a
+// handful of fields, decoded by hand (rl_wire.h, shared with the device plan) and encoded below.
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -23,186 +24,31 @@
 #include <vector>
 
 #include "rl_rls.h"
+#include "rl_rls_dev.h"
+#include "rl_wire.h"
 
 extern "C" uint32_t rl_matcher_counter_cap(rl_matcher* m);  // rl_match.cpp (library-internal)
-// Weak: the wire surface is also linked without the engine (the sanitizer build of tests/san); there every service
-// plans with the default engine's maximum.
+// Weak: the wire surface is also linked without the engine and the CUDA units (the sanitizer build of tests/san); there
+// every service plans on the CPU with the default engine's maximum.
 extern "C" __attribute__((weak)) uint32_t rl_engine_max_counters_per_request(rl_engine* e);
+extern "C" {
+__attribute__((weak)) int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, uint64_t n, const uint8_t* buf,
+                                          const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                                          const RlsDevReq** out_req);
+__attribute__((weak)) int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta);
+__attribute__((weak)) int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counters, uint8_t* limited,
+                                            uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
+                                            rl_counter* ctrs);
+__attribute__((weak)) int rl_rls_dev_wait(rl_rls_dev* st);
+__attribute__((weak)) const char* rl_rls_dev_error(rl_rls_dev* st);
+__attribute__((weak)) void rl_rls_dev_destroy(rl_rls_dev* st);
+}
 
 namespace {
 
-// ---- protobuf wire format (proto3) -----------------------------------------------------------------------------
-struct Rd {
-    const uint8_t* p;
-    const uint8_t* end;
-};
-
-// prost::encoding::decode_varint: at most 10 bytes, the 10th may only carry bit 63
-bool rd_varint(Rd& r, uint64_t& v) {
-    v = 0;
-    for (int i = 0; i < 10; i++) {
-        if (r.p >= r.end) return false;
-        const uint8_t b = *r.p++;
-        if (i == 9 && b > 1) return false;
-        v |= (uint64_t)(b & 0x7F) << (7 * i);
-        if (!(b & 0x80)) return true;
-    }
-    return false;
-}
-bool rd_key(Rd& r, uint32_t& tag, uint32_t& wt) {
-    uint64_t k;
-    if (!rd_varint(r, k) || k > 0xFFFFFFFFull) return false;  // "invalid key value"
-    wt = (uint32_t)k & 7u;
-    tag = (uint32_t)k >> 3;
-    return tag != 0 && wt <= 5;  // "invalid tag value: 0", "invalid wire type value"
-}
-bool rd_len(Rd& r, Rd& sub) {
-    uint64_t n;
-    if (!rd_varint(r, n) || n > (uint64_t)(r.end - r.p)) return false;
-    sub.p = r.p;
-    sub.end = r.p + n;
-    r.p += n;
-    return true;
-}
-bool rd_skip(Rd& r, uint32_t tag, uint32_t wt, int depth) {
-    uint64_t v;
-    Rd sub;
-    switch (wt) {
-        case 0: return rd_varint(r, v);
-        case 1:
-            if (r.end - r.p < 8) return false;
-            r.p += 8;
-            return true;
-        case 2: return rd_len(r, sub);
-        case 5:
-            if (r.end - r.p < 4) return false;
-            r.p += 4;
-            return true;
-        case 3:  // start group: skip to the matching end group (prost::encoding::skip_field)
-            if (depth >= 100) return false;
-            for (;;) {
-                uint32_t t2, w2;
-                if (!rd_key(r, t2, w2)) return false;
-                if (w2 == 4) return t2 == tag;
-                if (!rd_skip(r, t2, w2, depth + 1)) return false;
-            }
-        default: return false;  // a stray end group
-    }
-}
-
-// str::from_utf8: no overlong forms, no surrogates, nothing above U+10FFFF
-bool utf8_ok(const uint8_t* p, const uint8_t* end) {
-    while (p < end) {
-        const uint8_t c = *p;
-        if (c < 0x80) {
-            p++;
-            continue;
-        }
-        int n;
-        uint32_t cp;
-        if (c >= 0xC2 && c <= 0xDF) n = 1, cp = c & 0x1F;
-        else if (c >= 0xE0 && c <= 0xEF) n = 2, cp = c & 0x0F;
-        else if (c >= 0xF0 && c <= 0xF4) n = 3, cp = c & 0x07;
-        else return false;
-        if (end - p <= n) return false;
-        for (int i = 1; i <= n; i++) {
-            if ((p[i] & 0xC0) != 0x80) return false;
-            cp = (cp << 6) | (p[i] & 0x3F);
-        }
-        if (n == 2 && (cp < 0x800 || (cp >= 0xD800 && cp <= 0xDFFF))) return false;
-        if (n == 3 && (cp < 0x10000 || cp > 0x10FFFF)) return false;
-        p += n + 1;
-    }
-    return true;
-}
-
-bool rd_string(Rd& r, uint32_t wt, const uint8_t* base, uint32_t& off, uint32_t& len) {
-    Rd s;
-    if (wt != 2 || !rd_len(r, s) || !utf8_ok(s.p, s.end)) return false;
-    off = (uint32_t)(s.p - base);
-    len = (uint32_t)(s.end - s.p);
-    return true;
-}
-
-// RateLimitDescriptor.RateLimitOverride {1: uint32, 2: enum}: only validated (the path ignores it)
-bool decode_override(Rd r) {
-    while (r.p < r.end) {
-        uint32_t tag, wt;
-        uint64_t v;
-        if (!rd_key(r, tag, wt)) return false;
-        if (tag == 1 || tag == 2) {
-            if (wt != 0 || !rd_varint(r, v)) return false;
-        } else if (!rd_skip(r, tag, wt, 0)) {
-            return false;
-        }
-    }
-    return true;
-}
-
-struct EntrySink {
-    rl_rls_entry* out;
-    uint32_t cap;
-    uint32_t n = 0;
-};
-
-bool decode_entry(Rd r, const uint8_t* base, uint32_t descriptor, EntrySink& sink) {
-    rl_rls_entry e{descriptor, 0, 0, 0, 0};
-    while (r.p < r.end) {
-        uint32_t tag, wt;
-        if (!rd_key(r, tag, wt)) return false;
-        if (tag == 1) {
-            if (!rd_string(r, wt, base, e.key_off, e.key_len)) return false;
-        } else if (tag == 2) {
-            if (!rd_string(r, wt, base, e.val_off, e.val_len)) return false;
-        } else if (!rd_skip(r, tag, wt, 0)) {
-            return false;
-        }
-    }
-    if (sink.n < sink.cap) sink.out[sink.n] = e;
-    sink.n++;
-    return true;
-}
-
-bool decode_descriptor(Rd r, const uint8_t* base, uint32_t descriptor, EntrySink& sink) {
-    while (r.p < r.end) {
-        uint32_t tag, wt;
-        Rd sub;
-        if (!rd_key(r, tag, wt)) return false;
-        if (tag == 1) {
-            if (wt != 2 || !rd_len(r, sub) || !decode_entry(sub, base, descriptor, sink)) return false;
-        } else if (tag == 2) {
-            if (wt != 2 || !rd_len(r, sub) || !decode_override(sub)) return false;
-        } else if (!rd_skip(r, tag, wt, 0)) {
-            return false;
-        }
-    }
-    return true;
-}
-
-bool decode_request(const uint8_t* buf, uint64_t len, rl_rls_request& q, EntrySink& sink) {
-    if (len > 0xFFFFFFFFull) return false;
-    Rd r{buf, buf + len};
-    q = rl_rls_request{0, 0, 0, 0, 0};
-    while (r.p < r.end) {
-        uint32_t tag, wt;
-        Rd sub;
-        uint64_t v;
-        if (!rd_key(r, tag, wt)) return false;
-        if (tag == 1) {  // string domain = 1 (a repeated occurrence replaces the earlier one)
-            if (!rd_string(r, wt, buf, q.domain_off, q.domain_len)) return false;
-        } else if (tag == 2) {  // repeated RateLimitDescriptor descriptors = 2
-            if (wt != 2 || !rd_len(r, sub) || !decode_descriptor(sub, buf, q.n_descriptors, sink)) return false;
-            q.n_descriptors++;
-        } else if (tag == 3) {  // uint32 hits_addend = 3
-            if (wt != 0 || !rd_varint(r, v)) return false;
-            q.hits_addend = (uint32_t)v;
-        } else if (!rd_skip(r, tag, wt, 0)) {
-            return false;
-        }
-    }
-    q.n_entries = sink.n;
-    return true;
-}
+// the protobuf reader (rl_wire.h) is shared with the device plan
+using rl_wire::decode_request;
+using rl_wire::EntrySink;
 
 // ---- encoding ----------------------------------------------------------------------------------------------------
 void put_varint(std::vector<uint8_t>& o, uint64_t v) {
@@ -331,8 +177,6 @@ struct NsCounts {
     uint64_t authorized_calls = 0, authorized_hits = 0, limited_calls = 0;
 };
 
-enum : uint8_t { REQ_BAD_WIRE = 1, REQ_UNKNOWN_DOMAIN = 2, REQ_NO_LIMITS = 3, REQ_STORE = 4, REQ_UNSUPPORTED = 5 };
-
 struct ReqPlan {
     uint8_t kind = 0;
     uint32_t hits = 1;
@@ -368,6 +212,7 @@ struct rl_rls {
     int header_mode = RL_RLS_HEADERS_NONE;
     bool use_limit_name = false;
     Pool* pool = nullptr;
+    rl_rls_dev* dev = nullptr;  // the device plan's state (rl_rls_dev.cu), created by the first device plan
     std::string last_error;
 
     // the batch
@@ -653,6 +498,72 @@ void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uin
     }
 }
 
+int check_batch(rl_rls* s, int method, uint64_t n, const uint64_t* off) {
+    if (method != RL_RLS_SHOULD_RATE_LIMIT && method != RL_RLS_CHECK_RATE_LIMIT && method != RL_RLS_REPORT)
+        return sfail(s, "unknown method %d", method);
+    for (uint64_t i = 0; i < n; i++)
+        if (off[i + 1] < off[i]) return sfail(s, "request offsets must be non-decreasing (request %llu)", (unsigned long long)i);
+    return RL_OK;
+}
+
+// Stage 1 on the engine's device (rl_rls_dev.cu).  Leaves the service as rl_rls_plan does, except for what the kernels
+// wrote: the per-request outcomes are taken in by take_device_plan, and the CSR is copied to the host only with copy_csr
+// (rl_rls_plan_device; rl_rls_serve keeps it on the device).
+int plan_on_device(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us, bool copy_csr,
+                   const RlsDevReq*& req, uint64_t& n_ctr) {
+    if (!s->engine) return sfail(s, "the device plan needs a service created with an engine");
+    if (!rl_rls_dev_plan) return sfail(s, "this build of the library has no device plan");
+    int r = check_batch(s, method, n, off);
+    if (r) return r;
+    s->planned = s->finished = false;
+    s->method = method;
+    s->n = n;
+    const uint64_t now = now_us ? now_us : wall_us();
+    uint64_t n_store = 0;
+    r = rl_rls_dev_plan(&s->dev, s->engine, s->m, method, n, buf, off, now, &n_store, &n_ctr, &req);
+    if (r) {
+        s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
+        return r;
+    }
+    s->n_store = n_store;
+    s->load_counters = (method == RL_RLS_SHOULD_RATE_LIMIT && s->header_mode != RL_RLS_HEADERS_NONE) ? 1 : 0;  // server.rs:146
+    if (copy_csr) {
+        s->ctr_off.resize(n_store + 1);
+        s->ctrs.ensure(n_ctr);
+        s->delta.resize(n_store);
+        s->now.assign(n_store, now);
+        if ((r = rl_rls_dev_copy_plan(s->dev, s->ctr_off.data(), s->ctrs.data(), s->delta.data()))) {
+            s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
+            return r;
+        }
+    }
+    return RL_OK;
+}
+
+// The per-request outcomes of a device plan (in host memory once rl_rls_dev_copy_plan / _wait returned) into the
+// service's plan, store index and domains, on the worker pool.
+void take_device_plan(rl_rls* s, const RlsDevReq* req, const uint8_t* buf, const uint64_t* off) {
+    s->plan.resize(s->n);
+    s->domains.resize(s->n);
+    s->store_index.resize(s->n);
+    s->pool->run([&](uint32_t w) {
+        uint64_t lo, hi;
+        range_of(s->n, s->pool->n, w, lo, hi);
+        for (uint64_t i = lo; i < hi; i++) {
+            const RlsDevReq& R = req[i];
+            ReqPlan& P = s->plan[i];
+            P.kind = (uint8_t)R.kind;
+            P.hits = R.hits;
+            P.n_ctr = 0;  // (read by the CPU plan's scatter only)
+            P.store = R.store;
+            s->store_index[i] = R.store;
+            if (R.kind == REQ_BAD_WIRE) s->domains[i].clear();
+            else s->domains[i].assign((const char*)buf + off[i] + R.dom_off, R.dom_len);
+        }
+    });
+    s->planned = true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -692,6 +603,7 @@ int rl_rls_create(rl_matcher* m, rl_engine* engine, int header_mode, uint32_t th
 
 void rl_rls_destroy(rl_rls* s) {
     if (!s) return;
+    if (s->dev && rl_rls_dev_destroy) rl_rls_dev_destroy(s->dev);
     delete s->pool;
     delete s;
 }
@@ -700,10 +612,8 @@ const char* rl_rls_last_error(rl_rls* s) { return s ? s->last_error.c_str() : "n
 
 int rl_rls_plan(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
     if (!s || (n && (!off || !buf))) return RL_FATAL;
-    if (method != RL_RLS_SHOULD_RATE_LIMIT && method != RL_RLS_CHECK_RATE_LIMIT && method != RL_RLS_REPORT)
-        return sfail(s, "unknown method %d", method);
-    for (uint64_t i = 0; i < n; i++)
-        if (off[i + 1] < off[i]) return sfail(s, "request offsets must be non-decreasing (request %llu)", (unsigned long long)i);
+    int r = check_batch(s, method, n, off);
+    if (r) return r;
     s->planned = s->finished = false;
     s->method = method;
     s->n = n;
@@ -732,6 +642,16 @@ int rl_rls_plan(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uin
     s->now.assign(s->n_store, now_us ? now_us : wall_us());
     s->load_counters = (method == RL_RLS_SHOULD_RATE_LIMIT && s->header_mode != RL_RLS_HEADERS_NONE) ? 1 : 0;  // server.rs:146
     s->planned = true;
+    return RL_OK;
+}
+
+int rl_rls_plan_device(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!s || (n && (!off || !buf))) return RL_FATAL;
+    const RlsDevReq* req = nullptr;
+    uint64_t n_ctr = 0;
+    const int r = plan_on_device(s, method, n, buf, off, now_us, true, req, n_ctr);
+    if (r) return r;
+    take_device_plan(s, req, buf, off);
     return RL_OK;
 }
 
@@ -797,36 +717,39 @@ int rl_rls_responses(rl_rls* s, const uint8_t** out_buf, const uint64_t** out_of
 int rl_rls_serve(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
     if (!s) return RL_FATAL;
     if (!s->engine) return sfail(s, "the service was created without an engine: there is no CPU store to fall back to");
+    if (n && (!off || !buf)) return RL_FATAL;
+    // plan on the device: the store call's CSR stays there
     const double t0 = mono_us();
-    int r = rl_rls_plan(s, method, n, buf, off, now_us);
+    const RlsDevReq* req = nullptr;
+    uint64_t n_ctr = 0;
+    int r = plan_on_device(s, method, n, buf, off, now_us, false, req, n_ctr);
     if (r) return r;
     const double t1 = mono_us();
-    int st = RL_OK;
-    if (s->n_store) {
-        const uint64_t m = s->n_store;
-        s->o_limited.assign(m, 0);
-        s->o_first.assign(m, RL_NONE);
-        if (s->load_counters) {
-            s->o_rem.assign(s->ctrs.size(), 0);  // (slots of a refused call stay 0)
-            s->o_ttl.assign(s->ctrs.size(), 0);
-        }
-        if (method == RL_RLS_SHOULD_RATE_LIMIT)
-            st = rl_check_and_update_batch(s->engine, m, s->ctr_off.data(), s->ctrs.data(), s->delta.data(), s->now.data(),
-                                           s->load_counters, RL_MEM_HOST, s->o_limited.data(), s->o_first.data(),
-                                           s->load_counters ? s->o_rem.data() : nullptr, s->load_counters ? s->o_ttl.data() : nullptr);
-        else if (method == RL_RLS_CHECK_RATE_LIMIT)
-            st = rl_is_within_limits_batch(s->engine, m, s->ctr_off.data(), s->ctrs.data(), s->delta.data(), s->now.data(),
-                                           RL_MEM_HOST, s->o_limited.data(), s->o_first.data());
-        else
-            st = rl_update_batch(s->engine, m, s->ctr_off.data(), s->ctrs.data(), s->delta.data(), s->now.data(), RL_MEM_HOST);
-        if (st != RL_OK) s->last_error = std::string("store call failed: ") + rl_last_error(s->engine);
+    // the store call on the device arrays; only what the finish reads comes back
+    const uint64_t m = s->n_store;
+    s->o_limited.resize(m);
+    s->o_first.resize(m);
+    if (s->load_counters) {
+        s->o_rem.resize(n_ctr);
+        s->o_ttl.resize(n_ctr);
+        s->ctr_off.resize(m + 1);
+        s->ctrs.ensure(n_ctr);
+    }
+    const int st = rl_rls_dev_decide(s->dev, s->engine, method, s->load_counters, s->o_limited.data(), s->o_first.data(),
+                                     s->o_rem.data(), s->o_ttl.data(), s->ctr_off.data(), s->ctrs.data());
+    if (st != RL_OK) s->last_error = std::string("store call failed: ") + rl_last_error(s->engine);
+    if ((r = rl_rls_dev_wait(s->dev))) {
+        s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
+        return r;
     }
     const double t2 = mono_us();
-    r = rl_rls_finish(s, st, s->o_limited.data(), s->o_first.data(), s->o_rem.data(), s->o_ttl.data());
+    take_device_plan(s, req, buf, off);
     const double t3 = mono_us();
-    s->t_plan = t1 - t0;
+    r = rl_rls_finish(s, st, s->o_limited.data(), s->o_first.data(), s->o_rem.data(), s->o_ttl.data());
+    const double t4 = mono_us();
+    s->t_plan = (t1 - t0) + (t3 - t2);
     s->t_store = t2 - t1;
-    s->t_finish = t3 - t2;
+    s->t_finish = t4 - t3;
     return r;
 }
 

@@ -1,0 +1,289 @@
+// rl_rls_dev.cu — host side of the RLS device plan (rl_rls_dev.h; kernels in rl_rls_dev.cuh).  A translation unit of its
+// own: it sees an engine only through rl_internal.h and the public C-ABI, and a matcher only through its image.
+//
+// One plan: wire bytes and offsets -> pinned staging -> device (engine's stream); k_rls_plan; CUB exclusive sum; ONE
+// device->host read of the totals (the store request and counter counts); k_rls_scatter; the per-request array back
+// into pinned memory.  The store call then reads the CSR where it lies (RL_MEM_DEVICE).
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdarg>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include <cub/device/device_scan.cuh>
+
+#include "rl_internal.h"
+#include "rl_rls_dev.cuh"
+
+namespace {
+
+// device array that only grows
+template <class T>
+struct DBuf {
+    T* p = nullptr;
+    size_t cap = 0;
+    cudaError_t reserve(size_t n) {
+        if (p && n <= cap) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        const size_t want = std::max<size_t>(n + n / 2, 64);
+        const cudaError_t r = cudaMalloc((void**)&p, want * sizeof(T));
+        if (r == cudaSuccess) cap = want;
+        return r;
+    }
+    ~DBuf() {
+        if (p) cudaFree(p);
+    }
+};
+
+// pinned host array that only grows
+template <class T>
+struct HBuf {
+    T* p = nullptr;
+    size_t cap = 0;
+    cudaError_t reserve(size_t n) {
+        if (p && n <= cap) return cudaSuccess;
+        if (p) cudaFreeHost(p);
+        p = nullptr;
+        cap = 0;
+        const size_t want = std::max<size_t>(n + n / 2, 64);
+        const cudaError_t r = cudaMallocHost((void**)&p, want * sizeof(T));
+        if (r == cudaSuccess) cap = want;
+        return r;
+    }
+    ~HBuf() {
+        if (p) cudaFreeHost(p);
+    }
+};
+
+}  // namespace
+
+struct rl_rls_dev {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    std::string err;
+    // the matcher image: host copy (its header places the sections) and device copy
+    uint64_t gen = 0;
+    std::vector<uint32_t> image;
+    DBuf<uint32_t> d_image;
+    // the batch
+    uint64_t n = 0, n_store = 0, n_ctr = 0;
+    HBuf<uint8_t> h_buf;
+    HBuf<uint64_t> h_off;
+    HBuf<RlsDevReq> h_req;
+    HBuf<unsigned long long> h_total;
+    DBuf<uint8_t> d_buf, d_cub;
+    DBuf<uint64_t> d_off;
+    DBuf<rl_rls_entry> d_ent;
+    DBuf<rl_counter> d_scratch, d_ctrs;
+    DBuf<RlsDevReq> d_req;
+    DBuf<unsigned long long> d_count, d_start;
+    DBuf<uint32_t> d_ctr_off;
+    DBuf<uint64_t> d_delta, d_now;
+    // store call outputs
+    DBuf<uint8_t> d_lim;
+    DBuf<uint32_t> d_first;
+    DBuf<uint64_t> d_rem, d_ttl;
+};
+
+namespace {
+
+int dev_fail(rl_rls_dev* S, int status, const char* fmt, ...) {
+    char b[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(b, sizeof b, fmt, ap);
+    va_end(ap);
+    S->err = b;
+    return status;
+}
+
+#define RLS_CUDA(S, call)                                                                                                   \
+    do {                                                                                                                    \
+        const cudaError_t _r = (call);                                                                                      \
+        if (_r != cudaSuccess)                                                                                              \
+            return dev_fail((S), _r == cudaErrorMemoryAllocation ? RL_TRANSIENT : RL_FATAL, "CUDA error %s at %s:%d (%s)", \
+                            cudaGetErrorName(_r), __FILE__, __LINE__, cudaGetErrorString(_r));                              \
+    } while (0)
+
+uint32_t blocks_for(uint64_t n, uint32_t threads) { return (uint32_t)((n + threads - 1) / threads); }
+
+// upload the matcher's image when its generation moved since the last batch
+int refresh_image(rl_rls_dev* S, rl_matcher* m) {
+    const uint64_t g = rl_matcher_generation(m);
+    if (g == S->gen && !S->image.empty()) return RL_OK;
+    if (S->image.size() < 1024) S->image.resize(1024);
+    uint64_t need = 0, got = 0;
+    while (rl_matcher_image(m, S->image.data(), S->image.size(), &need, &got) != RL_OK) {
+        if (need <= S->image.size()) return dev_fail(S, RL_FATAL, "the matcher image could not be taken");
+        S->image.resize(need);
+    }
+    S->image.resize(need);
+    RLS_CUDA(S, S->d_image.reserve(need));
+    RLS_CUDA(S, cudaMemcpyAsync(S->d_image.p, S->image.data(), need * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
+    S->gen = got;
+    return RL_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, uint64_t n, const uint8_t* buf,
+                    const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                    const RlsDevReq** out_req) {
+    if (!st || !e || !m || !out_n_store || !out_n_ctr || !out_req) return RL_FATAL;
+    if (!*st) *st = new rl_rls_dev();
+    rl_rls_dev* S = *st;
+    S->n = S->n_store = S->n_ctr = 0;
+    RlTableView v;
+    int r = rl_internal_view(e, &v);  // the engine's device and stream (every earlier pipelined call is fenced)
+    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
+    S->device = v.device;
+    S->stream = v.stream;
+    if ((r = refresh_image(S, m))) return r;
+    const uint32_t engine_max = rl_engine_max_counters_per_request(e);
+    const uint32_t per_req = std::min(S->image[RL_IMG_H_COUNTER_CAP], engine_max);
+    if (n && (n + 1) * (uint64_t)per_req >= (1ull << 32))
+        return dev_fail(S, RL_FATAL, "a batch of %llu requests of up to %u counters each may exceed 2^32 counters",
+                        (unsigned long long)n, per_req);
+    const uint64_t bytes = n ? off[n] : 0;
+    // wire bytes and offsets through pinned staging onto the device
+    RLS_CUDA(S, S->h_buf.reserve(bytes + 1));
+    RLS_CUDA(S, S->h_off.reserve(n + 1));
+    RLS_CUDA(S, S->h_req.reserve(n + 1));
+    RLS_CUDA(S, S->h_total.reserve(1));
+    if (bytes) memcpy(S->h_buf.p, buf, bytes);
+    memcpy(S->h_off.p, off, (n + 1) * sizeof(uint64_t));
+    RLS_CUDA(S, S->d_buf.reserve(bytes + 1));
+    RLS_CUDA(S, S->d_off.reserve(n + 1));
+    RLS_CUDA(S, S->d_ent.reserve(bytes / 2 + 1));
+    RLS_CUDA(S, S->d_scratch.reserve(n * (uint64_t)per_req + 1));
+    RLS_CUDA(S, S->d_req.reserve(n + 1));
+    RLS_CUDA(S, S->d_count.reserve(n + 1));
+    RLS_CUDA(S, S->d_start.reserve(n + 1));
+    if (bytes) RLS_CUDA(S, cudaMemcpyAsync(S->d_buf.p, S->h_buf.p, bytes, cudaMemcpyHostToDevice, S->stream));
+    RLS_CUDA(S, cudaMemcpyAsync(S->d_off.p, S->h_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+    RlsPlanArgs a;
+    a.buf = S->d_buf.p;
+    a.off = S->d_off.p;
+    a.n = n;
+    a.img = rl_img_view(S->image.data(), S->d_image.p);
+    a.per_req = per_req;
+    a.ent = S->d_ent.p;
+    a.scratch = S->d_scratch.p;
+    a.req = S->d_req.p;
+    a.count = S->d_count.p;
+    const uint32_t threads = 128;
+    k_rls_plan<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
+    RLS_CUDA(S, cudaGetLastError());
+    size_t tmp = 0;
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
+    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
+    // the one read before the store call: how many store requests and counters the batch has
+    RLS_CUDA(S, cudaMemcpyAsync(S->h_total.p, S->d_start.p + n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S->stream));
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    const uint64_t n_store = S->h_total.p[0] >> 32, n_ctr = S->h_total.p[0] & 0xFFFFFFFFull;
+    RLS_CUDA(S, S->d_ctr_off.reserve(n_store + 1));
+    RLS_CUDA(S, S->d_ctrs.reserve(n_ctr + 1));
+    RLS_CUDA(S, S->d_delta.reserve(n_store + 1));
+    RLS_CUDA(S, S->d_now.reserve(n_store + 1));
+    RlsScatterArgs b;
+    b.req = S->d_req.p;
+    b.scratch = S->d_scratch.p;
+    b.start = S->d_start.p;
+    b.n = n;
+    b.per_req = per_req;
+    b.method = method;
+    b.now_us = now_us;
+    b.ctr_off = S->d_ctr_off.p;
+    b.ctrs = S->d_ctrs.p;
+    b.delta = S->d_delta.p;
+    b.now = S->d_now.p;
+    k_rls_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
+    RLS_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, 2);
+    if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_req.p, S->d_req.p, n * sizeof(RlsDevReq), cudaMemcpyDeviceToHost, S->stream));
+    S->n = n;
+    S->n_store = n_store;
+    S->n_ctr = n_ctr;
+    *out_n_store = n_store;
+    *out_n_ctr = n_ctr;
+    *out_req = S->h_req.p;
+    return RL_OK;
+}
+
+int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta) {
+    if (!S) return RL_FATAL;
+    RLS_CUDA(S, cudaSetDevice(S->device));
+    RLS_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_ctr) RLS_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_store) RLS_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    return RL_OK;
+}
+
+int rl_rls_dev_decide(rl_rls_dev* S, rl_engine* e, int method, int load_counters, uint8_t* limited, uint32_t* first_limited,
+                      uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
+    if (!S || !e) return RL_FATAL;
+    const uint64_t m = S->n_store, nc = S->n_ctr;
+    if (m == 0) return RL_OK;
+    RLS_CUDA(S, cudaSetDevice(S->device));
+    RLS_CUDA(S, S->d_lim.reserve(m));
+    RLS_CUDA(S, S->d_first.reserve(m));
+    if (load_counters) {
+        RLS_CUDA(S, S->d_rem.reserve(nc + 1));
+        RLS_CUDA(S, S->d_ttl.reserve(nc + 1));
+        // (slots of a refused call stay 0, as with host buffers)
+        RLS_CUDA(S, cudaMemsetAsync(S->d_rem.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+        RLS_CUDA(S, cudaMemsetAsync(S->d_ttl.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+    }
+    int st;
+    if (method == RL_RLS_SHOULD_RATE_LIMIT)
+        st = rl_check_and_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, load_counters, RL_MEM_DEVICE,
+                                       S->d_lim.p, S->d_first.p, load_counters ? S->d_rem.p : nullptr,
+                                       load_counters ? S->d_ttl.p : nullptr);
+    else if (method == RL_RLS_CHECK_RATE_LIMIT)
+        st = rl_is_within_limits_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, RL_MEM_DEVICE, S->d_lim.p,
+                                       S->d_first.p);
+    else
+        st = rl_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, RL_MEM_DEVICE);
+    if (st == RL_OK) st = rl_sync(e);  // a device-memory call reports its deferred errors here
+    if (st != RL_OK) return st;
+    if (method != RL_RLS_REPORT) {
+        if (cudaMemcpyAsync(limited, S->d_lim.p, m, cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(first_limited, S->d_first.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
+            return dev_fail(S, RL_FATAL, "copying the verdicts back failed");
+    }
+    if (load_counters) {
+        if (cudaMemcpyAsync(remaining, S->d_rem.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ttl_us, S->d_ttl.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (m + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ctrs, S->d_ctrs.p, nc * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
+            return dev_fail(S, RL_FATAL, "copying the counters back failed");
+    }
+    return RL_OK;
+}
+
+int rl_rls_dev_wait(rl_rls_dev* S) {
+    if (!S) return RL_FATAL;
+    RLS_CUDA(S, cudaSetDevice(S->device));
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    return RL_OK;
+}
+
+const char* rl_rls_dev_error(rl_rls_dev* S) { return S ? S->err.c_str() : "no device plan state"; }
+
+void rl_rls_dev_destroy(rl_rls_dev* S) {
+    if (!S) return;
+    cudaSetDevice(S->device);
+    if (S->stream) cudaStreamSynchronize(S->stream);
+    delete S;
+}
+
+}  // extern "C"

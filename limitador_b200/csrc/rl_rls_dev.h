@@ -1,0 +1,41 @@
+// rl_rls_dev.h — what the RLS service (rl_rls.cpp) and the device plan (rl_rls_dev.cu, kernels in rl_rls_dev.cuh) share.
+// Library-internal.  rl_rls.cpp reaches the rl_rls_dev_* functions through weak references, so that the wire surface still
+// links without the CUDA units (the sanitizer build of tests/san): there they are null and only the CPU plan exists.
+#pragma once
+#include <stdint.h>
+
+#include "../../include/rl_rls.h"
+
+// what the plan decided for one request
+enum : uint8_t { REQ_BAD_WIRE = 1, REQ_UNKNOWN_DOMAIN = 2, REQ_NO_LIMITS = 3, REQ_STORE = 4, REQ_UNSUPPORTED = 5 };
+
+// One request of a device plan, as the finish reads it: its kind, hits (hits_addend, 0 -> 1), position in the store
+// call (RL_RLS_NO_STORE if none) and its domain's byte range inside the message.
+struct RlsDevReq {
+    uint32_t kind, hits, store, dom_off, dom_len;
+};
+
+struct rl_rls_dev;  // per-service device state: the matcher image, staging and scratch buffers
+
+extern "C" {
+// Stage 1 on the engine's device and stream: the wire bytes go up through a pinned staging buffer, the kernels decode,
+// match and lay the store call out in device memory.  Returns after one synchronisation (the read of the batch's store
+// request and counter counts) with the per-request array's address: pinned host memory owned by *st, filled once
+// rl_rls_dev_copy_plan or rl_rls_dev_wait returned, valid until the next plan.  *st is created on first use.  RL_OK or
+// an error status (rl_rls_dev_error).
+int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, uint64_t n, const uint8_t* buf,
+                    const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                    const RlsDevReq** out_req);
+// Host copies of the planned store call: ctr_off [n_store + 1], ctrs [n_ctr], delta [n_store].
+int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta);
+// The store call of the planned batch from its device arrays (RL_MEM_DEVICE), then its outputs copied back: limited and
+// first_limited [n_store] (not for Report), and with load_counters remaining / ttl_us [n_ctr] together with ctr_off
+// [n_store + 1] and ctrs [n_ctr], which the headers are formatted from.  Returns the store call's status;
+// rl_last_error(e) tells why it failed.
+int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counters, uint8_t* limited, uint32_t* first_limited,
+                      uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
+// Wait for everything the plan and the store call enqueued (the per-request array and the outputs are then on the host).
+int rl_rls_dev_wait(rl_rls_dev* st);
+const char* rl_rls_dev_error(rl_rls_dev* st);
+void rl_rls_dev_destroy(rl_rls_dev* st);
+}

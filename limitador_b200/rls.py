@@ -1,9 +1,10 @@
 """ctypes binding of the Envoy RLS v3 wire surface (include/rl_rls.h, csrc/rl_rls.cpp).
 
 `RlsService` serves batches of `envoy.service.ratelimit.v3.RateLimitRequest` wire messages:
-decode + counters_that_apply on a pool of CPU workers, ONE engine call for the whole batch, then
-`RateLimitResponse` bytes (envoy_rls/server.rs:91-208, kuadrant_service.rs:27-186).  `plan`/`finish` are
-the CPU stages on their own (drivable without a GPU); `serve` runs all three through the engine.
+decode + counters_that_apply on the engine's GPU, ONE engine call for the whole batch, then
+`RateLimitResponse` bytes on a pool of CPU workers (envoy_rls/server.rs:91-208, kuadrant_service.rs:27-186).
+`plan`/`finish` are the CPU stages on their own (drivable without a GPU), `plan_device` is the GPU plan on its
+own; `serve` runs plan_device -> engine -> finish.
 `encode_request` / `decode_response` are small pure-Python helpers for callers and tests (the tests
 cross-check them against the protobuf runtime).
 """
@@ -26,7 +27,7 @@ NO_STORE = 0xFFFFFFFF
 RLS_SYMBOLS = (
     "rl_rls_decode_request", "rl_rls_encode_response", "rl_rls_create", "rl_rls_destroy", "rl_rls_last_error",
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
-    "rl_rls_last_timings",
+    "rl_rls_last_timings", "rl_rls_plan_device",
 )
 
 ENTRY_DTYPE = np.dtype([("descriptor", "<u4"), ("key_off", "<u4"), ("key_len", "<u4"), ("val_off", "<u4"), ("val_len", "<u4")])
@@ -54,6 +55,7 @@ def _lib():
     L.rl_rls_last_error.argtypes = [vp]
     L.rl_rls_last_error.restype = C.c_char_p
     L.rl_rls_plan.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_rls_plan_device.argtypes = [vp, i32, u64, vp, vp, u64]
     L.rl_rls_plan_view.argtypes = [vp, C.POINTER(u64), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
                                    C.POINTER(i32), C.POINTER(vp)]
     L.rl_rls_finish.argtypes = [vp, i32, vp, vp, vp, vp]
@@ -210,12 +212,20 @@ class RlsService:
             raise RlsError(self._lib.rl_rls_last_error(self._h).decode())
 
     def plan(self, method: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
-        """Stage 1 -> dict(n_store, ctr_off, ctrs, delta, now_us, load_counters, store_index): copies of the store call."""
+        """Stage 1 on the CPU workers -> dict(n_store, ctr_off, ctrs, delta, now_us, load_counters, store_index): copies of
+        the store call."""
+        return self._plan(self._lib.rl_rls_plan, method, buf, off, now_us)
+
+    def plan_device(self, method: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """Stage 1 on the engine's device (the service needs an engine); the same dict as `plan`, array for array."""
+        return self._plan(self._lib.rl_rls_plan_device, method, buf, off, now_us)
+
+    def _plan(self, fn, method, buf, off, now_us):
         buf = np.ascontiguousarray(buf, dtype=np.uint8)
         off = np.ascontiguousarray(off, dtype=np.uint64)
         n = len(off) - 1
         self._keep = (buf, off)
-        self._check(self._lib.rl_rls_plan(self._h, method, n, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
+        self._check(fn(self._h, method, n, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
         ns = C.c_uint64()
         p_off, p_ctr, p_delta, p_now, p_idx = (C.c_void_p() for _ in range(5))
         lc = C.c_int()
