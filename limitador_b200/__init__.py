@@ -5,8 +5,9 @@ from .limiter import (Authorization, CheckResult, Context, Counter, GpuCounterSt
                       RateLimiter)
 from .matcher import Matcher, MatcherError, counter_key  # noqa: F401
 from .rls import RlsService, RlsError  # noqa: F401
+from .http_api import HttpApi, HttpError  # noqa: F401
 from .crdt import CrdtTable, CrdtError  # noqa: F401
 
 __all__ = ["Engine", "EngineError", "Front", "owner_of", "RateLimiter", "Limit", "Counter", "Context", "CheckResult",
-           "Authorization", "GpuCounterStorage", "Matcher", "MatcherError", "counter_key", "RlsService", "RlsError", "CrdtTable", "CrdtError", "RECORD_DTYPE", "COUNTER_DTYPE",
+           "Authorization", "GpuCounterStorage", "Matcher", "MatcherError", "counter_key", "RlsService", "RlsError", "HttpApi", "HttpError", "CrdtTable", "CrdtError", "RECORD_DTYPE", "COUNTER_DTYPE",
            "LIMIT_DESC_DTYPE", "NONE"]

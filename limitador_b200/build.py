@@ -31,7 +31,7 @@ def _nvcc() -> str:
 
 
 # translation units and what (besides themselves) they are rebuilt for
-_PUBLIC = ("rl_engine.h", "rl_match.h", "rl_rls.h", "rl_crdt.h")
+_PUBLIC = ("rl_engine.h", "rl_match.h", "rl_rls.h", "rl_http.h", "rl_crdt.h")
 _UNITS = {
     "rl_engine.cu": "csrc",   # the kernels' headers live beside it: any change under csrc/ rebuilds it
     "rl_maint.cu": "csrc",

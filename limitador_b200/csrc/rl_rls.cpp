@@ -8,6 +8,8 @@
 // request is independent) —, the counters are laid out as one CSR, the store is called once for the whole batch, and
 // the responses are encoded by the worker pool.  No protobuf runtime: the four message types on the path have a
 // handful of fields, decoded by hand (rl_wire.h, shared with the device plan) and encoded below.
+// The HTTP API (include/rl_http.h) is served by the same stages over JSON bodies (rl_json.h): plan_range and plan_cpu
+// take either surface, the finish and the responses are its own, and it shares the RLS service's workers and metrics.
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -23,6 +25,8 @@
 #include <unordered_map>
 #include <vector>
 
+#include "rl_http.h"
+#include "rl_json.h"
 #include "rl_rls.h"
 #include "rl_rls_dev.h"
 #include "rl_wire.h"
@@ -39,6 +43,13 @@ __attribute__((weak)) int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off
 __attribute__((weak)) int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counters, uint8_t* limited,
                                             uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
                                             rl_counter* ctrs);
+__attribute__((weak)) int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
+                                           const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                                           const HttpDevReq** out_req, const HttpRun** out_runs, uint32_t* out_n_runs);
+__attribute__((weak)) int rl_http_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
+__attribute__((weak)) int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int endpoint, int* run_status, uint8_t* limited,
+                                             uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
+                                             rl_counter* ctrs);
 __attribute__((weak)) int rl_rls_dev_wait(rl_rls_dev* st);
 __attribute__((weak)) const char* rl_rls_dev_error(rl_rls_dev* st);
 __attribute__((weak)) void rl_rls_dev_destroy(rl_rls_dev* st);
@@ -179,9 +190,11 @@ struct NsCounts {
 
 struct ReqPlan {
     uint8_t kind = 0;
-    uint32_t hits = 1;
+    uint8_t hdr = 0;     // HTTP: response_headers (RL_HTTP_HEADERS_*)
+    uint32_t hits = 1;   // RLS: hits_addend, 0 -> 1
     uint32_t n_ctr = 0;
     uint32_t store = RL_RLS_NO_STORE;
+    uint64_t delta = 0;  // HTTP: the body's delta
 };
 
 struct WorkerOut {
@@ -189,6 +202,7 @@ struct WorkerOut {
     RawBuf<rl_counter> ctrs;            // the range's counters, request after request (ctr_off)
     std::vector<rl_rls_entry> entries;
     RawBuf<char> arena;                 // NUL-terminated copies of the keys and values (the bindings point into it)
+    RawBuf<uint8_t> txt, bits;          // HTTP: one body's unescaped strings and skip stack (rl_json.h)
     uint64_t n_store = 0;               // requests of the range that reach the store
     std::vector<rl_binding> binds;
     std::vector<uint32_t> bind_off, ctr_off;
@@ -200,6 +214,8 @@ struct WorkerOut {
     std::vector<uint64_t> resp_len;     // one per request of the worker's range
     std::vector<char> hdr;              // header values of the range's store requests (rl_matcher_response_headers_batch)
     std::vector<uint64_t> hdr_off;
+    std::vector<uint8_t> hval;          // HTTP: the range's X-RateLimit-* values, three per request (hval_len)
+    std::vector<uint64_t> hval_len;
     std::unordered_map<std::string, NsCounts> by_ns;  // the range's metrics, merged into the service's after the workers
     std::map<std::pair<std::string, std::string>, uint64_t> limited_by_name;
 };
@@ -244,9 +260,48 @@ struct rl_rls {
     double t_plan = 0, t_store = 0, t_finish = 0;
 };
 
+// The HTTP API (include/rl_http.h) over an RLS service: its own batch, the service's matcher, engine, workers, device
+// state and metrics.  The member names are the RLS service's, so that the plan stages below serve both.
+struct rl_http {
+    rl_rls* rls = nullptr;
+    rl_matcher* m = nullptr;
+    rl_engine* engine = nullptr;
+    Pool* pool = nullptr;
+    std::string last_error;
+
+    // the batch
+    int method = 0;  // the endpoint
+    uint64_t n = 0;
+    const uint8_t* buf = nullptr;  // only dereferenced during plan
+    bool planned = false, finished = false;
+    std::vector<ReqPlan> plan;
+    std::vector<std::string> domains;  // every body's namespace, unescaped
+    std::vector<WorkerOut> wout;
+    std::vector<uint32_t> store_index;
+    // store requests
+    uint64_t n_store = 0;
+    std::vector<uint32_t> ctr_off;
+    RawBuf<rl_counter> ctrs;
+    std::vector<uint64_t> delta, now;
+    std::vector<uint8_t> load;
+    // engine outputs (serve)
+    std::vector<int> run_status;
+    std::vector<int32_t> o_status;
+    std::vector<uint8_t> o_limited;
+    std::vector<uint32_t> o_first;
+    std::vector<uint64_t> o_rem, o_ttl;
+    // responses
+    std::vector<uint16_t> status;
+    RawBuf<uint8_t> body, hval;
+    std::vector<uint64_t> body_off, hval_off;
+    double t_plan = 0, t_store = 0, t_finish = 0;
+    uint32_t store_calls = 0;
+};
+
 namespace {
 
-int sfail(rl_rls* s, const char* fmt, ...) {
+template <class Svc>
+int sfail(Svc* s, const char* fmt, ...) {
     char b[512];
     va_list ap;
     va_start(ap, fmt);
@@ -263,10 +318,70 @@ void range_of(uint64_t n, uint32_t workers, uint32_t w, uint64_t& lo, uint64_t& 
     hi = std::min<uint64_t>(n, lo + per);
 }
 
+// Decode request i of an RLS batch (one wire message) into the worker's entries.  false: the request never reaches the
+// matcher (its kind is set); true: its context is `sink`'s entries and its namespace base[ns_off .. ns_off + ns_len).
+bool decode_one(rl_rls* s, const uint64_t* off, uint64_t i, WorkerOut& W, ReqPlan& P, EntrySink& sink, const uint8_t*& base,
+                uint32_t& ns_off, uint32_t& ns_len) {
+    const uint8_t* msg = s->buf + off[i];
+    const uint64_t len = off[i + 1] - off[i];
+    rl_rls_request q;
+    if (W.entries.size() < 16) W.entries.resize(16);
+    sink = EntrySink{W.entries.data(), (uint32_t)W.entries.size(), 0};
+    if (!decode_request(msg, len, q, sink)) {
+        P.kind = REQ_BAD_WIRE;
+        return false;
+    }
+    if (sink.n > sink.cap) {  // rare: more entries than the scratch holds — decode again into a larger one
+        W.entries.resize(sink.n);
+        sink = EntrySink{W.entries.data(), (uint32_t)W.entries.size(), 0};
+        decode_request(msg, len, q, sink);
+    }
+    P.hits = q.hits_addend ? q.hits_addend : 1;  // server.rs:131-135
+    s->domains[i].assign((const char*)msg + q.domain_off, q.domain_len);
+    if (q.domain_len == 0) {  // server.rs:106-116
+        P.kind = REQ_UNKNOWN_DOMAIN;
+        return false;
+    }
+    base = msg;
+    ns_off = q.domain_off;
+    ns_len = q.domain_len;
+    return true;
+}
+
+// The same for body i of an HTTP batch (rl_json.h): the strings are unescaped into the worker's txt, which `base` is.
+bool decode_one(rl_http* h, const uint64_t* off, uint64_t i, WorkerOut& W, ReqPlan& P, EntrySink& sink, const uint8_t*& base,
+                uint32_t& ns_off, uint32_t& ns_len) {
+    const uint8_t* body = h->buf + off[i];
+    const uint64_t len = off[i + 1] - off[i];
+    W.txt.ensure(len + 1);
+    W.bits.ensure(len / 8 + 1);
+    rl_json::Info q;
+    if (W.entries.size() < 16) W.entries.resize(16);
+    sink = EntrySink{W.entries.data(), (uint32_t)W.entries.size(), 0};
+    if (!rl_json::decode_info(body, len, W.txt.data(), W.bits.data(), q, sink)) {
+        P.kind = REQ_BAD_WIRE;
+        return false;
+    }
+    if (sink.n > sink.cap) {
+        W.entries.resize(sink.n);
+        sink = EntrySink{W.entries.data(), (uint32_t)W.entries.size(), 0};
+        rl_json::decode_info(body, len, W.txt.data(), W.bits.data(), q, sink);
+    }
+    P.delta = q.delta;
+    P.hdr = (uint8_t)q.headers;
+    h->domains[i].assign((const char*)W.txt.data() + q.ns_off, q.ns_len);
+    base = W.txt.data();
+    ns_off = q.ns_off;
+    ns_len = q.ns_len;
+    return true;
+}
+
 // Requests [lo, hi) of worker w: decode every message and lay its CEL context out (pass 1), then ONE matcher call for
 // the whole range (pass 2) — a reader section per range, not per request: eight workers taking the matcher's
-// reader/writer lock twice per request spent their time passing its cache line around and did not scale at all.
-void plan_range(rl_rls* s, const uint64_t* off, uint32_t w) {
+// reader/writer lock twice per request spent their time passing its cache line around and did not scale at all.  The
+// same body for both surfaces: only decode_one differs.
+template <class Svc>
+void plan_range(Svc* s, const uint64_t* off, uint32_t w) {
     uint64_t lo, hi;
     range_of(s->n, s->pool->n, w, lo, hi);
     WorkerOut& W = s->wout[w];
@@ -282,27 +397,11 @@ void plan_range(rl_rls* s, const uint64_t* off, uint32_t w) {
     for (uint64_t i = lo; i < hi; i++) {
         ReqPlan& P = s->plan[i];
         P = ReqPlan();
-        const uint8_t* msg = s->buf + off[i];
-        const uint64_t len = off[i + 1] - off[i];
-        rl_rls_request q;
-        if (W.entries.size() < 16) W.entries.resize(16);
-        EntrySink sink{W.entries.data(), (uint32_t)W.entries.size()};
-        if (!decode_request(msg, len, q, sink)) {
-            P.kind = REQ_BAD_WIRE;
-            continue;
-        }
-        if (sink.n > sink.cap) {  // rare: more entries than the scratch holds — decode again into a larger one
-            W.entries.resize(sink.n);
-            sink = EntrySink{W.entries.data(), (uint32_t)W.entries.size()};
-            decode_request(msg, len, q, sink);
-        }
-        P.hits = q.hits_addend ? q.hits_addend : 1;  // server.rs:131-135
-        s->domains[i].assign((const char*)msg + q.domain_off, q.domain_len);
-        if (q.domain_len == 0) {  // server.rs:106-116
-            P.kind = REQ_UNKNOWN_DOMAIN;
-            continue;
-        }
-        if (memchr(msg + q.domain_off, 0, q.domain_len) != nullptr) {
+        EntrySink sink{nullptr, 0, 0};
+        const uint8_t* msg = nullptr;
+        uint32_t ns_off = 0, ns_len = 0;
+        if (!decode_one(s, off, i, W, P, sink, msg, ns_off, ns_len)) continue;
+        if (memchr(msg + ns_off, 0, ns_len) != nullptr) {
             P.kind = REQ_NO_LIMITS;  // no namespace the matcher knows holds a NUL: nothing applies (lib.rs:434-440)
             continue;
         }
@@ -357,9 +456,15 @@ void plan_range(rl_rls* s, const uint64_t* off, uint32_t w) {
     }
 }
 
+// the delta of a store request: CheckRateLimit asks with delta 1 whatever hits_addend says (kuadrant_service.rs:62-65);
+// HTTP sends the body's own delta, also for /check (server.rs:144)
+uint64_t store_delta(const rl_rls* s, const ReqPlan& P) { return s->method == RL_RLS_CHECK_RATE_LIMIT ? 1 : P.hits; }
+uint64_t store_delta(const rl_http*, const ReqPlan& P) { return P.delta; }
+
 // Second pass of the plan: worker w copies its counters into the batch's CSR at the offsets the prefix over the workers
 // gave it (store requests in batch order: worker ranges are consecutive).
-void plan_scatter(rl_rls* s, uint32_t w, uint64_t store_base, uint64_t ctr_base) {
+template <class Svc>
+void plan_scatter(Svc* s, uint32_t w, uint64_t store_base, uint64_t ctr_base) {
     WorkerOut& W = s->wout[w];
     uint64_t j = store_base, c = ctr_base;
     for (uint64_t k = 0; k < W.req_of.size(); k++) {
@@ -370,8 +475,7 @@ void plan_scatter(rl_rls* s, uint32_t w, uint64_t store_base, uint64_t ctr_base)
         s->store_index[i] = (uint32_t)j;
         s->ctr_off[j] = (uint32_t)c;
         memcpy(s->ctrs.data() + c, W.ctrs.data() + W.ctr_off[k], (size_t)P.n_ctr * sizeof(rl_counter));
-        // CheckRateLimit asks with delta 1 whatever hits_addend says (kuadrant_service.rs:62-65)
-        s->delta[j] = s->method == RL_RLS_CHECK_RATE_LIMIT ? 1 : P.hits;
+        s->delta[j] = store_delta(s, P);
         c += P.n_ctr;
         j++;
     }
@@ -564,6 +668,225 @@ void take_device_plan(rl_rls* s, const RlsDevReq* req, const uint8_t* buf, const
     s->planned = true;
 }
 
+// Stage 1 on the CPU workers, for both surfaces (the caller has checked the batch and sets what is its own after it).
+template <class Svc>
+int plan_cpu(Svc* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    s->planned = s->finished = false;
+    s->method = method;
+    s->n = n;
+    s->buf = buf;
+    s->plan.resize(n);
+    s->domains.resize(n);
+    s->pool->run([&](uint32_t w) { plan_range(s, off, w); });
+    s->buf = nullptr;
+    // lay the workers' counters out as one CSR, requests in batch order: a prefix over the workers, then every worker
+    // copies its own slice
+    std::vector<uint64_t> store_base(s->pool->n + 1, 0), ctr_base(s->pool->n + 1, 0);
+    for (uint32_t w = 0; w < s->pool->n; w++) {
+        const WorkerOut& W = s->wout[w];
+        store_base[w + 1] = store_base[w] + W.n_store;
+        ctr_base[w + 1] = ctr_base[w] + (W.ctr_off.empty() ? 0 : W.ctr_off.back());
+    }
+    const uint64_t n_store = store_base[s->pool->n], n_ctr = ctr_base[s->pool->n];
+    if (n_ctr > 0xFFFFFFFFull) return sfail(s, "more than 2^32 counters in one batch");
+    s->store_index.assign(n, RL_RLS_NO_STORE);
+    s->ctr_off.assign(n_store + 1, 0);
+    s->ctr_off[n_store] = (uint32_t)n_ctr;
+    s->ctrs.ensure(n_ctr);
+    s->delta.assign(n_store, 0);
+    s->pool->run([&](uint32_t w) { plan_scatter(s, w, store_base[w], ctr_base[w]); });
+    s->n_store = n_store;
+    s->now.assign(s->n_store, now_us ? now_us : wall_us());
+    return RL_OK;
+}
+
+
+// ---- the HTTP API (include/rl_http.h) ------------------------------------------------------------------------------
+int check_http_batch(rl_http* h, int endpoint, uint64_t n, const uint64_t* off) {
+    if (endpoint != RL_HTTP_CHECK && endpoint != RL_HTTP_REPORT && endpoint != RL_HTTP_CHECK_AND_REPORT)
+        return sfail(h, "unknown endpoint %d", endpoint);
+    for (uint64_t i = 0; i < n; i++)
+        if (off[i + 1] < off[i]) return sfail(h, "body offsets must be non-decreasing (body %llu)", (unsigned long long)i);
+    return RL_OK;
+}
+
+// Responses [lo, hi) of worker w (server.rs:129-260): status, body, X-RateLimit-* values, and the metrics of
+// /check_and_report (server.rs:217-242).
+void finish_range_http(rl_http* h, const int32_t* store_status, const uint8_t* limited, const uint32_t* first, const uint64_t* rem,
+                       const uint64_t* ttl, uint32_t w) {
+    uint64_t lo, hi;
+    range_of(h->n, h->pool->n, w, lo, hi);
+    WorkerOut& W = h->wout[w];
+    W.resp.clear();
+    W.resp_len.assign(hi - lo, 0);
+    W.hval.clear();
+    W.hval_len.assign(3 * (hi - lo), 0);
+    W.by_ns.clear();
+    W.limited_by_name.clear();
+    const bool car = h->method == RL_HTTP_CHECK_AND_REPORT;
+    // the store requests of the range are one run of store indices: their header values in ONE matcher call, when one of
+    // them asks for the headers
+    uint64_t j0 = RL_RLS_NO_STORE, j1 = 0;
+    bool want = false;
+    for (uint64_t i = lo; i < hi; i++)
+        if (h->plan[i].kind == REQ_STORE) {
+            if (j0 == RL_RLS_NO_STORE) j0 = h->plan[i].store;
+            j1 = (uint64_t)h->plan[i].store + 1;
+            want = want || (car && h->plan[i].hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03);
+        }
+    bool headers_ok = false;
+    if (want) {
+        W.hdr_off.assign(j1 - j0 + 1, 0);
+        uint64_t need = 0;
+        W.hdr.resize(std::max<size_t>(W.hdr.size(), (size_t)(j1 - j0) * 96));
+        int r = rl_matcher_response_headers_batch(h->m, j1 - j0, h->ctr_off.data() + j0, h->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
+                                                  W.hdr_off.data(), &need);
+        if (r != RL_OK && need > W.hdr.size()) {
+            W.hdr.resize(need);
+            r = rl_matcher_response_headers_batch(h->m, j1 - j0, h->ctr_off.data() + j0, h->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
+                                                  W.hdr_off.data(), &need);
+        }
+        headers_ok = r == RL_OK;
+    }
+    const std::string* last_ns = nullptr;
+    NsCounts* last_counts = nullptr;
+    for (uint64_t i = lo; i < hi; i++) {
+        const ReqPlan& P = h->plan[i];
+        uint16_t status = 500;
+        bool decided = false, lim = false;
+        const char* vals[3] = {"", "", ""};
+        if (P.kind == REQ_BAD_WIRE) {
+            status = 400;  // what the Json extractor answers
+        } else if (P.kind == REQ_NO_LIMITS) {
+            status = 200;  // lib.rs:434-440: nothing applies, nothing is limited
+            decided = true;
+        } else if (P.kind == REQ_STORE) {
+            const uint32_t j = P.store;
+            const bool failed = (store_status && store_status[j] != RL_OK) || (h->method != RL_HTTP_REPORT && limited[j] == RL_VERDICT_ERROR);
+            if (!failed && h->method == RL_HTTP_REPORT) {
+                status = 200;
+            } else if (!failed) {
+                lim = limited[j] != 0;
+                status = lim ? 429 : 200;
+                decided = true;
+                if (car && P.hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03) {  // server.rs:262-280
+                    if (headers_ok) {
+                        vals[0] = W.hdr.data() + W.hdr_off[j - j0];
+                        vals[1] = vals[0] + strlen(vals[0]) + 1;
+                        vals[2] = vals[1] + strlen(vals[1]) + 1;
+                    } else {
+                        status = 500;
+                        decided = false;
+                    }
+                }
+            }
+        }  // REQ_UNSUPPORTED: 500
+        h->status[i] = status;
+        const char* body = "null";  // Json(()) and HttpResponse::...().json(())
+        if (status == 500 && !car) body = "Internal server error";  // ErrorResponse's Display
+        else if (status == 429 && !car) body = "Too many requests";
+        else if (status == 400) body = "";
+        const size_t bl = strlen(body);
+        W.resp.insert(W.resp.end(), (const uint8_t*)body, (const uint8_t*)body + bl);
+        W.resp_len[i - lo] = bl;
+        for (int k = 0; k < 3; k++) {
+            const size_t vl = strlen(vals[k]);
+            W.hval.insert(W.hval.end(), (const uint8_t*)vals[k], (const uint8_t*)vals[k] + vl);
+            W.hval_len[3 * (i - lo) + k] = vl;
+        }
+        if (!car || !decided) continue;
+        if (!last_ns || *last_ns != h->domains[i]) {
+            last_ns = &h->domains[i];
+            last_counts = &W.by_ns[h->domains[i]];
+        }
+        NsCounts& c = *last_counts;
+        if (lim) {
+            c.limited_calls++;
+            if (h->rls->use_limit_name) {
+                std::string name;
+                const uint32_t lid = first ? first[P.store] : RL_NONE;
+                if (lid != RL_NONE) {
+                    char nb[512];
+                    int has = 0;
+                    if (rl_matcher_limit_name_copy(h->m, lid, nb, sizeof nb, &has) == RL_OK && has) name = nb;
+                }
+                W.limited_by_name[{h->domains[i], name}]++;
+            }
+        } else {
+            c.authorized_calls++;
+            c.authorized_hits += P.delta;
+        }
+    }
+}
+
+// Stage 1 of an HTTP batch on the engine's device, through the RLS service's device state (rl_rls_dev.cu).
+int http_plan_on_device(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us, bool copy_csr,
+                        const HttpDevReq*& req, uint64_t& n_ctr, const HttpRun*& runs, uint32_t& n_runs) {
+    if (!h->engine) return sfail(h, "the device plan needs a service created with an engine");
+    if (!rl_http_dev_plan) return sfail(h, "this build of the library has no device plan");
+    int r = check_http_batch(h, endpoint, n, off);
+    if (r) return r;
+    h->planned = h->finished = false;
+    h->method = endpoint;
+    h->n = n;
+    const uint64_t now = now_us ? now_us : wall_us();
+    uint64_t n_store = 0;
+    rl_rls* s = h->rls;
+    r = rl_http_dev_plan(&s->dev, h->engine, h->m, endpoint, n, buf, off, now, &n_store, &n_ctr, &req, &runs, &n_runs);
+    if (r) {
+        h->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
+        return r;
+    }
+    h->n_store = n_store;
+    if (copy_csr) {
+        h->ctr_off.resize(n_store + 1);
+        h->ctrs.ensure(n_ctr);
+        h->delta.resize(n_store);
+        h->load.resize(n_store);
+        h->now.assign(n_store, now);
+        if ((r = rl_http_dev_copy_plan(s->dev, h->ctr_off.data(), h->ctrs.data(), h->delta.data(), h->load.data()))) {
+            h->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
+            return r;
+        }
+    }
+    return RL_OK;
+}
+
+// The per-body outcomes of a device plan into the service's plan, store index and namespaces.  The namespace comes from
+// the host's copy of the body, unescaped again (rl_json.h) when its source holds a backslash.
+void take_http_device_plan(rl_http* h, const HttpDevReq* req, const uint8_t* buf, const uint64_t* off) {
+    h->plan.resize(h->n);
+    h->domains.resize(h->n);
+    h->store_index.resize(h->n);
+    h->pool->run([&](uint32_t w) {
+        uint64_t lo, hi;
+        range_of(h->n, h->pool->n, w, lo, hi);
+        WorkerOut& W = h->wout[w];
+        for (uint64_t i = lo; i < hi; i++) {
+            const HttpDevReq& R = req[i];
+            ReqPlan& P = h->plan[i];
+            P = ReqPlan();
+            P.kind = (uint8_t)R.kind;
+            P.hdr = (uint8_t)R.headers;
+            P.delta = R.delta;
+            P.store = R.store;
+            h->store_index[i] = R.store;
+            const uint8_t* src = buf + off[i] + R.dom_off;
+            if (R.kind == REQ_BAD_WIRE) {
+                h->domains[i].clear();
+            } else if (memchr(src, '\\', R.dom_len) == nullptr) {  // (an escape makes the source longer than the string)
+                h->domains[i].assign((const char*)src, R.dom_len);
+            } else {
+                const uint64_t len = off[i + 1] - off[i];
+                W.txt.ensure(len + 1);
+                const uint32_t l = rl_json::unescape(buf + off[i], len, R.dom_off, W.txt.data());
+                h->domains[i].assign((const char*)W.txt.data() + R.dom_off, l);
+            }
+        }
+    });
+    h->planned = true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -614,32 +937,7 @@ int rl_rls_plan(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uin
     if (!s || (n && (!off || !buf))) return RL_FATAL;
     int r = check_batch(s, method, n, off);
     if (r) return r;
-    s->planned = s->finished = false;
-    s->method = method;
-    s->n = n;
-    s->buf = buf;
-    s->plan.resize(n);
-    s->domains.resize(n);
-    s->pool->run([&](uint32_t w) { plan_range(s, off, w); });
-    s->buf = nullptr;
-    // lay the workers' counters out as one CSR, requests in batch order: a prefix over the workers, then every worker
-    // copies its own slice
-    std::vector<uint64_t> store_base(s->pool->n + 1, 0), ctr_base(s->pool->n + 1, 0);
-    for (uint32_t w = 0; w < s->pool->n; w++) {
-        const WorkerOut& W = s->wout[w];
-        store_base[w + 1] = store_base[w] + W.n_store;
-        ctr_base[w + 1] = ctr_base[w] + (W.ctr_off.empty() ? 0 : W.ctr_off.back());
-    }
-    const uint64_t n_store = store_base[s->pool->n], n_ctr = ctr_base[s->pool->n];
-    if (n_ctr > 0xFFFFFFFFull) return sfail(s, "more than 2^32 counters in one batch");
-    s->store_index.assign(n, RL_RLS_NO_STORE);
-    s->ctr_off.assign(n_store + 1, 0);
-    s->ctr_off[n_store] = (uint32_t)n_ctr;
-    s->ctrs.ensure(n_ctr);
-    s->delta.assign(n_store, 0);
-    s->pool->run([&](uint32_t w) { plan_scatter(s, w, store_base[w], ctr_base[w]); });
-    s->n_store = n_store;
-    s->now.assign(s->n_store, now_us ? now_us : wall_us());
+    if ((r = plan_cpu(s, method, n, buf, off, now_us))) return r;
     s->load_counters = (method == RL_RLS_SHOULD_RATE_LIMIT && s->header_mode != RL_RLS_HEADERS_NONE) ? 1 : 0;  // server.rs:146
     s->planned = true;
     return RL_OK;
@@ -796,6 +1094,201 @@ int rl_rls_last_timings(rl_rls* s, double* out_plan_us, double* out_store_us, do
     if (out_plan_us) *out_plan_us = s->t_plan;
     if (out_store_us) *out_store_us = s->t_store;
     if (out_finish_us) *out_finish_us = s->t_finish;
+    return RL_OK;
+}
+
+// ---- the HTTP API --------------------------------------------------------------------------------------------------
+int rl_http_decode_body(const uint8_t* body, uint64_t len, uint8_t* txt, rl_http_info* out, rl_rls_entry* entries,
+                        uint32_t cap_entries) {
+    if (!out || (len && (!body || !txt)) || (cap_entries && !entries)) return RL_FATAL;
+    std::vector<uint8_t> bits(len / 8 + 1);
+    EntrySink sink{entries, cap_entries, 0};
+    rl_json::Info q;
+    if (!rl_json::decode_info(body, len, txt, bits.data(), q, sink)) return RL_FATAL;
+    *out = rl_http_info{q.ns_off, q.ns_len, q.delta, q.n_entries, q.headers};
+    return RL_OK;
+}
+
+int rl_http_create(rl_rls* rls, rl_http** out) {
+    if (!rls || !out) return RL_FATAL;
+    rl_http* h = new rl_http();
+    h->rls = rls;
+    h->m = rls->m;
+    h->engine = rls->engine;
+    h->pool = rls->pool;
+    h->wout.resize(rls->pool->n);
+    *out = h;
+    return RL_OK;
+}
+
+void rl_http_destroy(rl_http* h) { delete h; }
+
+const char* rl_http_last_error(rl_http* h) { return h ? h->last_error.c_str() : "null service"; }
+
+int rl_http_plan(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!h || (n && (!off || !buf))) return RL_FATAL;
+    int r = check_http_batch(h, endpoint, n, off);
+    if (r) return r;
+    if ((r = plan_cpu(h, endpoint, n, buf, off, now_us))) return r;
+    h->load.assign(h->n_store, 0);
+    for (uint64_t i = 0; i < n; i++)
+        if (h->plan[i].kind == REQ_STORE) h->load[h->plan[i].store] = rl_json::load_counters(endpoint, h->plan[i].hdr);
+    h->planned = true;
+    return RL_OK;
+}
+
+int rl_http_plan_device(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!h || (n && (!off || !buf))) return RL_FATAL;
+    const HttpDevReq* req = nullptr;
+    const HttpRun* runs = nullptr;
+    uint64_t n_ctr = 0;
+    uint32_t n_runs = 0;
+    const int r = http_plan_on_device(h, endpoint, n, buf, off, now_us, true, req, n_ctr, runs, n_runs);
+    if (r) return r;
+    take_http_device_plan(h, req, buf, off);
+    return RL_OK;
+}
+
+int rl_http_plan_view(rl_http* h, uint64_t* out_n_store, const uint32_t** out_ctr_off, const rl_counter** out_ctrs,
+                      const uint64_t** out_delta, const uint64_t** out_now_us, const uint8_t** out_load_counters,
+                      const uint32_t** out_store_index) {
+    if (!h) return RL_FATAL;
+    if (!h->planned) return sfail(h, "no planned batch");
+    if (out_n_store) *out_n_store = h->n_store;
+    if (out_ctr_off) *out_ctr_off = h->ctr_off.data();
+    if (out_ctrs) *out_ctrs = h->ctrs.data();
+    if (out_delta) *out_delta = h->delta.data();
+    if (out_now_us) *out_now_us = h->now.data();
+    if (out_load_counters) *out_load_counters = h->load.data();
+    if (out_store_index) *out_store_index = h->store_index.data();
+    return RL_OK;
+}
+
+int rl_http_finish(rl_http* h, const int32_t* store_status, const uint8_t* limited, const uint32_t* first_limited,
+                   const uint64_t* remaining, const uint64_t* ttl_us) {
+    if (!h) return RL_FATAL;
+    if (!h->planned) return sfail(h, "no planned batch");
+    if (h->n_store && h->method != RL_HTTP_REPORT && !limited) return sfail(h, "finish needs the verdicts of the store calls");
+    bool headers = false;
+    for (uint64_t i = 0; i < h->n && !headers; i++)
+        headers = h->plan[i].kind == REQ_STORE && h->method == RL_HTTP_CHECK_AND_REPORT && h->plan[i].hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03;
+    if (headers && (!remaining || !ttl_us)) return sfail(h, "finish needs remaining / ttl of the store calls (draft-03 headers)");
+    h->status.assign(h->n, 0);
+    h->pool->run([&](uint32_t w) { finish_range_http(h, store_status, limited, first_limited, remaining, ttl_us, w); });
+    // the workers' bodies and header values behind one another, their metrics merged into the RLS service's
+    const uint32_t nw = h->pool->n;
+    std::vector<uint64_t> bb(nw + 1, 0), hb(nw + 1, 0);
+    for (uint32_t w = 0; w < nw; w++) {
+        bb[w + 1] = bb[w] + h->wout[w].resp.size();
+        hb[w + 1] = hb[w] + h->wout[w].hval.size();
+    }
+    h->body.ensure(bb[nw]);
+    h->hval.ensure(hb[nw]);
+    h->body_off.assign(h->n + 1, 0);
+    h->hval_off.assign(3 * h->n + 1, 0);
+    h->pool->run([&](uint32_t w) {
+        uint64_t lo, hi;
+        range_of(h->n, nw, w, lo, hi);
+        const WorkerOut& W = h->wout[w];
+        if (!W.resp.empty()) memcpy(h->body.data() + bb[w], W.resp.data(), W.resp.size());
+        if (!W.hval.empty()) memcpy(h->hval.data() + hb[w], W.hval.data(), W.hval.size());
+        uint64_t at = bb[w], hat = hb[w];
+        for (uint64_t i = lo; i < hi; i++) {
+            at += W.resp_len[i - lo];
+            h->body_off[i + 1] = at;
+            for (int k = 0; k < 3; k++) {
+                hat += W.hval_len[3 * (i - lo) + k];
+                h->hval_off[3 * i + k + 1] = hat;
+            }
+        }
+    });
+    rl_rls* s = h->rls;
+    for (uint32_t w = 0; w < nw; w++) {
+        const WorkerOut& W = h->wout[w];
+        for (const auto& kv : W.by_ns) {
+            NsCounts& c = s->by_ns[kv.first];
+            c.authorized_calls += kv.second.authorized_calls;
+            c.authorized_hits += kv.second.authorized_hits;
+            c.limited_calls += kv.second.limited_calls;
+        }
+        for (const auto& kv : W.limited_by_name) s->limited_by_name[kv.first] += kv.second;
+    }
+    h->finished = true;
+    h->planned = false;  // a batch is finished once: its metrics are counted once
+    return RL_OK;
+}
+
+int rl_http_responses(rl_http* h, const uint16_t** out_status, const uint8_t** out_body, const uint64_t** out_body_off,
+                      const uint8_t** out_hdr, const uint64_t** out_hdr_off) {
+    if (!h) return RL_FATAL;
+    if (!h->finished) return sfail(h, "no finished batch");
+    static const uint8_t kEmpty = 0;
+    static const uint16_t kNone = 0;
+    if (out_status) *out_status = h->status.empty() ? &kNone : h->status.data();
+    if (out_body) *out_body = h->body.size() ? h->body.data() : &kEmpty;
+    if (out_body_off) *out_body_off = h->body_off.data();
+    if (out_hdr) *out_hdr = h->hval.size() ? h->hval.data() : &kEmpty;
+    if (out_hdr_off) *out_hdr_off = h->hval_off.data();
+    return RL_OK;
+}
+
+int rl_http_serve(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!h) return RL_FATAL;
+    if (!h->engine) return sfail(h, "the service was created without an engine: there is no CPU store to fall back to");
+    if (n && (!off || !buf)) return RL_FATAL;
+    const double t0 = mono_us();
+    const HttpDevReq* req = nullptr;
+    const HttpRun* runs = nullptr;
+    uint64_t n_ctr = 0;
+    uint32_t n_runs = 0;
+    int r = http_plan_on_device(h, endpoint, n, buf, off, now_us, false, req, n_ctr, runs, n_runs);
+    if (r) return r;
+    const double t1 = mono_us();
+    // one store call per run on the device arrays; only what the finish reads comes back
+    const uint64_t m = h->n_store;
+    bool any_load = false;
+    for (uint32_t k = 0; k < n_runs; k++) any_load = any_load || runs[k].load;
+    h->o_limited.resize(m);
+    h->o_first.resize(m);
+    if (any_load) {
+        h->o_rem.resize(n_ctr);
+        h->o_ttl.resize(n_ctr);
+        h->ctr_off.resize(m + 1);
+        h->ctrs.ensure(n_ctr);
+    }
+    h->run_status.assign(n_runs, RL_OK);
+    const int st = rl_http_dev_decide(h->rls->dev, h->engine, endpoint, h->run_status.data(), h->o_limited.data(), h->o_first.data(),
+                                      h->o_rem.data(), h->o_ttl.data(), h->ctr_off.data(), h->ctrs.data());
+    if (st != RL_OK) h->run_status.assign(n_runs, st);
+    for (uint32_t k = 0; k < n_runs; k++)
+        if (h->run_status[k] != RL_OK) h->last_error = std::string("store call failed: ") + rl_last_error(h->engine);
+    if ((r = rl_rls_dev_wait(h->rls->dev))) {
+        h->last_error = std::string("device plan: ") + rl_rls_dev_error(h->rls->dev);
+        return r;
+    }
+    h->o_status.resize(m);
+    for (uint32_t k = 0; k < n_runs; k++) {
+        const uint64_t j1 = k + 1 < n_runs ? runs[k + 1].store : m;
+        for (uint64_t j = runs[k].store; j < j1; j++) h->o_status[j] = h->run_status[k];
+    }
+    h->store_calls = n_runs;
+    const double t2 = mono_us();
+    take_http_device_plan(h, req, buf, off);
+    const double t3 = mono_us();
+    r = rl_http_finish(h, h->o_status.data(), h->o_limited.data(), h->o_first.data(), h->o_rem.data(), h->o_ttl.data());
+    const double t4 = mono_us();
+    h->t_plan = (t1 - t0) + (t3 - t2);
+    h->t_store = t2 - t1;
+    h->t_finish = t4 - t3;
+    return r;
+}
+
+int rl_http_last_timings(rl_http* h, double* out_plan_us, double* out_store_us, double* out_finish_us, uint32_t* out_store_calls) {
+    if (!h) return RL_FATAL;
+    if (out_plan_us) *out_plan_us = h->t_plan;
+    if (out_store_us) *out_store_us = h->t_store;
+    if (out_finish_us) *out_finish_us = h->t_finish;
+    if (out_store_calls) *out_store_calls = h->store_calls;
     return RL_OK;
 }
 

@@ -3,7 +3,9 @@
 //
 // One plan: wire bytes and offsets -> pinned staging -> device (engine's stream); k_rls_plan; CUB exclusive sum; ONE
 // device->host read of the totals (the store request and counter counts); k_rls_scatter; the per-request array back
-// into pinned memory.  The store call then reads the CSR where it lies (RL_MEM_DEVICE).
+// into pinned memory.  The store call then reads the CSR where it lies (RL_MEM_DEVICE).  The HTTP plan (rl_http_dev.cuh)
+// takes the same path through the same state: staging, image, scratch and the one read are shared, the kernels and the
+// per-request array are its own, and its read also brings the table of its store calls.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -15,6 +17,7 @@
 
 #include <cub/device/device_scan.cuh>
 
+#include "rl_http_dev.cuh"
 #include "rl_internal.h"
 #include "rl_rls_dev.cuh"
 
@@ -88,6 +91,14 @@ struct rl_rls_dev {
     DBuf<uint8_t> d_lim;
     DBuf<uint32_t> d_first;
     DBuf<uint64_t> d_rem, d_ttl;
+    // the HTTP plan's own arrays
+    DBuf<uint8_t> d_txt, d_bits, d_load;
+    DBuf<HttpDevReq> d_hreq;
+    HBuf<HttpDevReq> h_hreq;
+    DBuf<HttpScan> d_hcount, d_hstart;
+    DBuf<uint32_t> d_runs, d_ctr_run;
+    HBuf<uint32_t> h_runs;
+    uint32_t n_runs = 0;
 };
 
 namespace {
@@ -129,6 +140,81 @@ int refresh_image(rl_rls_dev* S, rl_matcher* m) {
     return RL_OK;
 }
 
+
+// What both plans start with: the engine's device and stream, the matcher image, the batch's bytes and offsets through
+// pinned staging onto the device, and the entry and counter scratch.  per_req = counters one request may carry.
+int stage_batch(rl_rls_dev* S, rl_engine* e, rl_matcher* m, uint64_t n, const uint8_t* buf, const uint64_t* off,
+                uint32_t& per_req) {
+    S->n = S->n_store = S->n_ctr = 0;
+    S->n_runs = 0;
+    RlTableView v;
+    int r = rl_internal_view(e, &v);  // the engine's device and stream (every earlier pipelined call is fenced)
+    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
+    S->device = v.device;
+    S->stream = v.stream;
+    if ((r = refresh_image(S, m))) return r;
+    const uint32_t engine_max = rl_engine_max_counters_per_request(e);
+    per_req = std::min(S->image[RL_IMG_H_COUNTER_CAP], engine_max);
+    if (n && (n + 1) * (uint64_t)per_req >= (1ull << 32))
+        return dev_fail(S, RL_FATAL, "a batch of %llu requests of up to %u counters each may exceed 2^32 counters",
+                        (unsigned long long)n, per_req);
+    const uint64_t bytes = n ? off[n] : 0;
+    // wire bytes and offsets through pinned staging onto the device
+    RLS_CUDA(S, S->h_buf.reserve(bytes + 1));
+    RLS_CUDA(S, S->h_off.reserve(n + 1));
+    RLS_CUDA(S, S->h_total.reserve(1));
+    if (bytes) memcpy(S->h_buf.p, buf, bytes);
+    memcpy(S->h_off.p, off, (n + 1) * sizeof(uint64_t));
+    RLS_CUDA(S, S->d_buf.reserve(bytes + 1));
+    RLS_CUDA(S, S->d_off.reserve(n + 1));
+    RLS_CUDA(S, S->d_ent.reserve(bytes / 2 + 1));
+    RLS_CUDA(S, S->d_scratch.reserve(n * (uint64_t)per_req + 1));
+    if (bytes) RLS_CUDA(S, cudaMemcpyAsync(S->d_buf.p, S->h_buf.p, bytes, cudaMemcpyHostToDevice, S->stream));
+    RLS_CUDA(S, cudaMemcpyAsync(S->d_off.p, S->h_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+    return RL_OK;
+}
+
+// the one read before the store call: `bytes` from the device to pinned host memory, then the stream is waited for
+int read_totals(rl_rls_dev* S, void* dst, const void* src, size_t bytes) {
+    RLS_CUDA(S, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S->stream));
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    return RL_OK;
+}
+
+// the store call's outputs from the device arrays to the caller's (with load_counters also the CSR the headers read)
+int copy_outputs(rl_rls_dev* S, bool verdicts, bool load_counters, uint8_t* limited, uint32_t* first_limited,
+                 uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
+    const uint64_t m = S->n_store, nc = S->n_ctr;
+    if (verdicts) {
+        if (cudaMemcpyAsync(limited, S->d_lim.p, m, cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(first_limited, S->d_first.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
+            return dev_fail(S, RL_FATAL, "copying the verdicts back failed");
+    }
+    if (load_counters) {
+        if (cudaMemcpyAsync(remaining, S->d_rem.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ttl_us, S->d_ttl.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (m + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+            cudaMemcpyAsync(ctrs, S->d_ctrs.p, nc * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
+            return dev_fail(S, RL_FATAL, "copying the counters back failed");
+    }
+    return RL_OK;
+}
+
+// the store call's output buffers; with load_counters remaining / ttl start at 0 (slots of a refused call stay 0, as
+// with host buffers)
+int reserve_outputs(rl_rls_dev* S, bool load_counters) {
+    const uint64_t m = S->n_store, nc = S->n_ctr;
+    RLS_CUDA(S, S->d_lim.reserve(m));
+    RLS_CUDA(S, S->d_first.reserve(m));
+    if (load_counters) {
+        RLS_CUDA(S, S->d_rem.reserve(nc + 1));
+        RLS_CUDA(S, S->d_ttl.reserve(nc + 1));
+        RLS_CUDA(S, cudaMemsetAsync(S->d_rem.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+        RLS_CUDA(S, cudaMemsetAsync(S->d_ttl.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+    }
+    return RL_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -139,35 +225,13 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     if (!st || !e || !m || !out_n_store || !out_n_ctr || !out_req) return RL_FATAL;
     if (!*st) *st = new rl_rls_dev();
     rl_rls_dev* S = *st;
-    S->n = S->n_store = S->n_ctr = 0;
-    RlTableView v;
-    int r = rl_internal_view(e, &v);  // the engine's device and stream (every earlier pipelined call is fenced)
-    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
-    S->device = v.device;
-    S->stream = v.stream;
-    if ((r = refresh_image(S, m))) return r;
-    const uint32_t engine_max = rl_engine_max_counters_per_request(e);
-    const uint32_t per_req = std::min(S->image[RL_IMG_H_COUNTER_CAP], engine_max);
-    if (n && (n + 1) * (uint64_t)per_req >= (1ull << 32))
-        return dev_fail(S, RL_FATAL, "a batch of %llu requests of up to %u counters each may exceed 2^32 counters",
-                        (unsigned long long)n, per_req);
-    const uint64_t bytes = n ? off[n] : 0;
-    // wire bytes and offsets through pinned staging onto the device
-    RLS_CUDA(S, S->h_buf.reserve(bytes + 1));
-    RLS_CUDA(S, S->h_off.reserve(n + 1));
+    uint32_t per_req = 0;
+    int r = stage_batch(S, e, m, n, buf, off, per_req);
+    if (r) return r;
     RLS_CUDA(S, S->h_req.reserve(n + 1));
-    RLS_CUDA(S, S->h_total.reserve(1));
-    if (bytes) memcpy(S->h_buf.p, buf, bytes);
-    memcpy(S->h_off.p, off, (n + 1) * sizeof(uint64_t));
-    RLS_CUDA(S, S->d_buf.reserve(bytes + 1));
-    RLS_CUDA(S, S->d_off.reserve(n + 1));
-    RLS_CUDA(S, S->d_ent.reserve(bytes / 2 + 1));
-    RLS_CUDA(S, S->d_scratch.reserve(n * (uint64_t)per_req + 1));
     RLS_CUDA(S, S->d_req.reserve(n + 1));
     RLS_CUDA(S, S->d_count.reserve(n + 1));
     RLS_CUDA(S, S->d_start.reserve(n + 1));
-    if (bytes) RLS_CUDA(S, cudaMemcpyAsync(S->d_buf.p, S->h_buf.p, bytes, cudaMemcpyHostToDevice, S->stream));
-    RLS_CUDA(S, cudaMemcpyAsync(S->d_off.p, S->h_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
     RlsPlanArgs a;
     a.buf = S->d_buf.p;
     a.off = S->d_off.p;
@@ -186,8 +250,7 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
     RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
     // the one read before the store call: how many store requests and counters the batch has
-    RLS_CUDA(S, cudaMemcpyAsync(S->h_total.p, S->d_start.p + n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, S->stream));
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    if ((r = read_totals(S, S->h_total.p, S->d_start.p + n, sizeof(unsigned long long)))) return r;
     const uint64_t n_store = S->h_total.p[0] >> 32, n_ctr = S->h_total.p[0] & 0xFFFFFFFFull;
     RLS_CUDA(S, S->d_ctr_off.reserve(n_store + 1));
     RLS_CUDA(S, S->d_ctrs.reserve(n_ctr + 1));
@@ -231,19 +294,11 @@ int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uin
 int rl_rls_dev_decide(rl_rls_dev* S, rl_engine* e, int method, int load_counters, uint8_t* limited, uint32_t* first_limited,
                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
     if (!S || !e) return RL_FATAL;
-    const uint64_t m = S->n_store, nc = S->n_ctr;
+    const uint64_t m = S->n_store;
     if (m == 0) return RL_OK;
     RLS_CUDA(S, cudaSetDevice(S->device));
-    RLS_CUDA(S, S->d_lim.reserve(m));
-    RLS_CUDA(S, S->d_first.reserve(m));
-    if (load_counters) {
-        RLS_CUDA(S, S->d_rem.reserve(nc + 1));
-        RLS_CUDA(S, S->d_ttl.reserve(nc + 1));
-        // (slots of a refused call stay 0, as with host buffers)
-        RLS_CUDA(S, cudaMemsetAsync(S->d_rem.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
-        RLS_CUDA(S, cudaMemsetAsync(S->d_ttl.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
-    }
-    int st;
+    int st = reserve_outputs(S, load_counters != 0);
+    if (st) return st;
     if (method == RL_RLS_SHOULD_RATE_LIMIT)
         st = rl_check_and_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, load_counters, RL_MEM_DEVICE,
                                        S->d_lim.p, S->d_first.p, load_counters ? S->d_rem.p : nullptr,
@@ -255,19 +310,142 @@ int rl_rls_dev_decide(rl_rls_dev* S, rl_engine* e, int method, int load_counters
         st = rl_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, RL_MEM_DEVICE);
     if (st == RL_OK) st = rl_sync(e);  // a device-memory call reports its deferred errors here
     if (st != RL_OK) return st;
-    if (method != RL_RLS_REPORT) {
-        if (cudaMemcpyAsync(limited, S->d_lim.p, m, cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
-            cudaMemcpyAsync(first_limited, S->d_first.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
-            return dev_fail(S, RL_FATAL, "copying the verdicts back failed");
-    }
-    if (load_counters) {
-        if (cudaMemcpyAsync(remaining, S->d_rem.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
-            cudaMemcpyAsync(ttl_us, S->d_ttl.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
-            cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (m + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
-            cudaMemcpyAsync(ctrs, S->d_ctrs.p, nc * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
-            return dev_fail(S, RL_FATAL, "copying the counters back failed");
-    }
+    return copy_outputs(S, method != RL_RLS_REPORT, load_counters != 0, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
+}
+
+int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
+                     const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                     const HttpDevReq** out_req, const HttpRun** out_runs, uint32_t* out_n_runs) {
+    if (!st || !e || !m || !out_n_store || !out_n_ctr || !out_req || !out_runs || !out_n_runs) return RL_FATAL;
+    if (!*st) *st = new rl_rls_dev();
+    rl_rls_dev* S = *st;
+    uint32_t per_req = 0;
+    int r = stage_batch(S, e, m, n, buf, off, per_req);
+    if (r) return r;
+    const uint64_t bytes = n ? off[n] : 0;
+    // the read before the store call: the head and up to kRunsRead store calls (a batch with more reads the rest after)
+    const uint64_t kRunsRead = 1024;
+    RLS_CUDA(S, S->h_hreq.reserve(n + 1));
+    RLS_CUDA(S, S->h_runs.reserve(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
+    RLS_CUDA(S, S->d_txt.reserve(bytes + 1));
+    RLS_CUDA(S, S->d_bits.reserve(bytes / 8 + n + 1));
+    RLS_CUDA(S, S->d_hreq.reserve(n + 1));
+    RLS_CUDA(S, S->d_hcount.reserve(n + 1));
+    RLS_CUDA(S, S->d_hstart.reserve(n + 1));
+    RLS_CUDA(S, S->d_runs.reserve(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
+    HttpPlanArgs a;
+    a.buf = S->d_buf.p;
+    a.off = S->d_off.p;
+    a.n = n;
+    a.img = rl_img_view(S->image.data(), S->d_image.p);
+    a.per_req = per_req;
+    a.endpoint = endpoint;
+    a.txt = S->d_txt.p;
+    a.bits = S->d_bits.p;
+    a.ent = S->d_ent.p;
+    a.scratch = S->d_scratch.p;
+    a.req = S->d_hreq.p;
+    a.count = S->d_hcount.p;
+    const uint32_t threads = 128;
+    k_http_plan<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
+    RLS_CUDA(S, cudaGetLastError());
+    size_t tmp = 0;
+    const HttpScan zero{0, 0, 0, 0, 0, {0, 0}};
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
+                                               S->stream));
+    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
+                                               S->stream));
+    HttpRunsArgs ra{S->d_hcount.p, S->d_hstart.p, n, S->d_runs.p};
+    k_http_runs<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(ra);
+    RLS_CUDA(S, cudaGetLastError());
+    const uint64_t first_read = RL_HTTP_RUNS_HEAD + 3 * std::min<uint64_t>(n, kRunsRead);
+    if ((r = read_totals(S, S->h_runs.p, S->d_runs.p, first_read * sizeof(uint32_t)))) return r;
+    const uint64_t n_store = S->h_runs.p[0], n_ctr = S->h_runs.p[1], n_runs = S->h_runs.p[2];
+    if (RL_HTTP_RUNS_HEAD + 3 * n_runs > first_read &&
+        (r = read_totals(S, S->h_runs.p + first_read, S->d_runs.p + first_read,
+                         (RL_HTTP_RUNS_HEAD + 3 * n_runs - first_read) * sizeof(uint32_t))))
+        return r;
+    RLS_CUDA(S, S->d_ctr_off.reserve(n_store + 1));
+    RLS_CUDA(S, S->d_ctr_run.reserve(n_store + n_runs + 1));
+    RLS_CUDA(S, S->d_ctrs.reserve(n_ctr + 1));
+    RLS_CUDA(S, S->d_delta.reserve(n_store + 1));
+    RLS_CUDA(S, S->d_now.reserve(n_store + 1));
+    RLS_CUDA(S, S->d_load.reserve(n_store + 1));
+    HttpScatterArgs b;
+    b.req = S->d_hreq.p;
+    b.scratch = S->d_scratch.p;
+    b.start = S->d_hstart.p;
+    b.runs = S->d_runs.p + RL_HTTP_RUNS_HEAD;
+    b.n = n;
+    b.per_req = per_req;
+    b.endpoint = endpoint;
+    b.now_us = now_us;
+    b.ctr_off = S->d_ctr_off.p;
+    b.ctr_run = S->d_ctr_run.p;
+    b.ctrs = S->d_ctrs.p;
+    b.delta = S->d_delta.p;
+    b.now = S->d_now.p;
+    b.load = S->d_load.p;
+    k_http_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
+    RLS_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, 3);
+    if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_hreq.p, S->d_hreq.p, n * sizeof(HttpDevReq), cudaMemcpyDeviceToHost, S->stream));
+    S->n = n;
+    S->n_store = n_store;
+    S->n_ctr = n_ctr;
+    S->n_runs = (uint32_t)n_runs;
+    *out_n_store = n_store;
+    *out_n_ctr = n_ctr;
+    *out_req = S->h_hreq.p;
+    *out_runs = reinterpret_cast<const HttpRun*>(S->h_runs.p + RL_HTTP_RUNS_HEAD);
+    *out_n_runs = (uint32_t)n_runs;
     return RL_OK;
+}
+
+int rl_http_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load) {
+    if (!S) return RL_FATAL;
+    RLS_CUDA(S, cudaSetDevice(S->device));
+    RLS_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_ctr) RLS_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_store) {
+        RLS_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaMemcpyAsync(load, S->d_load.p, S->n_store, cudaMemcpyDeviceToHost, S->stream));
+    }
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    return RL_OK;
+}
+
+int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_status, uint8_t* limited, uint32_t* first_limited,
+                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
+    if (!S || !e || !run_status) return RL_FATAL;
+    if (S->n_store == 0) return RL_OK;
+    RLS_CUDA(S, cudaSetDevice(S->device));
+    const HttpRun* runs = reinterpret_cast<const HttpRun*>(S->h_runs.p + RL_HTTP_RUNS_HEAD);
+    bool any_load = false;
+    for (uint32_t k = 0; k < S->n_runs; k++) any_load = any_load || runs[k].load;
+    int r = reserve_outputs(S, any_load);
+    if (r) return r;
+    // one store call per run, in batch order: run k's CSR starts at ctr_run[runs[k].store + k] and counts from 0
+    for (uint32_t k = 0; k < S->n_runs; k++) {
+        const HttpRun& R = runs[k];
+        const uint64_t j1 = k + 1 < S->n_runs ? runs[k + 1].store : S->n_store, m = j1 - R.store;
+        const uint32_t* off = S->d_ctr_run.p + R.store + k;
+        const rl_counter* c = S->d_ctrs.p + R.ctr;
+        const uint64_t *d = S->d_delta.p + R.store, *now = S->d_now.p + R.store;
+        int st;
+        if (endpoint == RL_HTTP_CHECK_AND_REPORT)
+            st = rl_check_and_update_batch(e, m, off, c, d, now, (int)R.load, RL_MEM_DEVICE, S->d_lim.p + R.store,
+                                           S->d_first.p + R.store, R.load ? S->d_rem.p + R.ctr : nullptr,
+                                           R.load ? S->d_ttl.p + R.ctr : nullptr);
+        else if (endpoint == RL_HTTP_CHECK)
+            st = rl_is_within_limits_batch(e, m, off, c, d, now, RL_MEM_DEVICE, S->d_lim.p + R.store, S->d_first.p + R.store);
+        else
+            st = rl_update_batch(e, m, off, c, d, now, RL_MEM_DEVICE);
+        if (st == RL_OK) st = rl_sync(e);  // a device-memory call reports its deferred errors here
+        run_status[k] = st;
+    }
+    return copy_outputs(S, endpoint != RL_HTTP_REPORT, any_load, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
 }
 
 int rl_rls_dev_wait(rl_rls_dev* S) {

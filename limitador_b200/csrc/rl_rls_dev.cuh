@@ -7,6 +7,7 @@
 //   (scan)         exclusive sum over `count` (CUB on the device; a host loop under the shim) -> every store request's
 //                  position in the store call and its first counter
 //   k_rls_scatter  the store call in batch order: store_index, ctr_off, ctrs, delta, now
+// The match after the decode (rl_match_ctx) is also the HTTP plan's (rl_http_dev.cuh).
 // Written so that the SAME source runs under tests/emu/cuda_shim.h (one CUDA thread after the other on the host): plain
 // per-thread code, no shared memory, no warp intrinsics, nothing that recurses.
 #pragma once
@@ -44,18 +45,20 @@ __device__ __forceinline__ const rl_rls_entry* rls_bound(const rl_rls_entry* E, 
     return nullptr;
 }
 
-// plan_range after the decode, then match_one: the request's kind; its counters at out[0 .. n_out)
-__device__ __forceinline__ uint8_t rls_match(const RlsPlanArgs& a, const uint8_t* msg, const rl_rls_request& q,
-                                             rl_rls_entry* E, uint32_t ne, rl_counter* out, uint32_t& n_out) {
+// The match body of both device plans (RLS and HTTP): plan_range's checks after the decode, then match_one.  The context
+// is E[0 .. ne) (byte ranges inside msg), the namespace msg[ns_off .. ns_off + ns_len); a.img is the matcher, a.per_req the
+// counters a request may carry.  Returns the request's kind; its counters at out[0 .. n_out).
+template <class Args>
+__device__ __forceinline__ uint8_t rl_match_ctx(const Args& a, const uint8_t* msg, uint32_t ns_off, uint32_t ns_len,
+                                                rl_rls_entry* E, uint32_t ne, rl_counter* out, uint32_t& n_out) {
     n_out = 0;
-    if (q.domain_len == 0) return REQ_UNKNOWN_DOMAIN;  // server.rs:106-116
     // no namespace the matcher knows holds a NUL: nothing applies (lib.rs:434-440)
-    if (rls_has_nul(msg + q.domain_off, q.domain_len)) return REQ_NO_LIMITS;
+    if (rls_has_nul(msg + ns_off, ns_len)) return REQ_NO_LIMITS;
     // the matcher compares NUL-terminated strings: an embedded NUL anywhere in the context is refused
     for (uint32_t k = 0; k < ne; k++)
         if (rls_has_nul(msg + E[k].key_off, E[k].key_len) || rls_has_nul(msg + E[k].val_off, E[k].val_len)) return REQ_UNSUPPORTED;
     const RlImage& I = a.img;
-    const uint32_t ns = rl_img_find_ns(I, msg + q.domain_off, q.domain_len);
+    const uint32_t ns = rl_img_find_ns(I, msg + ns_off, ns_len);
     if (ns == RL_IMG_EMPTY) return REQ_NO_LIMITS;  // no limit was ever added for the namespace
     for (uint32_t k = 0; k < ne; k++)  // bind: from here on an entry's `descriptor` holds its slot
         E[k].descriptor = rl_img_find_slot(I, E[k].descriptor, msg + E[k].key_off, E[k].key_len);
@@ -101,6 +104,14 @@ __device__ __forceinline__ uint8_t rls_match(const RlsPlanArgs& a, const uint8_t
         n_out++;
     }
     return n_out ? REQ_STORE : REQ_NO_LIMITS;
+}
+
+// the RLS plan after the decode: an empty domain is answered UNKNOWN before the match (server.rs:106-116)
+__device__ __forceinline__ uint8_t rls_match(const RlsPlanArgs& a, const uint8_t* msg, const rl_rls_request& q,
+                                             rl_rls_entry* E, uint32_t ne, rl_counter* out, uint32_t& n_out) {
+    n_out = 0;
+    if (q.domain_len == 0) return REQ_UNKNOWN_DOMAIN;
+    return rl_match_ctx(a, msg, q.domain_off, q.domain_len, E, ne, out, n_out);
 }
 
 __global__ void k_rls_plan(RlsPlanArgs a) {

@@ -15,7 +15,19 @@ struct RlsDevReq {
     uint32_t kind, hits, store, dom_off, dom_len;
 };
 
-struct rl_rls_dev;  // per-service device state: the matcher image, staging and scratch buffers
+// One body of an HTTP device plan (include/rl_http.h): kind, position in the store requests, the namespace's position in
+// the body (dom_off: first byte after its opening quote; dom_len: its unescaped length), response_headers (RL_HTTP_HEADERS_*)
+// and delta.
+struct HttpDevReq {
+    uint32_t kind, store, dom_off, dom_len, headers, _pad;
+    uint64_t delta;
+};
+// One store call of an HTTP batch: its first store request, its first counter and its load_counters flag.
+struct HttpRun {
+    uint32_t store, ctr, load;
+};
+
+struct rl_rls_dev;  // per-service device state (shared by the RLS and HTTP surfaces): the matcher image, staging and scratch buffers
 
 extern "C" {
 // Stage 1 on the engine's device and stream: the wire bytes go up through a pinned staging buffer, the kernels decode,
@@ -36,6 +48,17 @@ int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counter
                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
 // Wait for everything the plan and the store call enqueued (the per-request array and the outputs are then on the host).
 int rl_rls_dev_wait(rl_rls_dev* st);
+// The HTTP plan on the same state (rl_http_dev.cuh): as rl_rls_dev_plan, and the one read before the store call also
+// brings the store calls back: *out_runs[0 .. *out_n_runs) (pinned host memory owned by *st, valid until the next plan).
+int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
+                     const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
+                     const HttpDevReq** out_req, const HttpRun** out_runs, uint32_t* out_n_runs);
+// Host copies of the planned store requests: ctr_off [n_store + 1], ctrs [n_ctr], delta and load [n_store].
+int rl_http_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
+// One store call per run from the device arrays, then the outputs back as rl_rls_dev_decide copies them (remaining / ttl,
+// ctr_off and ctrs when a run loads counters).  run_status[r] = the status of run r's call.
+int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int endpoint, int* run_status, uint8_t* limited, uint32_t* first_limited,
+                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
 const char* rl_rls_dev_error(rl_rls_dev* st);
 void rl_rls_dev_destroy(rl_rls_dev* st);
 }

@@ -1,0 +1,209 @@
+"""ctypes binding of Limitador's HTTP API surface (include/rl_http.h, csrc/rl_rls.cpp).
+
+`HttpApi(rls_service)` serves batches of `CheckAndReportInfo` JSON bodies for one endpoint at a time — POST /check,
+/report or /check_and_report (limitador-server/src/http_api/server.rs:129-260) — through the RLS service's matcher,
+engine, workers and metrics: decode + counters_that_apply on the engine's GPU, one engine call per run of equal
+load_counters flags, then status / body / X-RateLimit-* headers on the CPU workers.  `plan` / `finish` are the CPU stages
+on their own (drivable without a GPU), `plan_device` is the GPU plan on its own; `serve` runs plan_device -> engine ->
+finish.  `encode_info` writes a body as serde_json serialises the struct.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import json
+from typing import Dict, List, Mapping, Optional, Sequence, Tuple
+
+import numpy as np
+
+from . import engine as _eng
+from . import rls as _rls
+
+CHECK, REPORT, CHECK_AND_REPORT = 0, 1, 2
+HEADERS_NONE, HEADERS_DRAFT_VERSION_03, HEADERS_OTHER = 0, 1, 2
+HEADER_NAMES = ("X-RateLimit-Limit", "X-RateLimit-Remaining", "X-RateLimit-Reset")
+
+HTTP_SYMBOLS = (
+    "rl_http_decode_body", "rl_http_create", "rl_http_destroy", "rl_http_last_error", "rl_http_plan", "rl_http_plan_device",
+    "rl_http_plan_view", "rl_http_finish", "rl_http_responses", "rl_http_serve", "rl_http_last_timings",
+)
+
+
+class HttpInfo(C.Structure):
+    _fields_ = [("ns_off", C.c_uint32), ("ns_len", C.c_uint32), ("delta", C.c_uint64), ("n_entries", C.c_uint32),
+                ("response_headers", C.c_uint32)]
+
+
+class HttpError(RuntimeError):
+    pass
+
+
+def _lib():
+    L = _rls._lib()
+    if getattr(L, "_rl_http_ready", False):
+        return L
+    vp, u32, u64, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int
+    L.rl_http_decode_body.argtypes = [vp, u64, vp, C.POINTER(HttpInfo), vp, u32]
+    L.rl_http_create.argtypes = [vp, C.POINTER(vp)]
+    L.rl_http_destroy.argtypes = [vp]
+    L.rl_http_destroy.restype = None
+    L.rl_http_last_error.argtypes = [vp]
+    L.rl_http_last_error.restype = C.c_char_p
+    L.rl_http_plan.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_plan_device.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_plan_view.argtypes = [vp, C.POINTER(u64), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                    C.POINTER(vp), C.POINTER(vp)]
+    L.rl_http_finish.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.rl_http_responses.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.rl_http_serve.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_last_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(u32)]
+    L._rl_http_ready = True
+    return L
+
+
+def encode_info(namespace: str, values: Mapping[str, str], delta: int, response_headers: Optional[str] = None) -> bytes:
+    """CheckAndReportInfo as serde_json::to_vec writes it: compact, fields in declaration order, `values` in the given
+    order, the short escapes and lower-case \\u00XX for other control characters, everything else as UTF-8."""
+    d = {"namespace": namespace, "values": dict(values), "delta": int(delta), "response_headers": response_headers}
+    return json.dumps(d, ensure_ascii=False, separators=(",", ":")).encode()
+
+
+pack_bodies = _rls.pack_requests  # -> (buf uint8, off uint64[n+1]): the batch layout rl_http_plan / rl_http_serve take
+
+
+def decode_body(body: bytes, cap_entries: int = 64):
+    """The native decoder on one body -> (namespace, values as (key, value) pairs in body order, delta, response_headers
+    state); raises HttpError for a body the Json extractor refuses (HTTP 400)."""
+    L = _lib()
+    arr = np.frombuffer(body, dtype=np.uint8) if body else np.zeros(1, dtype=np.uint8)
+    txt = np.zeros(max(len(body), 1), dtype=np.uint8)
+    q = HttpInfo()
+    ent = np.zeros(max(cap_entries, 1), dtype=_rls.ENTRY_DTYPE)
+    if L.rl_http_decode_body(arr.ctypes.data, len(body), txt.ctypes.data, C.byref(q), ent.ctypes.data, cap_entries) != 0:
+        raise HttpError("body refused")
+    if q.n_entries > cap_entries:
+        return decode_body(body, q.n_entries)
+    t = txt.tobytes()
+    s = lambda o, n: t[o:o + n].decode()  # noqa: E731
+    pairs = [(s(int(e["key_off"]), int(e["key_len"])), s(int(e["val_off"]), int(e["val_len"]))) for e in ent[:q.n_entries]]
+    return s(q.ns_off, q.ns_len), pairs, q.delta, q.response_headers
+
+
+_view = _rls._view
+
+
+class HttpApi:
+    """The HTTP API over an RlsService (its matcher, engine, workers and metrics).  Not thread-safe, and not to be used
+    concurrently with the RlsService: one batch of either surface at a time."""
+
+    def __init__(self, rls_service: _rls.RlsService):
+        self._lib = _lib()
+        self._rls = rls_service  # keep it alive
+        h = C.c_void_p()
+        if self._lib.rl_http_create(rls_service._h, C.byref(h)) != 0:
+            raise HttpError("rl_http_create failed")
+        self._h = h
+        self._n = 0
+
+    def close(self):
+        if self._h:
+            self._lib.rl_http_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, status):
+        if status != 0:
+            raise HttpError(self._lib.rl_http_last_error(self._h).decode())
+
+    def plan(self, endpoint: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """Stage 1 on the CPU workers -> dict(n_store, ctr_off, ctrs, delta, now_us, load_counters, store_index): copies
+        of the store requests (load_counters: one flag per store request)."""
+        return self._plan(self._lib.rl_http_plan, endpoint, buf, off, now_us)
+
+    def plan_device(self, endpoint: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """Stage 1 on the engine's device; the same dict as `plan`, array for array."""
+        return self._plan(self._lib.rl_http_plan_device, endpoint, buf, off, now_us)
+
+    def _plan(self, fn, endpoint, buf, off, now_us):
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        n = len(off) - 1
+        self._keep, self._n = (buf, off), n
+        self._check(fn(self._h, endpoint, n, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
+        ns = C.c_uint64()
+        p_off, p_ctr, p_delta, p_now, p_load, p_idx = (C.c_void_p() for _ in range(6))
+        self._check(self._lib.rl_http_plan_view(self._h, C.byref(ns), C.byref(p_off), C.byref(p_ctr), C.byref(p_delta),
+                                                C.byref(p_now), C.byref(p_load), C.byref(p_idx)))
+        m = ns.value
+        ctr_off = _view(p_off.value, m + 1, np.uint32).copy()
+        return {
+            "n_store": m, "ctr_off": ctr_off,
+            "ctrs": _view(p_ctr.value, int(ctr_off[-1]) if m else 0, _eng.COUNTER_DTYPE).copy(),
+            "delta": _view(p_delta.value, m, np.uint64).copy(), "now_us": _view(p_now.value, m, np.uint64).copy(),
+            "load_counters": _view(p_load.value, m, np.uint8).copy(), "store_index": _view(p_idx.value, n, np.uint32).copy(),
+        }
+
+    def finish(self, limited=None, first_limited=None, remaining=None, ttl_us=None, store_status=None):
+        """Stage 3.  store_status: one status per store request (None = all OK)."""
+        arrs = []
+
+        def ptr(a, dt):
+            if a is None:
+                return None
+            a = np.ascontiguousarray(a, dtype=dt)
+            arrs.append(a)
+            return a.ctypes.data if len(a) else None
+
+        self._check(self._lib.rl_http_finish(self._h, ptr(store_status, np.int32), ptr(limited, np.uint8),
+                                             ptr(first_limited, np.uint32), ptr(remaining, np.uint64), ptr(ttl_us, np.uint64)))
+        return self.responses()
+
+    def responses(self) -> List[Tuple[int, bytes, Dict[str, str]]]:
+        """-> [(status, body, headers)] of the last finished batch; headers holds the X-RateLimit-* headers present."""
+        ps, pb, pbo, ph, pho = (C.c_void_p() for _ in range(5))
+        self._check(self._lib.rl_http_responses(self._h, C.byref(ps), C.byref(pb), C.byref(pbo), C.byref(ph), C.byref(pho)))
+        n = self._n
+        status = _view(ps.value, n, np.uint16)
+        bo = _view(pbo.value, n + 1, np.uint64)
+        ho = _view(pho.value, 3 * n + 1, np.uint64)
+        body = _view(pb.value, int(bo[-1]) if n else 0, np.uint8).tobytes()
+        hv = _view(ph.value, int(ho[-1]) if n else 0, np.uint8).tobytes()
+        out = []
+        for i in range(n):
+            hdrs = {}
+            for k, name in enumerate(HEADER_NAMES):
+                v = hv[int(ho[3 * i + k]):int(ho[3 * i + k + 1])]
+                if v:
+                    hdrs[name] = v.decode()
+            out.append((int(status[i]), body[int(bo[i]):int(bo[i + 1])], hdrs))
+        return out
+
+    def serve(self, endpoint: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """plan_device -> the engine (one call per run) -> finish.  Needs an engine."""
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        self._keep, self._n = (buf, off), len(off) - 1
+        self._check(self._lib.rl_http_serve(self._h, endpoint, len(off) - 1, buf.ctypes.data if len(buf) else None,
+                                            off.ctypes.data, now_us))
+
+    def timings(self) -> Dict[str, float]:
+        a, b, c, k = C.c_double(), C.c_double(), C.c_double(), C.c_uint32()
+        self._lib.rl_http_last_timings(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(k))
+        return {"plan_us": a.value, "store_us": b.value, "finish_us": c.value, "store_calls": k.value}
+
+    def metrics(self) -> str:
+        """The shared metrics text (rl_rls_metrics_render): the same as the RLS service's."""
+        return self._rls.metrics()
+
+
+def store_runs(load_counters: np.ndarray) -> List[Tuple[int, int]]:
+    """The store calls of a plan: maximal runs [j0, j1) of equal load_counters flags."""
+    lc = np.asarray(load_counters)
+    if len(lc) == 0:
+        return []
+    cuts = [0] + [int(j) for j in np.flatnonzero(lc[1:] != lc[:-1]) + 1] + [len(lc)]
+    return list(zip(cuts[:-1], cuts[1:]))
