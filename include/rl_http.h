@@ -3,6 +3,7 @@
  * Replaces, batched,
  *   check / report / check_and_report      limitador-server/src/http_api/server.rs:129-260
  *   add_response_header                    limitador-server/src/http_api/server.rs:262-280
+ *   get_limits / get_counters              limitador-server/src/http_api/server.rs:88-125 (types request_types.rs:18-96)
  * over the JSON body CheckAndReportInfo {namespace, values, delta, response_headers}
  * (limitador-server/src/http_api/request_types.rs:10-16).  The HTTP server itself (routing, content type, body size
  * limit, /status, /metrics) stays with the caller: a batch here is a list of request bodies of one endpoint.
@@ -94,6 +95,32 @@ int rl_http_serve(rl_http *h, int endpoint, uint64_t n, const uint8_t *buf, cons
 /* Stage timings of the last serve call in microseconds, and the store calls it made. */
 int rl_http_last_timings(rl_http *h, double *out_plan_us, double *out_store_us, double *out_finish_us,
                          uint32_t *out_store_calls);
+
+/* ---- GET /limits/{namespace} and GET /counters/{namespace} --------------------------------------------------------
+ * ns[0 .. ns_len) is the path segment as the caller's router decoded it.  Bodies as actix Json + serde_json write them:
+ * compact, fields in declaration order, strings with the short escapes and lower-case \u00XX, everything else raw.
+ *   Limit    {"id":null,"namespace":..,"max_value":..,"seconds":..,"name":null|"..","conditions":[..],"variables":[..]}
+ *            (id: the matcher keeps no limit ids; conditions / variables: the sorted identity sources)
+ *   Counter  {"limit":{..},"set_variables":{source:value, sorted by source},"remaining":..,"expires_in_seconds":..}
+ * Arrays in a deterministic order: limits in counter order; counters by (the limit's position, key_lo, key_hi).
+ * Outcomes: 200 with the array (an unknown namespace: 200 []); /counters answers 500 `Internal server error` when the
+ * engine call fails or when a listed qualified counter has no recorded variables (keeping off, a dropped key, or a
+ * counter that came from an import or a direct engine call: see rl_rls_keep_counter_vars), never a counter with empty
+ * or guessed variables.  The response is read with rl_http_get_response. */
+int rl_http_get_limits(rl_http *h, const char *ns, uint32_t ns_len);
+/* The namespace's counters with ttl(now_us) > 0 (rl_get_counters; 0 = wall clock), the live limits' only, joined with the
+ * recorded variables on the engine's device. */
+int rl_http_get_counters(rl_http *h, const char *ns, uint32_t ns_len, uint64_t now_us);
+/* The rendering of GET /counters on its own (no engine needed): n counters with their remaining / ttl_us (as
+ * rl_get_counters reports them), counter i's recorded blob at blobs[blob_off[i] .. blob_off[i+1]) (the values in the
+ * order of the limit's variables, each a u32 little-endian length then the bytes) and unnamed[i] != 0 for a qualified
+ * counter without one.  Counters of other namespaces' or deleted limits are left out. */
+int rl_http_render_counters(rl_http *h, const char *ns, uint32_t ns_len, uint64_t n, const rl_counter *ctrs,
+                            const uint64_t *remaining, const uint64_t *ttl_us, const uint8_t *blobs, const uint64_t *blob_off,
+                            const uint8_t *unnamed);
+/* The last GET response: status, body (valid until the next GET call), and the qualified counters it found unnamed. */
+int rl_http_get_response(rl_http *h, uint16_t *out_status, const uint8_t **out_body, uint64_t *out_len,
+                         uint64_t *out_unnamed);
 
 #ifdef __cplusplus
 }

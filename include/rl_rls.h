@@ -114,6 +114,26 @@ int rl_rls_responses(rl_rls *s, const uint8_t **out_buf, const uint64_t **out_of
  * finish. */
 int rl_rls_serve(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
 
+/* ---- counter variables (GET /counters, include/rl_http.h) ------------------------------------------------------
+ * The store keeps a counter's 96-bit key digest only.  With keeping on, every device plan (rl_rls_serve,
+ * rl_rls_plan_device and their HTTP counterparts on the same service) records the variable values behind the keys it
+ * produced in a dictionary on the engine's device: (variable set, key) -> the values, in the order of the limit's sorted
+ * variables.  A key is recorded once, on the batch that first produced it (one device probe per variable set per store
+ * request after that).  The CPU plans (rl_rls_plan, rl_http_plan) do not record.
+ *   rl_rls_keep_counter_vars   off by default; max_keys slots (rounded up to a power of two; size it about twice the
+ *                              live qualified counters: a key probes at most 64 slots) and arena_bytes of values, both
+ *                              fixed until the next call.  (0, 0) turns it off and frees the memory; any call starts empty.
+ *   rl_rls_counter_vars_stats  entries, arena bytes in use, and keys dropped since it was turned on: a full table or
+ *                              arena never fails or delays a serve call, the key is simply not recorded (and its
+ *                              counters are "unnamed" in GET /counters until a later batch records it after a GC).
+ *   rl_rls_counter_vars_gc     keep exactly the entries the engine's present counters reference
+ *                              (rl_counters_export(NULL, now_us)) in a fresh table and a compacted arena (needs a second
+ *                              arena of the same size for the length of the call).  Serialise with serve, as rl_compact.
+ * Needs a service created with an engine. */
+int rl_rls_keep_counter_vars(rl_rls *s, uint64_t max_keys, uint64_t arena_bytes);
+int rl_rls_counter_vars_stats(rl_rls *s, uint64_t *out_keys, uint64_t *out_arena_used, uint64_t *out_dropped);
+int rl_rls_counter_vars_gc(rl_rls *s, uint64_t now_us, uint64_t *out_kept, uint64_t *out_freed);
+
 /* Prometheus text exposition of authorized_calls / authorized_hits / limited_calls (sorted by label values) plus
  * `limitador_up 1`: lines `name{limitador_namespace="ns"[,limit_name="x"]} value` as
  * metrics_exporter_prometheus renders them (prometheus_metrics.rs:415-447).  *out_len = bytes needed incl. NUL. */

@@ -20,6 +20,7 @@
 #include "rl_blake2b.h"
 #include "rl_match.h"
 #include "rl_match_image.h"
+#include "rl_match_records.h"
 
 namespace {
 
@@ -760,6 +761,33 @@ int rl_matcher_image(rl_matcher* m, uint32_t* out, uint64_t cap_words, uint64_t*
     memcpy(out, w.data(), w.size() * sizeof(uint32_t));
     return RL_OK;
 }
+
+}  // extern "C"
+
+bool rl_matcher_ns_limit_records(rl_matcher* m, const std::string& ns, std::vector<RlLimitRecord>& out) {
+    out.clear();
+    if (!m) return false;
+    std::shared_lock<std::shared_mutex> lock(m->mu);
+    const auto it = m->ns_ids.find(ns);
+    if (it == m->ns_ids.end()) return false;
+    for (const uint32_t lid : m->ns_limits[it->second]) {
+        const MLimit& L = m->limits[lid];
+        if (L.deleted) continue;
+        RlLimitRecord r;
+        r.limit_id = lid;
+        r.varset_id = L.varset_id;
+        r.max_value = L.max_value;
+        r.seconds = L.seconds;
+        r.has_name = L.has_name;
+        r.name = L.name;
+        r.conditions = L.conds;
+        r.variables = L.vars;
+        out.push_back(std::move(r));
+    }
+    return true;
+}
+
+extern "C" {
 
 void rl_counter_key(const char* const* sources, const char* const* values, uint32_t n, uint64_t* key_lo, uint64_t* key_hi) {
     *key_lo = *key_hi = 0;

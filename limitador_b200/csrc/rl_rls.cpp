@@ -27,6 +27,7 @@
 
 #include "rl_http.h"
 #include "rl_json.h"
+#include "rl_match_records.h"
 #include "rl_rls.h"
 #include "rl_rls_dev.h"
 #include "rl_wire.h"
@@ -51,6 +52,17 @@ __attribute__((weak)) int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int e
                                              uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
                                              rl_counter* ctrs);
 __attribute__((weak)) int rl_rls_dev_wait(rl_rls_dev* st);
+__attribute__((weak)) int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64_t arena_bytes);
+__attribute__((weak)) int rl_cv_dev_stats(rl_rls_dev* st, uint64_t* out_slots, uint64_t* out_keys, uint64_t* out_arena_used,
+                                          uint64_t* out_dropped);
+__attribute__((weak)) int rl_cv_dev_lookup(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* limit_id,
+                                           const uint64_t* key_lo, const uint64_t* key_hi, const uint8_t** out_blobs,
+                                           const uint64_t** out_blob_off, const uint8_t** out_unnamed);
+__attribute__((weak)) int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, uint64_t* out_kept,
+                                       uint64_t* out_freed);
+__attribute__((weak)) int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_t now_us, uint64_t cap,
+                                          uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi,
+                                          uint64_t* out_remaining, uint64_t* out_ttl_us, uint64_t* out_count);
 __attribute__((weak)) const char* rl_rls_dev_error(rl_rls_dev* st);
 __attribute__((weak)) void rl_rls_dev_destroy(rl_rls_dev* st);
 }
@@ -296,6 +308,10 @@ struct rl_http {
     std::vector<uint64_t> body_off, hval_off;
     double t_plan = 0, t_store = 0, t_finish = 0;
     uint32_t store_calls = 0;
+    // the last GET response
+    uint16_t get_status = 0;
+    std::string get_body;
+    uint64_t get_unnamed = 0;
 };
 
 namespace {
@@ -887,6 +903,130 @@ void take_http_device_plan(rl_http* h, const HttpDevReq* req, const uint8_t* buf
     h->planned = true;
 }
 
+// ---- GET /limits and GET /counters (include/rl_http.h) -----------------------------------------------------------
+// A string as serde_json writes it (ser.rs format_escaped_str): the short escapes, \u00XX (lower-case hex) for the other
+// control characters, every other byte as it is (the strings are UTF-8 already).
+void json_str(std::string& o, const char* p, size_t n) {
+    static const char kHex[] = "0123456789abcdef";
+    o.push_back('"');
+    for (size_t i = 0; i < n; i++) {
+        const unsigned char c = (unsigned char)p[i];
+        switch (c) {
+            case '"': o += "\\\""; break;
+            case '\\': o += "\\\\"; break;
+            case '\b': o += "\\b"; break;
+            case '\f': o += "\\f"; break;
+            case '\n': o += "\\n"; break;
+            case '\r': o += "\\r"; break;
+            case '\t': o += "\\t"; break;
+            default:
+                if (c < 0x20) {
+                    o += "\\u00";
+                    o.push_back(kHex[c >> 4]);
+                    o.push_back(kHex[c & 15]);
+                } else {
+                    o.push_back((char)c);
+                }
+        }
+    }
+    o.push_back('"');
+}
+void json_str(std::string& o, const std::string& s) { json_str(o, s.data(), s.size()); }
+
+void json_str_list(std::string& o, const std::vector<std::string>& v) {
+    o.push_back('[');
+    for (size_t i = 0; i < v.size(); i++) {
+        if (i) o.push_back(',');
+        json_str(o, v[i]);
+    }
+    o.push_back(']');
+}
+
+// request_types.rs Limit; id is always null (the matcher keeps no limit ids)
+void json_limit(std::string& o, const std::string& ns, const RlLimitRecord& L) {
+    o += "{\"id\":null,\"namespace\":";
+    json_str(o, ns);
+    o += ",\"max_value\":" + std::to_string(L.max_value) + ",\"seconds\":" + std::to_string(L.seconds) + ",\"name\":";
+    if (L.has_name) json_str(o, L.name);
+    else o += "null";
+    o += ",\"conditions\":";
+    json_str_list(o, L.conditions);
+    o += ",\"variables\":";
+    json_str_list(o, L.variables);
+    o.push_back('}');
+}
+
+void get_answer(rl_http* h, uint16_t status, std::string body, uint64_t unnamed) {
+    h->get_status = status;
+    h->get_body = std::move(body);
+    h->get_unnamed = unnamed;
+}
+
+// Counter i's set_variables from its blob, or false when the blob does not hold exactly one value per variable.
+bool blob_values(const uint8_t* b, uint64_t len, size_t n_vars, std::vector<std::pair<const char*, uint32_t>>& out) {
+    out.clear();
+    uint64_t at = 0;
+    while (at < len) {
+        if (len - at < 4) return false;
+        const uint32_t l = (uint32_t)b[at] | (uint32_t)b[at + 1] << 8 | (uint32_t)b[at + 2] << 16 | (uint32_t)b[at + 3] << 24;
+        at += 4;
+        if (len - at < l) return false;
+        out.emplace_back((const char*)b + at, l);
+        at += l;
+    }
+    return out.size() == n_vars;
+}
+
+// The /counters body of namespace ns over the given counters (the rendering stage of rl_http_get_counters).
+void render_counters(rl_http* h, const std::string& ns, uint64_t n, const rl_counter* ctrs, const uint64_t* rem, const uint64_t* ttl,
+                     const uint8_t* blobs, const uint64_t* blob_off, const uint8_t* unnamed) {
+    std::vector<RlLimitRecord> lims;
+    if (!rl_matcher_ns_limit_records(h->m, ns, lims)) return get_answer(h, 200, "[]", 0);
+    std::unordered_map<uint32_t, uint32_t> pos;  // limit id -> position among the namespace's live limits
+    for (uint32_t k = 0; k < lims.size(); k++) pos[lims[k].limit_id] = k;
+    struct Row {
+        uint32_t pos;
+        uint64_t lo, hi, i;
+    };
+    std::vector<Row> rows;
+    for (uint64_t i = 0; i < n; i++) {
+        const auto it = pos.find(ctrs[i].limit_id);
+        if (it != pos.end()) rows.push_back({it->second, ctrs[i].key_lo, ctrs[i].key_hi, i});
+    }
+    std::sort(rows.begin(), rows.end(), [](const Row& a, const Row& b) {
+        return a.pos != b.pos ? a.pos < b.pos : a.lo != b.lo ? a.lo < b.lo : a.hi != b.hi ? a.hi < b.hi : a.i < b.i;
+    });
+    std::string o = "[";
+    uint64_t bad = 0;
+    std::vector<std::pair<const char*, uint32_t>> vals;
+    for (const Row& r : rows) {
+        const RlLimitRecord& L = lims[r.pos];
+        const uint64_t i = r.i;
+        if (!L.variables.empty() &&
+            ((unnamed && unnamed[i]) || !blob_values(blobs + blob_off[i], blob_off[i + 1] - blob_off[i], L.variables.size(), vals))) {
+            bad++;
+            continue;
+        }
+        if (o.size() > 1) o.push_back(',');
+        o += "{\"limit\":";
+        json_limit(o, ns, L);
+        o += ",\"set_variables\":{";
+        for (size_t v = 0; v < L.variables.size(); v++) {  // sorted by source, as a BTreeMap
+            if (v) o.push_back(',');
+            json_str(o, L.variables[v]);
+            o.push_back(':');
+            json_str(o, vals[v].first, vals[v].second);
+        }
+        o += "},\"remaining\":" + std::to_string(rem[i]) + ",\"expires_in_seconds\":" + std::to_string(ttl[i] / 1000000ull) + "}";
+    }
+    o.push_back(']');
+    if (bad) {
+        h->last_error = std::to_string(bad) + " qualified counter(s) of namespace have no recorded variables";
+        return get_answer(h, 500, "Internal server error", bad);
+    }
+    get_answer(h, 200, std::move(o), 0);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1289,6 +1429,127 @@ int rl_http_last_timings(rl_http* h, double* out_plan_us, double* out_store_us, 
     if (out_store_us) *out_store_us = h->t_store;
     if (out_finish_us) *out_finish_us = h->t_finish;
     if (out_store_calls) *out_store_calls = h->store_calls;
+    return RL_OK;
+}
+
+// ---- counter variables and the GET endpoints -------------------------------------------------------------------
+int rl_rls_keep_counter_vars(rl_rls* s, uint64_t max_keys, uint64_t arena_bytes) {
+    if (!s) return RL_FATAL;
+    if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
+    if (!rl_cv_dev_configure) return sfail(s, "this build of the library has no device plan");
+    const int r = rl_cv_dev_configure(&s->dev, s->engine, max_keys, arena_bytes);
+    if (r) s->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
+    return r;
+}
+
+int rl_rls_counter_vars_stats(rl_rls* s, uint64_t* out_keys, uint64_t* out_arena_used, uint64_t* out_dropped) {
+    if (!s) return RL_FATAL;
+    if (!rl_cv_dev_stats) return sfail(s, "this build of the library has no device plan");
+    const int r = rl_cv_dev_stats(s->dev, nullptr, out_keys, out_arena_used, out_dropped);
+    if (r) s->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
+    return r;
+}
+
+int rl_rls_counter_vars_gc(rl_rls* s, uint64_t now_us, uint64_t* out_kept, uint64_t* out_freed) {
+    if (!s) return RL_FATAL;
+    if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
+    if (!rl_cv_dev_gc) return sfail(s, "this build of the library has no device plan");
+    const int r = rl_cv_dev_gc(&s->dev, s->engine, s->m, now_us ? now_us : wall_us(), out_kept, out_freed);
+    if (r) s->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
+    return r;
+}
+
+int rl_http_get_limits(rl_http* h, const char* ns, uint32_t ns_len) {
+    if (!h || (ns_len && !ns)) return RL_FATAL;
+    const std::string name(ns ? ns : "", ns_len);
+    std::vector<RlLimitRecord> lims;
+    rl_matcher_ns_limit_records(h->m, name, lims);  // an unknown namespace has none: 200 []
+    std::string o = "[";
+    for (size_t k = 0; k < lims.size(); k++) {
+        if (k) o.push_back(',');
+        json_limit(o, name, lims[k]);
+    }
+    o.push_back(']');
+    get_answer(h, 200, std::move(o), 0);
+    return RL_OK;
+}
+
+int rl_http_get_counters(rl_http* h, const char* ns, uint32_t ns_len, uint64_t now_us) {
+    if (!h || (ns_len && !ns)) return RL_FATAL;
+    if (!h->engine || !rl_get_counters || !rl_cv_dev_lookup) return sfail(h, "GET /counters needs a service created with an engine");
+    const std::string name(ns ? ns : "", ns_len);
+    std::vector<RlLimitRecord> lims;
+    if (!rl_matcher_ns_limit_records(h->m, name, lims) || lims.empty()) {
+        get_answer(h, 200, "[]", 0);
+        return RL_OK;
+    }
+    const uint64_t now = now_us ? now_us : wall_us();
+    std::vector<uint32_t> ids;
+    for (const auto& L : lims) ids.push_back(L.limit_id);
+    // every counter of the namespace with ttl > 0 (in_memory.rs:158-187); it may hold deleted limits' counters too
+    std::vector<uint32_t> lid;
+    std::vector<uint64_t> lo, hi, rem, ttl;
+    uint64_t cap = 4096, found = 0;
+    for (;;) {
+        lid.resize(cap);
+        lo.resize(cap);
+        hi.resize(cap);
+        rem.resize(cap);
+        ttl.resize(cap);
+        if (rl_get_counters(h->engine, ids.data(), (uint32_t)ids.size(), now, cap, lid.data(), lo.data(), hi.data(), rem.data(),
+                            ttl.data(), &found) != RL_OK) {
+            h->last_error = std::string("get_counters failed: ") + rl_last_error(h->engine);
+            get_answer(h, 500, "Internal server error", 0);
+            return RL_OK;
+        }
+        if (found <= cap) break;
+        cap = found + found / 8;
+    }
+    // the live limits' counters only, then their variables from the device dictionary
+    std::vector<uint8_t> live(1, 0);
+    for (const uint32_t x : ids) {
+        if (x >= live.size()) live.resize(x + 1, 0);
+        live[x] = 1;
+    }
+    uint64_t k = 0;
+    for (uint64_t i = 0; i < found; i++)
+        if (lid[i] < live.size() && live[lid[i]]) {
+            lid[k] = lid[i];
+            lo[k] = lo[i];
+            hi[k] = hi[i];
+            rem[k] = rem[i];
+            ttl[k] = ttl[i];
+            k++;
+        }
+    const uint8_t *blobs = nullptr, *unnamed = nullptr;
+    const uint64_t* blob_off = nullptr;
+    rl_rls* s = h->rls;
+    if (rl_cv_dev_lookup(&s->dev, h->engine, h->m, k, lid.data(), lo.data(), hi.data(), &blobs, &blob_off, &unnamed) != RL_OK) {
+        h->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
+        get_answer(h, 500, "Internal server error", 0);
+        return RL_OK;
+    }
+    std::vector<rl_counter> ctrs(k);
+    for (uint64_t i = 0; i < k; i++) ctrs[i] = rl_counter{lid[i], 0, lo[i], hi[i]};
+    render_counters(h, name, k, ctrs.data(), rem.data(), ttl.data(), blobs, blob_off, unnamed);
+    return RL_OK;
+}
+
+int rl_http_render_counters(rl_http* h, const char* ns, uint32_t ns_len, uint64_t n, const rl_counter* ctrs, const uint64_t* remaining,
+                            const uint64_t* ttl_us, const uint8_t* blobs, const uint64_t* blob_off, const uint8_t* unnamed) {
+    if (!h || (ns_len && !ns) || (n && (!ctrs || !remaining || !ttl_us || !blob_off))) return RL_FATAL;
+    static const uint8_t kNone = 0;
+    render_counters(h, std::string(ns ? ns : "", ns_len), n, ctrs, remaining, ttl_us, blobs ? blobs : &kNone, blob_off, unnamed);
+    return RL_OK;
+}
+
+int rl_http_get_response(rl_http* h, uint16_t* out_status, const uint8_t** out_body, uint64_t* out_len, uint64_t* out_unnamed) {
+    if (!h) return RL_FATAL;
+    if (!h->get_status) return sfail(h, "no GET response");
+    if (out_status) *out_status = h->get_status;
+    if (out_body) *out_body = (const uint8_t*)h->get_body.data();
+    if (out_len) *out_len = h->get_body.size();
+    if (out_unnamed) *out_unnamed = h->get_unnamed;
     return RL_OK;
 }
 

@@ -17,6 +17,7 @@
 
 #include <cub/device/device_scan.cuh>
 
+#include "rl_cvars_dev.cuh"
 #include "rl_http_dev.cuh"
 #include "rl_internal.h"
 #include "rl_rls_dev.cuh"
@@ -37,6 +38,20 @@ struct DBuf {
         const cudaError_t r = cudaMalloc((void**)&p, want * sizeof(T));
         if (r == cudaSuccess) cap = want;
         return r;
+    }
+    // exactly n elements (0: none), the old contents dropped
+    cudaError_t exact(size_t n) {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        if (n == 0) return cudaSuccess;
+        const cudaError_t r = cudaMalloc((void**)&p, n * sizeof(T));
+        if (r == cudaSuccess) cap = n;
+        return r;
+    }
+    void swap(DBuf& o) {
+        std::swap(p, o.p);
+        std::swap(cap, o.cap);
     }
     ~DBuf() {
         if (p) cudaFree(p);
@@ -99,6 +114,19 @@ struct rl_rls_dev {
     DBuf<uint32_t> d_runs, d_ctr_run;
     HBuf<uint32_t> h_runs;
     uint32_t n_runs = 0;
+    // the counter variable dictionary (rl_cvars_dev.cuh): off while cv_slots == 0
+    uint64_t cv_slots = 0, cv_arena_bytes = 0;
+    DBuf<CvSlot> d_cv_slots;
+    DBuf<uint8_t> d_cv_arena;
+    DBuf<unsigned long long> d_cv_ctl;
+    // lookup and GC scratch
+    DBuf<uint32_t> d_cv_lid;
+    DBuf<uint64_t> d_cv_lo, d_cv_hi, d_cv_val, d_cv_exp, d_cv_src;
+    DBuf<unsigned long long> d_cv_len, d_cv_pos;
+    DBuf<uint8_t> d_cv_mark, d_cv_out;
+    std::vector<unsigned long long> h_cv_pos;
+    std::vector<uint64_t> h_cv_src;
+    std::vector<uint8_t> h_cv_out, h_cv_unnamed;
 };
 
 namespace {
@@ -215,6 +243,47 @@ int reserve_outputs(rl_rls_dev* S, bool load_counters) {
     return RL_OK;
 }
 
+CvDict cv_dict(rl_rls_dev* S) {
+    return CvDict{S->d_cv_slots.p, S->cv_slots - 1, S->d_cv_arena.p, S->cv_arena_bytes, S->d_cv_ctl.p};
+}
+
+// k_counter_vars_record after a plan's scatter, when keeping is on: the plan's scratch is still the batch's.  Returns the
+// kernels launched (0 or 1).
+template <class Dec>
+int record_vars(rl_rls_dev* S, uint64_t n, uint32_t per_req, const unsigned long long* rls_count, const HttpScan* http_count,
+                uint32_t& launched) {
+    launched = 0;
+    if (!S->cv_slots || n == 0) return RL_OK;
+    CvRecordArgs a;
+    a.buf = S->d_buf.p;
+    a.off = S->d_off.p;
+    a.n = n;
+    a.img = rl_img_view(S->image.data(), S->d_image.p);
+    a.per_req = per_req;
+    a.ent = S->d_ent.p;
+    a.scratch = S->d_scratch.p;
+    a.rls_count = rls_count;
+    a.http_count = http_count;
+    a.txt = S->d_txt.p;
+    a.bits = S->d_bits.p;
+    a.dict = cv_dict(S);
+    const uint32_t threads = 128;
+    k_counter_vars_record<Dec><<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
+    RLS_CUDA(S, cudaGetLastError());
+    launched = 1;
+    return RL_OK;
+}
+
+// the engine's device and stream, and the matcher's image as it stands now
+int bind_engine(rl_rls_dev* S, rl_engine* e, rl_matcher* m) {
+    RlTableView v;
+    const int r = rl_internal_view(e, &v);
+    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
+    S->device = v.device;
+    S->stream = v.stream;
+    return m ? refresh_image(S, m) : RL_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -270,7 +339,9 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     b.now = S->d_now.p;
     k_rls_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
     RLS_CUDA(S, cudaGetLastError());
-    rl_internal_launched(e, 2);
+    uint32_t rec = 0;
+    if ((r = record_vars<CvWire>(S, n, per_req, S->d_count.p, nullptr, rec))) return r;
+    rl_internal_launched(e, 2 + rec);
     if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_req.p, S->d_req.p, n * sizeof(RlsDevReq), cudaMemcpyDeviceToHost, S->stream));
     S->n = n;
     S->n_store = n_store;
@@ -389,7 +460,9 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
     b.load = S->d_load.p;
     k_http_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
     RLS_CUDA(S, cudaGetLastError());
-    rl_internal_launched(e, 3);
+    uint32_t rec = 0;
+    if ((r = record_vars<CvJson>(S, n, per_req, nullptr, S->d_hcount.p, rec))) return r;
+    rl_internal_launched(e, 3 + rec);
     if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_hreq.p, S->d_hreq.p, n * sizeof(HttpDevReq), cudaMemcpyDeviceToHost, S->stream));
     S->n = n;
     S->n_store = n_store;
@@ -452,6 +525,169 @@ int rl_rls_dev_wait(rl_rls_dev* S) {
     if (!S) return RL_FATAL;
     RLS_CUDA(S, cudaSetDevice(S->device));
     RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    return RL_OK;
+}
+
+int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64_t arena_bytes) {
+    if (!st || !e) return RL_FATAL;
+    if (!*st) *st = new rl_rls_dev();
+    rl_rls_dev* S = *st;
+    int r = bind_engine(S, e, nullptr);
+    if (r) return r;
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));  // no batch may still write the old dictionary
+    S->cv_slots = S->cv_arena_bytes = 0;
+    RLS_CUDA(S, S->d_cv_slots.exact(0));
+    RLS_CUDA(S, S->d_cv_arena.exact(0));
+    RLS_CUDA(S, S->d_cv_ctl.exact(0));
+    if (max_keys == 0 && arena_bytes == 0) return RL_OK;
+    if (max_keys == 0 || arena_bytes == 0 || max_keys > (1ull << 40))
+        return dev_fail(S, RL_FATAL, "keeping counter variables needs max_keys in [1, 2^40] and arena_bytes > 0");
+    uint64_t slots = 16;
+    while (slots < max_keys) slots *= 2;
+    RLS_CUDA(S, S->d_cv_slots.exact(slots));
+    RLS_CUDA(S, S->d_cv_arena.exact(arena_bytes));
+    RLS_CUDA(S, S->d_cv_ctl.exact(RL_CV_CTL_WORDS));
+    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_slots.p, 0, slots * sizeof(CvSlot), S->stream));
+    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_ctl.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    S->cv_slots = slots;
+    S->cv_arena_bytes = arena_bytes;
+    return RL_OK;
+}
+
+int rl_cv_dev_stats(rl_rls_dev* S, uint64_t* out_slots, uint64_t* out_keys, uint64_t* out_arena_used, uint64_t* out_dropped) {
+    uint64_t w[RL_CV_CTL_WORDS] = {0, 0, 0, 0};
+    if (S && S->cv_slots) {
+        RLS_CUDA(S, cudaSetDevice(S->device));
+        RLS_CUDA(S, cudaMemcpyAsync(w, S->d_cv_ctl.p, sizeof w, cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    }
+    if (out_slots) *out_slots = S ? S->cv_slots : 0;
+    if (out_keys) *out_keys = w[RL_CV_KEYS];
+    if (out_arena_used) *out_arena_used = S ? std::min<uint64_t>(w[RL_CV_CURSOR], S->cv_arena_bytes) : 0;
+    if (out_dropped) *out_dropped = w[RL_CV_DROPPED];
+    return RL_OK;
+}
+
+int rl_cv_dev_lookup(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* limit_id, const uint64_t* key_lo,
+                     const uint64_t* key_hi, const uint8_t** out_blobs, const uint64_t** out_blob_off, const uint8_t** out_unnamed) {
+    if (!st || !e || !m || (n && (!limit_id || !key_lo || !key_hi)) || !out_blobs || !out_blob_off || !out_unnamed) return RL_FATAL;
+    if (!*st) *st = new rl_rls_dev();
+    rl_rls_dev* S = *st;
+    int r = bind_engine(S, e, m);
+    if (r) return r;
+    S->h_cv_pos.assign(n + 1, 0);
+    S->h_cv_src.assign(n + 1, 0);
+    S->h_cv_unnamed.assign(n + 1, 0);
+    S->h_cv_out.assign(1, 0);
+    if (!S->cv_slots) {  // keeping is off: every qualified counter is unnamed
+        const RlImage I = rl_img_view(S->image.data(), S->image.data());
+        for (uint64_t i = 0; i < n; i++) S->h_cv_unnamed[i] = limit_id[i] < I.n_limits && I.lims[5ull * limit_id[i] + 4] != 0;
+    } else if (n) {
+        RLS_CUDA(S, S->d_cv_lid.reserve(n));
+        RLS_CUDA(S, S->d_cv_lo.reserve(n));
+        RLS_CUDA(S, S->d_cv_hi.reserve(n));
+        RLS_CUDA(S, S->d_cv_src.reserve(n));
+        RLS_CUDA(S, S->d_cv_len.reserve(n + 1));
+        RLS_CUDA(S, S->d_cv_pos.reserve(n + 1));
+        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_lid.p, limit_id, n * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
+        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_lo.p, key_lo, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_hi.p, key_hi, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+        CvLookupArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S),
+                       S->d_cv_len.p, S->d_cv_src.p};
+        const uint32_t threads = 256;
+        k_counter_vars_lookup<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
+        RLS_CUDA(S, cudaGetLastError());
+        size_t tmp = 0;
+        RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
+        RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
+        RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
+        unsigned long long total = 0;
+        RLS_CUDA(S, cudaMemcpyAsync(&total, S->d_cv_pos.p + n, sizeof total, cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+        RLS_CUDA(S, S->d_cv_out.reserve(total + 1));
+        CvGatherArgs g{S->d_cv_pos.p, S->d_cv_len.p, S->d_cv_src.p, n, S->d_cv_arena.p, S->d_cv_out.p};
+        k_counter_vars_gather<<<blocks_for(n, threads), threads, 0, S->stream>>>(g);
+        RLS_CUDA(S, cudaGetLastError());
+        rl_internal_launched(e, 2);
+        S->h_cv_out.resize(total + 1);
+        if (total) RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), S->d_cv_out.p, total, cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_pos.data(), S->d_cv_pos.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_src.data(), S->d_cv_src.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+        for (uint64_t i = 0; i < n; i++) S->h_cv_unnamed[i] = S->h_cv_src[i] == RL_CV_NONE;
+    }
+    *out_blobs = S->h_cv_out.data();
+    *out_blob_off = reinterpret_cast<const uint64_t*>(S->h_cv_pos.data());
+    *out_unnamed = S->h_cv_unnamed.data();
+    return RL_OK;
+}
+
+int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, uint64_t* out_kept, uint64_t* out_freed) {
+    if (!st || !e || !m) return RL_FATAL;
+    if (out_kept) *out_kept = 0;
+    if (out_freed) *out_freed = 0;
+    if (!*st || !(*st)->cv_slots) return RL_OK;
+    rl_rls_dev* S = *st;
+    int r = bind_engine(S, e, m);
+    if (r) return r;
+    uint64_t before[RL_CV_CTL_WORDS];
+    RLS_CUDA(S, cudaMemcpyAsync(before, S->d_cv_ctl.p, sizeof before, cudaMemcpyDeviceToHost, S->stream));
+    // the engine's live counters, on the device
+    uint64_t n = 0;
+    if ((r = rl_counters_export(e, nullptr, 0, now_us, 0, RL_MEM_DEVICE, nullptr, nullptr, nullptr, nullptr, nullptr, &n)))
+        return dev_fail(S, r, "%s", rl_last_error(e));
+    RLS_CUDA(S, S->d_cv_lid.reserve(n + 1));
+    RLS_CUDA(S, S->d_cv_lo.reserve(n + 1));
+    RLS_CUDA(S, S->d_cv_hi.reserve(n + 1));
+    RLS_CUDA(S, S->d_cv_val.reserve(n + 1));
+    RLS_CUDA(S, S->d_cv_exp.reserve(n + 1));
+    uint64_t got = 0;
+    if ((r = rl_counters_export(e, nullptr, 0, now_us, n, RL_MEM_DEVICE, S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, S->d_cv_val.p,
+                                S->d_cv_exp.p, &got)))
+        return dev_fail(S, r, "%s", rl_last_error(e));
+    n = std::min(n, got);
+    // mark what they reference, then copy it into a fresh table and arena
+    const uint64_t slots = S->cv_slots;
+    RLS_CUDA(S, S->d_cv_mark.reserve(slots));
+    RLS_CUDA(S, S->d_cv_len.reserve(slots + 1));
+    RLS_CUDA(S, S->d_cv_pos.reserve(slots + 1));
+    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p, 0, slots, S->stream));
+    const uint32_t threads = 256;
+    if (n) {
+        CvMarkArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S), S->d_cv_mark.p};
+        k_counter_vars_mark<<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
+        RLS_CUDA(S, cudaGetLastError());
+    }
+    k_counter_vars_kept<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(cv_dict(S), S->d_cv_mark.p, S->d_cv_len.p);
+    RLS_CUDA(S, cudaGetLastError());
+    size_t tmp = 0;
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
+    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    DBuf<CvSlot> slots2;
+    DBuf<uint8_t> arena2;
+    DBuf<unsigned long long> ctl2;
+    RLS_CUDA(S, slots2.exact(slots));
+    RLS_CUDA(S, arena2.exact(S->cv_arena_bytes));
+    RLS_CUDA(S, ctl2.exact(RL_CV_CTL_WORDS));
+    RLS_CUDA(S, cudaMemsetAsync(slots2.p, 0, slots * sizeof(CvSlot), S->stream));
+    RLS_CUDA(S, cudaMemsetAsync(ctl2.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
+    // the count of dropped keys carries over
+    RLS_CUDA(S, cudaMemcpyAsync(ctl2.p + RL_CV_DROPPED, S->d_cv_ctl.p + RL_CV_DROPPED, sizeof(unsigned long long),
+                                cudaMemcpyDeviceToDevice, S->stream));
+    CvRebuildArgs b{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, CvDict{slots2.p, slots - 1, arena2.p, S->cv_arena_bytes, ctl2.p}};
+    k_counter_vars_rebuild<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(b);
+    RLS_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, n ? 3 : 2);
+    RLS_CUDA(S, cudaStreamSynchronize(S->stream));  // the old dictionary is read until here
+    S->d_cv_slots.swap(slots2);
+    S->d_cv_arena.swap(arena2);
+    S->d_cv_ctl.swap(ctl2);
+    uint64_t after[RL_CV_CTL_WORDS];
+    RLS_CUDA(S, cudaMemcpy(after, S->d_cv_ctl.p, sizeof after, cudaMemcpyDeviceToHost));
+    if (out_kept) *out_kept = after[RL_CV_KEYS];
+    if (out_freed) *out_freed = before[RL_CV_KEYS] - std::min(before[RL_CV_KEYS], after[RL_CV_KEYS]);
     return RL_OK;
 }
 

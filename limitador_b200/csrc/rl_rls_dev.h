@@ -59,6 +59,19 @@ int rl_http_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, u
 // ctr_off and ctrs when a run loads counters).  run_status[r] = the status of run r's call.
 int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int endpoint, int* run_status, uint8_t* limited, uint32_t* first_limited,
                        uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
+// The counter variable dictionary (rl_cvars_dev.cuh) on the same state, on the engine's device.  Both plans record into it
+// after their scatter while it is on.  configure: (0, 0) turns it off and frees it; otherwise max_keys (rounded up to a
+// power of two: the slots) and the arena's bytes.
+int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64_t arena_bytes);
+int rl_cv_dev_stats(rl_rls_dev* st, uint64_t* out_slots, uint64_t* out_keys, uint64_t* out_arena_used, uint64_t* out_dropped);
+// The blobs of n counters: counter i's at (*out_blobs)[(*out_blob_off)[i] .. [i + 1]); (*out_unnamed)[i] = 1 for a
+// qualified counter without an entry (every qualified counter while keeping is off).  Host memory owned by *st, valid
+// until the next call on it.
+int rl_cv_dev_lookup(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* limit_id, const uint64_t* key_lo,
+                     const uint64_t* key_hi, const uint8_t** out_blobs, const uint64_t** out_blob_off, const uint8_t** out_unnamed);
+// Keep exactly the entries the engine's counters reference (rl_counters_export(NULL, now_us)), in a fresh table and a
+// compacted arena.
+int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, uint64_t* out_kept, uint64_t* out_freed);
 const char* rl_rls_dev_error(rl_rls_dev* st);
 void rl_rls_dev_destroy(rl_rls_dev* st);
 }

@@ -5,7 +5,9 @@
 engine, workers and metrics: decode + counters_that_apply on the engine's GPU, one engine call per run of equal
 load_counters flags, then status / body / X-RateLimit-* headers on the CPU workers.  `plan` / `finish` are the CPU stages
 on their own (drivable without a GPU), `plan_device` is the GPU plan on its own; `serve` runs plan_device -> engine ->
-finish.  `encode_info` writes a body as serde_json serialises the struct.
+finish.  `encode_info` writes a body as serde_json serialises the struct.  `get_counters` / `get_limits` answer
+GET /counters/{namespace} and GET /limits/{namespace} (server.rs:88-125); `render_counters` is the rendering of the
+former on its own.
 """
 from __future__ import annotations
 
@@ -24,7 +26,8 @@ HEADER_NAMES = ("X-RateLimit-Limit", "X-RateLimit-Remaining", "X-RateLimit-Reset
 
 HTTP_SYMBOLS = (
     "rl_http_decode_body", "rl_http_create", "rl_http_destroy", "rl_http_last_error", "rl_http_plan", "rl_http_plan_device",
-    "rl_http_plan_view", "rl_http_finish", "rl_http_responses", "rl_http_serve", "rl_http_last_timings",
+    "rl_http_plan_view", "rl_http_finish", "rl_http_responses", "rl_http_serve", "rl_http_last_timings", "rl_http_get_limits",
+    "rl_http_get_counters", "rl_http_render_counters", "rl_http_get_response",
 )
 
 
@@ -56,6 +59,10 @@ def _lib():
     L.rl_http_responses.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.rl_http_serve.argtypes = [vp, i32, u64, vp, vp, u64]
     L.rl_http_last_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(u32)]
+    L.rl_http_get_limits.argtypes = [vp, C.c_char_p, u32]
+    L.rl_http_get_counters.argtypes = [vp, C.c_char_p, u32, u64]
+    L.rl_http_render_counters.argtypes = [vp, C.c_char_p, u32, u64, vp, vp, vp, vp, vp, vp]
+    L.rl_http_get_response.argtypes = [vp, C.POINTER(C.c_uint16), C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
     L._rl_http_ready = True
     return L
 
@@ -194,6 +201,41 @@ class HttpApi:
         a, b, c, k = C.c_double(), C.c_double(), C.c_double(), C.c_uint32()
         self._lib.rl_http_last_timings(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(k))
         return {"plan_us": a.value, "store_us": b.value, "finish_us": c.value, "store_calls": k.value}
+
+    def get_limits(self, namespace: str) -> Tuple[int, bytes]:
+        """GET /limits/{namespace} -> (status, body)."""
+        ns = namespace.encode()
+        self._check(self._lib.rl_http_get_limits(self._h, ns, len(ns)))
+        return self._get_response()[:2]
+
+    def get_counters(self, namespace: str, now_us: int = 0) -> Tuple[int, bytes]:
+        """GET /counters/{namespace} at now_us (0 = wall clock) -> (status, body).  Needs an engine, and the RLS service
+        keeping counter variables (RlsService.keep_counter_vars) for any qualified counter to be listed."""
+        ns = namespace.encode()
+        self._check(self._lib.rl_http_get_counters(self._h, ns, len(ns), now_us))
+        status, body, self.last_unnamed = self._get_response()
+        return status, body
+
+    def render_counters(self, namespace: str, ctrs, remaining, ttl_us, blobs: bytes, blob_off, unnamed=None) -> Tuple[int, bytes]:
+        """The rendering stage of get_counters on its own: counters (COUNTER_DTYPE), remaining / ttl_us per counter, the
+        blobs packed (counter i's at blobs[blob_off[i]:blob_off[i + 1]]) and the unnamed flags -> (status, body)."""
+        ns = namespace.encode()
+        ctrs = np.ascontiguousarray(ctrs, dtype=_eng.COUNTER_DTYPE)
+        n = len(ctrs)
+        rem = np.ascontiguousarray(remaining, dtype=np.uint64)
+        ttl = np.ascontiguousarray(ttl_us, dtype=np.uint64)
+        bl = np.frombuffer(bytes(blobs) or b"\0", dtype=np.uint8)
+        bo = np.ascontiguousarray(blob_off, dtype=np.uint64)
+        un = None if unnamed is None else np.ascontiguousarray(unnamed, dtype=np.uint8)
+        p = lambda a: a.ctypes.data if a is not None and len(a) else None  # noqa: E731
+        self._check(self._lib.rl_http_render_counters(self._h, ns, len(ns), n, p(ctrs), p(rem), p(ttl), p(bl), p(bo), p(un)))
+        status, body, self.last_unnamed = self._get_response()
+        return status, body
+
+    def _get_response(self):
+        st, pb, ln, un = C.c_uint16(), C.c_void_p(), C.c_uint64(), C.c_uint64()
+        self._check(self._lib.rl_http_get_response(self._h, C.byref(st), C.byref(pb), C.byref(ln), C.byref(un)))
+        return int(st.value), _view(pb.value, ln.value, np.uint8).tobytes(), un.value
 
     def metrics(self) -> str:
         """The shared metrics text (rl_rls_metrics_render): the same as the RLS service's."""

@@ -27,7 +27,8 @@ NO_STORE = 0xFFFFFFFF
 RLS_SYMBOLS = (
     "rl_rls_decode_request", "rl_rls_encode_response", "rl_rls_create", "rl_rls_destroy", "rl_rls_last_error",
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
-    "rl_rls_last_timings", "rl_rls_plan_device",
+    "rl_rls_last_timings", "rl_rls_plan_device", "rl_rls_keep_counter_vars", "rl_rls_counter_vars_stats",
+    "rl_rls_counter_vars_gc",
 )
 
 ENTRY_DTYPE = np.dtype([("descriptor", "<u4"), ("key_off", "<u4"), ("key_len", "<u4"), ("val_off", "<u4"), ("val_len", "<u4")])
@@ -63,6 +64,9 @@ def _lib():
     L.rl_rls_serve.argtypes = [vp, i32, u64, vp, vp, u64]
     L.rl_rls_metrics_render.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.rl_rls_last_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    L.rl_rls_keep_counter_vars.argtypes = [vp, u64, u64]
+    L.rl_rls_counter_vars_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.rl_rls_counter_vars_gc.argtypes = [vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L._rl_rls_ready = True
     return L
 
@@ -287,6 +291,22 @@ class RlsService:
         a, b, c = C.c_double(), C.c_double(), C.c_double()
         self._lib.rl_rls_last_timings(self._h, C.byref(a), C.byref(b), C.byref(c))
         return {"plan_us": a.value, "store_us": b.value, "finish_us": c.value}
+
+    def keep_counter_vars(self, max_keys: int, arena_bytes: int):
+        """Record the variable values behind the counter keys of every device plan (GET /counters needs them) in a
+        dictionary of max_keys slots and arena_bytes of values on the engine's device; (0, 0) turns it off."""
+        self._check(self._lib.rl_rls_keep_counter_vars(self._h, max_keys, arena_bytes))
+
+    def counter_vars_stats(self) -> Dict[str, int]:
+        k, a, d = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        self._check(self._lib.rl_rls_counter_vars_stats(self._h, C.byref(k), C.byref(a), C.byref(d)))
+        return {"keys": k.value, "arena_used": a.value, "dropped": d.value}
+
+    def counter_vars_gc(self, now_us: int = 0) -> Dict[str, int]:
+        """Keep the entries the engine's present counters reference (0 = wall clock) -> {kept, freed}."""
+        k, f = C.c_uint64(), C.c_uint64()
+        self._check(self._lib.rl_rls_counter_vars_gc(self._h, now_us, C.byref(k), C.byref(f)))
+        return {"kept": k.value, "freed": f.value}
 
     def metrics(self) -> str:
         need = C.c_uint64()
