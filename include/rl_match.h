@@ -12,8 +12,11 @@
  *   seconds, conditions, variables — max_value, name and id excluded) -> dense limit_id, namespace -> ns_id,
  *   (namespace, variable set) -> varset_id, resolved variable values -> 96-bit counter key.
  *
- * Expressions accepted (anything else is refused at rl_matcher_add_limit with RL_FATAL, so that a deployment
- * can keep such limits on the reference's interpreter):
+ * Expressions accepted (anything else is refused at rl_matcher_add_limit with RL_FATAL "unsupported condition
+ * expression", so that a deployment can keep such limits on the reference's interpreter).  Two dialects, chosen per
+ * matcher with rl_matcher_set_dialect (rl_match_dialect.h); variables take the same grammar in both.
+ *
+ * RL_MATCH_DIALECT_TABLE (the default):
  *   operand   := IDENT                                      a root binding (ASCII identifier, NO dots: `req.method`
  *                                                           is CEL member access on the variable `req`, which the
  *                                                           reference never binds — limit/cel.rs:314-322)
@@ -25,6 +28,24 @@
  *                                                           reinterpreted)
  *   variable  := operand
  *
+ * RL_MATCH_DIALECT_BOOLEAN: the table dialect's conditions and boolean formulas whose result provably does not depend on
+ * how a CEL implementation propagates errors through && / || (DESIGN.md §9b).  Tokens may be separated by whitespace;
+ * operand and QUOTED are as above (a QUOTED also holds no line break; raw, byte and triple-quoted strings are refused);
+ * IDENT is no CEL reserved word, nor `descriptors` or `has`.
+ *   atom      := operand ('==' | '!=') QUOTED | QUOTED ('==' | '!=') operand
+ *              | operand '.' ('startsWith' | 'endsWith' | 'contains') '(' QUOTED ')'
+ *              | operand 'in' '[' [QUOTED (',' QUOTED)*] ']'
+ *   group     := any formula of atoms with '&&', '||', '!' and parentheses in which every atom has the SAME operand and
+ *                which holds at most RL_MATCH_MAX_ATOMS (6) atoms; a '!' directly before an ==, != or `in` needs
+ *                parentheses (CEL reads `!x == 'a'` as `(!x) == 'a'`).  An unbound or missing operand (a descriptor
+ *                index past the request's list included) makes the whole group false, whatever its formula: every
+ *                atom errors, and the reference's Predicate::test turns that into false (cel.rs:321-339).
+ *   presence  := 'has(descriptors[' N '].' IDENT ')' | QUOTED 'in descriptors[' N ']'
+ *                true iff descriptor N exists and holds the key; only positively, and only as a top-level conjunct
+ *   condition := (group | presence) ('&&' (group | presence))*
+ * Refused: || or ! across two operands, a presence test under ! or ||, `matches`, `size`, any literal that is not a
+ * string, `limit.name` / `limit.id`, dotted root operands, more than 6 atoms in one group, and all other CEL.
+ *
  * Output = exactly the inputs of rl_check_and_update_batch (include/rl_engine.h): a CSR of rl_counter.
  * Counters come out in the limits' registration order (the reference iterates a HashSet: unspecified).
  * Pure host code; no CUDA call is made by anything in this header.
@@ -35,6 +56,7 @@
 #include <stdint.h>
 
 #include "rl_engine.h"
+#include "rl_match_dialect.h" /* rl_matcher_set_dialect: which of the two grammars below later limits are parsed in */
 
 #ifdef __cplusplus
 extern "C" {

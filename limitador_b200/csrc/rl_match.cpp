@@ -3,9 +3,11 @@
 // Host-only code.  The reference walks a CEL AST per condition and per variable for every limit of the
 // namespace (limit.rs:157-174, cel.rs:185-227,314-334), building string maps on the way; here every
 // operand of every accepted expression is interned into a SLOT when the limit is added, a request's
-// bindings are dropped into the slot array once, and a limit is a list of (slot, ==|!=, literal) tests plus
-// a list of slots that must be present.  The counter key of a variable set is digested once per request
-// and shared by the limits that use the same variables.
+// bindings are dropped into the slot array once, and a limit is a list of TESTS plus a list of slots that
+// must be present.  A test is a presence test on one slot, or up to RL_MATCH_MAX_ATOMS value atoms over one
+// slot and the truth table of the boolean formula that combines them (`x == 'a'` is one atom and the table
+// 0b10, `x != 'a'` the table 0b01).  The counter key of a variable set is digested once per request and
+// shared by the limits that use the same variables.
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
@@ -73,10 +75,25 @@ struct SlotTable {
     }
 };
 
-struct Pred {
+// a value atom: RL_ATOM_* against one literal, or against a list of them for RL_ATOM_IN
+struct Atom {
+    uint32_t op;
+    std::vector<std::string> lits;
+};
+
+// a test of one operand (see rl_match_image.h): no atoms = present; else table bit `atom bits` of its value
+struct Test {
     uint32_t slot;
-    bool neq;
-    std::string lit;
+    std::vector<Atom> atoms;
+    uint64_t table;
+};
+
+// a test as parsed, before its operand is interned
+struct ParsedTest {
+    uint32_t desc;
+    std::string key;
+    std::vector<Atom> atoms;
+    uint64_t table;
 };
 
 struct MLimit {
@@ -85,7 +102,7 @@ struct MLimit {
     uint32_t ns_id = 0, varset_id = 0;
     uint64_t max_value = 0, seconds = 0;
     std::vector<std::string> conds, vars;  // sorted, unique (the identity)
-    std::vector<Pred> preds;
+    std::vector<Test> tests;
     std::vector<uint32_t> var_slots;  // same order as vars
 };
 
@@ -177,6 +194,332 @@ bool parse_variable(const char* src, uint32_t& desc, std::string& key) {
     return *p == 0;
 }
 
+// ---- the boolean dialect (RL_MATCH_DIALECT_BOOLEAN, see rl_match.h) ------------------------------
+// A recursive-descent parser over a token list, then the normal form: the top-level && split into conjuncts, each one
+// a presence test or an operand group (one operand, at most RL_MATCH_MAX_ATOMS atoms) compiled to its truth table.
+// Everything the normal form does not hold is refused on the parsed form.
+class BoolParser {
+  public:
+    explicit BoolParser(const char* src) : src_(src) {}
+
+    bool parse(std::vector<ParsedTest>& out) {
+        if (!lex()) return false;
+        int root;
+        if (!parse_or(0, root) || tok_[pos_].kind != T_END) return false;
+        std::vector<int> conj;
+        split_and(root, conj);
+        for (const int c : conj) {
+            ParsedTest t;
+            if (nodes_[c].kind == N_PRESENT) {  // only ever a top-level conjunct, and only positively
+                t.desc = nodes_[c].desc;
+                t.key = nodes_[c].key;
+                t.table = 0;
+                out.push_back(std::move(t));
+                continue;
+            }
+            std::vector<int> atoms;
+            if (!group_atoms(c, atoms) || atoms.size() > RL_MATCH_MAX_ATOMS) return false;
+            t.desc = nodes_[atoms[0]].desc;
+            t.key = nodes_[atoms[0]].key;
+            for (const int a : atoms) {
+                if (nodes_[a].desc != t.desc || nodes_[a].key != t.key) return false;  // || or ! spanning two operands
+                t.atoms.push_back(nodes_[a].atom);
+            }
+            t.table = 0;
+            for (uint32_t bits = 0; bits < (1u << atoms.size()); bits++)
+                if (eval(c, atoms, bits)) t.table |= 1ull << bits;
+            out.push_back(std::move(t));
+        }
+        return true;
+    }
+
+  private:
+    enum TokKind { T_END, T_IDENT, T_STR, T_INT, T_PUNCT };
+    struct Tok {
+        TokKind kind;
+        std::string text;  // identifier, unquoted string, digits or punctuation
+    };
+    enum NodeKind { N_ATOM, N_PRESENT, N_NOT, N_AND, N_OR };
+    struct Node {
+        NodeKind kind;
+        int a = -1, b = -1;  // operands of N_NOT (a), N_AND / N_OR (a, b)
+        uint32_t desc = 0;   // N_ATOM / N_PRESENT: the operand
+        std::string key;
+        Atom atom;           // N_ATOM
+        bool negated = false;  // N_ATOM: written with !=
+        bool relation = false;  // an ==, != or `in` not inside parentheses
+    };
+    static constexpr int kMaxDepth = 32;  // nesting of ( and !
+
+    const char* src_;
+    std::vector<Tok> tok_;
+    size_t pos_ = 0;
+    std::vector<Node> nodes_;
+
+    bool lex() {
+        const char* p = src_;
+        for (;;) {
+            skip_ws(p);
+            if (!*p) break;
+            const unsigned char c = (unsigned char)*p;
+            if (is_ident_start(c)) {
+                const char* s = p;
+                while (is_word((unsigned char)*p)) p++;
+                if (*p == '\'' || *p == '"') return false;  // r'..', b'..': raw and byte strings
+                tok_.push_back({T_IDENT, std::string(s, p)});
+            } else if (c >= '0' && c <= '9') {
+                const char* s = p;
+                while (*p >= '0' && *p <= '9') p++;
+                tok_.push_back({T_INT, std::string(s, p)});
+            } else if (c == '\'' || c == '"') {
+                if (p[1] == *p && p[2] == *p) return false;  // triple-quoted
+                const char q = *p++;
+                const char* s = p;
+                // no escape processing here: a backslash anywhere refuses the expression, as in the table dialect
+                while (*p && *p != q && *p != '\\' && *p != '\n' && *p != '\r') p++;
+                if (*p != q) return false;
+                tok_.push_back({T_STR, std::string(s, p)});
+                p++;
+            } else {
+                static const char* const kPunct[] = {"&&", "||", "==", "!=", "(", ")", "[", "]", ".", ",", "!"};
+                bool hit = false;
+                for (const char* k : kPunct) {
+                    const size_t n = strlen(k);
+                    if (strncmp(p, k, n) == 0) {
+                        tok_.push_back({T_PUNCT, k});
+                        p += n;
+                        hit = true;
+                        break;
+                    }
+                }
+                if (!hit) return false;
+            }
+        }
+        tok_.push_back({T_END, ""});
+        return true;
+    }
+
+    bool is(TokKind k, const char* text = nullptr, size_t ahead = 0) const {
+        const size_t i = std::min(pos_ + ahead, tok_.size() - 1);
+        return tok_[i].kind == k && (!text || tok_[i].text == text);
+    }
+    bool take(TokKind k, const char* text = nullptr) {
+        if (!is(k, text)) return false;
+        pos_++;
+        return true;
+    }
+    int node(Node n) {
+        nodes_.push_back(std::move(n));
+        return (int)nodes_.size() - 1;
+    }
+
+    static bool reserved(const std::string& w) {
+        static const char* const kWords[] = {"true",  "false",    "null",     "in",     "as",     "break",   "const",
+                                             "continue", "else",  "for",      "function", "if",   "import",  "let",
+                                             "loop",  "package",  "namespace", "return", "var",   "void",    "while",
+                                             "descriptors", "has"};
+        for (const char* k : kWords)
+            if (w == k) return true;
+        return false;
+    }
+
+    // descriptors[N] after the identifier: N into desc
+    bool descriptor_index(uint32_t& desc) {
+        if (!take(T_PUNCT, "[") || !is(T_INT)) return false;
+        uint64_t n = 0;
+        for (const char d : tok_[pos_].text) {
+            n = n * 10 + (uint64_t)(d - '0');
+            if (n >= RL_BIND_ROOT) return false;
+        }
+        pos_++;
+        desc = (uint32_t)n;
+        return take(T_PUNCT, "]");
+    }
+
+    // IDENT | descriptors[N].IDENT | descriptors[N]['key']
+    bool operand(uint32_t& desc, std::string& key) {
+        if (!is(T_IDENT)) return false;
+        if (tok_[pos_].text != "descriptors") {
+            if (reserved(tok_[pos_].text)) return false;
+            key = tok_[pos_++].text;
+            desc = RL_BIND_ROOT;
+            return true;
+        }
+        pos_++;
+        if (!descriptor_index(desc)) return false;
+        if (take(T_PUNCT, ".")) {
+            if (!is(T_IDENT)) return false;
+            key = tok_[pos_++].text;
+            return true;
+        }
+        if (!take(T_PUNCT, "[") || !is(T_STR) || tok_[pos_].text.empty()) return false;
+        key = tok_[pos_++].text;
+        return take(T_PUNCT, "]");
+    }
+
+    bool parse_or(int depth, int& out) {
+        if (!parse_and(depth, out)) return false;
+        while (take(T_PUNCT, "||")) {
+            int r;
+            if (!parse_and(depth, r)) return false;
+            Node n{N_OR};
+            n.a = out;
+            n.b = r;
+            out = node(std::move(n));
+        }
+        return true;
+    }
+
+    bool parse_and(int depth, int& out) {
+        if (!parse_unary(depth, out)) return false;
+        while (take(T_PUNCT, "&&")) {
+            int r;
+            if (!parse_unary(depth, r)) return false;
+            Node n{N_AND};
+            n.a = out;
+            n.b = r;
+            out = node(std::move(n));
+        }
+        return true;
+    }
+
+    // an ==, != or `in` binds looser than a leading `!` in CEL (`!x == 'a'` is `(!x) == 'a'` there): refused after a `!`
+    bool parse_unary(int depth, int& out) {
+        if (depth > kMaxDepth) return false;
+        if (take(T_PUNCT, "!")) {
+            int a;
+            if (!(is(T_PUNCT, "!") || is(T_PUNCT, "(") || is(T_IDENT)) || !parse_unary(depth + 1, a)) return false;
+            if (nodes_[a].relation) return false;
+            Node n{N_NOT};
+            n.a = a;
+            out = node(std::move(n));
+            return true;
+        }
+        return parse_primary(depth, out);
+    }
+
+    bool parse_primary(int depth, int& out) {
+        if (take(T_PUNCT, "(")) {
+            if (!parse_or(depth + 1, out) || !take(T_PUNCT, ")")) return false;
+            nodes_[out].relation = false;
+            return true;
+        }
+        if (is(T_IDENT, "has") && is(T_PUNCT, "(", 1)) {  // has(descriptors[N].IDENT)
+            pos_ += 2;
+            Node n{N_PRESENT};
+            if (!take(T_IDENT, "descriptors") || !descriptor_index(n.desc) || !take(T_PUNCT, ".") || !is(T_IDENT)) return false;
+            n.key = tok_[pos_++].text;
+            if (!take(T_PUNCT, ")")) return false;
+            out = node(std::move(n));
+            return true;
+        }
+        Node n{N_ATOM};
+        if (is(T_STR)) {  // 'key' in descriptors[N], or 'lit' ==|!= operand
+            const std::string lit = tok_[pos_++].text;
+            if (take(T_IDENT, "in")) {
+                Node p{N_PRESENT};
+                if (lit.empty() || !take(T_IDENT, "descriptors") || !descriptor_index(p.desc)) return false;
+                p.key = lit;
+                p.relation = true;
+                out = node(std::move(p));
+                return true;
+            }
+            if (is(T_PUNCT, "==") || is(T_PUNCT, "!=")) {
+                n.negated = tok_[pos_++].text == "!=";
+                if (!operand(n.desc, n.key)) return false;
+                n.atom = {RL_ATOM_EQ, {lit}};
+                n.relation = true;
+                out = node(std::move(n));
+                return true;
+            }
+            return false;
+        }
+        if (!operand(n.desc, n.key)) return false;
+        if (is(T_PUNCT, "==") || is(T_PUNCT, "!=")) {  // operand ==|!= 'lit'
+            n.negated = tok_[pos_++].text == "!=";
+            if (!is(T_STR)) return false;
+            n.atom = {RL_ATOM_EQ, {tok_[pos_++].text}};
+            n.relation = true;
+            out = node(std::move(n));
+            return true;
+        }
+        if (take(T_PUNCT, ".")) {  // operand.startsWith|endsWith|contains('lit')
+            if (!is(T_IDENT)) return false;
+            const std::string& f = tok_[pos_++].text;
+            if (f == "startsWith") n.atom.op = RL_ATOM_PREFIX;
+            else if (f == "endsWith") n.atom.op = RL_ATOM_SUFFIX;
+            else if (f == "contains") n.atom.op = RL_ATOM_CONTAINS;
+            else return false;
+            if (!take(T_PUNCT, "(") || !is(T_STR)) return false;
+            n.atom.lits.push_back(tok_[pos_++].text);
+            if (!take(T_PUNCT, ")")) return false;
+            out = node(std::move(n));
+            return true;
+        }
+        if (take(T_IDENT, "in")) {  // operand in ['lit', ...] (possibly empty, no trailing comma)
+            if (!take(T_PUNCT, "[")) return false;
+            n.atom.op = RL_ATOM_IN;
+            if (!take(T_PUNCT, "]")) {
+                do {
+                    if (!is(T_STR)) return false;
+                    n.atom.lits.push_back(tok_[pos_++].text);
+                } while (take(T_PUNCT, ","));
+                if (!take(T_PUNCT, "]")) return false;
+            }
+            n.relation = true;
+            out = node(std::move(n));
+            return true;
+        }
+        return false;
+    }
+
+    void split_and(int n, std::vector<int>& out) const {
+        if (nodes_[n].kind == N_AND) {
+            split_and(nodes_[n].a, out);
+            split_and(nodes_[n].b, out);
+        } else {
+            out.push_back(n);
+        }
+    }
+
+    // the atoms of an operand group, left to right; false if a presence test sits inside it
+    bool group_atoms(int n, std::vector<int>& out) const {
+        const Node& x = nodes_[n];
+        if (x.kind == N_PRESENT) return false;  // negated, or inside ||: refused
+        if (x.kind == N_ATOM) {
+            out.push_back(n);
+            return true;
+        }
+        if (!group_atoms(x.a, out)) return false;
+        return x.b < 0 || group_atoms(x.b, out);
+    }
+
+    // the group's formula with atom atoms[j] = bit j of `bits`
+    bool eval(int n, const std::vector<int>& atoms, uint32_t bits) const {
+        const Node& x = nodes_[n];
+        switch (x.kind) {
+            case N_ATOM: {
+                const size_t j = (size_t)(std::find(atoms.begin(), atoms.end(), n) - atoms.begin());
+                return (((bits >> j) & 1u) != 0) != x.negated;
+            }
+            case N_NOT: return !eval(x.a, atoms, bits);
+            case N_AND: return eval(x.a, atoms, bits) && eval(x.b, atoms, bits);
+            case N_OR: return eval(x.a, atoms, bits) || eval(x.b, atoms, bits);
+            default: return false;
+        }
+    }
+};
+
+// a condition of the table dialect as a one-atom test
+bool parse_table_condition(const char* src, ParsedTest& t) {
+    bool neq;
+    std::string lit;
+    if (!parse_condition(src, t.desc, t.key, neq, lit)) return false;
+    t.atoms = {Atom{RL_ATOM_EQ, {lit}}};
+    t.table = neq ? 0x1 : 0x2;  // bit 1: the value equals the literal
+    return true;
+}
+
 // per-thread request scratch: slot -> value of the current request (stamped, never cleared)
 struct Scratch {
     std::vector<const char*> val;
@@ -195,6 +538,7 @@ thread_local Scratch tls_scratch;
 struct rl_matcher {
     std::shared_mutex mu;
     uint32_t counter_cap = RL_MAX_COUNTERS_PER_REQUEST;  // rl_matcher_set_counter_cap
+    uint32_t dialect = RL_MATCH_DIALECT_TABLE;           // rl_matcher_set_dialect: how later add_limit calls parse
     std::mutex err_mu;  // last_error is also written by matching calls, which hold `mu` shared
     std::string last_error;
     SlotTable slots;
@@ -214,6 +558,14 @@ int mfail(rl_matcher* m, const char* fmt, ...) {
     va_start(ap, fmt);
     vsnprintf(buf, sizeof buf, fmt, ap);
     va_end(ap);
+    // a long expression is cut at the buffer's end: never in the middle of a UTF-8 sequence
+    size_t n = strlen(buf), s = n;
+    while (s > 0 && ((unsigned char)buf[s - 1] & 0xC0) == 0x80) s--;
+    if (s > 0 && (unsigned char)buf[s - 1] >= 0xC0) {
+        const unsigned char lead = (unsigned char)buf[s - 1];
+        const size_t need = lead >= 0xF0 ? 4 : lead >= 0xE0 ? 3 : 2;
+        if (n - (s - 1) < need) buf[s - 1] = 0;
+    }
     std::lock_guard<std::mutex> g(m->err_mu);
     m->last_error = buf;
     return RL_FATAL;
@@ -252,14 +604,24 @@ int match_one(const rl_matcher* m, uint32_t ns_id, const rl_binding* binds, uint
         const MLimit& L = m->limits[lid];
         if (L.deleted) continue;
         bool ok = true;
-        for (const Pred& p : L.preds) {
-            const char* v = (s.stamp[p.slot] == ep) ? s.val[p.slot] : nullptr;
+        for (const Test& t : L.tests) {
+            const char* v = (s.stamp[t.slot] == ep) ? s.val[t.slot] : nullptr;
             if (!v) {  // unbound name / missing key: the predicate is false (cel.rs:315-331)
                 ok = false;
                 break;
             }
-            const bool eq = strcmp(v, p.lit.c_str()) == 0;
-            if (eq == p.neq) {
+            if (t.atoms.empty()) continue;  // a presence test: bound is all it asks
+            const uint32_t n = (uint32_t)strlen(v);
+            uint32_t bits = 0;
+            for (size_t j = 0; j < t.atoms.size(); j++) {
+                const Atom& a = t.atoms[j];
+                bool hit = false;
+                for (size_t k = 0; k < a.lits.size() && !hit; k++)
+                    hit = rl_str_op(a.op == RL_ATOM_IN ? RL_ATOM_EQ : a.op, (const uint8_t*)v, n, (const uint8_t*)a.lits[k].data(),
+                                    (uint32_t)a.lits[k].size());
+                bits |= (uint32_t)hit << j;
+            }
+            if (!((t.table >> bits) & 1)) {
                 ok = false;
                 break;
             }
@@ -354,13 +716,19 @@ int rl_matcher_add_limit_ex(rl_matcher* m, const char* ns, uint64_t max_value, u
     struct Parsed {
         uint32_t desc;
         std::string key;
-        bool neq;
-        std::string lit;
     };
-    std::vector<Parsed> pc(L.conds.size()), pv(L.vars.size());
-    for (size_t i = 0; i < L.conds.size(); i++)
-        if (!parse_condition(L.conds[i].c_str(), pc[i].desc, pc[i].key, pc[i].neq, pc[i].lit))
-            return mfail(m, "unsupported condition expression: %s", L.conds[i].c_str());
+    std::vector<ParsedTest> pc;
+    std::vector<Parsed> pv(L.vars.size());
+    for (size_t i = 0; i < L.conds.size(); i++) {
+        bool ok;
+        if (m->dialect == RL_MATCH_DIALECT_BOOLEAN) {
+            ok = BoolParser(L.conds[i].c_str()).parse(pc);
+        } else {
+            pc.emplace_back();
+            ok = parse_table_condition(L.conds[i].c_str(), pc.back());
+        }
+        if (!ok) return mfail(m, "unsupported condition expression: %s", L.conds[i].c_str());
+    }
     for (size_t i = 0; i < L.vars.size(); i++)
         if (!parse_variable(L.vars[i].c_str(), pv[i].desc, pv[i].key))
             return mfail(m, "unsupported variable expression: %s", L.vars[i].c_str());
@@ -400,7 +768,7 @@ int rl_matcher_add_limit_ex(rl_matcher* m, const char* ns, uint64_t max_value, u
             if (vit == m->varsets.end()) vit = m->varsets.emplace(vk, (uint32_t)m->varsets.size() + 1).first;
             L.varset_id = vit->second;
         }
-        for (const auto& c : pc) L.preds.push_back({m->slots.intern(c.desc, c.key), c.neq, c.lit});
+        for (auto& c : pc) L.tests.push_back({m->slots.intern(c.desc, c.key), std::move(c.atoms), c.table});
         for (const auto& v : pv) L.var_slots.push_back(m->slots.intern(v.desc, v.key));
         m->by_identity.emplace(ident, lid);
         m->ns_limits[L.ns_id].push_back(lid);
@@ -414,6 +782,14 @@ int rl_matcher_add_limit_ex(rl_matcher* m, const char* ns, uint64_t max_value, u
     out_desc->qualified = R.vars.empty() ? 0 : 1;  // counter.rs:108-110
     out_desc->max_value = R.max_value;
     out_desc->window_us = R.seconds * 1000000ull;  // counter.rs:76-78
+    return RL_OK;
+}
+
+int rl_matcher_set_dialect(rl_matcher* m, uint32_t dialect) {
+    if (!m) return RL_FATAL;
+    if (dialect != RL_MATCH_DIALECT_TABLE && dialect != RL_MATCH_DIALECT_BOOLEAN) return mfail(m, "unknown dialect %u", dialect);
+    std::unique_lock<std::shared_mutex> lock(m->mu);
+    m->dialect = dialect;  // the limits already added keep their tests: the image does not change
     return RL_OK;
 }
 
@@ -716,22 +1092,38 @@ int rl_matcher_image(rl_matcher* m, uint32_t* out, uint64_t cap_words, uint64_t*
         while (tab[p] != RL_IMG_EMPTY) p = (p + 1) & slot_mask;
         tab[p] = s;
     }
-    // limits, their predicates and variables
+    // limits, their tests, the tests' atoms and the limits' variables
     const uint32_t n_limits = (uint32_t)m->limits.size();
-    std::vector<uint32_t> preds, vars;
+    std::vector<uint32_t> tests, atoms, vars;
     w[RL_IMG_H_LIMS] = (uint32_t)w.size();
     for (uint32_t lid = 0; lid < n_limits; lid++) {
         const MLimit& L = m->limits[lid];
-        w.push_back((uint32_t)(preds.size() / 4));
-        w.push_back((uint32_t)L.preds.size());
+        w.push_back((uint32_t)(tests.size() / 4));
+        w.push_back((uint32_t)L.tests.size());
         w.push_back((uint32_t)(vars.size() / 3));
         w.push_back((uint32_t)L.var_slots.size());
         w.push_back(L.varset_id);
-        for (const Pred& p : L.preds) {
-            preds.push_back(p.slot);
-            preds.push_back(p.neq ? 1u : 0u);
-            preds.push_back(put_str(p.lit));
-            preds.push_back((uint32_t)p.lit.size());
+        for (const Test& t : L.tests) {
+            tests.push_back(t.slot);
+            tests.push_back((uint32_t)(atoms.size() / 3) << 3 | (uint32_t)t.atoms.size());
+            tests.push_back((uint32_t)t.table);
+            tests.push_back((uint32_t)(t.table >> 32));
+            for (const Atom& a : t.atoms) {
+                atoms.push_back(a.op);
+                if (a.op != RL_ATOM_IN) {
+                    atoms.push_back(put_str(a.lits[0]));
+                    atoms.push_back((uint32_t)a.lits[0].size());
+                    continue;
+                }
+                atoms.push_back((uint32_t)arena.size());
+                atoms.push_back((uint32_t)a.lits.size());
+                for (const std::string& l : a.lits) {
+                    const uint32_t n = (uint32_t)l.size();
+                    const char le[4] = {(char)n, (char)(n >> 8), (char)(n >> 16), (char)(n >> 24)};
+                    arena.append(le, 4);
+                    arena += l;
+                }
+            }
         }
         for (size_t j = 0; j < L.var_slots.size(); j++) {
             vars.push_back(L.var_slots[j]);
@@ -739,8 +1131,11 @@ int rl_matcher_image(rl_matcher* m, uint32_t* out, uint64_t cap_words, uint64_t*
             vars.push_back((uint32_t)L.vars[j].size());
         }
     }
-    w[RL_IMG_H_PREDS] = (uint32_t)w.size();
-    w.insert(w.end(), preds.begin(), preds.end());
+    if (atoms.size() / 3 >= (1u << 29)) return mfail(m, "more than 2^29 value atoms in one matcher image");
+    w[RL_IMG_H_TESTS] = (uint32_t)w.size();
+    w.insert(w.end(), tests.begin(), tests.end());
+    w[RL_IMG_H_ATOMS] = (uint32_t)w.size();
+    w.insert(w.end(), atoms.begin(), atoms.end());
     w[RL_IMG_H_VARS] = (uint32_t)w.size();
     w.insert(w.end(), vars.begin(), vars.end());
     w[RL_IMG_H_ARENA] = (uint32_t)w.size();

@@ -66,11 +66,11 @@ __device__ __forceinline__ uint8_t rl_match_ctx(const Args& a, const uint8_t* ms
         const uint32_t lid = I.ns_lims[x];
         const uint32_t* L = I.lims + 5ull * lid;
         bool ok = true;
-        for (uint32_t p = L[0]; ok && p < L[0] + L[1]; p++) {
-            const uint32_t* P = I.preds + 4ull * p;
-            const rl_rls_entry* b = rls_bound(E, ne, P[0]);
-            // an unbound name / missing key makes the predicate false (cel.rs:315-331)
-            ok = b && (b->val_len == P[3] && rl_img_bytes_eq(msg + b->val_off, I.arena + P[2], P[3])) != (P[1] != 0);
+        for (uint32_t t = L[0]; ok && t < L[0] + L[1]; t++) {
+            const uint32_t* T = I.tests + 4ull * t;
+            const rl_rls_entry* b = rls_bound(E, ne, T[0]);
+            // an unbound name / missing key makes the predicate false (cel.rs:315-331); a presence test asks no more
+            ok = b && ((T[1] & 7u) == 0 || rl_img_test(I, T, msg + b->val_off, b->val_len));
         }
         for (uint32_t v = L[2]; ok && v < L[2] + L[3]; v++) ok = rls_bound(E, ne, I.vars[3ull * v]) != nullptr;  // limit.rs:133-148
         if (!ok) continue;

@@ -24,6 +24,10 @@ MATCH_SYMBOLS = (
     "rl_front_check_and_update_bindings", "rl_matcher_set_counter_cap", "rl_matcher_counters_batch_ns",
     "rl_matcher_response_headers_batch",
 )
+DIALECT_SYMBOLS = ("rl_matcher_set_dialect",)  # include/rl_match_dialect.h
+
+# rl_matcher_set_dialect (include/rl_match.h): the condition grammar of later add_limit calls
+DIALECTS = {"table": 0, "boolean": 1}
 
 
 class RlBinding(C.Structure):
@@ -52,6 +56,7 @@ def _lib():
     L.rl_matcher_last_error_copy.argtypes = [vp, C.c_char_p, u32]
     L.rl_matcher_delete_limit.argtypes = [vp, u32]
     L.rl_matcher_set_counter_cap.argtypes = [vp, u32]
+    L.rl_matcher_set_dialect.argtypes = [vp, u32]
     L.rl_matcher_counters_batch_ns.argtypes = [vp, u64, C.POINTER(C.c_char_p), vp, C.POINTER(RlBinding), vp, vp, u64, vp]
     L.rl_matcher_response_headers_batch.argtypes = [vp, u64, vp, vp, vp, vp, vp, u64, vp, C.POINTER(u64)]
     L.rl_matcher_namespace_id.argtypes = [vp, C.c_char_p, C.POINTER(u32)]
@@ -91,12 +96,22 @@ def _bindings(root: Optional[Dict[str, str]], descriptors: Optional[List[Dict[st
 
 
 class Matcher:
-    def __init__(self):
+    def __init__(self, dialect: str = "table"):
+        """dialect "table" accepts `operand ==|!= 'literal'` conditions only; "boolean" also accepts single-operand
+        boolean formulas (&&, ||, !, in, startsWith, endsWith, contains) and positive has() conjuncts (rl_match.h)."""
         self._lib = _lib()
         h = C.c_void_p()
         if self._lib.rl_matcher_create(C.byref(h)) != 0:
             raise MatcherError("rl_matcher_create failed")
         self._h = h
+        if dialect != "table":
+            self.set_dialect(dialect)
+
+    def set_dialect(self, dialect: str):
+        """The condition grammar of the later add_limit calls; limits already added keep their meaning."""
+        if dialect not in DIALECTS:
+            raise MatcherError(f"unknown dialect {dialect!r}")
+        self._check(self._lib.rl_matcher_set_dialect(self._h, DIALECTS[dialect]))
 
     def close(self):
         if self._h:
