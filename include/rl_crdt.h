@@ -15,8 +15,9 @@
  * The semantics are eventually consistent, not bit-exact against a single stream: the reference applies concurrent
  * increments and merges in whatever order its threads run.  What IS exact, and tested against the CPU restatement
  * (oracle/crdt_oracle.c, pinned by the reference's own eleven unit tests): a batch in which every key appears once
- * equals the reference applied to that batch in any order; merge batches may repeat keys (merge_at commutes for one
- * clock reading: the earliest unexpired expiry and the per-actor maxima do not depend on the order).
+ * equals the reference applied to that batch in any order; an inc batch that repeats keys equals one such order (see
+ * rl_crdt_inc); merge batches may repeat keys (merge_at commutes for one clock reading: the earliest unexpired expiry
+ * and the per-actor maxima do not depend on the order).
  *
  * Differences a caller can observe: the reference PANICS when a gossiped key has no local counter
  * (`limits.get(&update.key).unwrap()`, distributed/mod.rs:242); here the row is created and treated as locally
@@ -67,8 +68,14 @@ const char *rl_crdt_last_error(rl_crdt *c);
 
 /* inc_actor_at for n counters, all at the clock reading now_us: counter keys[i] of actor[i] += increment[i] within a
  * window of window_us[i] (a counter that is absent or expired starts a new window at now_us and takes the increment as
- * its value).  A key should appear once per call (repeats are applied in an unspecified order, like concurrent callers
- * of the reference). */
+ * its value).  Keys may repeat, and every increment counts:
+ *   - one actor's repeats of a key are exact: the sum of its increments on an absent or expired counter, its old value
+ *     plus that sum on a live one (wrapping mod 2^64), which is what every order of them gives;
+ *   - repeats of a key by several actors equal the sequential order that starts with one of them, like concurrent
+ *     callers of the reference: on an absent or expired counter that request's window starts and its actor's value
+ *     becomes the sum of that actor's increments, while the other actors add theirs onto the values they held.
+ * Except: a window that leaves the expiry at or before now_us (window_us 0, or now_us + window_us wrapping past 2^64)
+ * starts over at every increment, and the result of repeating such a key within one call is unspecified. */
 int rl_crdt_inc(rl_crdt *c, uint64_t n, const rl_crdt_key *keys, const uint32_t *actor, const uint64_t *increment,
                 const uint64_t *window_us, uint64_t now_us, int mem);
 /* merge_at for n updates at the clock reading now_us.  Keys may repeat. */

@@ -68,9 +68,14 @@ __global__ void k_crdt_inc(RlCrdtTab T, uint32_t n, const rl_crdt_key* __restric
     unsigned long long* val = rl_crdt_values(row) + a;
     const unsigned long long cur = rlm_ld64(exp);
     if (cur <= now) {  // expired_at is inclusive; a fresh row (expiry 0) starts its first window here
-        // update_if_expired: only the thread whose CAS moves the expiry stores, the others add (:55-59, :70-74)
+        // update_if_expired: only the thread whose CAS moves the expiry stores, the others add (:55-59, :70-74).  The
+        // store is an add of (increment - the stale value read before the CAS): the other threads of this call that
+        // target the slot add only after they have seen the CAS, and an exchange landing after their adds would erase
+        // them.  The fence keeps the stale read before the CAS for every observer.
+        const unsigned long long stale = rlm_ld64(val);
+        rlm_fence();
         if (atomicCAS(exp, cur, (unsigned long long)(now + window_us[i])) == cur) {
-            atomicExch(val, (unsigned long long)increment[i]);
+            atomicAdd(val, (unsigned long long)increment[i] - stale);
             return;
         }
     }

@@ -26,9 +26,18 @@ __device__ __forceinline__ ulonglong2 rlm_cas128(void* addr, ulonglong2 cmp, ulo
     return old;
 }
 #else
-inline ulonglong2 rlm_ld(const void* p) { return *reinterpret_cast<const ulonglong2*>(p); }
+// An emulator may hand control to another thread before each of these: tests/emu/cuda_simt.h's interleaving mode
+// defines RLM_EMU_SWITCH.  Without it nothing happens.
+#ifndef RLM_EMU_SWITCH
+#define RLM_EMU_SWITCH() ((void)0)
+#endif
+inline ulonglong2 rlm_ld(const void* p) {
+    RLM_EMU_SWITCH();
+    return *reinterpret_cast<const ulonglong2*>(p);
+}
 inline void rlm_st(void* p, unsigned long long a, unsigned long long b) { *reinterpret_cast<ulonglong2*>(p) = make_ulonglong2(a, b); }
 inline ulonglong2 rlm_cas128(void* addr, ulonglong2 cmp, ulonglong2 val) {
+    RLM_EMU_SWITCH();
     ulonglong2* p = reinterpret_cast<ulonglong2*>(addr);
     const ulonglong2 old = *p;
     if (old.x == cmp.x && old.y == cmp.y) *p = val;
@@ -40,7 +49,10 @@ inline ulonglong2 rlm_cas128(void* addr, ulonglong2 cmp, ulonglong2 val) {
 #if !defined(RL_SHIM) && !defined(RL_SIMT)
 __device__ __forceinline__ unsigned long long rlm_ld64(const void* p) { return __ldcg(reinterpret_cast<const unsigned long long*>(p)); }
 #else
-inline unsigned long long rlm_ld64(const void* p) { return *reinterpret_cast<const unsigned long long*>(p); }
+inline unsigned long long rlm_ld64(const void* p) {
+    RLM_EMU_SWITCH();
+    return *reinterpret_cast<const unsigned long long*>(p);
+}
 #endif
 
 // atomic OR of a 32-bit word; returns the old value
@@ -48,8 +60,16 @@ inline unsigned long long rlm_ld64(const void* p) { return *reinterpret_cast<con
 __device__ __forceinline__ unsigned rlm_or(unsigned* p, unsigned v) { return atomicOr(p, v); }
 #else
 inline unsigned rlm_or(unsigned* p, unsigned v) {
+    RLM_EMU_SWITCH();
     const unsigned o = *p;
     *p = o | v;
     return o;
 }
+#endif
+
+// a fence between a thread's global accesses, for every observer
+#if !defined(RL_SHIM) && !defined(RL_SIMT)
+__device__ __forceinline__ void rlm_fence() { __threadfence(); }
+#else
+inline void rlm_fence() {}  // the emulators have one memory: every access is already ordered
 #endif

@@ -8,6 +8,14 @@
 // Strict where the hardware is lenient: a lane that names an exited lane in a mask, lanes of one rendezvous that
 // disagree on the operation or the mask, and a block that stops making progress are all reported (abort with a message),
 // because on a GPU they are hangs or undefined behaviour.
+//
+// Interleaving mode (simt_interleave, off by default): a fiber otherwise gives way only at a rendezvous or a barrier, so
+// a kernel without either runs each thread from start to finish.  With the mode on, every global atomic below and the
+// memory helpers of rl_devmem.cuh (rlm_ld, rlm_ld64, rlm_cas128, rlm_or) first hand control back to the scheduler with
+// probability p, and every pass of the scheduler visits the block's fibers in a seeded random order; p = 1 switches at
+// every one of them.  A kernel whose threads claim and then write shared words thus runs under many interleavings of
+// those steps, deterministically for one seed.  Blocks still run one after the other: only the threads of one block
+// interleave, so a test puts the work that must collide inside one block.
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
@@ -16,6 +24,7 @@
 
 #include <functional>
 #include <memory>
+#include <utility>
 #include <vector>
 
 #define RL_SIMT 1
@@ -36,8 +45,14 @@ struct ulonglong2 {
 };
 static inline ulonglong2 make_ulonglong2(unsigned long long x, unsigned long long y) { return ulonglong2{x, y}; }
 
+namespace simt {
+static void interleave_point();
+}
+#define RLM_EMU_SWITCH() simt::interleave_point()  // rl_devmem.cuh's memory helpers are switch points too
+
 template <class T>
 static inline T atomicAdd(T* p, T v) {
+    simt::interleave_point();
     const T o = *p;
     *p = o + v;
     return o;
@@ -45,24 +60,28 @@ static inline T atomicAdd(T* p, T v) {
 static inline unsigned long long atomicAdd(unsigned long long* p, unsigned v) { return atomicAdd(p, (unsigned long long)v); }
 template <class T>
 static inline T atomicMax(T* p, T v) {
+    simt::interleave_point();
     const T o = *p;
     if (v > o) *p = v;
     return o;
 }
 template <class T>
 static inline T atomicMin(T* p, T v) {
+    simt::interleave_point();
     const T o = *p;
     if (v < o) *p = v;
     return o;
 }
 template <class T>
 static inline T atomicCAS(T* p, T cmp, T val) {
+    simt::interleave_point();
     const T o = *p;
     if (o == cmp) *p = val;
     return o;
 }
 template <class T>
 static inline T atomicExch(T* p, T v) {
+    simt::interleave_point();
     const T o = *p;
     *p = v;
     return o;
@@ -102,6 +121,21 @@ struct Block {
 
 static Block* g_block = nullptr;
 
+// the interleaving mode (see the header comment)
+struct Interleave {
+    bool on = false;
+    double p = 1.0;
+    uint64_t state = 0;
+};
+static Interleave g_interleave;
+
+static uint64_t next_random() {  // splitmix64
+    uint64_t z = (g_interleave.state += 0x9E3779B97F4A7C15ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 [[noreturn]] static void die(const char* what) {
     fprintf(stderr, "cuda_simt: %s (block %u, thread %u)\n", what, blockIdx.x, threadIdx.x);
     abort();
@@ -110,6 +144,16 @@ static Block* g_block = nullptr;
 static void yield() {
     Block* b = g_block;
     swapcontext(&b->fibers[b->current].ctx, &b->sched);
+}
+
+// A switch point: with the interleaving mode on, inside a launch, give way to the other fibers with probability p.  A
+// switch is progress (the fiber can always resume), so the deadlock check counts it.
+static void interleave_point() {
+    Block* b = g_block;
+    if (!g_interleave.on || !b) return;
+    if (g_interleave.p < 1.0 && (double)(next_random() >> 11) * 0x1.0p-53 >= g_interleave.p) return;
+    b->progress++;
+    yield();
 }
 
 static void trampoline() {
@@ -210,6 +254,13 @@ static inline unsigned __shfl_sync(unsigned mask, unsigned v, int src) { return 
 static inline void __syncwarp(unsigned mask = 0xFFFFFFFFu) { simt::rendezvous(simt::OP_SYNCWARP, mask, 0); }
 static inline void __syncthreads() { simt::syncthreads(); }
 
+// Turn the interleaving mode on (seed, switch probability p in (0, 1]) or off.
+static inline void simt_interleave(bool on, uint64_t seed = 0, double p = 1.0) {
+    simt::g_interleave.on = on;
+    simt::g_interleave.p = p;
+    simt::g_interleave.state = seed;
+}
+
 // run body() once per thread of a <<<grid, block>>> launch: blocks one after the other, the threads of a block as fibers
 template <class F>
 static void simt_launch(unsigned grid, unsigned block, F&& body) {
@@ -233,11 +284,16 @@ static void simt_launch(unsigned grid, unsigned block, F&& body) {
             f.ctx.uc_link = nullptr;
             makecontext(&f.ctx, simt::trampoline, 0);
         }
+        std::vector<unsigned> order(block);
         while (B.live) {
             const unsigned long long before = B.progress;
-            // the threads take turns, starting from a thread that depends on the block: no lane is always first
+            // the threads take turns, starting from a thread that depends on the block: no lane is always first; in the
+            // interleaving mode every pass takes them in a fresh random order
+            for (unsigned k = 0; k < block; k++) order[k] = (k + bx) % block;
+            if (simt::g_interleave.on)
+                for (unsigned k = block; k > 1; k--) std::swap(order[k - 1], order[simt::next_random() % k]);
             for (unsigned k = 0; k < block; k++) {
-                const unsigned t = (k + bx) % block;
+                const unsigned t = order[k];
                 simt::Fiber& f = B.fibers[t];
                 if (f.done) continue;
                 B.current = t;

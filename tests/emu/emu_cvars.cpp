@@ -4,7 +4,16 @@
 // kernel over its scratch (the scatter writes nothing the recording reads, so it is left out); the lookup with its
 // scan and gather; the GC's mark, kept lengths, scan and rebuild, with host loops in place of the CUB scans.  Also
 // compiled into tests/san/san_cvars.cpp for the ASan + UBSan run.
+// Built a second time with -DEMU_SIMT under tests/emu/cuda_simt.h, whose interleaving mode lets the recording threads of a
+// block race for the same new keys; there the recording kernel runs in 256-thread blocks (the GPU uses 128), so that all
+// 256 requests of a block can collide.
+#ifdef EMU_SIMT
+#include "cuda_simt.h"
+#define shim_launch simt_launch
+static uint64_t shim_seed = 0;
+#else
 #include "cuda_shim.h"
+#endif
 // (the shim must come first: it defines __global__ & co. away)
 #include <algorithm>
 #include <cstring>
@@ -23,6 +32,11 @@ struct EmuDict {
 
 const uint32_t kThreads = 128;
 uint32_t grid(uint64_t n) { return (uint32_t)((n + kThreads - 1) / kThreads); }
+#ifdef EMU_SIMT
+const uint32_t kRecordThreads = 256;
+#else
+const uint32_t kRecordThreads = kThreads;
+#endif
 
 // the scratch a plan leaves and the recording reads (exact sizes, so that ASan sees any access past them)
 struct Scratch {
@@ -47,8 +61,9 @@ void record(EmuDict* d, const RlImage& img, uint32_t per_req, uint64_t n, const 
     a.txt = s.txt.data();
     a.bits = s.bits.data();
     a.dict = d->view();
-    if (!s.rls_count.empty()) shim_launch(grid(n), kThreads, [&] { k_counter_vars_record<CvWire>(a); });
-    else shim_launch(grid(n), kThreads, [&] { k_counter_vars_record<CvJson>(a); });
+    const uint32_t blocks = (uint32_t)((n + kRecordThreads - 1) / kRecordThreads);
+    if (!s.rls_count.empty()) shim_launch(blocks, kRecordThreads, [&] { k_counter_vars_record<CvWire>(a); });
+    else shim_launch(blocks, kRecordThreads, [&] { k_counter_vars_record<CvJson>(a); });
 }
 
 }  // namespace
@@ -56,6 +71,10 @@ void record(EmuDict* d, const RlImage& img, uint32_t per_req, uint64_t n, const 
 extern "C" {
 
 void emu_cv_seed(uint64_t s) { shim_seed = s; }
+#ifdef EMU_SIMT
+// cuda_simt.h's interleaving mode for the launches that follow (on = 0: off, the default)
+void emu_cv_interleave(int on, uint64_t seed, double p) { simt_interleave(on != 0, seed, p); }
+#endif
 
 // max_keys rounded up to a power of two (at least 16) slots, as rl_cv_dev_configure sizes them
 void* emu_cv_create(uint64_t max_keys, uint64_t arena_bytes) {

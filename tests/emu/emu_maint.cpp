@@ -23,6 +23,10 @@ static uint64_t shim_seed = 0;
 extern "C" {
 
 void emu_seed(uint64_t s) { shim_seed = s; }
+#ifdef EMU_SIMT
+// cuda_simt.h's interleaving mode for the launches that follow (on = 0: off, the default)
+void emu_simt_interleave(int on, uint64_t seed, double p) { simt_interleave(on != 0, seed, p); }
+#endif
 
 // ---- per-namespace metrics ------------------------------------------------------------------------------------------
 // out = authorized_calls[ns_cap] | authorized_hits[ns_cap] | limited_calls[ns_cap] | limited_by_limit[limits_cap] | dropped

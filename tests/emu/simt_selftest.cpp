@@ -1,6 +1,8 @@
 // simt_selftest.cpp — the fiber emulator (cuda_simt.h) checked on its own: results of the warp intrinsics and the block
 // barrier against closed forms, and — run with an argument — the three mistakes it must refuse (they are hangs or undefined
 // behaviour on a GPU): a *_sync mask naming an exited lane, lanes disagreeing on the mask, a barrier not every thread reaches.
+// Also the interleaving mode: a read-modify-write made of a plain load and store with a switch point between them must lose
+// updates under it, and the same update as an atomic must not — the mode can show a race at all.
 #include "cuda_simt.h"
 
 #include <cstdio>
@@ -26,6 +28,22 @@ __global__ void k_ok(unsigned* out_match, unsigned* out_sum, unsigned* out_ballo
     }
     if (t == 0) out_block_sum[blockIdx.x] = g_smem[0];
     __syncthreads();  // nobody overwrites g_smem for the next block's use before thread 0 has read it (blocks run in turn)
+}
+
+__global__ void k_racy_inc(unsigned long long* counter) {
+    const unsigned long long v = *counter;  // plain load ...
+    simt::interleave_point();
+    *counter = v + 1;                       // ... and plain store: another fiber's update in between is lost
+}
+__global__ void k_atomic_inc(unsigned long long* counter) { atomicAdd(counter, 1ull); }
+
+// the two counters after one 256-thread block of each kernel under the interleaving mode
+static void race(uint64_t seed, double p, unsigned long long* racy, unsigned long long* atomic) {
+    *racy = *atomic = 0;
+    simt_interleave(true, seed, p);
+    simt_launch(1, 256, [&] { k_racy_inc(racy); });
+    simt_launch(1, 256, [&] { k_atomic_inc(atomic); });
+    simt_interleave(false);
 }
 
 __global__ void k_exited_lane() {
@@ -71,6 +89,16 @@ int main(int argc, char** argv) {
     }
     for (unsigned g = 0; g < grid; g++)
         if (bs[g] != block * (block + 1) / 2) return 3;
-    printf("ok simt\n");
+    // interleaving mode off (the default): every thread runs to its end, the racy update loses nothing
+    unsigned long long racy = 0, atomic = 0;
+    simt_launch(1, 256, [&] { k_racy_inc(&racy); });
+    if (racy != 256) return 4;
+    // on: the racy update loses some increments, whether every switch point switches or half of them do; the atomic none
+    race(1, 1.0, &racy, &atomic);
+    if (racy >= 256 || atomic != 256) return 5;
+    const unsigned long long lost_p1 = 256 - racy;
+    race(2, 0.5, &racy, &atomic);
+    if (racy >= 256 || atomic != 256) return 6;
+    printf("ok simt (racy update lost %llu and %llu of 256 increments)\n", lost_p1, 256 - racy);
     return 0;
 }

@@ -420,19 +420,36 @@ def emu_maint_lib(simt: bool = False):
     L.emu_crdt_scan.restype = u64
     L.emu_import.restype = u64
     L.emu_import.argtypes = [vp, u32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp, vp]
+    if simt:
+        L.emu_simt_interleave.argtypes = [C.c_int, u64, C.c_double]
+        L.emu_simt_interleave.restype = None
     return L
 
 
 class EmuCrdt:
-    """The CRDT kernels on the host (same interface as limitador_b200.crdt.CrdtTable)."""
+    """The CRDT kernels on the host (same interface as limitador_b200.crdt.CrdtTable).  interleave=(seed, p) (simt=True
+    only): every call runs under cuda_simt.h's interleaving mode, the n-th call of the table with seed + n."""
 
-    def __init__(self, capacity_rows, actors, self_actor, simt=False):
+    def __init__(self, capacity_rows, actors, self_actor, simt=False, interleave=None):
         from limitador_b200 import crdt as CR
+        assert interleave is None or simt
         self.CR = CR
         self.L = emu_maint_lib(simt)
         self.actors, self.self_actor = actors, self_actor
         self.h = self.L.emu_crdt_create(capacity_rows, actors, self_actor)
         self.capacity = capacity_rows
+        self.interleave, self.calls = interleave, 0
+
+    def _call(self, f, *args):
+        if self.interleave is None:
+            return f(*args)
+        seed, p = self.interleave
+        self.calls += 1
+        self.L.emu_simt_interleave(1, seed + self.calls, p)
+        try:
+            return f(*args)
+        finally:
+            self.L.emu_simt_interleave(0, 0, 1.0)  # the library is shared: leave the mode off for everybody else
 
     def __del__(self):
         try:
@@ -446,33 +463,33 @@ class EmuCrdt:
         a = np.ascontiguousarray(np.broadcast_to(np.asarray(actor, dtype=np.uint32), (n,)))
         inc = np.ascontiguousarray(np.broadcast_to(np.asarray(increment, dtype=np.uint64), (n,)))
         win = np.ascontiguousarray(np.broadcast_to(np.asarray(window_us, dtype=np.uint64), (n,)))
-        return self.L.emu_crdt_inc(self.h, n, _p(keys), _p(a), _p(inc), _p(win), now_us)
+        return self._call(self.L.emu_crdt_inc, self.h, n, _p(keys), _p(a), _p(inc), _p(win), now_us)
 
     def merge(self, ups, actors, values, now_us):
         ups = np.ascontiguousarray(ups, dtype=self.CR.UPDATE_DTYPE)
         actors = np.ascontiguousarray(actors, dtype=np.uint32)
         values = np.ascontiguousarray(values, dtype=np.uint64)
-        return self.L.emu_crdt_merge(self.h, len(ups), _p(ups), _p(actors), _p(values), len(values), now_us)
+        return self._call(self.L.emu_crdt_merge, self.h, len(ups), _p(ups), _p(actors), _p(values), len(values), now_us)
 
     def read(self, keys, now_us):
         keys = np.ascontiguousarray(keys, dtype=self.CR.KEY_DTYPE)
         val = np.zeros(len(keys), dtype=np.uint64)
         exp = np.zeros(len(keys), dtype=np.uint64)
-        assert self.L.emu_crdt_read(self.h, len(keys), _p(keys), now_us, _p(val), _p(exp)) == 0
+        assert self._call(self.L.emu_crdt_read, self.h, len(keys), _p(keys), now_us, _p(val), _p(exp)) == 0
         return val, exp
 
     def export(self, now_us, cap=1 << 16):
         k = np.zeros(cap, dtype=self.CR.KEY_DTYPE)
         val = np.zeros(cap, dtype=np.uint64)
         exp = np.zeros(cap, dtype=np.uint64)
-        n = self.L.emu_crdt_scan(self.h, 0, now_us, cap, _p(k), _p(val), _p(exp), None)
+        n = self._call(self.L.emu_crdt_scan, self.h, 0, now_us, cap, _p(k), _p(val), _p(exp), None)
         return sorted(zip(k["lo"][:n].tolist(), k["hi"][:n].tolist(), val[:n].tolist(), exp[:n].tolist()))
 
     def dump(self, cap=1 << 16):
         k = np.zeros(cap, dtype=self.CR.KEY_DTYPE)
         exp = np.zeros(cap, dtype=np.uint64)
         vals = np.zeros(cap * self.actors, dtype=np.uint64)
-        n = self.L.emu_crdt_scan(self.h, 1, 0, cap, _p(k), None, _p(exp), _p(vals))
+        n = self._call(self.L.emu_crdt_scan, self.h, 1, 0, cap, _p(k), None, _p(exp), _p(vals))
         v = vals[:n * self.actors].reshape(n, self.actors)
         return sorted((int(k["lo"][i]), int(k["hi"][i]), int(exp[i]), tuple(v[i].tolist())) for i in range(n))
 

@@ -24,9 +24,13 @@ T0 = 1_700_000_000_000_000
 
 
 @functools.cache
-def _emu():
-    L = H.host_lib("emu_cvars.cpp", "librl_emu_cvars.so")
+def _emu(simt=False):
+    """tests/emu/emu_cvars.cpp under the host shim, or with simt=True under the fiber emulator (tests/emu/cuda_simt.h)."""
+    L = H.host_lib("emu_cvars.cpp", "librl_emu_cvars_simt.so" if simt else "librl_emu_cvars.so", ["EMU_SIMT"] if simt else [])
     vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
+    if simt:
+        L.emu_cv_interleave.argtypes = [C.c_int, u64, C.c_double]
+        L.emu_cv_interleave.restype = None
     L.emu_cv_seed.argtypes = [u64]
     L.emu_cv_create.restype = vp
     L.emu_cv_create.argtypes = [u64, u64]
@@ -45,11 +49,13 @@ def _emu():
 
 
 class Dict:
-    """One dictionary under the shim."""
+    """One dictionary under the shim; with interleave=(seed, p), under the fiber emulator with its interleaving mode on
+    for every record call."""
 
-    def __init__(self, max_keys=1 << 14, arena_bytes=1 << 20):
-        self.L = _emu()
+    def __init__(self, max_keys=1 << 14, arena_bytes=1 << 20, interleave=None):
+        self.L = _emu(interleave is not None)
         self.h = self.L.emu_cv_create(max_keys, arena_bytes)
+        self.interleave = interleave
 
     def __del__(self):
         self.L.emu_cv_destroy(self.h)
@@ -59,8 +65,14 @@ class Dict:
         if len(buf) == 0:
             buf = np.zeros(1, np.uint8)
         img, _ = matcher_image(m)
-        return self.L.emu_cv_plan_record(self.h, int(http), img.ctypes.data, endpoint, len(msgs), buf.ctypes.data, off.ctypes.data,
-                                         engine_max)
+        if self.interleave:
+            self.L.emu_cv_interleave(1, *self.interleave)
+        try:
+            return self.L.emu_cv_plan_record(self.h, int(http), img.ctypes.data, endpoint, len(msgs), buf.ctypes.data,
+                                             off.ctypes.data, engine_max)
+        finally:
+            if self.interleave:
+                self.L.emu_cv_interleave(0, 0, 1.0)
 
     def stats(self):
         v = [C.c_uint64() for _ in range(4)]
