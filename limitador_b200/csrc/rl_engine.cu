@@ -7,7 +7,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -18,6 +17,7 @@
 #include <utility>
 #include <vector>
 
+#include "rl_cuda_host.h"
 #include "rl_kernels.cuh"
 #include "rl_shard.cuh"
 #include "rl_internal.h"
@@ -46,28 +46,6 @@ struct HostGroup {
     uint32_t limit_of_cell[RL_MAX_CELLS];
     HostGroup() {
         for (auto& l : limit_of_cell) l = RL_NONE_U32;
-    }
-};
-
-// Device memory owned by its holder: freed when the holder goes away.
-template <class T>
-struct DevBuf {
-    T* p = nullptr;
-    size_t n = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() {
-        if (p) cudaFree(p);
-    }
-    cudaError_t reserve(size_t want) {
-        if (want <= n) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        n = 0;
-        cudaError_t r = cudaMalloc((void**)&p, want * sizeof(T));
-        if (r == cudaSuccess) n = want;
-        return r;
     }
 };
 
@@ -136,7 +114,7 @@ struct rl_engine {
     // bucket helper
     DevBuf<uint32_t> d_bucket;
     DevBuf<unsigned long long> d_bucket_counts;
-    uint32_t* h_misc = nullptr;  // pinned mirror of d_misc
+    PinnedBuf<uint32_t> h_misc;  // pinned mirror of d_misc
 
     rl_stats stats{};
     std::string last_error = "";
@@ -176,26 +154,13 @@ namespace {
 
 enum { MISC_ERR = 0, MISC_FLAGS = 1, MISC_CHANGED = 3, MISC_XCHG = 7, MISC_N = 8 };
 
-int fail(rl_engine* e, int status, const char* fmt, ...) {
-    char buf[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
-    va_end(ap);
-    if (e) e->last_error = buf;
+template <class... A>
+int fail(rl_engine* e, int status, const char* fmt, A... a) {
+    if (e) e->last_error = rl_format(fmt, a...);
     return status;
 }
 
 int pipe_fence(rl_engine* e);
-
-#define RL_CUDA(e, call)                                                                          \
-    do {                                                                                          \
-        cudaError_t _r = (call);                                                                  \
-        if (_r != cudaSuccess)                                                                    \
-            return fail((e), _r == cudaErrorMemoryAllocation ? RL_TRANSIENT : RL_FATAL,           \
-                        "CUDA error %s at %s:%d (%s)", cudaGetErrorName(_r), __FILE__, __LINE__,  \
-                        cudaGetErrorString(_r));                                                  \
-    } while (0)
 
 #define RL_LAUNCH_CHECK(e)                    \
     do {                                      \
@@ -327,9 +292,9 @@ int check_device_error(rl_engine* e) {
         int rf = pipe_fence(e);
         if (rf) return rf;
     }
-    RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(e->h_misc.p, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    const uint32_t code = e->h_misc[MISC_ERR];
+    const uint32_t code = e->h_misc.p[MISC_ERR];
     if (code == RL_DEV_OK) return RL_OK;
     RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_ERR, 0, sizeof(uint32_t), e->stream));
     switch (code) {
@@ -343,7 +308,7 @@ int check_device_error(rl_engine* e) {
         case RL_DEV_TOO_MANY_COUNTERS:
             return fail(e, RL_FATAL, "a request has more than %u counters", e->max_ctrs_req);
         case RL_DEV_EXCHANGE: {
-            const uint32_t d = e->h_misc[MISC_XCHG];
+            const uint32_t d = e->h_misc.p[MISC_XCHG];
             RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_XCHG, 0, sizeof(uint32_t), e->stream));
             const char* what = (d >> 28) == 1 ? "records of source rank" : (d >> 28) == 2 ? "verdicts of owner rank" : "inbox larger than max_batch, rank";
             return fail(e, RL_FATAL, "peer exchange failed at step %u: %s %u did not arrive within %.0f s (or a block fill was out of range)",
@@ -358,9 +323,9 @@ int check_device_error(rl_engine* e) {
 // max_counters_per_request counters, key out of range): refuse the WHOLE call before anything touches the
 // table, so that the caller can fix the batch and retry without double counting (ADVICE r1).
 int check_resolve_error(rl_engine* e) {
-    RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(e->h_misc.p, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    if (e->h_misc[MISC_ERR] == RL_DEV_OK) return RL_OK;
+    if (e->h_misc.p[MISC_ERR] == RL_DEV_OK) return RL_OK;
     int r = check_device_error(e);
     if (r == RL_OK) r = RL_FATAL;
     e->last_error += " — the call was refused before the table was touched";
@@ -568,10 +533,10 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
     if (mode == 2) return launch_main<AccSrc, 2>(e, D, B, src);
     auto main0 = [&]() { return wide ? launch_main<AccSrcWide, 0>(e, D, B, AccSrcWide{src}) : launch_main<AccSrc, 0>(e, D, B, src); };
     // does the batch contain coupled (multi-row) requests?
-    RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+    RL_CUDA(e, cudaMemcpyAsync(e->h_misc.p, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
     e->stats.fixed_point_rounds = 0;
-    if (e->h_misc[MISC_FLAGS] & 1u) {
+    if (e->h_misc.p[MISC_FLAGS] & 1u) {
         RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_FLAGS, 0, sizeof(uint32_t), e->stream));
         RL_CUDA(e, e->d_fl_prev.reserve(e->max_batch));
         RL_CUDA(e, e->d_fl_next.reserve(e->max_batch));
@@ -606,11 +571,11 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
             k_fl_step<<<ceil_div(n_req, 256), 256, 0, e->stream>>>(n_req, B.fl_prev, B.fl_next,
                                                                     e->d_misc.p + MISC_CHANGED);
             RL_LAUNCH_CHECK(e);
-            RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+            RL_CUDA(e, cudaMemcpyAsync(e->h_misc.p, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost,
                                        e->stream));
             RL_CUDA(e, cudaStreamSynchronize(e->stream));
             e->stats.fixed_point_rounds = round + 1;
-            if (!(e->h_misc[MISC_CHANGED] & 1u)) break;
+            if (!(e->h_misc.p[MISC_CHANGED] & 1u)) break;
         }
     }
     B.phase = RL_PHASE_COMMIT;
@@ -858,7 +823,7 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     if (r) return r;
     RL_CUDA(e, e->d_misc.reserve(MISC_N));
     RL_CUDA(e, cudaMemsetAsync(e->d_misc.p, 0, MISC_N * sizeof(uint32_t), e->stream));
-    RL_CUDA(e, cudaMallocHost((void**)&e->h_misc, MISC_N * sizeof(uint32_t)));
+    RL_CUDA(e, e->h_misc.exact(MISC_N));
     RL_CUDA(e, e->d_acc.reserve(e->max_counters));
     if (e->max_ctrs_req > RL_MAX_CTRS_PER_REQ) RL_CUDA(e, e->d_perm.reserve(e->max_counters));
     RL_CUDA(e, e->d_kstats.reserve(32));
@@ -917,8 +882,7 @@ void rl_engine_destroy(rl_engine* e) {
     }
     for (cudaStream_t st : {e->sq, e->sp, e->sm, e->own_stream})
         if (st) cudaStreamDestroy(st);
-    if (e->h_misc) cudaFreeHost(e->h_misc);
-    delete e;  // frees the device buffers, on the device made current above
+    delete e;  // frees the device and pinned buffers, on the device made current above
 }
 
 int rl_engine_set_stream(rl_engine* e, void* cuda_stream) {
@@ -1563,9 +1527,9 @@ static int resolve_csr(rl_engine* e, uint64_t n, const CsrDev& c, const RlResolv
     k_resolve_csr<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, write_defaults);
     RL_LAUNCH_CHECK(e);
     if (e->max_ctrs_req > RL_MAX_CTRS_PER_REQ) {
-        RL_CUDA(e, cudaMemcpyAsync(e->h_misc, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+        RL_CUDA(e, cudaMemcpyAsync(e->h_misc.p, e->d_misc.p, MISC_N * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
         RL_CUDA(e, cudaStreamSynchronize(e->stream));
-        if (e->h_misc[MISC_ERR] == RL_DEV_TOO_MANY_COUNTERS) {
+        if (e->h_misc.p[MISC_ERR] == RL_DEV_TOO_MANY_COUNTERS) {
             // every other refusal has a lower code (the error word is a sticky max): the wide pass finds it again
             RL_CUDA(e, cudaMemsetAsync(e->d_misc.p + MISC_ERR, 0, 2 * sizeof(uint32_t), e->stream));  // error + flags
             k_resolve_csr_wide<<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, O, write_defaults,

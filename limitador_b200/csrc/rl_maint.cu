@@ -4,10 +4,10 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdio>
 #include <cstring>
 #include <vector>
 
+#include "rl_cuda_host.h"
 #include "rl_internal.h"
 #include "rl_maint.cuh"
 
@@ -17,7 +17,7 @@ struct MaintState {
     int device = 0;
     // metrics accumulators (device): authorized_calls | authorized_hits | limited_calls [ns_cap], limited_by_limit
     // [limits_cap], dropped [1]
-    unsigned long long* d_metrics = nullptr;
+    DevBuf<unsigned long long> d_metrics;
     uint32_t ns_cap = 0, limits_cap = 0;
     bool metrics_on = false;
 };
@@ -26,8 +26,7 @@ void maint_free(void* p) {
     MaintState* s = static_cast<MaintState*>(p);
     if (!s) return;
     cudaSetDevice(s->device);
-    if (s->d_metrics) cudaFree(s->d_metrics);
-    delete s;
+    delete s;  // frees the accumulators, on the device made current above
 }
 
 MaintState* state_of(rl_engine* e, int device) {
@@ -40,36 +39,20 @@ MaintState* state_of(rl_engine* e, int device) {
     return static_cast<MaintState*>(*slot);
 }
 
-#define RLM_CUDA(e, call)                                                                                   \
-    do {                                                                                                    \
-        cudaError_t _r = (call);                                                                            \
-        if (_r != cudaSuccess) {                                                                            \
-            char _b[256];                                                                                   \
-            snprintf(_b, sizeof _b, "CUDA error %s at %s:%d (%s)", cudaGetErrorName(_r), __FILE__, __LINE__, \
-                     cudaGetErrorString(_r));                                                               \
-            return rl_internal_fail((e), _r == cudaErrorMemoryAllocation ? RL_TRANSIENT : RL_FATAL, _b);    \
-        }                                                                                                   \
-    } while (0)
-
-// A device scratch array freed at scope exit (every exit path of a call, the error ones included).
-template <class E>
-struct Scratch {
-    E* p = nullptr;
-    ~Scratch() {
-        if (p) cudaFree(p);
-    }
-    cudaError_t alloc(size_t n) { return cudaMalloc((void**)&p, (n ? n : 1) * sizeof(E)); }
-};
+template <class... A>
+int fail(rl_engine* e, int status, const char* fmt, A... a) {
+    return rl_internal_fail(e, status, rl_format(fmt, a...).c_str());
+}
 
 size_t metrics_words(uint32_t ns_cap, uint32_t limits_cap) { return (size_t)3 * ns_cap + limits_cap + 1; }
 
 RlNsMetricsDev metrics_dev(const MaintState* s) {
     RlNsMetricsDev M;
-    M.authorized_calls = s->d_metrics;
-    M.authorized_hits = s->d_metrics + s->ns_cap;
-    M.limited_calls = s->d_metrics + 2 * (size_t)s->ns_cap;
-    M.limited_by_limit = s->d_metrics + 3 * (size_t)s->ns_cap;
-    M.dropped = s->d_metrics + 3 * (size_t)s->ns_cap + s->limits_cap;
+    M.authorized_calls = s->d_metrics.p;
+    M.authorized_hits = s->d_metrics.p + s->ns_cap;
+    M.limited_calls = s->d_metrics.p + 2 * (size_t)s->ns_cap;
+    M.limited_by_limit = s->d_metrics.p + 3 * (size_t)s->ns_cap;
+    M.dropped = s->d_metrics.p + 3 * (size_t)s->ns_cap + s->limits_cap;
     M.ns_cap = s->ns_cap;
     M.limits_cap = s->limits_cap;
     return M;
@@ -78,24 +61,23 @@ RlNsMetricsDev metrics_dev(const MaintState* s) {
 // Make the accumulators cover ns_cap namespaces and limits_cap limits; growing keeps the counts (rare: a full
 // device synchronisation, then a copy).
 int metrics_reserve(rl_engine* e, MaintState* s, uint32_t ns_cap, uint32_t limits_cap) {
-    if (s->d_metrics && ns_cap <= s->ns_cap && limits_cap <= s->limits_cap) return RL_OK;
+    if (s->d_metrics.p && ns_cap <= s->ns_cap && limits_cap <= s->limits_cap) return RL_OK;
     const uint32_t new_ns = std::max<uint32_t>({ns_cap, s->ns_cap, 1024u}), new_lim = std::max<uint32_t>({limits_cap, s->limits_cap, 1024u});
-    const uint32_t grow_ns = s->d_metrics && new_ns > s->ns_cap ? std::max(new_ns, 2 * s->ns_cap) : new_ns;
-    const uint32_t grow_lim = s->d_metrics && new_lim > s->limits_cap ? std::max(new_lim, 2 * s->limits_cap) : new_lim;
+    const uint32_t grow_ns = s->d_metrics.p && new_ns > s->ns_cap ? std::max(new_ns, 2 * s->ns_cap) : new_ns;
+    const uint32_t grow_lim = s->d_metrics.p && new_lim > s->limits_cap ? std::max(new_lim, 2 * s->limits_cap) : new_lim;
     if (grow_ns >= (1u << 31)) return rl_internal_fail(e, RL_FATAL, "namespace ids must stay below 2^31 for the metrics reduction");
-    unsigned long long* d_new = nullptr;
-    RLM_CUDA(e, cudaDeviceSynchronize());
-    RLM_CUDA(e, cudaMalloc((void**)&d_new, metrics_words(grow_ns, grow_lim) * sizeof(unsigned long long)));
-    RLM_CUDA(e, cudaMemset(d_new, 0, metrics_words(grow_ns, grow_lim) * sizeof(unsigned long long)));
-    if (s->d_metrics) {
+    DevBuf<unsigned long long> d_new;
+    RL_CUDA(e, cudaDeviceSynchronize());
+    RL_CUDA(e, d_new.exact(metrics_words(grow_ns, grow_lim)));
+    RL_CUDA(e, cudaMemset(d_new.p, 0, metrics_words(grow_ns, grow_lim) * sizeof(unsigned long long)));
+    if (s->d_metrics.p) {
         const size_t w = sizeof(unsigned long long);
         for (int k = 0; k < 3; k++)
-            RLM_CUDA(e, cudaMemcpy(d_new + (size_t)k * grow_ns, s->d_metrics + (size_t)k * s->ns_cap, s->ns_cap * w, cudaMemcpyDeviceToDevice));
-        RLM_CUDA(e, cudaMemcpy(d_new + 3 * (size_t)grow_ns, s->d_metrics + 3 * (size_t)s->ns_cap, s->limits_cap * w, cudaMemcpyDeviceToDevice));
-        RLM_CUDA(e, cudaMemcpy(d_new + 3 * (size_t)grow_ns + grow_lim, s->d_metrics + 3 * (size_t)s->ns_cap + s->limits_cap, w, cudaMemcpyDeviceToDevice));
-        cudaFree(s->d_metrics);
+            RL_CUDA(e, cudaMemcpy(d_new.p + (size_t)k * grow_ns, s->d_metrics.p + (size_t)k * s->ns_cap, s->ns_cap * w, cudaMemcpyDeviceToDevice));
+        RL_CUDA(e, cudaMemcpy(d_new.p + 3 * (size_t)grow_ns, s->d_metrics.p + 3 * (size_t)s->ns_cap, s->limits_cap * w, cudaMemcpyDeviceToDevice));
+        RL_CUDA(e, cudaMemcpy(d_new.p + 3 * (size_t)grow_ns + grow_lim, s->d_metrics.p + 3 * (size_t)s->ns_cap + s->limits_cap, w, cudaMemcpyDeviceToDevice));
     }
-    s->d_metrics = d_new;
+    s->d_metrics.swap(d_new);  // the old accumulators are freed on return
     s->ns_cap = grow_ns;
     s->limits_cap = grow_lim;
     return RL_OK;
@@ -108,7 +90,7 @@ int launch_metrics(rl_engine* e, MaintState* s, cudaStream_t st, uint32_t n, con
     const uint32_t blocks = std::min<uint32_t>((n + threads - 1) / threads, rl_internal_sm_count(e) * 8u);  // grid-stride beyond 8 CTAs per SM
     k_ns_metrics<<<blocks, threads, 0, st>>>(static_cast<const unsigned long long*>(d_recs), record_bytes == 16 ? 2u : 4u, n,
                                              d_limited, d_first, metrics_dev(s));
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 1);
     return RL_OK;
 }
@@ -152,16 +134,13 @@ int rl_ns_metrics_accumulate(rl_engine* e, uint64_t n, const void* recs, uint32_
     if (r || n == 0) return r;
     if (mem == RL_MEM_DEVICE) return launch_metrics(e, s, v.stream, (uint32_t)n, recs, (int)record_bytes, limited, first_limited);
     // host arrays: staged for the call
-    Scratch<uint8_t> d_recs, d_lim;
-    Scratch<uint32_t> d_first;
-    RLM_CUDA(e, d_recs.alloc(n * record_bytes));
-    RLM_CUDA(e, d_lim.alloc(n));
-    if (first_limited) RLM_CUDA(e, d_first.alloc(n));
-    RLM_CUDA(e, cudaMemcpyAsync(d_recs.p, recs, n * record_bytes, cudaMemcpyHostToDevice, v.stream));
-    RLM_CUDA(e, cudaMemcpyAsync(d_lim.p, limited, n, cudaMemcpyHostToDevice, v.stream));
-    if (first_limited) RLM_CUDA(e, cudaMemcpyAsync(d_first.p, first_limited, n * sizeof(uint32_t), cudaMemcpyHostToDevice, v.stream));
+    In<uint8_t> d_recs, d_lim;
+    In<uint32_t> d_first;
+    RL_CUDA(e, d_recs.set(static_cast<const uint8_t*>(recs), n * record_bytes, mem, v.stream));
+    RL_CUDA(e, d_lim.set(limited, n, mem, v.stream));
+    RL_CUDA(e, d_first.set(first_limited, n, mem, v.stream));
     r = launch_metrics(e, s, v.stream, (uint32_t)n, d_recs.p, (int)record_bytes, d_lim.p, d_first.p);
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged copies are freed
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged copies are freed
     return r;
 }
 
@@ -180,10 +159,10 @@ int rl_ns_metrics_read(rl_engine* e, uint32_t ns_cap, uint64_t* out_authorized_c
     }
     if (out_limited_by_limit)
         for (uint32_t i = 0; i < limits_cap; i++) out_limited_by_limit[i] = 0;
-    if (!s->d_metrics) return RL_OK;
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));  // the view fenced the pipeline onto this stream
+    if (!s->d_metrics.p) return RL_OK;
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));  // the view fenced the pipeline onto this stream
     std::vector<unsigned long long> h(metrics_words(s->ns_cap, s->limits_cap));
-    RLM_CUDA(e, cudaMemcpy(h.data(), s->d_metrics, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    RL_CUDA(e, cudaMemcpy(h.data(), s->d_metrics.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     const uint32_t nn = std::min(ns_cap, s->ns_cap), nl = std::min(limits_cap, s->limits_cap);
     for (uint32_t i = 0; i < nn; i++) {
         if (out_authorized_calls) out_authorized_calls[i] = h[i];
@@ -193,7 +172,7 @@ int rl_ns_metrics_read(rl_engine* e, uint32_t ns_cap, uint64_t* out_authorized_c
     if (out_limited_by_limit)
         for (uint32_t i = 0; i < nl; i++) out_limited_by_limit[i] = h[3 * (size_t)s->ns_cap + i];
     if (out_dropped) *out_dropped = h[3 * (size_t)s->ns_cap + s->limits_cap];
-    if (reset) RLM_CUDA(e, cudaMemset(s->d_metrics, 0, h.size() * sizeof(unsigned long long)));
+    if (reset) RL_CUDA(e, cudaMemset(s->d_metrics.p, 0, h.size() * sizeof(unsigned long long)));
     return RL_OK;
 }
 
@@ -204,17 +183,17 @@ int rl_compact(rl_engine* e, uint32_t min_tombstone_pct, rl_compact_stats* out) 
     if (out) memset(out, 0, sizeof *out);
     const uint32_t P = 1u << v.log2P;
     const uint64_t R = 1ull << v.log2R;
-    Scratch<uint32_t> d_census;  // live[P] | tomb[P]
-    RLM_CUDA(e, d_census.alloc(2 * (size_t)P));
-    RLM_CUDA(e, cudaMemsetAsync(d_census.p, 0, 2 * (size_t)P * sizeof(uint32_t), v.stream));
+    DevBuf<uint32_t> d_census;  // live[P] | tomb[P]
+    RL_CUDA(e, d_census.alloc(2 * (size_t)P));
+    RL_CUDA(e, cudaMemsetAsync(d_census.p, 0, 2 * (size_t)P * sizeof(uint32_t), v.stream));
     const uint32_t threads = 256;
     const uint32_t blocks = (uint32_t)((v.capacity + threads - 1) / threads);
     k_region_census<<<blocks, threads, 0, v.stream>>>(v.rows, v.row_bytes, v.log2R, v.capacity, d_census.p, d_census.p + P);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 1);
     std::vector<uint32_t> census(2 * (size_t)P);
-    RLM_CUDA(e, cudaMemcpyAsync(census.data(), d_census.p, census.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream));
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+    RL_CUDA(e, cudaMemcpyAsync(census.data(), d_census.p, census.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));
     std::vector<uint8_t> sel(P, 0);
     uint64_t live = 0, tomb = 0, chosen = 0, tomb_chosen = 0;
     for (uint32_t g = 0; g < P; g++) {
@@ -234,25 +213,25 @@ int rl_compact(rl_engine* e, uint32_t min_tombstone_pct, rl_compact_stats* out) 
         out->regions_rebuilt = chosen;
     }
     if (!chosen) return RL_OK;
-    Scratch<uint8_t> d_sel, d_scratch;
-    Scratch<unsigned long long> d_counts;
-    RLM_CUDA(e, d_sel.alloc(P));
+    DevBuf<uint8_t> d_sel, d_scratch;
+    DevBuf<unsigned long long> d_counts;
+    RL_CUDA(e, d_sel.alloc(P));
     if (d_scratch.alloc((size_t)v.capacity * v.row_bytes) != cudaSuccess) {
         cudaGetLastError();
         return rl_internal_fail(e, RL_TRANSIENT, "rl_compact: no device memory for the scratch slab (one copy of the table)");
     }
-    RLM_CUDA(e, d_counts.alloc(3));
-    RLM_CUDA(e, cudaMemcpyAsync(d_sel.p, sel.data(), P, cudaMemcpyHostToDevice, v.stream));
-    RLM_CUDA(e, cudaMemsetAsync(d_counts.p, 0, 3 * sizeof(unsigned long long), v.stream));
+    RL_CUDA(e, d_counts.alloc(3));
+    RL_CUDA(e, cudaMemcpyAsync(d_sel.p, sel.data(), P, cudaMemcpyHostToDevice, v.stream));
+    RL_CUDA(e, cudaMemsetAsync(d_counts.p, 0, 3 * sizeof(unsigned long long), v.stream));
     k_compact_move<<<blocks, threads, 0, v.stream>>>(v.rows, d_scratch.p, v.row_bytes, v.log2R, v.capacity, d_sel.p);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     k_compact_reinsert<<<blocks, threads, 0, v.stream>>>(v.rows, d_scratch.p, v.row_bytes, v.log2P, v.log2R, v.capacity, d_sel.p, d_counts.p);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 2);
     r = rl_internal_reset_hot_rows(e);  // table row indices changed
     unsigned long long counts[3] = {0, 0, 0};
-    RLM_CUDA(e, cudaMemcpyAsync(counts, d_counts.p, sizeof counts, cudaMemcpyDeviceToHost, v.stream));
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));  // before the scratch slab is freed
+    RL_CUDA(e, cudaMemcpyAsync(counts, d_counts.p, sizeof counts, cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));  // before the scratch slab is freed
     if (r) return r;
     if (out) {
         out->rows_moved = counts[0];
@@ -274,26 +253,22 @@ int rl_counters_import(rl_engine* e, uint64_t n, const uint32_t* limit_id, const
     if (n >= (1ull << 48)) return rl_internal_fail(e, RL_FATAL, "rl_counters_import: n must stay below 2^48");
     if (n == 0) return RL_OK;
     // inputs on the device: the caller's arrays, or staged for the call
-    Scratch<uint32_t> s_lid;
-    Scratch<uint64_t> s_words;  // key_lo | key_hi | value | expiry, n each
-    RlImportIn I{limit_id, key_lo, key_hi, value, expiry_us, n};
-    if (mem == RL_MEM_HOST) {
-        RLM_CUDA(e, s_lid.alloc(n));
-        RLM_CUDA(e, s_words.alloc(4 * n));
-        RLM_CUDA(e, cudaMemcpyAsync(s_lid.p, limit_id, n * sizeof(uint32_t), cudaMemcpyHostToDevice, v.stream));
-        const uint64_t* src[4] = {key_lo, key_hi, value, expiry_us};
-        for (int k = 0; k < 4; k++)
-            RLM_CUDA(e, cudaMemcpyAsync(s_words.p + k * n, src[k], n * sizeof(uint64_t), cudaMemcpyHostToDevice, v.stream));
-        I = RlImportIn{s_lid.p, s_words.p, s_words.p + n, s_words.p + 2 * n, s_words.p + 3 * n, n};
-    }
+    In<uint32_t> lid;
+    In<uint64_t> lo, hi, val, exp;
+    RL_CUDA(e, lid.set(limit_id, n, mem, v.stream));
+    RL_CUDA(e, lo.set(key_lo, n, mem, v.stream));
+    RL_CUDA(e, hi.set(key_hi, n, mem, v.stream));
+    RL_CUDA(e, val.set(value, n, mem, v.stream));
+    RL_CUDA(e, exp.set(expiry_us, n, mem, v.stream));
+    const RlImportIn I{lid.p, lo.p, hi.p, val.p, exp.p, n};
     const RlImportTab T{v.rows, v.row_bytes, v.log2P, v.log2R, v.limits, v.limits_cap};
-    Scratch<unsigned long long> d_err, d_row_of;
-    Scratch<uint8_t> d_unq;
-    Scratch<unsigned> d_mask;  // per-row cell mask of this call
-    RLM_CUDA(e, d_err.alloc(1));
-    RLM_CUDA(e, d_unq.alloc(v.limits_cap));
-    RLM_CUDA(e, cudaMemsetAsync(d_err.p, 0xFF, sizeof(unsigned long long), v.stream));
-    RLM_CUDA(e, cudaMemsetAsync(d_unq.p, 0, v.limits_cap, v.stream));
+    DevBuf<unsigned long long> d_err, d_row_of;
+    DevBuf<uint8_t> d_unq;
+    DevBuf<unsigned> d_mask;  // per-row cell mask of this call
+    RL_CUDA(e, d_err.alloc(1));
+    RL_CUDA(e, d_unq.alloc(v.limits_cap));
+    RL_CUDA(e, cudaMemsetAsync(d_err.p, 0xFF, sizeof(unsigned long long), v.stream));
+    RL_CUDA(e, cudaMemsetAsync(d_unq.p, 0, v.limits_cap, v.stream));
     const uint32_t threads = 256;
     const uint32_t blocks = (uint32_t)((n + threads - 1) / threads);
     unsigned long long err = ~0ull;
@@ -303,45 +278,44 @@ int rl_counters_import(rl_engine* e, uint64_t n, const uint32_t* limit_id, const
         static const char* const reason[] = {"", "limit id not registered in this engine", "qualified counter with key_hi >= 2^32",
                                              "qualified counter with expiry 0", "the same counter appears twice",
                                              "its table region is full"};
-        char b[256];
-        snprintf(b, sizeof b, "rl_counters_import: entry %llu refused (%s) in the %s pass; no counter changed",
-                 (unsigned long long)idx, why <= RLM_IMP_TABLE_FULL ? reason[why] : "?", pass);
-        return rl_internal_fail(e, why == RLM_IMP_TABLE_FULL ? RL_TRANSIENT : RL_FATAL, b);
+        return fail(e, why == RLM_IMP_TABLE_FULL ? RL_TRANSIENT : RL_FATAL,
+                    "rl_counters_import: entry %llu refused (%s) in the %s pass; no counter changed", (unsigned long long)idx,
+                    why <= RLM_IMP_TABLE_FULL ? reason[why] : "?", pass);
     };
     // pass 1: every entry names a registered limit and a valid key / expiry
     k_import_resolve<<<blocks, threads, 0, v.stream>>>(T, I, d_err.p, d_unq.p);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 1);
-    RLM_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+    RL_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));
     if (err != ~0ull) return report("resolve");
     // pass 2: find or claim the rows; duplicates and full regions are found before any cell is written
-    RLM_CUDA(e, d_row_of.alloc(n));
+    RL_CUDA(e, d_row_of.alloc(n));
     if (d_mask.alloc(v.capacity) != cudaSuccess) {
         cudaGetLastError();
         return rl_internal_fail(e, RL_TRANSIENT, "rl_counters_import: no device memory for the per-row cell mask");
     }
-    RLM_CUDA(e, cudaMemsetAsync(d_mask.p, 0, v.capacity * sizeof(unsigned), v.stream));
-    RLM_CUDA(e, cudaMemsetAsync(d_row_of.p, 0, n * sizeof(unsigned long long), v.stream));
+    RL_CUDA(e, cudaMemsetAsync(d_mask.p, 0, v.capacity * sizeof(unsigned), v.stream));
+    RL_CUDA(e, cudaMemsetAsync(d_row_of.p, 0, n * sizeof(unsigned long long), v.stream));
     k_import_claim<<<blocks, threads, 0, v.stream>>>(T, I, d_row_of.p, d_mask.p, d_err.p);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 1);
-    RLM_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+    RL_CUDA(e, cudaMemcpyAsync(&err, d_err.p, sizeof err, cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));
     if (err != ~0ull) {  // give back the rows this call claimed: the table is byte-identical to before the call
         k_import_release<<<blocks, threads, 0, v.stream>>>(T, n, d_row_of.p);
-        RLM_CUDA(e, cudaGetLastError());
+        RL_CUDA(e, cudaGetLastError());
         rl_internal_launched(e, 1);
-        RLM_CUDA(e, cudaStreamSynchronize(v.stream));
+        RL_CUDA(e, cudaStreamSynchronize(v.stream));
         return report("claim");
     }
     // pass 3: the cells
     k_import_write<<<blocks, threads, 0, v.stream>>>(T, I, d_row_of.p);
-    RLM_CUDA(e, cudaGetLastError());
+    RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 1);
     std::vector<uint8_t> unq(v.limits_cap);
-    RLM_CUDA(e, cudaMemcpyAsync(unq.data(), d_unq.p, unq.size(), cudaMemcpyDeviceToHost, v.stream));
-    RLM_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged inputs are freed
+    RL_CUDA(e, cudaMemcpyAsync(unq.data(), d_unq.p, unq.size(), cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged inputs are freed
     rl_internal_mark_present(e, unq.data(), v.limits_cap);
     return RL_OK;
 }

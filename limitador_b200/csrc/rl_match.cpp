@@ -9,7 +9,6 @@
 // 0b10, `x != 'a'` the table 0b01).  The counter key of a variable set is digested once per request and
 // shared by the limits that use the same variables.
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -20,6 +19,7 @@
 #include <vector>
 
 #include "rl_blake2b.h"
+#include "rl_error.h"
 #include "rl_match.h"
 #include "rl_match_image.h"
 #include "rl_match_records.h"
@@ -552,22 +552,11 @@ struct rl_matcher {
 
 namespace {
 
-int mfail(rl_matcher* m, const char* fmt, ...) {
-    char buf[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
-    va_end(ap);
-    // a long expression is cut at the buffer's end: never in the middle of a UTF-8 sequence
-    size_t n = strlen(buf), s = n;
-    while (s > 0 && ((unsigned char)buf[s - 1] & 0xC0) == 0x80) s--;
-    if (s > 0 && (unsigned char)buf[s - 1] >= 0xC0) {
-        const unsigned char lead = (unsigned char)buf[s - 1];
-        const size_t need = lead >= 0xF0 ? 4 : lead >= 0xE0 ? 3 : 2;
-        if (n - (s - 1) < need) buf[s - 1] = 0;
-    }
+template <class... A>
+int mfail(rl_matcher* m, const char* fmt, A... a) {
+    std::string msg = rl_format(fmt, a...);
     std::lock_guard<std::mutex> g(m->err_mu);
-    m->last_error = buf;
+    m->last_error = std::move(msg);
     return RL_FATAL;
 }
 

@@ -13,7 +13,6 @@
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <functional>
@@ -25,6 +24,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "rl_error.h"
 #include "rl_http.h"
 #include "rl_json.h"
 #include "rl_match_records.h"
@@ -316,14 +316,9 @@ struct rl_http {
 
 namespace {
 
-template <class Svc>
-int sfail(Svc* s, const char* fmt, ...) {
-    char b[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(b, sizeof b, fmt, ap);
-    va_end(ap);
-    s->last_error = b;
+template <class Svc, class... A>
+int sfail(Svc* s, const char* fmt, A... a) {
+    s->last_error = rl_format(fmt, a...);
     return RL_FATAL;
 }
 

@@ -9,76 +9,17 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
 
 #include <cub/device/device_scan.cuh>
 
+#include "rl_cuda_host.h"
 #include "rl_cvars_dev.cuh"
 #include "rl_http_dev.cuh"
 #include "rl_internal.h"
 #include "rl_rls_dev.cuh"
-
-namespace {
-
-// device array that only grows
-template <class T>
-struct DBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (p && n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = std::max<size_t>(n + n / 2, 64);
-        const cudaError_t r = cudaMalloc((void**)&p, want * sizeof(T));
-        if (r == cudaSuccess) cap = want;
-        return r;
-    }
-    // exactly n elements (0: none), the old contents dropped
-    cudaError_t exact(size_t n) {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        if (n == 0) return cudaSuccess;
-        const cudaError_t r = cudaMalloc((void**)&p, n * sizeof(T));
-        if (r == cudaSuccess) cap = n;
-        return r;
-    }
-    void swap(DBuf& o) {
-        std::swap(p, o.p);
-        std::swap(cap, o.cap);
-    }
-    ~DBuf() {
-        if (p) cudaFree(p);
-    }
-};
-
-// pinned host array that only grows
-template <class T>
-struct HBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (p && n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = std::max<size_t>(n + n / 2, 64);
-        const cudaError_t r = cudaMallocHost((void**)&p, want * sizeof(T));
-        if (r == cudaSuccess) cap = want;
-        return r;
-    }
-    ~HBuf() {
-        if (p) cudaFreeHost(p);
-    }
-};
-
-}  // namespace
 
 struct rl_rls_dev {
     int device = 0;
@@ -87,43 +28,43 @@ struct rl_rls_dev {
     // the matcher image: host copy (its header places the sections) and device copy
     uint64_t gen = 0;
     std::vector<uint32_t> image;
-    DBuf<uint32_t> d_image;
+    DevBuf<uint32_t> d_image;
     // the batch
     uint64_t n = 0, n_store = 0, n_ctr = 0;
-    HBuf<uint8_t> h_buf;
-    HBuf<uint64_t> h_off;
-    HBuf<RlsDevReq> h_req;
-    HBuf<unsigned long long> h_total;
-    DBuf<uint8_t> d_buf, d_cub;
-    DBuf<uint64_t> d_off;
-    DBuf<rl_rls_entry> d_ent;
-    DBuf<rl_counter> d_scratch, d_ctrs;
-    DBuf<RlsDevReq> d_req;
-    DBuf<unsigned long long> d_count, d_start;
-    DBuf<uint32_t> d_ctr_off;
-    DBuf<uint64_t> d_delta, d_now;
+    PinnedBuf<uint8_t> h_buf;
+    PinnedBuf<uint64_t> h_off;
+    PinnedBuf<RlsDevReq> h_req;
+    PinnedBuf<unsigned long long> h_total;
+    DevBuf<uint8_t> d_buf, d_cub;
+    DevBuf<uint64_t> d_off;
+    DevBuf<rl_rls_entry> d_ent;
+    DevBuf<rl_counter> d_scratch, d_ctrs;
+    DevBuf<RlsDevReq> d_req;
+    DevBuf<unsigned long long> d_count, d_start;
+    DevBuf<uint32_t> d_ctr_off;
+    DevBuf<uint64_t> d_delta, d_now;
     // store call outputs
-    DBuf<uint8_t> d_lim;
-    DBuf<uint32_t> d_first;
-    DBuf<uint64_t> d_rem, d_ttl;
+    DevBuf<uint8_t> d_lim;
+    DevBuf<uint32_t> d_first;
+    DevBuf<uint64_t> d_rem, d_ttl;
     // the HTTP plan's own arrays
-    DBuf<uint8_t> d_txt, d_bits, d_load;
-    DBuf<HttpDevReq> d_hreq;
-    HBuf<HttpDevReq> h_hreq;
-    DBuf<HttpScan> d_hcount, d_hstart;
-    DBuf<uint32_t> d_runs, d_ctr_run;
-    HBuf<uint32_t> h_runs;
+    DevBuf<uint8_t> d_txt, d_bits, d_load;
+    DevBuf<HttpDevReq> d_hreq;
+    PinnedBuf<HttpDevReq> h_hreq;
+    DevBuf<HttpScan> d_hcount, d_hstart;
+    DevBuf<uint32_t> d_runs, d_ctr_run;
+    PinnedBuf<uint32_t> h_runs;
     uint32_t n_runs = 0;
     // the counter variable dictionary (rl_cvars_dev.cuh): off while cv_slots == 0
     uint64_t cv_slots = 0, cv_arena_bytes = 0;
-    DBuf<CvSlot> d_cv_slots;
-    DBuf<uint8_t> d_cv_arena;
-    DBuf<unsigned long long> d_cv_ctl;
+    DevBuf<CvSlot> d_cv_slots;
+    DevBuf<uint8_t> d_cv_arena;
+    DevBuf<unsigned long long> d_cv_ctl;
     // lookup and GC scratch
-    DBuf<uint32_t> d_cv_lid;
-    DBuf<uint64_t> d_cv_lo, d_cv_hi, d_cv_val, d_cv_exp, d_cv_src;
-    DBuf<unsigned long long> d_cv_len, d_cv_pos;
-    DBuf<uint8_t> d_cv_mark, d_cv_out;
+    DevBuf<uint32_t> d_cv_lid;
+    DevBuf<uint64_t> d_cv_lo, d_cv_hi, d_cv_val, d_cv_exp, d_cv_src;
+    DevBuf<unsigned long long> d_cv_len, d_cv_pos;
+    DevBuf<uint8_t> d_cv_mark, d_cv_out;
     std::vector<unsigned long long> h_cv_pos;
     std::vector<uint64_t> h_cv_src;
     std::vector<uint8_t> h_cv_out, h_cv_unnamed;
@@ -131,23 +72,11 @@ struct rl_rls_dev {
 
 namespace {
 
-int dev_fail(rl_rls_dev* S, int status, const char* fmt, ...) {
-    char b[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(b, sizeof b, fmt, ap);
-    va_end(ap);
-    S->err = b;
+template <class... A>
+int fail(rl_rls_dev* S, int status, const char* fmt, A... a) {
+    S->err = rl_format(fmt, a...);
     return status;
 }
-
-#define RLS_CUDA(S, call)                                                                                                   \
-    do {                                                                                                                    \
-        const cudaError_t _r = (call);                                                                                      \
-        if (_r != cudaSuccess)                                                                                              \
-            return dev_fail((S), _r == cudaErrorMemoryAllocation ? RL_TRANSIENT : RL_FATAL, "CUDA error %s at %s:%d (%s)", \
-                            cudaGetErrorName(_r), __FILE__, __LINE__, cudaGetErrorString(_r));                              \
-    } while (0)
 
 uint32_t blocks_for(uint64_t n, uint32_t threads) { return (uint32_t)((n + threads - 1) / threads); }
 
@@ -158,12 +87,12 @@ int refresh_image(rl_rls_dev* S, rl_matcher* m) {
     if (S->image.size() < 1024) S->image.resize(1024);
     uint64_t need = 0, got = 0;
     while (rl_matcher_image(m, S->image.data(), S->image.size(), &need, &got) != RL_OK) {
-        if (need <= S->image.size()) return dev_fail(S, RL_FATAL, "the matcher image could not be taken");
+        if (need <= S->image.size()) return fail(S, RL_FATAL, "the matcher image could not be taken");
         S->image.resize(need);
     }
     S->image.resize(need);
-    RLS_CUDA(S, S->d_image.reserve(need));
-    RLS_CUDA(S, cudaMemcpyAsync(S->d_image.p, S->image.data(), need * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
+    RL_CUDA(S, S->d_image.grow(need));
+    RL_CUDA(S, cudaMemcpyAsync(S->d_image.p, S->image.data(), need * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
     S->gen = got;
     return RL_OK;
 }
@@ -177,35 +106,35 @@ int stage_batch(rl_rls_dev* S, rl_engine* e, rl_matcher* m, uint64_t n, const ui
     S->n_runs = 0;
     RlTableView v;
     int r = rl_internal_view(e, &v);  // the engine's device and stream (every earlier pipelined call is fenced)
-    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
+    if (r) return fail(S, r, "%s", rl_last_error(e));
     S->device = v.device;
     S->stream = v.stream;
     if ((r = refresh_image(S, m))) return r;
     const uint32_t engine_max = rl_engine_max_counters_per_request(e);
     per_req = std::min(S->image[RL_IMG_H_COUNTER_CAP], engine_max);
     if (n && (n + 1) * (uint64_t)per_req >= (1ull << 32))
-        return dev_fail(S, RL_FATAL, "a batch of %llu requests of up to %u counters each may exceed 2^32 counters",
+        return fail(S, RL_FATAL, "a batch of %llu requests of up to %u counters each may exceed 2^32 counters",
                         (unsigned long long)n, per_req);
     const uint64_t bytes = n ? off[n] : 0;
     // wire bytes and offsets through pinned staging onto the device
-    RLS_CUDA(S, S->h_buf.reserve(bytes + 1));
-    RLS_CUDA(S, S->h_off.reserve(n + 1));
-    RLS_CUDA(S, S->h_total.reserve(1));
+    RL_CUDA(S, S->h_buf.grow(bytes + 1));
+    RL_CUDA(S, S->h_off.grow(n + 1));
+    RL_CUDA(S, S->h_total.grow(1));
     if (bytes) memcpy(S->h_buf.p, buf, bytes);
     memcpy(S->h_off.p, off, (n + 1) * sizeof(uint64_t));
-    RLS_CUDA(S, S->d_buf.reserve(bytes + 1));
-    RLS_CUDA(S, S->d_off.reserve(n + 1));
-    RLS_CUDA(S, S->d_ent.reserve(bytes / 2 + 1));
-    RLS_CUDA(S, S->d_scratch.reserve(n * (uint64_t)per_req + 1));
-    if (bytes) RLS_CUDA(S, cudaMemcpyAsync(S->d_buf.p, S->h_buf.p, bytes, cudaMemcpyHostToDevice, S->stream));
-    RLS_CUDA(S, cudaMemcpyAsync(S->d_off.p, S->h_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+    RL_CUDA(S, S->d_buf.grow(bytes + 1));
+    RL_CUDA(S, S->d_off.grow(n + 1));
+    RL_CUDA(S, S->d_ent.grow(bytes / 2 + 1));
+    RL_CUDA(S, S->d_scratch.grow(n * (uint64_t)per_req + 1));
+    if (bytes) RL_CUDA(S, cudaMemcpyAsync(S->d_buf.p, S->h_buf.p, bytes, cudaMemcpyHostToDevice, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(S->d_off.p, S->h_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
     return RL_OK;
 }
 
 // the one read before the store call: `bytes` from the device to pinned host memory, then the stream is waited for
 int read_totals(rl_rls_dev* S, void* dst, const void* src, size_t bytes) {
-    RLS_CUDA(S, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S->stream));
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
 
@@ -216,14 +145,14 @@ int copy_outputs(rl_rls_dev* S, bool verdicts, bool load_counters, uint8_t* limi
     if (verdicts) {
         if (cudaMemcpyAsync(limited, S->d_lim.p, m, cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
             cudaMemcpyAsync(first_limited, S->d_first.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
-            return dev_fail(S, RL_FATAL, "copying the verdicts back failed");
+            return fail(S, RL_FATAL, "copying the verdicts back failed");
     }
     if (load_counters) {
         if (cudaMemcpyAsync(remaining, S->d_rem.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
             cudaMemcpyAsync(ttl_us, S->d_ttl.p, nc * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
             cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (m + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
             cudaMemcpyAsync(ctrs, S->d_ctrs.p, nc * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess)
-            return dev_fail(S, RL_FATAL, "copying the counters back failed");
+            return fail(S, RL_FATAL, "copying the counters back failed");
     }
     return RL_OK;
 }
@@ -232,13 +161,13 @@ int copy_outputs(rl_rls_dev* S, bool verdicts, bool load_counters, uint8_t* limi
 // with host buffers)
 int reserve_outputs(rl_rls_dev* S, bool load_counters) {
     const uint64_t m = S->n_store, nc = S->n_ctr;
-    RLS_CUDA(S, S->d_lim.reserve(m));
-    RLS_CUDA(S, S->d_first.reserve(m));
+    RL_CUDA(S, S->d_lim.grow(m));
+    RL_CUDA(S, S->d_first.grow(m));
     if (load_counters) {
-        RLS_CUDA(S, S->d_rem.reserve(nc + 1));
-        RLS_CUDA(S, S->d_ttl.reserve(nc + 1));
-        RLS_CUDA(S, cudaMemsetAsync(S->d_rem.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
-        RLS_CUDA(S, cudaMemsetAsync(S->d_ttl.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+        RL_CUDA(S, S->d_rem.grow(nc + 1));
+        RL_CUDA(S, S->d_ttl.grow(nc + 1));
+        RL_CUDA(S, cudaMemsetAsync(S->d_rem.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
+        RL_CUDA(S, cudaMemsetAsync(S->d_ttl.p, 0, (nc + 1) * sizeof(uint64_t), S->stream));
     }
     return RL_OK;
 }
@@ -269,7 +198,7 @@ int record_vars(rl_rls_dev* S, uint64_t n, uint32_t per_req, const unsigned long
     a.dict = cv_dict(S);
     const uint32_t threads = 128;
     k_counter_vars_record<Dec><<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     launched = 1;
     return RL_OK;
 }
@@ -278,7 +207,7 @@ int record_vars(rl_rls_dev* S, uint64_t n, uint32_t per_req, const unsigned long
 int bind_engine(rl_rls_dev* S, rl_engine* e, rl_matcher* m) {
     RlTableView v;
     const int r = rl_internal_view(e, &v);
-    if (r) return dev_fail(S, r, "%s", rl_last_error(e));
+    if (r) return fail(S, r, "%s", rl_last_error(e));
     S->device = v.device;
     S->stream = v.stream;
     return m ? refresh_image(S, m) : RL_OK;
@@ -297,10 +226,10 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     uint32_t per_req = 0;
     int r = stage_batch(S, e, m, n, buf, off, per_req);
     if (r) return r;
-    RLS_CUDA(S, S->h_req.reserve(n + 1));
-    RLS_CUDA(S, S->d_req.reserve(n + 1));
-    RLS_CUDA(S, S->d_count.reserve(n + 1));
-    RLS_CUDA(S, S->d_start.reserve(n + 1));
+    RL_CUDA(S, S->h_req.grow(n + 1));
+    RL_CUDA(S, S->d_req.grow(n + 1));
+    RL_CUDA(S, S->d_count.grow(n + 1));
+    RL_CUDA(S, S->d_start.grow(n + 1));
     RlsPlanArgs a;
     a.buf = S->d_buf.p;
     a.off = S->d_off.p;
@@ -313,18 +242,18 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     a.count = S->d_count.p;
     const uint32_t threads = 128;
     k_rls_plan<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     size_t tmp = 0;
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
-    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_count.p, S->d_start.p, (int64_t)(n + 1), S->stream));
     // the one read before the store call: how many store requests and counters the batch has
     if ((r = read_totals(S, S->h_total.p, S->d_start.p + n, sizeof(unsigned long long)))) return r;
     const uint64_t n_store = S->h_total.p[0] >> 32, n_ctr = S->h_total.p[0] & 0xFFFFFFFFull;
-    RLS_CUDA(S, S->d_ctr_off.reserve(n_store + 1));
-    RLS_CUDA(S, S->d_ctrs.reserve(n_ctr + 1));
-    RLS_CUDA(S, S->d_delta.reserve(n_store + 1));
-    RLS_CUDA(S, S->d_now.reserve(n_store + 1));
+    RL_CUDA(S, S->d_ctr_off.grow(n_store + 1));
+    RL_CUDA(S, S->d_ctrs.grow(n_ctr + 1));
+    RL_CUDA(S, S->d_delta.grow(n_store + 1));
+    RL_CUDA(S, S->d_now.grow(n_store + 1));
     RlsScatterArgs b;
     b.req = S->d_req.p;
     b.scratch = S->d_scratch.p;
@@ -338,11 +267,11 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     b.delta = S->d_delta.p;
     b.now = S->d_now.p;
     k_rls_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     uint32_t rec = 0;
     if ((r = record_vars<CvWire>(S, n, per_req, S->d_count.p, nullptr, rec))) return r;
     rl_internal_launched(e, 2 + rec);
-    if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_req.p, S->d_req.p, n * sizeof(RlsDevReq), cudaMemcpyDeviceToHost, S->stream));
+    if (n) RL_CUDA(S, cudaMemcpyAsync(S->h_req.p, S->d_req.p, n * sizeof(RlsDevReq), cudaMemcpyDeviceToHost, S->stream));
     S->n = n;
     S->n_store = n_store;
     S->n_ctr = n_ctr;
@@ -354,11 +283,11 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
 
 int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta) {
     if (!S) return RL_FATAL;
-    RLS_CUDA(S, cudaSetDevice(S->device));
-    RLS_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_ctr) RLS_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_store) RLS_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    RL_CUDA(S, cudaSetDevice(S->device));
+    RL_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_ctr) RL_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_store) RL_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
 
@@ -367,7 +296,7 @@ int rl_rls_dev_decide(rl_rls_dev* S, rl_engine* e, int method, int load_counters
     if (!S || !e) return RL_FATAL;
     const uint64_t m = S->n_store;
     if (m == 0) return RL_OK;
-    RLS_CUDA(S, cudaSetDevice(S->device));
+    RL_CUDA(S, cudaSetDevice(S->device));
     int st = reserve_outputs(S, load_counters != 0);
     if (st) return st;
     if (method == RL_RLS_SHOULD_RATE_LIMIT)
@@ -396,14 +325,14 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
     const uint64_t bytes = n ? off[n] : 0;
     // the read before the store call: the head and up to kRunsRead store calls (a batch with more reads the rest after)
     const uint64_t kRunsRead = 1024;
-    RLS_CUDA(S, S->h_hreq.reserve(n + 1));
-    RLS_CUDA(S, S->h_runs.reserve(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
-    RLS_CUDA(S, S->d_txt.reserve(bytes + 1));
-    RLS_CUDA(S, S->d_bits.reserve(bytes / 8 + n + 1));
-    RLS_CUDA(S, S->d_hreq.reserve(n + 1));
-    RLS_CUDA(S, S->d_hcount.reserve(n + 1));
-    RLS_CUDA(S, S->d_hstart.reserve(n + 1));
-    RLS_CUDA(S, S->d_runs.reserve(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
+    RL_CUDA(S, S->h_hreq.grow(n + 1));
+    RL_CUDA(S, S->h_runs.grow(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
+    RL_CUDA(S, S->d_txt.grow(bytes + 1));
+    RL_CUDA(S, S->d_bits.grow(bytes / 8 + n + 1));
+    RL_CUDA(S, S->d_hreq.grow(n + 1));
+    RL_CUDA(S, S->d_hcount.grow(n + 1));
+    RL_CUDA(S, S->d_hstart.grow(n + 1));
+    RL_CUDA(S, S->d_runs.grow(RL_HTTP_RUNS_HEAD + 3 * (n + 1)));
     HttpPlanArgs a;
     a.buf = S->d_buf.p;
     a.off = S->d_off.p;
@@ -419,17 +348,17 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
     a.count = S->d_hcount.p;
     const uint32_t threads = 128;
     k_http_plan<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     size_t tmp = 0;
     const HttpScan zero{0, 0, 0, 0, 0, {0, 0}};
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
                                                S->stream));
-    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_hcount.p, S->d_hstart.p, HttpScanOp(), zero, (int64_t)(n + 1),
                                                S->stream));
     HttpRunsArgs ra{S->d_hcount.p, S->d_hstart.p, n, S->d_runs.p};
     k_http_runs<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(ra);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     const uint64_t first_read = RL_HTTP_RUNS_HEAD + 3 * std::min<uint64_t>(n, kRunsRead);
     if ((r = read_totals(S, S->h_runs.p, S->d_runs.p, first_read * sizeof(uint32_t)))) return r;
     const uint64_t n_store = S->h_runs.p[0], n_ctr = S->h_runs.p[1], n_runs = S->h_runs.p[2];
@@ -437,12 +366,12 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
         (r = read_totals(S, S->h_runs.p + first_read, S->d_runs.p + first_read,
                          (RL_HTTP_RUNS_HEAD + 3 * n_runs - first_read) * sizeof(uint32_t))))
         return r;
-    RLS_CUDA(S, S->d_ctr_off.reserve(n_store + 1));
-    RLS_CUDA(S, S->d_ctr_run.reserve(n_store + n_runs + 1));
-    RLS_CUDA(S, S->d_ctrs.reserve(n_ctr + 1));
-    RLS_CUDA(S, S->d_delta.reserve(n_store + 1));
-    RLS_CUDA(S, S->d_now.reserve(n_store + 1));
-    RLS_CUDA(S, S->d_load.reserve(n_store + 1));
+    RL_CUDA(S, S->d_ctr_off.grow(n_store + 1));
+    RL_CUDA(S, S->d_ctr_run.grow(n_store + n_runs + 1));
+    RL_CUDA(S, S->d_ctrs.grow(n_ctr + 1));
+    RL_CUDA(S, S->d_delta.grow(n_store + 1));
+    RL_CUDA(S, S->d_now.grow(n_store + 1));
+    RL_CUDA(S, S->d_load.grow(n_store + 1));
     HttpScatterArgs b;
     b.req = S->d_hreq.p;
     b.scratch = S->d_scratch.p;
@@ -459,11 +388,11 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
     b.now = S->d_now.p;
     b.load = S->d_load.p;
     k_http_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     uint32_t rec = 0;
     if ((r = record_vars<CvJson>(S, n, per_req, nullptr, S->d_hcount.p, rec))) return r;
     rl_internal_launched(e, 3 + rec);
-    if (n) RLS_CUDA(S, cudaMemcpyAsync(S->h_hreq.p, S->d_hreq.p, n * sizeof(HttpDevReq), cudaMemcpyDeviceToHost, S->stream));
+    if (n) RL_CUDA(S, cudaMemcpyAsync(S->h_hreq.p, S->d_hreq.p, n * sizeof(HttpDevReq), cudaMemcpyDeviceToHost, S->stream));
     S->n = n;
     S->n_store = n_store;
     S->n_ctr = n_ctr;
@@ -478,14 +407,14 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
 
 int rl_http_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load) {
     if (!S) return RL_FATAL;
-    RLS_CUDA(S, cudaSetDevice(S->device));
-    RLS_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_ctr) RLS_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaSetDevice(S->device));
+    RL_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_ctr) RL_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
     if (S->n_store) {
-        RLS_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaMemcpyAsync(load, S->d_load.p, S->n_store, cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(load, S->d_load.p, S->n_store, cudaMemcpyDeviceToHost, S->stream));
     }
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
 
@@ -493,7 +422,7 @@ int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_statu
                        uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
     if (!S || !e || !run_status) return RL_FATAL;
     if (S->n_store == 0) return RL_OK;
-    RLS_CUDA(S, cudaSetDevice(S->device));
+    RL_CUDA(S, cudaSetDevice(S->device));
     const HttpRun* runs = reinterpret_cast<const HttpRun*>(S->h_runs.p + RL_HTTP_RUNS_HEAD);
     bool any_load = false;
     for (uint32_t k = 0; k < S->n_runs; k++) any_load = any_load || runs[k].load;
@@ -523,8 +452,8 @@ int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_statu
 
 int rl_rls_dev_wait(rl_rls_dev* S) {
     if (!S) return RL_FATAL;
-    RLS_CUDA(S, cudaSetDevice(S->device));
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    RL_CUDA(S, cudaSetDevice(S->device));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
 
@@ -534,22 +463,22 @@ int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64
     rl_rls_dev* S = *st;
     int r = bind_engine(S, e, nullptr);
     if (r) return r;
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));  // no batch may still write the old dictionary
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));  // no batch may still write the old dictionary
     S->cv_slots = S->cv_arena_bytes = 0;
-    RLS_CUDA(S, S->d_cv_slots.exact(0));
-    RLS_CUDA(S, S->d_cv_arena.exact(0));
-    RLS_CUDA(S, S->d_cv_ctl.exact(0));
+    RL_CUDA(S, S->d_cv_slots.exact(0));
+    RL_CUDA(S, S->d_cv_arena.exact(0));
+    RL_CUDA(S, S->d_cv_ctl.exact(0));
     if (max_keys == 0 && arena_bytes == 0) return RL_OK;
     if (max_keys == 0 || arena_bytes == 0 || max_keys > (1ull << 40))
-        return dev_fail(S, RL_FATAL, "keeping counter variables needs max_keys in [1, 2^40] and arena_bytes > 0");
+        return fail(S, RL_FATAL, "keeping counter variables needs max_keys in [1, 2^40] and arena_bytes > 0");
     uint64_t slots = 16;
     while (slots < max_keys) slots *= 2;
-    RLS_CUDA(S, S->d_cv_slots.exact(slots));
-    RLS_CUDA(S, S->d_cv_arena.exact(arena_bytes));
-    RLS_CUDA(S, S->d_cv_ctl.exact(RL_CV_CTL_WORDS));
-    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_slots.p, 0, slots * sizeof(CvSlot), S->stream));
-    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_ctl.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+    RL_CUDA(S, S->d_cv_slots.exact(slots));
+    RL_CUDA(S, S->d_cv_arena.exact(arena_bytes));
+    RL_CUDA(S, S->d_cv_ctl.exact(RL_CV_CTL_WORDS));
+    RL_CUDA(S, cudaMemsetAsync(S->d_cv_slots.p, 0, slots * sizeof(CvSlot), S->stream));
+    RL_CUDA(S, cudaMemsetAsync(S->d_cv_ctl.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     S->cv_slots = slots;
     S->cv_arena_bytes = arena_bytes;
     return RL_OK;
@@ -558,9 +487,9 @@ int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64
 int rl_cv_dev_stats(rl_rls_dev* S, uint64_t* out_slots, uint64_t* out_keys, uint64_t* out_arena_used, uint64_t* out_dropped) {
     uint64_t w[RL_CV_CTL_WORDS] = {0, 0, 0, 0};
     if (S && S->cv_slots) {
-        RLS_CUDA(S, cudaSetDevice(S->device));
-        RLS_CUDA(S, cudaMemcpyAsync(w, S->d_cv_ctl.p, sizeof w, cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+        RL_CUDA(S, cudaSetDevice(S->device));
+        RL_CUDA(S, cudaMemcpyAsync(w, S->d_cv_ctl.p, sizeof w, cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaStreamSynchronize(S->stream));
     }
     if (out_slots) *out_slots = S ? S->cv_slots : 0;
     if (out_keys) *out_keys = w[RL_CV_KEYS];
@@ -584,37 +513,37 @@ int rl_cv_dev_lookup(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, c
         const RlImage I = rl_img_view(S->image.data(), S->image.data());
         for (uint64_t i = 0; i < n; i++) S->h_cv_unnamed[i] = limit_id[i] < I.n_limits && I.lims[5ull * limit_id[i] + 4] != 0;
     } else if (n) {
-        RLS_CUDA(S, S->d_cv_lid.reserve(n));
-        RLS_CUDA(S, S->d_cv_lo.reserve(n));
-        RLS_CUDA(S, S->d_cv_hi.reserve(n));
-        RLS_CUDA(S, S->d_cv_src.reserve(n));
-        RLS_CUDA(S, S->d_cv_len.reserve(n + 1));
-        RLS_CUDA(S, S->d_cv_pos.reserve(n + 1));
-        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_lid.p, limit_id, n * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
-        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_lo.p, key_lo, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
-        RLS_CUDA(S, cudaMemcpyAsync(S->d_cv_hi.p, key_hi, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+        RL_CUDA(S, S->d_cv_lid.grow(n));
+        RL_CUDA(S, S->d_cv_lo.grow(n));
+        RL_CUDA(S, S->d_cv_hi.grow(n));
+        RL_CUDA(S, S->d_cv_src.grow(n));
+        RL_CUDA(S, S->d_cv_len.grow(n + 1));
+        RL_CUDA(S, S->d_cv_pos.grow(n + 1));
+        RL_CUDA(S, cudaMemcpyAsync(S->d_cv_lid.p, limit_id, n * sizeof(uint32_t), cudaMemcpyHostToDevice, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(S->d_cv_lo.p, key_lo, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(S->d_cv_hi.p, key_hi, n * sizeof(uint64_t), cudaMemcpyHostToDevice, S->stream));
         CvLookupArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S),
                        S->d_cv_len.p, S->d_cv_src.p};
         const uint32_t threads = 256;
         k_counter_vars_lookup<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
-        RLS_CUDA(S, cudaGetLastError());
+        RL_CUDA(S, cudaGetLastError());
         size_t tmp = 0;
-        RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
-        RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
-        RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
+        RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
+        RL_CUDA(S, S->d_cub.grow(tmp + 1));
+        RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(n + 1), S->stream));
         unsigned long long total = 0;
-        RLS_CUDA(S, cudaMemcpyAsync(&total, S->d_cv_pos.p + n, sizeof total, cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
-        RLS_CUDA(S, S->d_cv_out.reserve(total + 1));
+        RL_CUDA(S, cudaMemcpyAsync(&total, S->d_cv_pos.p + n, sizeof total, cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaStreamSynchronize(S->stream));
+        RL_CUDA(S, S->d_cv_out.grow(total + 1));
         CvGatherArgs g{S->d_cv_pos.p, S->d_cv_len.p, S->d_cv_src.p, n, S->d_cv_arena.p, S->d_cv_out.p};
         k_counter_vars_gather<<<blocks_for(n, threads), threads, 0, S->stream>>>(g);
-        RLS_CUDA(S, cudaGetLastError());
+        RL_CUDA(S, cudaGetLastError());
         rl_internal_launched(e, 2);
         S->h_cv_out.resize(total + 1);
-        if (total) RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), S->d_cv_out.p, total, cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_pos.data(), S->d_cv_pos.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaMemcpyAsync(S->h_cv_src.data(), S->d_cv_src.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
-        RLS_CUDA(S, cudaStreamSynchronize(S->stream));
+        if (total) RL_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), S->d_cv_out.p, total, cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(S->h_cv_pos.data(), S->d_cv_pos.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaMemcpyAsync(S->h_cv_src.data(), S->d_cv_src.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        RL_CUDA(S, cudaStreamSynchronize(S->stream));
         for (uint64_t i = 0; i < n; i++) S->h_cv_unnamed[i] = S->h_cv_src[i] == RL_CV_NONE;
     }
     *out_blobs = S->h_cv_out.data();
@@ -632,60 +561,60 @@ int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, 
     int r = bind_engine(S, e, m);
     if (r) return r;
     uint64_t before[RL_CV_CTL_WORDS];
-    RLS_CUDA(S, cudaMemcpyAsync(before, S->d_cv_ctl.p, sizeof before, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(before, S->d_cv_ctl.p, sizeof before, cudaMemcpyDeviceToHost, S->stream));
     // the engine's live counters, on the device
     uint64_t n = 0;
     if ((r = rl_counters_export(e, nullptr, 0, now_us, 0, RL_MEM_DEVICE, nullptr, nullptr, nullptr, nullptr, nullptr, &n)))
-        return dev_fail(S, r, "%s", rl_last_error(e));
-    RLS_CUDA(S, S->d_cv_lid.reserve(n + 1));
-    RLS_CUDA(S, S->d_cv_lo.reserve(n + 1));
-    RLS_CUDA(S, S->d_cv_hi.reserve(n + 1));
-    RLS_CUDA(S, S->d_cv_val.reserve(n + 1));
-    RLS_CUDA(S, S->d_cv_exp.reserve(n + 1));
+        return fail(S, r, "%s", rl_last_error(e));
+    RL_CUDA(S, S->d_cv_lid.grow(n + 1));
+    RL_CUDA(S, S->d_cv_lo.grow(n + 1));
+    RL_CUDA(S, S->d_cv_hi.grow(n + 1));
+    RL_CUDA(S, S->d_cv_val.grow(n + 1));
+    RL_CUDA(S, S->d_cv_exp.grow(n + 1));
     uint64_t got = 0;
     if ((r = rl_counters_export(e, nullptr, 0, now_us, n, RL_MEM_DEVICE, S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, S->d_cv_val.p,
                                 S->d_cv_exp.p, &got)))
-        return dev_fail(S, r, "%s", rl_last_error(e));
+        return fail(S, r, "%s", rl_last_error(e));
     n = std::min(n, got);
     // mark what they reference, then copy it into a fresh table and arena
     const uint64_t slots = S->cv_slots;
-    RLS_CUDA(S, S->d_cv_mark.reserve(slots));
-    RLS_CUDA(S, S->d_cv_len.reserve(slots + 1));
-    RLS_CUDA(S, S->d_cv_pos.reserve(slots + 1));
-    RLS_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p, 0, slots, S->stream));
+    RL_CUDA(S, S->d_cv_mark.grow(slots));
+    RL_CUDA(S, S->d_cv_len.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_pos.grow(slots + 1));
+    RL_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p, 0, slots, S->stream));
     const uint32_t threads = 256;
     if (n) {
         CvMarkArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S), S->d_cv_mark.p};
         k_counter_vars_mark<<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
-        RLS_CUDA(S, cudaGetLastError());
+        RL_CUDA(S, cudaGetLastError());
     }
     k_counter_vars_kept<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(cv_dict(S), S->d_cv_mark.p, S->d_cv_len.p);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     size_t tmp = 0;
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
-    RLS_CUDA(S, S->d_cub.reserve(tmp + 1));
-    RLS_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
-    DBuf<CvSlot> slots2;
-    DBuf<uint8_t> arena2;
-    DBuf<unsigned long long> ctl2;
-    RLS_CUDA(S, slots2.exact(slots));
-    RLS_CUDA(S, arena2.exact(S->cv_arena_bytes));
-    RLS_CUDA(S, ctl2.exact(RL_CV_CTL_WORDS));
-    RLS_CUDA(S, cudaMemsetAsync(slots2.p, 0, slots * sizeof(CvSlot), S->stream));
-    RLS_CUDA(S, cudaMemsetAsync(ctl2.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    DevBuf<CvSlot> slots2;
+    DevBuf<uint8_t> arena2;
+    DevBuf<unsigned long long> ctl2;
+    RL_CUDA(S, slots2.exact(slots));
+    RL_CUDA(S, arena2.exact(S->cv_arena_bytes));
+    RL_CUDA(S, ctl2.exact(RL_CV_CTL_WORDS));
+    RL_CUDA(S, cudaMemsetAsync(slots2.p, 0, slots * sizeof(CvSlot), S->stream));
+    RL_CUDA(S, cudaMemsetAsync(ctl2.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
     // the count of dropped keys carries over
-    RLS_CUDA(S, cudaMemcpyAsync(ctl2.p + RL_CV_DROPPED, S->d_cv_ctl.p + RL_CV_DROPPED, sizeof(unsigned long long),
+    RL_CUDA(S, cudaMemcpyAsync(ctl2.p + RL_CV_DROPPED, S->d_cv_ctl.p + RL_CV_DROPPED, sizeof(unsigned long long),
                                 cudaMemcpyDeviceToDevice, S->stream));
     CvRebuildArgs b{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, CvDict{slots2.p, slots - 1, arena2.p, S->cv_arena_bytes, ctl2.p}};
     k_counter_vars_rebuild<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(b);
-    RLS_CUDA(S, cudaGetLastError());
+    RL_CUDA(S, cudaGetLastError());
     rl_internal_launched(e, n ? 3 : 2);
-    RLS_CUDA(S, cudaStreamSynchronize(S->stream));  // the old dictionary is read until here
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));  // the old dictionary is read until here
     S->d_cv_slots.swap(slots2);
     S->d_cv_arena.swap(arena2);
     S->d_cv_ctl.swap(ctl2);
     uint64_t after[RL_CV_CTL_WORDS];
-    RLS_CUDA(S, cudaMemcpy(after, S->d_cv_ctl.p, sizeof after, cudaMemcpyDeviceToHost));
+    RL_CUDA(S, cudaMemcpy(after, S->d_cv_ctl.p, sizeof after, cudaMemcpyDeviceToHost));
     if (out_kept) *out_kept = after[RL_CV_KEYS];
     if (out_freed) *out_freed = before[RL_CV_KEYS] - std::min(before[RL_CV_KEYS], after[RL_CV_KEYS]);
     return RL_OK;

@@ -138,3 +138,26 @@ def test_peer_exchange_refuses_an_inbox_larger_than_the_engine():
     owner = exchange.owner_of(0, world)
     with pytest.raises(EngineError):
         engines[owner].sync()
+
+
+def test_shard_refuses_a_slab_the_device_cannot_hold():
+    """A slab larger than the device is refused with RL_TRANSIENT and its exact size in bytes (the shard is freed before
+    the message is written), and the engine stays usable: the refused allocation does not fail its next launch."""
+    from limitador_b200.engine import RL_TRANSIENT
+    world, cap, lag = 32, 1 << 27, 4
+    depth = lag + 2
+    align = lambda x: (x + 255) & ~255
+    slab_bytes = (align(depth * world * cap * RECORD_DTYPE.itemsize) + align(depth * world * cap)
+                  + align(depth * world * 16))  # records | verdicts | one 16-byte control block per (buffer, peer)
+    assert slab_bytes > 4 * (80 << 30)  # far beyond an 80 GB device
+    w = streams.WORKLOADS["C2"](batch=1024, n_rows=2000, n_ns=1)
+    e = Engine(capacity_rows=w.capacity_rows, cells_per_row=w.cells_per_row, max_batch=w.batch, flags=2)
+    e.limits_set(w.limits)
+    with pytest.raises(EngineError) as err:
+        Shard(e, 0, world, cap, lag)
+    assert err.value.status == RL_TRANSIENT
+    assert f"cannot allocate the {slab_bytes}-byte exchange slab" in str(err.value)
+    recs = w.batch_records(0)
+    lim = e.check_and_update_records(recs, True, stride=w.cells_per_row)[0]
+    assert np.array_equal(lim, H.oracle_with_limits(w.limits, 1 << 16).batch_records(0, recs, True, w.cells_per_row)[0])
+    e.close()
