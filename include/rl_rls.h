@@ -129,10 +129,36 @@ int rl_rls_serve(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const ui
  *   rl_rls_counter_vars_gc     keep exactly the entries the engine's present counters reference
  *                              (rl_counters_export(NULL, now_us)) in a fresh table and a compacted arena (needs a second
  *                              arena of the same size for the length of the call).  Serialise with serve, as rl_compact.
+ *   rl_rls_counter_vars_export / _import   carry the dictionary through a counter snapshot (rl_counters_export /
+ *                              rl_counters_import), so that a restored counter is named in GET /counters at once.  Export
+ *                              with the same ns_ids and now_us as the counters; import before the counters.  The import
+ *                              checks every entry against the matcher's limits as they stand (the variable set, the blob's
+ *                              layout, UTF-8 without NUL, and BLAKE2b-96 over (source, value) equal to the key), so a
+ *                              file from another configuration, or a corrupted one, can never name a counter wrongly.
+ *                              Serialise both with serve, as rl_compact.
  * Needs a service created with an engine. */
 int rl_rls_keep_counter_vars(rl_rls *s, uint64_t max_keys, uint64_t arena_bytes);
 int rl_rls_counter_vars_stats(rl_rls *s, uint64_t *out_keys, uint64_t *out_arena_used, uint64_t *out_dropped);
 int rl_rls_counter_vars_gc(rl_rls *s, uint64_t now_us, uint64_t *out_kept, uint64_t *out_freed);
+/* The dictionary entries that the counters rl_counters_export(e, ns_ids, n_ns, now_us, ...) would list refer to,
+ * each entry once, in no particular order.  Host memory.  blob_off has cap + 1 entries; blob i is
+ * blobs[blob_off[i] .. blob_off[i+1]), in the dictionary's own format: for each variable of the variable set,
+ * in digest order, a u32 LE length and then the bytes.  With cap = 0, or with cap / bytes_cap too small, nothing is
+ * written and only *out_count / *out_bytes are set.  With keeping off the count is 0.  Changes nothing. */
+int rl_rls_counter_vars_export(rl_rls *s, const uint32_t *ns_ids, uint32_t n_ns, uint64_t now_us,
+                               uint64_t cap, uint64_t bytes_cap,
+                               uint32_t *out_varset, uint64_t *out_key_lo, uint64_t *out_key_hi,
+                               uint64_t *out_blob_off, uint8_t *out_blobs,
+                               uint64_t *out_count, uint64_t *out_bytes);
+/* Add entries to the dictionary.  All or nothing.  Keeping must be on.  blob_off has n + 1 entries, non-decreasing.
+ * RL_FATAL, with nothing changed and rl_rls_last_error naming the first refused entry and why: a variable set that is
+ * not a qualified limit's, a blob that is not exactly one (length, value) per variable, a value that is not UTF-8 or
+ * holds a NUL, values that do not digest to the key, a key named twice.  RL_TRANSIENT, with nothing changed (the
+ * dropped count included): no room in the arena, or a key without a free slot within 64 probes.  A key the dictionary
+ * holds already is skipped (by the digest its values are the same) and does not count in *out_added. */
+int rl_rls_counter_vars_import(rl_rls *s, uint64_t n, const uint32_t *varset, const uint64_t *key_lo,
+                               const uint64_t *key_hi, const uint64_t *blob_off, const uint8_t *blobs,
+                               uint64_t *out_added);
 
 /* Prometheus text exposition of authorized_calls / authorized_hits / limited_calls (sorted by label values) plus
  * `limitador_up 1`: lines `name{limitador_namespace="ns"[,limit_name="x"]} value` as

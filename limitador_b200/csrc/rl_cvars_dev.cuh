@@ -17,6 +17,9 @@
 //   k_counter_vars_lookup / _gather   GET /counters: per counter the blob's length or "unnamed", a scan, the packed blobs
 //   k_counter_vars_mark / _rebuild    GC: mark the entries the engine's live counters reference, then copy them into a
 //                       fresh table and a compacted arena
+//   k_counter_vars_export / _check / _import   snapshots: the GC's mark, then the marked entries laid out for the host;
+//                       an import checks every entry against the image (rl_cv_check_entry), then copies the dictionary
+//                       into a fresh table (_occupied, _kept, _rebuild) and claims the new entries there
 // Written, like rl_rls_dev.cuh, so that the same source runs under tests/emu/cuda_shim.h: per-thread code and global
 // atomics only.
 #pragma once
@@ -65,15 +68,17 @@ RL_HD uint64_t rl_cv_find(const CvDict& D, uint32_t varset, uint64_t lo, uint64_
     return RL_CV_NONE;
 }
 
-// Claim a slot for a key whose blob is already written; false: no free slot within the probe length.  A slot that
-// already holds the fingerprint is the key's own (recorded by another thread of the batch): nothing to do.
-__device__ __forceinline__ bool rl_cv_claim(const CvDict& D, uint32_t varset, uint64_t lo, uint64_t hi, uint64_t off,
-                                            uint32_t len) {
+enum : int { RL_CV_NO_ROOM = 0, RL_CV_CLAIMED = 1, RL_CV_HELD = 2 };
+
+// Claim a slot for a key whose blob is already written: RL_CV_CLAIMED, RL_CV_NO_ROOM (no free slot within the probe
+// length) or RL_CV_HELD (a slot already holds the fingerprint).
+__device__ __forceinline__ int rl_cv_claim_slot(const CvDict& D, uint32_t varset, uint64_t lo, uint64_t hi, uint64_t off,
+                                                uint32_t len) {
     const unsigned long long fp = rl_cv_fp(varset, lo, hi);
     for (uint64_t k = 0, P = rl_cv_probe_len(D); k < P; k++) {
         const uint64_t p = (fp + k) & D.mask;
         const unsigned long long prev = atomicCAS(&D.slots[p].fp, 0ull, fp);
-        if (prev == fp) return true;
+        if (prev == fp) return RL_CV_HELD;
         if (prev != 0) continue;
         CvSlot& s = D.slots[p];
         s.key_lo = lo;
@@ -82,9 +87,15 @@ __device__ __forceinline__ bool rl_cv_claim(const CvDict& D, uint32_t varset, ui
         s.off = off;
         s.len = len;
         atomicAdd(&D.ctl[RL_CV_KEYS], 1ull);
-        return true;
+        return RL_CV_CLAIMED;
     }
-    return false;
+    return RL_CV_NO_ROOM;
+}
+// The recording and the GC: a slot that already holds the fingerprint is the key's own (recorded by another thread of
+// the batch): nothing to do.  false: no free slot within the probe length.
+__device__ __forceinline__ bool rl_cv_claim(const CvDict& D, uint32_t varset, uint64_t lo, uint64_t hi, uint64_t off,
+                                            uint32_t len) {
+    return rl_cv_claim_slot(D, varset, lo, hi, off, len) != RL_CV_NO_ROOM;
 }
 
 struct CvRecordArgs {
@@ -274,4 +285,135 @@ __global__ void k_counter_vars_rebuild(CvRebuildArgs a) {
     const uint64_t at = a.pos[p];
     for (uint32_t t = 0; t < s.len; t++) a.to.arena[at + t] = a.from.arena[s.off + t];
     if (!rl_cv_claim(a.to, s.varset, s.key_lo, s.key_hi, at, s.len)) atomicAdd(&a.to.ctl[RL_CV_DROPPED], 1ull);
+}
+
+// ---- snapshots (include/rl_rls.h: rl_rls_counter_vars_export / _import) ---------------------------------------------
+// Export: the GC's mark over the counters rl_counters_export selects, the kept lengths and their scan (each blob's
+// position), a scan of the marks (each entry's index), then k_counter_vars_export lays the entries out for the host.
+struct CvExportArgs {
+    CvDict d;
+    const uint8_t* mark;               // [slots]
+    const unsigned long long* pos;     // [slots + 1]: exclusive sum of the kept lengths
+    const unsigned long long* idx;     // [slots + 1]: exclusive sum of the marks
+    uint32_t* varset;                  // [idx[slots]]
+    uint64_t* key_lo;
+    uint64_t* key_hi;
+    uint64_t* blob_off;                // [idx[slots] + 1]
+    uint8_t* blobs;                    // [pos[slots]]
+};
+
+__global__ void k_counter_vars_export(CvExportArgs a) {
+    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p > a.d.mask + 1) return;
+    if (p == a.d.mask + 1) {
+        a.blob_off[a.idx[p]] = a.pos[p];
+        return;
+    }
+    if (!a.mark[p]) return;
+    const CvSlot& s = a.d.slots[p];
+    const uint64_t k = a.idx[p], at = a.pos[p];
+    a.varset[k] = s.varset;
+    a.key_lo[k] = s.key_lo;
+    a.key_hi[k] = s.key_hi;
+    a.blob_off[k] = at;
+    for (uint32_t t = 0; t < s.len; t++) a.blobs[at + t] = a.d.arena[s.off + t];
+}
+
+// Why an imported entry is refused.  The call's word `bad` ends as the least (entry << 8 | reason), RL_CV_GOOD if none.
+enum : uint32_t {
+    RL_CV_BAD_VARSET = 1,     // not the variable set of a qualified limit of the image
+    RL_CV_BAD_LENGTH = 2,     // a length prefix or a value runs past the blob (or the blob has too few values)
+    RL_CV_BAD_TRAILING = 3,   // bytes after the set's last value
+    RL_CV_BAD_VALUE = 4,      // a value that is not UTF-8 or holds a NUL: the recording never stores one
+    RL_CV_BAD_DIGEST = 5,     // BLAKE2b-96 over (source, value) is not the key
+    RL_CV_BAD_DUPLICATE = 6,  // the import names the key twice
+};
+#define RL_CV_GOOD 0xFFFFFFFFFFFFFFFFull
+
+// One entry against the image: its variable set's sources (vs_vars[2 * vs] = first variable, [2 * vs + 1] = variables; 0
+// variables: no qualified limit has the set) and its blob b[0 .. n), which must be exactly one (u32 LE length, bytes)
+// per variable and digest to (lo, hi).  0 or an RL_CV_BAD_* reason.
+RL_HD uint32_t rl_cv_check_entry(const RlImage& I, const uint32_t* vs_vars, uint32_t n_vs, uint32_t vs, uint64_t lo, uint64_t hi,
+                                 const uint8_t* b, uint64_t n) {
+    if (vs == 0 || vs >= n_vs || vs_vars[2ull * vs + 1] == 0) return RL_CV_BAD_VARSET;
+    rl_b2::KeyDigest d;
+    uint64_t at = 0;
+    for (uint32_t v = vs_vars[2ull * vs], end = v + vs_vars[2ull * vs + 1]; v < end; v++) {
+        if (n - at < 4) return RL_CV_BAD_LENGTH;
+        const uint64_t len = (uint64_t)b[at] | (uint64_t)b[at + 1] << 8 | (uint64_t)b[at + 2] << 16 | (uint64_t)b[at + 3] << 24;
+        at += 4;
+        if (len > n - at) return RL_CV_BAD_LENGTH;
+        const uint8_t* val = b + at;
+        for (uint64_t t = 0; t < len; t++)
+            if (val[t] == 0) return RL_CV_BAD_VALUE;
+        if (!rl_wire::utf8_ok(val, val + len)) return RL_CV_BAD_VALUE;
+        const uint32_t* V = I.vars + 3ull * v;
+        d.str((const char*)I.arena + V[1], V[2]);
+        d.str((const char*)val, len);
+        at += len;
+    }
+    if (at != n) return RL_CV_BAD_TRAILING;
+    uint64_t dlo, dhi;
+    d.finish(dlo, dhi);
+    return dlo == lo && dhi == hi ? 0 : RL_CV_BAD_DIGEST;
+}
+
+struct CvImportArgs {
+    const uint32_t* varset;          // [n]
+    const uint64_t* key_lo;
+    const uint64_t* key_hi;
+    const uint64_t* blob_off;        // [n + 1], non-decreasing (checked on the host)
+    const uint8_t* blobs;
+    uint64_t n;
+    RlImage img;
+    const uint32_t* vs_vars;         // [2 * n_vs] (rl_cv_check_entry)
+    uint32_t n_vs;
+    CvDict dict;                     // check: the dictionary as it stands; import: the fresh one
+    unsigned long long* len;         // [n + 1]: the check's output, read by the import: the blob's length for a new key, 0
+                                     // for a key already present (a valid blob has at least 4 bytes); len[n] = 0
+    const unsigned long long* pos;   // import: [n + 1], exclusive sum of len
+    uint64_t base;                   // import: the fresh arena's bytes before the first imported blob
+    unsigned long long* bad;         // [1], RL_CV_GOOD before the check
+};
+
+// One thread per entry: refuse it, or leave its length for the import (0 when the dictionary has the key already: by
+// the digest, with the same values).
+__global__ void k_counter_vars_check(CvImportArgs a) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > a.n) return;
+    a.len[i] = 0;
+    if (i == a.n) return;
+    const uint64_t o = a.blob_off[i], n = a.blob_off[i + 1] - o;
+    const uint32_t why = rl_cv_check_entry(a.img, a.vs_vars, a.n_vs, a.varset[i], a.key_lo[i], a.key_hi[i], a.blobs + o, n);
+    if (why) {
+        atomicMin(a.bad, (unsigned long long)i << 8 | why);
+        return;
+    }
+    if (rl_cv_find(a.dict, a.varset[i], a.key_lo[i], a.key_hi[i]) == RL_CV_NONE) a.len[i] = n;
+}
+
+// After k_counter_vars_rebuild copied every entry of the dictionary into the fresh one: one thread per new entry copies
+// its blob to base + pos[i] and claims its slot.  No room counts in the fresh table's `dropped`; a slot that already
+// holds the key means the import names it twice.
+__global__ void k_counter_vars_import(CvImportArgs a) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > a.n) return;
+    if (i == a.n) {
+        a.dict.ctl[RL_CV_CURSOR] = a.base + a.pos[i];
+        return;
+    }
+    const uint64_t n = a.len[i];
+    if (n == 0) return;
+    const uint64_t at = a.base + a.pos[i];
+    const uint8_t* b = a.blobs + a.blob_off[i];
+    for (uint64_t t = 0; t < n; t++) a.dict.arena[at + t] = b[t];
+    const int r = rl_cv_claim_slot(a.dict, a.varset[i], a.key_lo[i], a.key_hi[i], at, (uint32_t)n);
+    if (r == RL_CV_NO_ROOM) atomicAdd(&a.dict.ctl[RL_CV_DROPPED], 1ull);
+    if (r == RL_CV_HELD) atomicMin(a.bad, (unsigned long long)i << 8 | RL_CV_BAD_DUPLICATE);
+}
+
+// every occupied slot (the import copies the whole dictionary into the fresh table)
+__global__ void k_counter_vars_occupied(CvDict d, uint8_t* mark) {
+    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p <= d.mask) mark[p] = d.slots[p].fp != 0;
 }

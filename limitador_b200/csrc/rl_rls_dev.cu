@@ -11,9 +11,11 @@
 #include <algorithm>
 #include <cstring>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include <cub/device/device_scan.cuh>
+#include <cuda/std/functional>
 
 #include "rl_cuda_host.h"
 #include "rl_cvars_dev.cuh"
@@ -64,6 +66,7 @@ struct rl_rls_dev {
     DevBuf<uint32_t> d_cv_lid;
     DevBuf<uint64_t> d_cv_lo, d_cv_hi, d_cv_val, d_cv_exp, d_cv_src;
     DevBuf<unsigned long long> d_cv_len, d_cv_pos;
+    DevBuf<unsigned long long> d_cv_idx;  // export: each entry's index
     DevBuf<uint8_t> d_cv_mark, d_cv_out;
     std::vector<unsigned long long> h_cv_pos;
     std::vector<uint64_t> h_cv_src;
@@ -201,6 +204,83 @@ int record_vars(rl_rls_dev* S, uint64_t n, uint32_t per_req, const unsigned long
     RL_CUDA(S, cudaGetLastError());
     launched = 1;
     return RL_OK;
+}
+
+// The first half of the GC and of the export: the engine's counters rl_counters_export(ns_ids, now_us) lists, on the
+// device, and the dictionary slots they reference marked in d_cv_mark [slots + 1] (mark[slots] = 0: the export scans
+// it).  d_cv_len and d_cv_pos get room for kept_positions.  launched = the kernels run (0 or 1).
+int mark_live(rl_rls_dev* S, rl_engine* e, const uint32_t* ns_ids, uint32_t n_ns, uint64_t now_us, uint32_t& launched) {
+    launched = 0;
+    uint64_t n = 0;
+    int r;
+    if ((r = rl_counters_export(e, ns_ids, n_ns, now_us, 0, RL_MEM_DEVICE, nullptr, nullptr, nullptr, nullptr, nullptr, &n)))
+        return fail(S, r, "%s", rl_last_error(e));
+    RL_CUDA(S, S->d_cv_lid.grow(n + 1));
+    RL_CUDA(S, S->d_cv_lo.grow(n + 1));
+    RL_CUDA(S, S->d_cv_hi.grow(n + 1));
+    RL_CUDA(S, S->d_cv_val.grow(n + 1));
+    RL_CUDA(S, S->d_cv_exp.grow(n + 1));
+    uint64_t got = 0;
+    if ((r = rl_counters_export(e, ns_ids, n_ns, now_us, n, RL_MEM_DEVICE, S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, S->d_cv_val.p,
+                                S->d_cv_exp.p, &got)))
+        return fail(S, r, "%s", rl_last_error(e));
+    n = std::min(n, got);
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, S->d_cv_mark.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_len.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_pos.grow(slots + 1));
+    RL_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p, 0, slots + 1, S->stream));
+    if (n) {
+        const uint32_t threads = 256;
+        CvMarkArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S), S->d_cv_mark.p};
+        k_counter_vars_mark<<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
+        RL_CUDA(S, cudaGetLastError());
+        launched = 1;
+    }
+    return RL_OK;
+}
+
+// d_cv_pos = where each marked slot's blob goes in a compacted arena (d_cv_pos[slots] = the kept bytes): one kernel
+int kept_positions(rl_rls_dev* S) {
+    const uint64_t slots = S->cv_slots;
+    const uint32_t threads = 256;
+    k_counter_vars_kept<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(cv_dict(S), S->d_cv_mark.p, S->d_cv_len.p);
+    RL_CUDA(S, cudaGetLastError());
+    size_t tmp = 0;
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    return RL_OK;
+}
+
+// The marked entries copied into a fresh table and arena of the configured sizes (the count of dropped keys carries
+// over): one kernel.  The caller swaps them in.
+int rebuild_fresh(rl_rls_dev* S, DevBuf<CvSlot>& slots2, DevBuf<uint8_t>& arena2, DevBuf<unsigned long long>& ctl2) {
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, slots2.exact(slots));
+    RL_CUDA(S, arena2.exact(S->cv_arena_bytes));
+    RL_CUDA(S, ctl2.exact(RL_CV_CTL_WORDS));
+    RL_CUDA(S, cudaMemsetAsync(slots2.p, 0, slots * sizeof(CvSlot), S->stream));
+    RL_CUDA(S, cudaMemsetAsync(ctl2.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(ctl2.p + RL_CV_DROPPED, S->d_cv_ctl.p + RL_CV_DROPPED, sizeof(unsigned long long),
+                                cudaMemcpyDeviceToDevice, S->stream));
+    CvRebuildArgs b{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, CvDict{slots2.p, slots - 1, arena2.p, S->cv_arena_bytes, ctl2.p}};
+    const uint32_t threads = 256;
+    k_counter_vars_rebuild<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(b);
+    RL_CUDA(S, cudaGetLastError());
+    return RL_OK;
+}
+
+const char* cv_reason(uint64_t why) {
+    switch (why) {
+        case RL_CV_BAD_VARSET: return "not the variable set of a qualified limit";
+        case RL_CV_BAD_LENGTH: return "a length runs past the blob";
+        case RL_CV_BAD_TRAILING: return "bytes after the last value";
+        case RL_CV_BAD_VALUE: return "a value that is not UTF-8 or holds a NUL";
+        case RL_CV_BAD_DIGEST: return "the values do not digest to the key";
+        case RL_CV_BAD_DUPLICATE: return "the import names the key twice";
+        default: return "unknown reason";
+    }
 }
 
 // the engine's device and stream, and the matcher's image as it stands now
@@ -562,53 +642,15 @@ int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, 
     if (r) return r;
     uint64_t before[RL_CV_CTL_WORDS];
     RL_CUDA(S, cudaMemcpyAsync(before, S->d_cv_ctl.p, sizeof before, cudaMemcpyDeviceToHost, S->stream));
-    // the engine's live counters, on the device
-    uint64_t n = 0;
-    if ((r = rl_counters_export(e, nullptr, 0, now_us, 0, RL_MEM_DEVICE, nullptr, nullptr, nullptr, nullptr, nullptr, &n)))
-        return fail(S, r, "%s", rl_last_error(e));
-    RL_CUDA(S, S->d_cv_lid.grow(n + 1));
-    RL_CUDA(S, S->d_cv_lo.grow(n + 1));
-    RL_CUDA(S, S->d_cv_hi.grow(n + 1));
-    RL_CUDA(S, S->d_cv_val.grow(n + 1));
-    RL_CUDA(S, S->d_cv_exp.grow(n + 1));
-    uint64_t got = 0;
-    if ((r = rl_counters_export(e, nullptr, 0, now_us, n, RL_MEM_DEVICE, S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, S->d_cv_val.p,
-                                S->d_cv_exp.p, &got)))
-        return fail(S, r, "%s", rl_last_error(e));
-    n = std::min(n, got);
-    // mark what they reference, then copy it into a fresh table and arena
-    const uint64_t slots = S->cv_slots;
-    RL_CUDA(S, S->d_cv_mark.grow(slots));
-    RL_CUDA(S, S->d_cv_len.grow(slots + 1));
-    RL_CUDA(S, S->d_cv_pos.grow(slots + 1));
-    RL_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p, 0, slots, S->stream));
-    const uint32_t threads = 256;
-    if (n) {
-        CvMarkArgs a{S->d_cv_lid.p, S->d_cv_lo.p, S->d_cv_hi.p, n, rl_img_view(S->image.data(), S->d_image.p), cv_dict(S), S->d_cv_mark.p};
-        k_counter_vars_mark<<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
-        RL_CUDA(S, cudaGetLastError());
-    }
-    k_counter_vars_kept<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(cv_dict(S), S->d_cv_mark.p, S->d_cv_len.p);
-    RL_CUDA(S, cudaGetLastError());
-    size_t tmp = 0;
-    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
-    RL_CUDA(S, S->d_cub.grow(tmp + 1));
-    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, S->d_cv_len.p, S->d_cv_pos.p, (int64_t)(slots + 1), S->stream));
+    // mark what the engine's live counters reference, then copy it into a fresh table and arena
+    uint32_t launched = 0;
+    if ((r = mark_live(S, e, nullptr, 0, now_us, launched))) return r;
+    if ((r = kept_positions(S))) return r;
     DevBuf<CvSlot> slots2;
     DevBuf<uint8_t> arena2;
     DevBuf<unsigned long long> ctl2;
-    RL_CUDA(S, slots2.exact(slots));
-    RL_CUDA(S, arena2.exact(S->cv_arena_bytes));
-    RL_CUDA(S, ctl2.exact(RL_CV_CTL_WORDS));
-    RL_CUDA(S, cudaMemsetAsync(slots2.p, 0, slots * sizeof(CvSlot), S->stream));
-    RL_CUDA(S, cudaMemsetAsync(ctl2.p, 0, RL_CV_CTL_WORDS * sizeof(unsigned long long), S->stream));
-    // the count of dropped keys carries over
-    RL_CUDA(S, cudaMemcpyAsync(ctl2.p + RL_CV_DROPPED, S->d_cv_ctl.p + RL_CV_DROPPED, sizeof(unsigned long long),
-                                cudaMemcpyDeviceToDevice, S->stream));
-    CvRebuildArgs b{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, CvDict{slots2.p, slots - 1, arena2.p, S->cv_arena_bytes, ctl2.p}};
-    k_counter_vars_rebuild<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(b);
-    RL_CUDA(S, cudaGetLastError());
-    rl_internal_launched(e, n ? 3 : 2);
+    if ((r = rebuild_fresh(S, slots2, arena2, ctl2))) return r;
+    rl_internal_launched(e, launched + 2);
     RL_CUDA(S, cudaStreamSynchronize(S->stream));  // the old dictionary is read until here
     S->d_cv_slots.swap(slots2);
     S->d_cv_arena.swap(arena2);
@@ -617,6 +659,169 @@ int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, 
     RL_CUDA(S, cudaMemcpy(after, S->d_cv_ctl.p, sizeof after, cudaMemcpyDeviceToHost));
     if (out_kept) *out_kept = after[RL_CV_KEYS];
     if (out_freed) *out_freed = before[RL_CV_KEYS] - std::min(before[RL_CV_KEYS], after[RL_CV_KEYS]);
+    return RL_OK;
+}
+
+int rl_cv_dev_export(rl_rls_dev** st, rl_engine* e, rl_matcher* m, const uint32_t* ns_ids, uint32_t n_ns, uint64_t now_us,
+                     uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset, uint64_t* out_key_lo, uint64_t* out_key_hi,
+                     uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes) {
+    if (!st || !e || !m || !out_count || !out_bytes) return RL_FATAL;
+    *out_count = *out_bytes = 0;
+    if (!*st || !(*st)->cv_slots) return RL_OK;
+    rl_rls_dev* S = *st;
+    int r = bind_engine(S, e, m);
+    if (r) return r;
+    uint32_t launched = 0;
+    if ((r = mark_live(S, e, ns_ids, n_ns, now_us, launched))) return r;
+    if ((r = kept_positions(S))) return r;
+    // each entry's index: a scan over the marks
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, S->d_cv_idx.grow(slots + 1));
+    size_t tmp = 0;
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull, (int64_t)(slots + 1),
+                                               S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull,
+                                               (int64_t)(slots + 1), S->stream));
+    unsigned long long tot[2] = {0, 0};
+    RL_CUDA(S, cudaMemcpyAsync(&tot[0], S->d_cv_idx.p + slots, sizeof tot[0], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[1], S->d_cv_pos.p + slots, sizeof tot[1], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    rl_internal_launched(e, launched + 1);
+    const uint64_t count = tot[0], bytes = tot[1];
+    *out_count = count;
+    *out_bytes = bytes;
+    if (cap == 0 || cap < count || bytes_cap < bytes) return RL_OK;
+    if (!out_varset || !out_key_lo || !out_key_hi || !out_blob_off || (bytes && !out_blobs))
+        return fail(S, RL_FATAL, "exporting counter variables: cap > 0 needs every output array");
+    // one packed array on the device, one copy to the host: varset (padded to 8 bytes), key_lo, key_hi, blob_off, blobs
+    const uint64_t o_lo = (4 * count + 7) / 8 * 8, o_hi = o_lo + 8 * count, o_off = o_hi + 8 * count, o_blob = o_off + 8 * (count + 1);
+    RL_CUDA(S, S->d_cv_out.grow(o_blob + bytes));
+    uint8_t* P = S->d_cv_out.p;
+    CvExportArgs a{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, S->d_cv_idx.p, reinterpret_cast<uint32_t*>(P),
+                   reinterpret_cast<uint64_t*>(P + o_lo), reinterpret_cast<uint64_t*>(P + o_hi),
+                   reinterpret_cast<uint64_t*>(P + o_off), P + o_blob};
+    const uint32_t threads = 256;
+    k_counter_vars_export<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(a);
+    RL_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    S->h_cv_out.resize(o_blob + bytes);
+    RL_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), P, o_blob + bytes, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    const uint8_t* h = S->h_cv_out.data();
+    memcpy(out_varset, h, 4 * count);
+    memcpy(out_key_lo, h + o_lo, 8 * count);
+    memcpy(out_key_hi, h + o_hi, 8 * count);
+    memcpy(out_blob_off, h + o_off, 8 * (count + 1));
+    if (bytes) memcpy(out_blobs, h + o_blob, bytes);
+    return RL_OK;
+}
+
+int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* varset, const uint64_t* key_lo,
+                     const uint64_t* key_hi, const uint64_t* blob_off, const uint8_t* blobs, uint64_t* out_added) {
+    if (!st || !e || !m || (n && (!varset || !key_lo || !key_hi || !blob_off))) return RL_FATAL;
+    if (out_added) *out_added = 0;
+    if (!*st) *st = new rl_rls_dev();
+    rl_rls_dev* S = *st;
+    if (!S->cv_slots) return fail(S, RL_FATAL, "importing counter variables needs keeping on (rl_rls_keep_counter_vars)");
+    if (n == 0) return RL_OK;
+    for (uint64_t i = 0; i < n; i++)
+        if (blob_off[i + 1] < blob_off[i])
+            return fail(S, RL_FATAL, "counter variable entry %llu refused: blob_off decreases after it", (unsigned long long)i);
+    const uint64_t bytes = blob_off[n];
+    if (bytes && !blobs) return fail(S, RL_FATAL, "importing counter variables: blobs is NULL");
+    int r = bind_engine(S, e, m);
+    if (r) return r;
+    // varset -> (first variable, variables) of the image's qualified limits
+    const RlImage H = rl_img_view(S->image.data(), S->image.data());
+    uint32_t n_vs = 1;
+    for (uint32_t l = 0; l < H.n_limits; l++) n_vs = std::max(n_vs, H.lims[5ull * l + 4] + 1);
+    std::vector<uint32_t> vs_vars(2ull * n_vs, 0);
+    for (uint32_t l = 0; l < H.n_limits; l++) {
+        const uint32_t* L = H.lims + 5ull * l;
+        if (L[4] && L[3]) {
+            vs_vars[2ull * L[4]] = L[2];
+            vs_vars[2ull * L[4] + 1] = L[3];
+        }
+    }
+    In<uint32_t> d_vs, d_vt;
+    In<uint64_t> d_lo, d_hi, d_off;
+    In<uint8_t> d_blobs;
+    RL_CUDA(S, d_vs.set(varset, n, RL_MEM_HOST, S->stream));
+    RL_CUDA(S, d_lo.set(key_lo, n, RL_MEM_HOST, S->stream));
+    RL_CUDA(S, d_hi.set(key_hi, n, RL_MEM_HOST, S->stream));
+    RL_CUDA(S, d_off.set(blob_off, n + 1, RL_MEM_HOST, S->stream));
+    RL_CUDA(S, d_blobs.set(blobs, bytes, RL_MEM_HOST, S->stream));
+    RL_CUDA(S, d_vt.set(vs_vars.data(), vs_vars.size(), RL_MEM_HOST, S->stream));
+    DevBuf<unsigned long long> len, pos, bad;
+    RL_CUDA(S, len.exact(n + 1));
+    RL_CUDA(S, pos.exact(n + 1));
+    RL_CUDA(S, bad.exact(1));
+    RL_CUDA(S, cudaMemsetAsync(bad.p, 0xFF, sizeof(unsigned long long), S->stream));
+    CvImportArgs a{d_vs.p, d_lo.p, d_hi.p, d_off.p, d_blobs.p, n, rl_img_view(S->image.data(), S->d_image.p), d_vt.p, n_vs,
+                   cv_dict(S), len.p, pos.p, 0, bad.p};
+    // check every entry against the image and the dictionary; each new blob's position after the kept ones
+    const uint32_t threads = 128;
+    k_counter_vars_check<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
+    RL_CUDA(S, cudaGetLastError());
+    size_t tmp = 0;
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(nullptr, tmp, len.p, pos.p, (int64_t)(n + 1), S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveSum(S->d_cub.p, tmp, len.p, pos.p, (int64_t)(n + 1), S->stream));
+    // every entry the dictionary holds, in a compacted arena
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, S->d_cv_mark.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_len.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_pos.grow(slots + 1));
+    k_counter_vars_occupied<<<blocks_for(slots, 256), 256, 0, S->stream>>>(cv_dict(S), S->d_cv_mark.p);
+    RL_CUDA(S, cudaGetLastError());
+    if ((r = kept_positions(S))) return r;
+    rl_internal_launched(e, 3);
+    uint64_t before[RL_CV_CTL_WORDS];
+    unsigned long long tot[3];  // bad, the new bytes, the kept bytes
+    RL_CUDA(S, cudaMemcpyAsync(before, S->d_cv_ctl.p, sizeof before, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[0], bad.p, sizeof tot[0], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[1], pos.p + n, sizeof tot[1], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[2], S->d_cv_pos.p + slots, sizeof tot[2], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    if (tot[0] != RL_CV_GOOD) return fail(S, RL_FATAL, "counter variable entry %llu refused: %s", tot[0] >> 8, cv_reason(tot[0] & 0xFF));
+    if (tot[1] == 0) return RL_OK;  // every key is held already
+    if (tot[1] + tot[2] > S->cv_arena_bytes)
+        return fail(S, RL_TRANSIENT, "the dictionary's arena has no room: %llu bytes kept + %llu imported > %llu", tot[2], tot[1],
+                    (unsigned long long)S->cv_arena_bytes);
+    // commit: a fresh table with every entry, then the new ones; swapped in only if each found its slot
+    DevBuf<CvSlot> slots2;
+    DevBuf<uint8_t> arena2;
+    DevBuf<unsigned long long> ctl2;
+    if ((r = rebuild_fresh(S, slots2, arena2, ctl2))) return r;
+    a.dict = CvDict{slots2.p, slots - 1, arena2.p, S->cv_arena_bytes, ctl2.p};
+    a.base = tot[2];
+    k_counter_vars_import<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(a);
+    RL_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, 2);
+    uint64_t after[RL_CV_CTL_WORDS];
+    RL_CUDA(S, cudaMemcpyAsync(after, ctl2.p, sizeof after, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[0], bad.p, sizeof tot[0], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    if (tot[0] != RL_CV_GOOD) {  // which thread saw the other's slot depends on the schedule: name the later entry
+        std::unordered_map<uint64_t, uint64_t> seen;  // (a hash of) the key -> first entry
+        for (uint64_t i = 0; i < n; i++) {
+            const uint64_t h = rl_cv_fp(varset[i], key_lo[i], key_hi[i]);
+            auto it = seen.find(h);
+            if (it != seen.end() && varset[it->second] == varset[i] && key_lo[it->second] == key_lo[i] && key_hi[it->second] == key_hi[i])
+                return fail(S, RL_FATAL, "counter variable entry %llu refused: %s (entry %llu)", (unsigned long long)i,
+                            cv_reason(RL_CV_BAD_DUPLICATE), (unsigned long long)it->second);
+            seen.emplace(h, i);
+        }
+        return fail(S, RL_FATAL, "counter variable entry %llu refused: %s", tot[0] >> 8, cv_reason(tot[0] & 0xFF));
+    }
+    if (after[RL_CV_DROPPED] != before[RL_CV_DROPPED])
+        return fail(S, RL_TRANSIENT, "the dictionary has no room: %llu entries found no free slot within %u probes",
+                    (unsigned long long)(after[RL_CV_DROPPED] - before[RL_CV_DROPPED]), RL_CV_PROBE);
+    S->d_cv_slots.swap(slots2);
+    S->d_cv_arena.swap(arena2);
+    S->d_cv_ctl.swap(ctl2);
+    if (out_added) *out_added = after[RL_CV_KEYS] - before[RL_CV_KEYS];
     return RL_OK;
 }
 

@@ -72,6 +72,14 @@ int rl_cv_dev_lookup(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, c
 // Keep exactly the entries the engine's counters reference (rl_counters_export(NULL, now_us)), in a fresh table and a
 // compacted arena.
 int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, uint64_t* out_kept, uint64_t* out_freed);
+// Snapshots (include/rl_rls.h: rl_rls_counter_vars_export / _import).  Export: the entries the counters
+// rl_counters_export(ns_ids, now_us) lists reference, into host arrays.  Import: every entry checked against the image
+// (variable set, blob, UTF-8, digest), then committed all or nothing into a fresh table.
+int rl_cv_dev_export(rl_rls_dev** st, rl_engine* e, rl_matcher* m, const uint32_t* ns_ids, uint32_t n_ns, uint64_t now_us,
+                     uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset, uint64_t* out_key_lo, uint64_t* out_key_hi,
+                     uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes);
+int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* varset, const uint64_t* key_lo,
+                     const uint64_t* key_hi, const uint64_t* blob_off, const uint8_t* blobs, uint64_t* out_added);
 const char* rl_rls_dev_error(rl_rls_dev* st);
 void rl_rls_dev_destroy(rl_rls_dev* st);
 }

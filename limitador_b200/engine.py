@@ -511,15 +511,19 @@ class Engine:
             ptrs, mem = [_p(c) for c in cols], MEM_HOST
         self._check(self._lib.rl_counters_import(self._h, n, *ptrs, mem))
 
-    def save_counters(self, path: str, now_us: int = 0):
-        """Write the limits (rl_limits_get) and every counter (export_counters(now_us)) to one .npz file at `path`;
-        the counters sorted by (limit_id, key) so that the same table always gives the same file."""
+    def _snapshot_arrays(self, now_us: int = 0) -> dict:
+        """The arrays of a save_counters file, in file order: the limits (rl_limits_get) and every counter
+        (export_counters(now_us)) sorted by (limit_id, key) so that the same table always gives the same file."""
         limits = self.limits_get()
         lid, lo, hi, val, exp = self.export_counters(now_us)
         order = np.lexsort((hi, lo, lid))
+        return dict(version=np.uint32(SNAPSHOT_VERSION), limits=limits, limit_id=lid[order], key_lo=lo[order],
+                    key_hi=hi[order], value=val[order], expiry_us=exp[order])
+
+    def save_counters(self, path: str, now_us: int = 0):
+        """Write the limits and every counter (_snapshot_arrays(now_us)) to one .npz file at `path`."""
         with open(path, "wb") as f:
-            np.savez(f, version=np.uint32(SNAPSHOT_VERSION), limits=limits, limit_id=lid[order], key_lo=lo[order],
-                     key_hi=hi[order], value=val[order], expiry_us=exp[order])
+            np.savez(f, **self._snapshot_arrays(now_us))
 
     def load_counters(self, path: str):
         """Import a save_counters file.  Limit ids are interned by the caller: this engine must have registered the same

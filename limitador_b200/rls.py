@@ -28,7 +28,7 @@ RLS_SYMBOLS = (
     "rl_rls_decode_request", "rl_rls_encode_response", "rl_rls_create", "rl_rls_destroy", "rl_rls_last_error",
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
     "rl_rls_last_timings", "rl_rls_plan_device", "rl_rls_keep_counter_vars", "rl_rls_counter_vars_stats",
-    "rl_rls_counter_vars_gc",
+    "rl_rls_counter_vars_gc", "rl_rls_counter_vars_export", "rl_rls_counter_vars_import",
 )
 
 ENTRY_DTYPE = np.dtype([("descriptor", "<u4"), ("key_off", "<u4"), ("key_len", "<u4"), ("val_off", "<u4"), ("val_len", "<u4")])
@@ -67,6 +67,8 @@ def _lib():
     L.rl_rls_keep_counter_vars.argtypes = [vp, u64, u64]
     L.rl_rls_counter_vars_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     L.rl_rls_counter_vars_gc.argtypes = [vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.rl_rls_counter_vars_export.argtypes = [vp, vp, u32, u64, u64, u64, vp, vp, vp, vp, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.rl_rls_counter_vars_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, C.POINTER(u64)]
     L._rl_rls_ready = True
     return L
 
@@ -307,6 +309,74 @@ class RlsService:
         k, f = C.c_uint64(), C.c_uint64()
         self._check(self._lib.rl_rls_counter_vars_gc(self._h, now_us, C.byref(k), C.byref(f)))
         return {"kept": k.value, "freed": f.value}
+
+    # -- snapshots: the dictionary beside the counters --
+    def export_counter_vars(self, now_us: int = 0, ns_ids=None):
+        """The dictionary entries the counters Engine.export_counters(now_us, ns_ids) lists refer to -> numpy arrays
+        (varset uint32, key_lo, key_hi, blob_off [n + 1], blobs uint8): entry i's values are blobs[blob_off[i] ..
+        blob_off[i + 1]), a u32 little-endian length then the bytes per variable, in no particular order.  Empty while
+        keeping is off."""
+        ids = None if ns_ids is None else np.ascontiguousarray(ns_ids, dtype=np.uint32)
+        n_ids = 0 if ids is None else len(ids)
+        p_ids = None if ids is None else (ids.ctypes.data if n_ids else np.zeros(1, np.uint32).ctypes.data)
+        cnt, nb, cap, bcap = C.c_uint64(0), C.c_uint64(0), 0, 0
+        while True:  # count, then fetch (again if the dictionary grew in between)
+            vs, lo, hi = np.zeros(max(cap, 1), np.uint32), np.zeros(max(cap, 1), np.uint64), np.zeros(max(cap, 1), np.uint64)
+            off, blobs = np.zeros(cap + 1, np.uint64), np.zeros(max(bcap, 1), np.uint8)
+            self._check(self._lib.rl_rls_counter_vars_export(self._h, p_ids, n_ids, now_us, cap, bcap, vs.ctypes.data,
+                                                             lo.ctypes.data, hi.ctypes.data, off.ctypes.data,
+                                                             blobs.ctypes.data, C.byref(cnt), C.byref(nb)))
+            if cap and cnt.value <= cap and nb.value <= bcap:
+                n = cnt.value
+                return vs[:n], lo[:n], hi[:n], off[:n + 1], blobs[:int(off[n])]
+            if cnt.value == 0:
+                return vs[:0], lo[:0], hi[:0], np.zeros(1, np.uint64), blobs[:0]
+            cap, bcap = int(cnt.value), int(nb.value)
+
+    def import_counter_vars(self, varset, key_lo, key_hi, blob_off, blobs) -> int:
+        """Add dictionary entries (the arrays export_counter_vars returns), all or nothing -> the keys added (keys the
+        dictionary holds already are skipped).  Every entry must match a qualified limit of the matcher and digest to its
+        key; a refused call raises RlsError naming the first refused entry and changes nothing."""
+        vs = np.ascontiguousarray(varset, dtype=np.uint32)
+        lo, hi = np.ascontiguousarray(key_lo, dtype=np.uint64), np.ascontiguousarray(key_hi, dtype=np.uint64)
+        off, b = np.ascontiguousarray(blob_off, dtype=np.uint64), np.ascontiguousarray(blobs, dtype=np.uint8)
+        n = len(vs)
+        if len(lo) != n or len(hi) != n or len(off) != n + 1:
+            raise ValueError("import_counter_vars: varset, key_lo and key_hi need n entries and blob_off n + 1")
+        if n and int(off.max()) > len(b):
+            raise ValueError("import_counter_vars: blob_off points past blobs")
+        added = C.c_uint64(0)
+        self._check(self._lib.rl_rls_counter_vars_import(self._h, n, vs.ctypes.data, lo.ctypes.data, hi.ctypes.data,
+                                                         off.ctypes.data, b.ctypes.data if len(b) else None, C.byref(added)))
+        return added.value
+
+    def save_counters(self, path: str, now_us: int = 0):
+        """Engine.save_counters(path, now_us) of the service's engine, plus the dictionary entries those counters refer
+        to (cv_varset, cv_key_lo, cv_key_hi, cv_blob_off, cv_blobs), sorted by (varset, key) so that the same state
+        always gives the same file.  Engine.load_counters reads the file as well (it ignores the cv_ arrays)."""
+        vs, lo, hi, off, blobs = self.export_counter_vars(now_us)
+        order = np.lexsort((hi, lo, vs))
+        ln = np.diff(off)[order]
+        new_off = np.zeros(len(order) + 1, np.uint64)
+        np.cumsum(ln, out=new_off[1:])
+        # byte t of sorted blob k comes from off[order[k]] + (t - new_off[k])
+        src = np.repeat(off[:-1][order].astype(np.int64) - new_off[:-1].astype(np.int64), ln.astype(np.int64))
+        src += np.arange(int(new_off[-1]), dtype=np.int64)
+        arrays = self._engine._snapshot_arrays(now_us)
+        arrays.update(cv_varset=vs[order], cv_key_lo=lo[order], cv_key_hi=hi[order], cv_blob_off=new_off, cv_blobs=blobs[src])
+        with open(path, "wb") as f:
+            np.savez(f, **arrays)
+
+    def load_counters(self, path: str) -> int:
+        """Import a save_counters file: the dictionary entries first (keeping must be on), then the counters through
+        Engine.load_counters.  Returns the keys added to the dictionary.  A file without cv_ arrays (Engine.save_counters)
+        loads exactly as Engine.load_counters loads it.  If the counter import is refused after the dictionary import,
+        the added entries refer to no counter, and the next counter_vars_gc drops them."""
+        with np.load(path) as z:
+            cv = [z[k] for k in ("cv_varset", "cv_key_lo", "cv_key_hi", "cv_blob_off", "cv_blobs")] if "cv_varset" in z else None
+        added = self.import_counter_vars(*cv) if cv is not None else 0
+        self._engine.load_counters(path)
+        return added
 
     def metrics(self) -> str:
         need = C.c_uint64()
