@@ -160,6 +160,56 @@ int rl_rls_counter_vars_import(rl_rls *s, uint64_t n, const uint32_t *varset, co
                                const uint64_t *key_hi, const uint64_t *blob_off, const uint8_t *blobs,
                                uint64_t *out_added);
 
+/* ---- configuration (RateLimiter::configure_with, limitador/src/lib.rs:475-505) -----------------------------------
+ * rl_rls_configure makes the service's matcher and engine hold exactly the limits of `limits`, as limitador-server does
+ * with its limits file at start and on every change of it:
+ *   - a limit's identity is (namespace, seconds, set of conditions, set of variables); of two entries with one identity
+ *     the first wins (HashSet::insert);
+ *   - a live limit of the new set is kept: its limit_id, counters (value and expiry) and position in its namespace stay.
+ *     If its max_value or name differs it takes the entry's max_value, name and id; if only the id differs nothing
+ *     changes (Storage::update_limit, storage/mod.rs:67-83);
+ *   - a live limit absent from the new set is deleted with its counters, qualified and unqualified (rl_limits_delete,
+ *     ONE call for all of them); added again later, it starts from fresh counters under its old limit_id;
+ *   - added limits follow the kept ones of their namespace, in the given order (the order of the counters of a request,
+ *     of X-RateLimit-Limit and of GET /limits);
+ *   - all or nothing: nothing changes (matcher, engine, device match image, counters, metrics) unless every entry is
+ *     accepted.  Refused: an expression the matcher's dialect does not accept; a namespace that would hold more limits
+ *     than one request may carry counters (the smaller of the matcher's counter cap and the engine's
+ *     max_counters_per_request; 16 without an engine); anything rl_limits_set refuses (the limits set before it are
+ *     dropped again and the old maxima restored).  RL_FATAL, report->first_refused = the entry's index, and
+ *     rl_rls_last_error says "entry <index>: <reason>".  A failure of the engine's delete call itself returns its status
+ *     with first_refused = RL_NONE.
+ * dry_run != 0 (limitador-server --validate): the entries are parsed, checked against the matcher and counted, nothing
+ * changes, and the engine is not asked.  engine == NULL: the matcher alone changes.  The matcher's generation is bumped
+ * once, so the next device plan uploads the new match image.  Pipelined record calls issued before are fenced first
+ * (RL_FLAG_PIPELINE).  The counter-variable dictionary is not collected: after a call with deleted > 0, run
+ * rl_rls_counter_vars_gc to get the deleted counters' entries back.  Serialise with serve, as rl_compact. */
+typedef struct rl_limit_spec {
+    const char *ns;
+    uint64_t max_value;
+    uint64_t seconds;
+    const char *const *conditions;
+    uint32_t n_cond;
+    uint32_t _pad0;
+    const char *const *variables;
+    uint32_t n_var;
+    uint32_t _pad1;
+    const char *name; /* nullable */
+    const char *id;   /* nullable; GET /limits renders it */
+} rl_limit_spec;
+typedef struct rl_configure_report {
+    uint32_t kept;          /* live limits of the new set with max_value and name unchanged */
+    uint32_t added;         /* new limits, and deleted ones that came back */
+    uint32_t updated;       /* kept limits that took a new max_value or name */
+    uint32_t deleted;       /* live limits deleted, with their counters */
+    uint32_t first_refused; /* index of the refused entry, or RL_NONE */
+    uint32_t _pad;
+} rl_configure_report;
+int rl_rls_configure(rl_rls *s, const rl_limit_spec *limits, uint32_t n, int dry_run, rl_configure_report *out_report);
+/* Status::config_version / config_err_since (limitador-server/src/main.rs:218-235): successful rl_rls_configure calls,
+ * and failed ones since the last success.  Dry runs do not count. */
+int rl_rls_config_status(rl_rls *s, uint64_t *out_version, uint64_t *out_err_since);
+
 /* Prometheus text exposition of authorized_calls / authorized_hits / limited_calls (sorted by label values) plus
  * `limitador_up 1`: lines `name{limitador_namespace="ns"[,limit_name="x"]} value` as
  * metrics_exporter_prometheus renders them (prometheus_metrics.rs:415-447).  *out_len = bytes needed incl. NUL. */

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <shared_mutex>
@@ -97,8 +98,8 @@ struct ParsedTest {
 };
 
 struct MLimit {
-    std::string ns, name;
-    bool has_name = false, deleted = false;
+    std::string ns, name, id;
+    bool has_name = false, has_id = false, deleted = false;
     uint32_t ns_id = 0, varset_id = 0;
     uint64_t max_value = 0, seconds = 0;
     std::vector<std::string> conds, vars;  // sorted, unique (the identity)
@@ -535,18 +536,27 @@ thread_local Scratch tls_scratch;
 
 }  // namespace
 
-struct rl_matcher {
+struct MLock {
     std::shared_mutex mu;
     uint32_t counter_cap = RL_MAX_COUNTERS_PER_REQUEST;  // rl_matcher_set_counter_cap
     uint32_t dialect = RL_MATCH_DIALECT_TABLE;           // rl_matcher_set_dialect: how later add_limit calls parse
     std::mutex err_mu;  // last_error is also written by matching calls, which hold `mu` shared
     std::string last_error;
+};
+
+// Everything the limits define: rl_matcher_configure stages a whole new set of limits on a copy and swaps it in.
+struct MTables {
     SlotTable slots;
     std::vector<MLimit> limits;
     std::unordered_map<std::string, uint32_t> ns_ids;
     std::vector<std::vector<uint32_t>> ns_limits;  // registration order
     std::map<std::string, uint32_t> by_identity;
     std::map<std::string, uint32_t> varsets;  // (namespace, variables) -> id, from 1
+};
+
+// The lock first and the tables behind it, in that order: matching threads bump the lock's reader count on every batch,
+// and the tables they read stay off its cache line.
+struct rl_matcher : MLock, MTables {
     uint64_t generation = 1;                  // rl_matcher_generation: bumped by every change of the limits or the cap
 };
 
@@ -653,6 +663,128 @@ int match_one(const rl_matcher* m, uint32_t ns_id, const rl_binding* binds, uint
     return RL_OK;
 }
 
+// The identity (limit.rs:177-214) as by_identity keys it: namespace, seconds, the sorted condition and variable sets.
+std::string identity_of(const MLimit& L) {
+    return L.ns + '\0' + std::to_string(L.seconds) + '\0' + joined(L.conds) + '\0' + joined(L.vars);
+}
+
+// A limit as parsed (Limit::new), before any table of the matcher is touched.
+struct ParsedLimit {
+    MLimit L;
+    std::vector<ParsedTest> conds;
+    std::vector<std::pair<uint32_t, std::string>> vars;  // (descriptor, key) of each variable, in L.vars order
+    std::string ident;                                   // the identity (limit.rs:177-214)
+};
+
+// The parse-only half of rl_matcher_add_limit_ex: false, with the reason in err, for an expression the dialect refuses.
+bool parse_limit(uint32_t dialect, const char* ns, uint64_t max_value, uint64_t seconds, const char* const* conditions,
+                 uint32_t n_cond, const char* const* variables, uint32_t n_var, const char* name, const char* id,
+                 ParsedLimit& P, std::string& err) {
+    MLimit& L = P.L;
+    L.ns = ns;
+    L.max_value = max_value;
+    L.seconds = seconds;
+    if (name) {
+        L.name = name;
+        L.has_name = true;
+    }
+    if (id) {
+        L.id = id;
+        L.has_id = true;
+    }
+    for (uint32_t i = 0; i < n_cond; i++) L.conds.emplace_back(conditions[i] ? conditions[i] : "");
+    for (uint32_t i = 0; i < n_var; i++) L.vars.emplace_back(variables[i] ? variables[i] : "");
+    // the identity holds SETS of expression sources (limit.rs:31-48: BTreeSet)
+    std::sort(L.conds.begin(), L.conds.end());
+    L.conds.erase(std::unique(L.conds.begin(), L.conds.end()), L.conds.end());
+    std::sort(L.vars.begin(), L.vars.end());
+    L.vars.erase(std::unique(L.vars.begin(), L.vars.end()), L.vars.end());
+    for (size_t i = 0; i < L.conds.size(); i++) {
+        bool ok;
+        if (dialect == RL_MATCH_DIALECT_BOOLEAN) {
+            ok = BoolParser(L.conds[i].c_str()).parse(P.conds);
+        } else {
+            P.conds.emplace_back();
+            ok = parse_table_condition(L.conds[i].c_str(), P.conds.back());
+        }
+        if (!ok) {
+            err = rl_format("unsupported condition expression: %s", L.conds[i].c_str());
+            return false;
+        }
+    }
+    P.vars.resize(L.vars.size());
+    for (size_t i = 0; i < L.vars.size(); i++)
+        if (!parse_variable(L.vars[i].c_str(), P.vars[i].first, P.vars[i].second)) {
+            err = rl_format("unsupported variable expression: %s", L.vars[i].c_str());
+            return false;
+        }
+    P.ident = identity_of(L);
+    return true;
+}
+
+// The table half of rl_matcher_add_limit_ex (Storage::add_limit / update_limit) on t; returns the limit's id.
+uint32_t place_limit(MTables& t, ParsedLimit&& P, int keep_existing, int* out_existed) {
+    MLimit& L = P.L;
+    uint32_t lid;
+    auto it = t.by_identity.find(P.ident);
+    if (it != t.by_identity.end()) {
+        // update_limit (storage/mod.rs:67-83): same identity, new max_value / name; a deleted one comes back
+        lid = it->second;
+        MLimit& E = t.limits[lid];
+        if (out_existed) *out_existed = E.deleted ? 0 : 1;
+        // Storage::add_limit is a HashSet::insert: on an equal (live) element it is a no-op and the OLD
+        // max_value / name stay (storage/mod.rs:60-65); only update_limit swaps them (:67-83)
+        if (!(keep_existing && !E.deleted)) {
+            // update_limit replaces the whole Limit, id included, only when max_value or name differ
+            if (E.deleted || E.max_value != L.max_value || E.has_name != L.has_name || E.name != L.name) {
+                E.id = L.id;
+                E.has_id = L.has_id;
+            }
+            E.max_value = L.max_value;
+            E.name = L.name;
+            E.has_name = L.has_name;
+        }
+        if (E.deleted) {  // deleted and added again: it is the namespace's newest limit
+            auto& order = t.ns_limits[E.ns_id];
+            order.erase(std::remove(order.begin(), order.end(), lid), order.end());
+            order.push_back(lid);
+            E.deleted = false;
+        }
+        return lid;
+    }
+    lid = (uint32_t)t.limits.size();
+    auto nit = t.ns_ids.find(L.ns);
+    if (nit == t.ns_ids.end()) {
+        nit = t.ns_ids.emplace(L.ns, (uint32_t)t.ns_ids.size()).first;
+        t.ns_limits.emplace_back();
+    }
+    L.ns_id = nit->second;
+    if (!L.vars.empty()) {
+        const std::string vk = L.ns + '\0' + joined(L.vars);
+        auto vit = t.varsets.find(vk);
+        if (vit == t.varsets.end()) vit = t.varsets.emplace(vk, (uint32_t)t.varsets.size() + 1).first;
+        L.varset_id = vit->second;
+    }
+    for (auto& c : P.conds) L.tests.push_back({t.slots.intern(c.desc, c.key), std::move(c.atoms), c.table});
+    for (const auto& v : P.vars) L.var_slots.push_back(t.slots.intern(v.first, v.second));
+    t.by_identity.emplace(std::move(P.ident), lid);
+    t.ns_limits[L.ns_id].push_back(lid);
+    t.limits.push_back(std::move(L));
+    return lid;
+}
+
+rl_limit_desc desc_of(const MTables& t, uint32_t lid) {
+    const MLimit& R = t.limits[lid];
+    rl_limit_desc d;
+    d.limit_id = lid;
+    d.ns_id = R.ns_id;
+    d.varset_id = R.varset_id;
+    d.qualified = R.vars.empty() ? 0 : 1;  // counter.rs:108-110
+    d.max_value = R.max_value;
+    d.window_us = R.seconds * 1000000ull;  // counter.rs:76-78
+    return d;
+}
+
 }  // namespace
 
 extern "C" {
@@ -686,91 +818,14 @@ int rl_matcher_add_limit_ex(rl_matcher* m, const char* ns, uint64_t max_value, u
     if (!m || !ns || !out_desc || (n_cond && !conditions) || (n_var && !variables)) return RL_FATAL;
     if (out_existed) *out_existed = 0;
     std::unique_lock<std::shared_mutex> lock(m->mu);
-    MLimit L;
-    L.ns = ns;
-    L.max_value = max_value;
-    L.seconds = seconds;
-    if (name) {
-        L.name = name;
-        L.has_name = true;
-    }
-    for (uint32_t i = 0; i < n_cond; i++) L.conds.emplace_back(conditions[i] ? conditions[i] : "");
-    for (uint32_t i = 0; i < n_var; i++) L.vars.emplace_back(variables[i] ? variables[i] : "");
-    // the identity holds SETS of expression sources (limit.rs:31-48: BTreeSet)
-    std::sort(L.conds.begin(), L.conds.end());
-    L.conds.erase(std::unique(L.conds.begin(), L.conds.end()), L.conds.end());
-    std::sort(L.vars.begin(), L.vars.end());
-    L.vars.erase(std::unique(L.vars.begin(), L.vars.end()), L.vars.end());
     // parse before touching any table: a refused limit leaves the matcher unchanged
-    struct Parsed {
-        uint32_t desc;
-        std::string key;
-    };
-    std::vector<ParsedTest> pc;
-    std::vector<Parsed> pv(L.vars.size());
-    for (size_t i = 0; i < L.conds.size(); i++) {
-        bool ok;
-        if (m->dialect == RL_MATCH_DIALECT_BOOLEAN) {
-            ok = BoolParser(L.conds[i].c_str()).parse(pc);
-        } else {
-            pc.emplace_back();
-            ok = parse_table_condition(L.conds[i].c_str(), pc.back());
-        }
-        if (!ok) return mfail(m, "unsupported condition expression: %s", L.conds[i].c_str());
-    }
-    for (size_t i = 0; i < L.vars.size(); i++)
-        if (!parse_variable(L.vars[i].c_str(), pv[i].desc, pv[i].key))
-            return mfail(m, "unsupported variable expression: %s", L.vars[i].c_str());
-
-    const std::string ident = L.ns + '\0' + std::to_string(seconds) + '\0' + joined(L.conds) + '\0' + joined(L.vars);
-    uint32_t lid;
-    auto it = m->by_identity.find(ident);
-    if (it != m->by_identity.end()) {
-        // update_limit (storage/mod.rs:67-83): same identity, new max_value / name; a deleted one comes back
-        lid = it->second;
-        MLimit& E = m->limits[lid];
-        if (out_existed) *out_existed = E.deleted ? 0 : 1;
-        // Storage::add_limit is a HashSet::insert: on an equal (live) element it is a no-op and the OLD
-        // max_value / name stay (storage/mod.rs:60-65); only update_limit swaps them (:67-83)
-        if (!(keep_existing && !E.deleted)) {
-            E.max_value = max_value;
-            E.name = L.name;
-            E.has_name = L.has_name;
-        }
-        if (E.deleted) {  // deleted and added again: it is the namespace's newest limit
-            auto& order = m->ns_limits[E.ns_id];
-            order.erase(std::remove(order.begin(), order.end(), lid), order.end());
-            order.push_back(lid);
-            E.deleted = false;
-        }
-    } else {
-        lid = (uint32_t)m->limits.size();
-        auto nit = m->ns_ids.find(L.ns);
-        if (nit == m->ns_ids.end()) {
-            nit = m->ns_ids.emplace(L.ns, (uint32_t)m->ns_ids.size()).first;
-            m->ns_limits.emplace_back();
-        }
-        L.ns_id = nit->second;
-        if (!L.vars.empty()) {
-            const std::string vk = L.ns + '\0' + joined(L.vars);
-            auto vit = m->varsets.find(vk);
-            if (vit == m->varsets.end()) vit = m->varsets.emplace(vk, (uint32_t)m->varsets.size() + 1).first;
-            L.varset_id = vit->second;
-        }
-        for (auto& c : pc) L.tests.push_back({m->slots.intern(c.desc, c.key), std::move(c.atoms), c.table});
-        for (const auto& v : pv) L.var_slots.push_back(m->slots.intern(v.desc, v.key));
-        m->by_identity.emplace(ident, lid);
-        m->ns_limits[L.ns_id].push_back(lid);
-        m->limits.push_back(std::move(L));
-    }
+    ParsedLimit P;
+    std::string err;
+    if (!parse_limit(m->dialect, ns, max_value, seconds, conditions, n_cond, variables, n_var, name, nullptr, P, err))
+        return mfail(m, "%s", err.c_str());
+    const uint32_t lid = place_limit(*m, std::move(P), keep_existing, out_existed);
     m->generation++;
-    const MLimit& R = m->limits[lid];
-    out_desc->limit_id = lid;
-    out_desc->ns_id = R.ns_id;
-    out_desc->varset_id = R.varset_id;
-    out_desc->qualified = R.vars.empty() ? 0 : 1;  // counter.rs:108-110
-    out_desc->max_value = R.max_value;
-    out_desc->window_us = R.seconds * 1000000ull;  // counter.rs:76-78
+    *out_desc = desc_of(*m, lid);
     return RL_OK;
 }
 
@@ -1164,11 +1219,77 @@ bool rl_matcher_ns_limit_records(rl_matcher* m, const std::string& ns, std::vect
         r.seconds = L.seconds;
         r.has_name = L.has_name;
         r.name = L.name;
+        r.has_id = L.has_id;
+        r.id = L.id;
         r.conditions = L.conds;
         r.variables = L.vars;
         out.push_back(std::move(r));
     }
     return true;
+}
+
+int rl_matcher_configure(rl_matcher* m, const rl_limit_spec* specs, uint32_t n, uint32_t max_limits_per_ns, bool dry_run,
+                         RlConfigurePlan& plan, const std::function<int(RlConfigurePlan&)>& apply) {
+    plan = RlConfigurePlan();
+    if (!m || (n && !specs)) return RL_FATAL;
+    std::unique_lock<std::shared_mutex> lock(m->mu);
+    const auto refuse = [&](uint32_t i, std::string why) {
+        plan.refused = i;
+        plan.error = rl_format("entry %u: %s", i, why.c_str());
+        return RL_FATAL;
+    };
+    // 1. every entry parsed in the dialect in force; the first of two entries with one identity wins (HashSet::insert)
+    std::vector<ParsedLimit> parsed(n);
+    std::vector<uint8_t> first(n, 0);
+    std::map<std::string, uint32_t> wanted;  // identity -> entry
+    std::unordered_map<std::string, uint32_t> per_ns;
+    const uint32_t cap = std::min(max_limits_per_ns, m->counter_cap);
+    for (uint32_t i = 0; i < n; i++) {
+        const rl_limit_spec& x = specs[i];
+        if (!x.ns || (x.n_cond && !x.conditions) || (x.n_var && !x.variables)) return refuse(i, "null namespace or expression list");
+        std::string err;
+        if (!parse_limit(m->dialect, x.ns, x.max_value, x.seconds, x.conditions, x.n_cond, x.variables, x.n_var, x.name, x.id, parsed[i], err))
+            return refuse(i, err);
+        if (!wanted.emplace(parsed[i].ident, i).second) continue;
+        first[i] = 1;
+        if (++per_ns[parsed[i].L.ns] > cap)
+            return refuse(i, rl_format("namespace %s would hold more than %u limits, the counters one request may carry", x.ns, cap));
+    }
+    // 2. staged on a copy of the tables: live limits absent from the new set are deleted, kept ones stay where they are,
+    // added ones follow in the given order
+    MTables t = *m;
+    for (uint32_t lid = 0; lid < t.limits.size(); lid++) {
+        MLimit& L = t.limits[lid];
+        if (L.deleted) continue;
+        if (wanted.count(identity_of(L))) continue;
+        L.deleted = true;
+        plan.deleted.push_back(lid);
+    }
+    for (uint32_t i = 0; i < n; i++) {
+        if (!first[i]) continue;
+        ParsedLimit& P = parsed[i];
+        const auto it = t.by_identity.find(P.ident);
+        const MLimit* E = it == t.by_identity.end() ? nullptr : &t.limits[it->second];
+        if (E && !E->deleted && E->max_value == P.L.max_value && E->has_name == P.L.has_name && E->name == P.L.name) {
+            plan.kept++;  // update_limit compares max_value and name only: the old id stays too
+            continue;
+        }
+        const bool update = E && !E->deleted;
+        const uint64_t old_max = update ? E->max_value : 0;
+        const uint32_t lid = place_limit(t, std::move(P), 0, nullptr);
+        plan.set.push_back(desc_of(t, lid));
+        plan.set_entry.push_back(i);
+        plan.set_added.push_back(update ? 0 : 1);
+        plan.old_max.push_back(old_max);
+        (update ? plan.updated : plan.added)++;
+    }
+    if (dry_run) return RL_OK;
+    // 3. the engine (the caller's apply), then the matcher in one step
+    const int r = apply ? apply(plan) : RL_OK;
+    if (r != RL_OK) return r;
+    static_cast<MTables&>(*m) = std::move(t);
+    m->generation++;
+    return RL_OK;
 }
 
 extern "C" {

@@ -70,6 +70,9 @@ __attribute__((weak)) int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_mat
 __attribute__((weak)) int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_t now_us, uint64_t cap,
                                           uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi,
                                           uint64_t* out_remaining, uint64_t* out_ttl_us, uint64_t* out_count);
+__attribute__((weak)) int rl_limits_set(rl_engine* e, const rl_limit_desc* limits, uint32_t n);
+__attribute__((weak)) int rl_limits_delete(rl_engine* e, const uint32_t* limit_ids, uint32_t n);
+__attribute__((weak)) int rl_fence(rl_engine* e);
 __attribute__((weak)) const char* rl_rls_dev_error(rl_rls_dev* st);
 __attribute__((weak)) void rl_rls_dev_destroy(rl_rls_dev* st);
 }
@@ -277,6 +280,8 @@ struct rl_rls {
     std::map<std::string, NsCounts> by_ns;
     std::map<std::pair<std::string, std::string>, uint64_t> limited_by_name;
     double t_plan = 0, t_store = 0, t_finish = 0;
+    // rl_rls_configure outcomes (Status::config_success / config_failure)
+    uint64_t config_version = 0, config_err_since = 0;
 };
 
 // The HTTP API (include/rl_http.h) over an RLS service: its own batch, the service's matcher, engine, workers, device
@@ -944,9 +949,12 @@ void json_str_list(std::string& o, const std::vector<std::string>& v) {
     o.push_back(']');
 }
 
-// request_types.rs Limit; id is always null (the matcher keeps no limit ids)
+// request_types.rs Limit; id is null for limits added without one (rl_matcher_add_limit)
 void json_limit(std::string& o, const std::string& ns, const RlLimitRecord& L) {
-    o += "{\"id\":null,\"namespace\":";
+    o += "{\"id\":";
+    if (L.has_id) json_str(o, L.id);
+    else o += "null";
+    o += ",\"namespace\":";
     json_str(o, ns);
     o += ",\"max_value\":" + std::to_string(L.max_value) + ",\"seconds\":" + std::to_string(L.seconds) + ",\"name\":";
     if (L.has_name) json_str(o, L.name);
@@ -1193,6 +1201,48 @@ int rl_rls_serve(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const ui
     return r;
 }
 
+// The engine's half of rl_rls_configure, on the matcher's staged plan: register the added limits and the new maxima, then
+// delete the removed limits in one call.  On a refusal, what was set is undone, so that the engine is as it was.
+static int configure_engine(rl_engine* e, RlConfigurePlan& plan) {
+    if (!rl_limits_set || !rl_limits_delete || !rl_fence) {
+        plan.error = "this build of the library has no engine";
+        return RL_FATAL;
+    }
+    int r = rl_fence(e);  // pipelined record calls still read the limit tables that rl_limits_set marks for upload
+    if (r) {
+        plan.error = std::string("fencing the pipelined calls: ") + rl_last_error(e);
+        return r;
+    }
+    const auto undo = [&](size_t upto) {
+        std::vector<uint32_t> drop;
+        for (size_t k = 0; k < upto; k++) {
+            if (plan.set_added[k]) {
+                drop.push_back(plan.set[k].limit_id);
+                continue;
+            }
+            rl_limit_desc d = plan.set[k];
+            d.max_value = plan.old_max[k];
+            rl_limits_set(e, &d, 1);
+        }
+        if (!drop.empty()) rl_limits_delete(e, drop.data(), (uint32_t)drop.size());
+    };
+    for (size_t k = 0; k < plan.set.size(); k++) {
+        if ((r = rl_limits_set(e, &plan.set[k], 1)) == RL_OK) continue;
+        const std::string why = rl_last_error(e);
+        undo(k);
+        plan.refused = plan.set_entry[k];
+        plan.error = rl_format("entry %u: the engine refused the limit: %s", plan.set_entry[k], why.c_str());
+        return r;
+    }
+    if (!plan.deleted.empty() && (r = rl_limits_delete(e, plan.deleted.data(), (uint32_t)plan.deleted.size())) != RL_OK) {
+        const std::string why = rl_last_error(e);
+        undo(plan.set.size());
+        plan.error = "deleting the removed limits: " + why;
+        return r;
+    }
+    return RL_OK;
+}
+
 int rl_rls_metrics_render(rl_rls* s, char* out, uint64_t cap, uint64_t* out_len) {
     if (!s || !out_len) return RL_FATAL;
     std::string t;
@@ -1236,6 +1286,38 @@ int rl_rls_last_timings(rl_rls* s, double* out_plan_us, double* out_store_us, do
     if (out_plan_us) *out_plan_us = s->t_plan;
     if (out_store_us) *out_store_us = s->t_store;
     if (out_finish_us) *out_finish_us = s->t_finish;
+    return RL_OK;
+}
+
+int rl_rls_configure(rl_rls* s, const rl_limit_spec* limits, uint32_t n, int dry_run, rl_configure_report* out_report) {
+    if (!s || (n && !limits)) return RL_FATAL;
+    if (out_report) *out_report = rl_configure_report{0, 0, 0, 0, RL_NONE, 0};
+    const uint32_t engine_max = (s->engine && rl_engine_max_counters_per_request)
+                                    ? rl_engine_max_counters_per_request(s->engine) : RL_MAX_COUNTERS_PER_REQUEST;
+    RlConfigurePlan plan;
+    std::function<int(RlConfigurePlan&)> apply;
+    if (s->engine) apply = [s](RlConfigurePlan& p) { return configure_engine(s->engine, p); };
+    const int r = rl_matcher_configure(s->m, limits, n, engine_max, dry_run != 0, plan, apply);
+    if (out_report) {
+        *out_report = rl_configure_report{plan.kept, plan.added, plan.updated, (uint32_t)plan.deleted.size(), plan.refused, 0};
+        if (r != RL_OK) out_report->kept = out_report->added = out_report->updated = out_report->deleted = 0;
+    }
+    if (r != RL_OK) s->last_error = plan.error.empty() ? "configure: invalid arguments" : plan.error;
+    if (!dry_run) {
+        if (r == RL_OK) {
+            s->config_version++;
+            s->config_err_since = 0;
+        } else {
+            s->config_err_since++;
+        }
+    }
+    return r;
+}
+
+int rl_rls_config_status(rl_rls* s, uint64_t* out_version, uint64_t* out_err_since) {
+    if (!s) return RL_FATAL;
+    if (out_version) *out_version = s->config_version;
+    if (out_err_since) *out_err_since = s->config_err_since;
     return RL_OK;
 }
 

@@ -28,7 +28,8 @@ RLS_SYMBOLS = (
     "rl_rls_decode_request", "rl_rls_encode_response", "rl_rls_create", "rl_rls_destroy", "rl_rls_last_error",
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
     "rl_rls_last_timings", "rl_rls_plan_device", "rl_rls_keep_counter_vars", "rl_rls_counter_vars_stats",
-    "rl_rls_counter_vars_gc", "rl_rls_counter_vars_export", "rl_rls_counter_vars_import",
+    "rl_rls_counter_vars_gc", "rl_rls_counter_vars_export", "rl_rls_counter_vars_import", "rl_rls_configure",
+    "rl_rls_config_status",
 )
 
 ENTRY_DTYPE = np.dtype([("descriptor", "<u4"), ("key_off", "<u4"), ("key_len", "<u4"), ("val_off", "<u4"), ("val_len", "<u4")])
@@ -41,6 +42,31 @@ class RlsRequest(C.Structure):
 
 class RlsError(RuntimeError):
     pass
+
+
+class ConfigureError(RlsError):
+    """A configuration refused by RlsService.configure_with; `index` is the refused entry (None when the engine's delete
+    call failed).  Nothing changed."""
+
+    def __init__(self, msg: str, index: Optional[int]):
+        super().__init__(msg)
+        self.index = index
+
+
+class LimitSpec(C.Structure):
+    _fields_ = [("ns", C.c_char_p), ("max_value", C.c_uint64), ("seconds", C.c_uint64),
+                ("conditions", C.POINTER(C.c_char_p)), ("n_cond", C.c_uint32), ("_pad0", C.c_uint32),
+                ("variables", C.POINTER(C.c_char_p)), ("n_var", C.c_uint32), ("_pad1", C.c_uint32),
+                ("name", C.c_char_p), ("id", C.c_char_p)]
+
+
+class ConfigureReport(C.Structure):
+    _fields_ = [("kept", C.c_uint32), ("added", C.c_uint32), ("updated", C.c_uint32), ("deleted", C.c_uint32),
+                ("first_refused", C.c_uint32), ("_pad", C.c_uint32)]
+
+
+def _field(limit, key):
+    return limit[key] if isinstance(limit, dict) else getattr(limit, key)
 
 
 def _lib():
@@ -69,6 +95,8 @@ def _lib():
     L.rl_rls_counter_vars_gc.argtypes = [vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.rl_rls_counter_vars_export.argtypes = [vp, vp, u32, u64, u64, u64, vp, vp, vp, vp, vp, C.POINTER(u64), C.POINTER(u64)]
     L.rl_rls_counter_vars_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, C.POINTER(u64)]
+    L.rl_rls_configure.argtypes = [vp, C.POINTER(LimitSpec), u32, i32, C.POINTER(ConfigureReport)]
+    L.rl_rls_config_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L._rl_rls_ready = True
     return L
 
@@ -377,6 +405,42 @@ class RlsService:
         added = self.import_counter_vars(*cv) if cv is not None else 0
         self._engine.load_counters(path)
         return added
+
+    # -- configuration --
+    def configure_with(self, limits, dry_run: bool = False) -> Dict[str, int]:
+        """RateLimiter::configure_with (lib.rs:475-505) over rl_rls_configure: the service then holds exactly `limits`
+        (limiter.Limit objects, or dicts as limits_file.parse_limits returns them).  Kept limits keep their counters; the
+        first of two entries with one identity wins; all or nothing.  dry_run checks and counts without changing anything.
+        -> {kept, added, updated, deleted}; raises ConfigureError naming the refused entry."""
+        limits = list(limits)
+        keep = []  # the encoded strings live until the call returns
+
+        def enc(v):
+            return None if v is None else str(v).encode()
+
+        specs = (LimitSpec * max(len(limits), 1))()
+        for i, l in enumerate(limits):
+            conds, vars_ = [str(c) for c in _field(l, "conditions")], [str(v) for v in _field(l, "variables")]
+            ca, va = _m._strs(conds), _m._strs(vars_)
+            keep += [ca, va]
+            specs[i] = LimitSpec(enc(_field(l, "namespace")), int(_field(l, "max_value")), int(_field(l, "seconds")), ca, len(conds), 0,
+                                 va, len(vars_), 0, enc(_field(l, "name")), enc(_field(l, "id")))
+        rep = ConfigureReport()
+        if self._lib.rl_rls_configure(self._h, specs, len(limits), int(dry_run), C.byref(rep)) != 0:
+            raise ConfigureError(self._lib.rl_rls_last_error(self._h).decode(),
+                                 None if rep.first_refused == NO_STORE else rep.first_refused)
+        return {"kept": rep.kept, "added": rep.added, "updated": rep.updated, "deleted": rep.deleted}
+
+    def load_limits_file(self, path: str, dry_run: bool = False) -> Dict[str, int]:
+        """configure_with the limits of a limitador-server limits file (limits_file.load_limits_file)."""
+        from . import limits_file
+        return self.configure_with(limits_file.load_limits_file(path), dry_run)
+
+    def config_status(self) -> Dict[str, int]:
+        """Status::config_version / config_err_since (limitador-server main.rs:218-235) of the configure_with calls."""
+        v, e = C.c_uint64(), C.c_uint64()
+        self._check(self._lib.rl_rls_config_status(self._h, C.byref(v), C.byref(e)))
+        return {"config_version": v.value, "config_err_since": e.value}
 
     def metrics(self) -> str:
         need = C.c_uint64()
