@@ -16,6 +16,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/rl_engine.h"
 #include "rl_core.h"
 
@@ -395,6 +397,9 @@ struct AccSrcWide : AccSrc {
 //   pass 2  the same sweep hands out the positions (stable: earlier warps, then rank inside the warp);
 //   tail    region totals are accumulated by atomics; the LAST block to finish turns them into the work
 //           items of k_main (one global round trip, the rest out of shared memory).
+// Record batches ask for 4 resident CTAs per SM (64 registers, no spill at U = 4): with RL_FLAG_PIPELINE the next
+// batch's front runs beside the current replay, and every register it holds is one k_main cannot (DESIGN.md §3.2).
+// Access batches ask for 3, the residency they had without a bound (ptxas: 70 registers, no spill).
 template <int NT>
 __device__ __forceinline__ uint32_t rl_block_excl_scan(uint32_t v, uint32_t* s_warp, uint32_t& total) {
     // exclusive prefix of v over the NT threads of the block; s_warp: NT/32 words of shared memory
@@ -438,7 +443,7 @@ __device__ __forceinline__ uint32_t rl_batch_n(const RlBatch& B) {
 }
 
 template <int CELLS, class Src>
-__global__ void __launch_bounds__(RL_PART_THREADS) k_front(RlDev D, RlBatch B, Src src) {
+__global__ void __launch_bounds__(RL_PART_THREADS, Src::kAccessIsRequest ? 4 : 3) k_front(RlDev D, RlBatch B, Src src) {
     extern __shared__ uint32_t wcnt[];  // [RL_PART_WARPS][P+1] per-warp counts -> positions, then loc[P+2]
     __shared__ uint32_t s_warp[RL_PART_WARPS], s_warp2[RL_PART_WARPS];
     __shared__ uint32_t s_last;
@@ -714,15 +719,16 @@ __global__ void __launch_bounds__(RL_PART_THREADS) k_front(RlDev D, RlBatch B, S
 //      issues the gather of its 32-B record; while that is in flight the CTA groups the accesses by
 //      TABLE ROW with a shared-memory hash table (the probe already resolved key -> row, so the
 //      32-bit row index is the exact identity of the key: one CAS, no key comparison), and the
-//      claimer ("rep") of a row issues the load of the row state;
+//      claimer ("rep") of a row loads the row state and stages it in shared memory;
 //   2. every access gets its stable ordinal inside its row group from one packed shared-memory
 //      counter per row (8 bits per warp, added warp-aggregated): ordinal order == thread order ==
-//      stream order;
-//   3. the rep stages the row state in shared memory;
-//   4. the group is replayed by ALL its threads in lock-step run-length rounds (rl_core.h,
+//      stream order; one barrier covers the grouping, the staging and the ordinals;
+//   3. the group is replayed by ALL its threads in lock-step run-length rounds (rl_core.h,
 //      hypotheses A and B; B in closed form for runs of equal deltas) — two barriers per
 //      round, one round for a saturated or an unconstrained hot key;
-//   5. the rep writes the dirty cells back.
+//   4. the rep writes the dirty cells back.
+// Nothing of steps 1-2 but the row's slot is kept in registers across the replay: C2's instantiation holds 6 CTAs
+// per SM without a spill (DESIGN.md §3.2).
 // Counter values never need atomics: a region belongs to one CTA at a time, a row to one group.
 template <int CELLS, int CH>
 struct RlMainSmem {
@@ -737,14 +743,16 @@ struct RlMainSmem {
     uint32_t g_rep[GT];
     uint32_t cells_arr[CH];
     uint32_t g_min[2][2][CH];  // [round parity][A|B][gid]
-    uint32_t g_flags[CH];      // by gid: bit2 = replay again (chained chunk, state changed under it)
+    uint32_t g_flags[CH];      // by gid: bit2 = replay again (chained chunk, an earlier chunk declared it writes the row)
     uint32_t g_dirty[CH];
-    uint32_t rflag[GT];        // chained chunks: row of g_row[] is "ordered" (see below)
+    uint32_t rflag[GT];        // chained chunks: row of g_row[] is "ordered" (see below): bit 0 set, and bit 1 if an
+                               // earlier chunk declared it writes the row
     uint32_t need_bits[64];    // earlier chunks (bit per chunk) whose commit I must wait for
     uint32_t scan_off[CH];     // dependency scan: offsets of the earlier chunks' sets, CH chunks at a time
     uint32_t scan_w[NW];
     uint32_t w_cnt;
     uint32_t item;
+    long long tph;      // RL_FLAG_KERNEL_STATS: clock of thread 0 at the last phase boundary
     // followed in dynamic shared memory by t_pfx[num_tiles + 1] (my partition's list: exclusive prefix of its per-tile
     // run lengths) and t_loc[num_tiles] (where each tile's run starts in part_idx/part_row): sized by the batch's
     // tile count, not by RL_MAX_TILES — shared memory a 128-tile batch does not need would come out of k_main's L1
@@ -754,10 +762,36 @@ __host__ __device__ constexpr size_t rl_main_smem_bytes(uint32_t num_tiles) {
     return sizeof(RlMainSmem<CELLS, CH>) + (2 * (size_t)num_tiles + 1) * sizeof(uint32_t);
 }
 
-// Per-thread view of the limits its access touches, in the access's own cell order.
+// Per-thread view of the limits its access touches (`cells`, of the row group whose descriptors are `desc`).
+// RlMyLimits: copies in registers, in the access's own cell order.  RlDescLimits: the descriptors, indexed by cell and
+// read where a replay round needs them — k_main's view for more than one cell, where a copy in registers would be
+// live across every round of the chunk (DESIGN.md §3.2).
 struct RlMyLimits {
     uint64_t mx[RL_MAX_CELLS];
     uint32_t qmask;  // bit k: k-th touched cell belongs to a qualified limit
+    template <int CELLS>
+    __device__ __forceinline__ void load(const RlCellDesc* desc, uint32_t cells) {
+        const uint32_t n = rl_cells_n(cells);
+        qmask = 0;
+#pragma unroll
+        for (int k = 0; k < CELLS; k++) {
+            mx[k] = 0;
+            if ((uint32_t)k < n) {
+                const uint32_t c = rl_cells_at(cells, k);
+                mx[k] = desc[c].max_value;
+                qmask |= (desc[c].qualified ? 1u : 0u) << k;
+            }
+        }
+    }
+    __device__ __forceinline__ uint64_t max_value(int k, uint32_t) const { return mx[k]; }
+    __device__ __forceinline__ bool qualified(int k, uint32_t) const { return (qmask >> k) & 1u; }
+};
+struct RlDescLimits {
+    const RlCellDesc* lim;
+    template <int CELLS>
+    __device__ __forceinline__ void load(const RlCellDesc* desc, uint32_t) { lim = desc; }
+    __device__ __forceinline__ uint64_t max_value(int, uint32_t c) const { return lim[c].max_value; }
+    __device__ __forceinline__ bool qualified(int, uint32_t c) const { return lim[c].qualified; }
 };
 
 // Hypotheses A and B for one access against the staged row state (shared memory).
@@ -765,9 +799,9 @@ struct RlMyLimits {
 //          first limited counter (in_memory.rs:110-112,130-132,141-143)
 //   b_ok : every touched cell is live at `now` and stays within its limit after adding
 //          `dsum` (this request's delta plus those of the run before it)
-template <int CELLS, bool WIDE = false>
+template <int CELLS, bool WIDE = false, class Lim>
 __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const unsigned long long* se,
-                                           const RlMyLimits& L, uint32_t cells, uint64_t posorig, uint64_t delta,
+                                           const Lim& L, uint32_t cells, uint64_t posorig, uint64_t delta,
                                            uint64_t dsum, uint64_t now, bool lc, bool check_limit, bool& a_ok,
                                            bool& b_ok, uint32_t& fl) {
     const uint32_t n = rl_cells_n(cells);
@@ -779,11 +813,11 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
             const uint32_t c = rl_cells_at(cells, k);
             const uint64_t v = sv[c], e = se[c];
             const bool reached = lc || fl == RL_NONE_U32;  // !lc: the walk returns at the first limited counter
-            if (reached && ((L.qmask >> k) & 1u) && e == 0) absent_reached = true;
+            if (reached && L.qualified(k, c) && e == 0) absent_reached = true;
             const uint64_t vv = (e <= now) ? 0 : v;
-            if (reached && fl == RL_NONE_U32 && vv + delta > L.mx[k]) fl = rl_pos_of<WIDE>(posorig, k);
+            if (reached && fl == RL_NONE_U32 && vv + delta > L.max_value(k, c)) fl = rl_pos_of<WIDE>(posorig, k);
             if (e <= now) live_all = false;
-            if (v + dsum > L.mx[k]) within_all = false;
+            if (v + dsum > L.max_value(k, c)) within_all = false;
         }
     }
     a_ok = (fl != RL_NONE_U32) && !absent_reached;
@@ -796,6 +830,19 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
 #ifndef RL_MID_CTAS
 #define RL_MID_CTAS 5  // resident 128-thread k_main CTAs per SM asked of the compiler for 3..4-cell rows (registers = 512 / this)
 #endif
+// The record-form check_and_update replay of 4-cell row groups in 128-access chunks (C2's k_main) asks for 6 (80
+// registers): C2 makes ~800 chunks per 65536-request batch, and 5 CTAs x 132 SMs leave a second turn of items that
+// sets the step's length.  6 (792 slots) beat 7 and 8 on an H100: more CTAs share an SM's issue slots and leave the
+// next front no room (DESIGN.md §3.2).  tests/test_kernel_budgets.py holds it to 80 registers, no spill.
+#ifndef RL_RECORD_MID_CTAS
+#define RL_RECORD_MID_CTAS 6
+#endif
+template <int CELLS, class Src, int MODE, int CH, bool LC>
+constexpr int rl_main_ctas() {
+    if (CELLS <= 2) return 8;
+    if (CELLS > 4) return 4;
+    return (CELLS == 4 && Src::kAccessIsRequest && MODE == 0 && CH == 128 && !LC) ? RL_RECORD_MID_CTAS : RL_MID_CTAS;
+}
 #ifndef RL_WAIT_NS
 #define RL_WAIT_NS 100  // back-off of the chained-commit wait loops
 #endif
@@ -806,8 +853,8 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
 #define RL_PHASE_TICK(i)                                                         \
     if (D.kstats != nullptr && tid == 0) {                                       \
         const long long tnow = clock64();                                        \
-        atomicAdd(D.kstats + 8 + (i), (unsigned long long)(tnow - tph));         \
-        tph = tnow;                                                              \
+        atomicAdd(D.kstats + 8 + (i), (unsigned long long)(tnow - sm.tph));      \
+        sm.tph = tnow;                                                           \
     }
 #define RL_KSTAT_ADD(i, v) \
     if (D.kstats != nullptr) atomicAdd(D.kstats + (i), (unsigned long long)(v))
@@ -820,9 +867,9 @@ __device__ __forceinline__ void rl_eval_ab(const unsigned long long* sv, const u
 // memory) — the default path (single-row request, load_counters off).  Same arithmetic as
 // rl_walk_check_single / rl_walk_update (rl_core.h), without a private copy of the row.
 //   in_memory.rs:122-127 (insert on lookup), :110-112,130-132 (early return), :146-153 (update)
-template <int CELLS, bool WIDE = false>
+template <int CELLS, bool WIDE = false, class Lim>
 __device__ __forceinline__ uint32_t rl_apply_check_smem(unsigned long long* sv, unsigned long long* se,
-                                                        const RlMyLimits& L, const RlCellDesc* gdesc, uint32_t cells,
+                                                        const Lim& L, const RlCellDesc* gdesc, uint32_t cells,
                                                         uint64_t posorig, uint64_t delta, uint64_t now,
                                                         uint32_t& dirty) {
     const uint32_t n = rl_cells_n(cells);
@@ -832,7 +879,7 @@ __device__ __forceinline__ uint32_t rl_apply_check_smem(unsigned long long* sv, 
         if ((uint32_t)k < n && fl == RL_NONE_U32) {
             const uint32_t c = rl_cells_at(cells, k);
             uint64_t v = sv[c], e = se[c];
-            if (((L.qmask >> k) & 1u) && e == 0) {
+            if (L.qualified(k, c) && e == 0) {
                 e = now + gdesc[c].window_us;
                 v = 0;
                 sv[c] = 0;
@@ -840,7 +887,7 @@ __device__ __forceinline__ uint32_t rl_apply_check_smem(unsigned long long* sv, 
                 dirty |= 1u << c;
             }
             const uint64_t vv = (e <= now) ? 0 : v;
-            if (vv + delta > L.mx[k]) fl = rl_pos_of<WIDE>(posorig, k);
+            if (vv + delta > L.max_value(k, c)) fl = rl_pos_of<WIDE>(posorig, k);
         }
     }
     if (fl != RL_NONE_U32) return fl;
@@ -889,10 +936,10 @@ __device__ __forceinline__ void rl_apply_update_smem(unsigned long long* sv, uns
 //   ord/cnt  my stream-order ordinal inside the group and the group's size
 //   peers    the lanes of my warp that belong to my group (leader = lowest of them; solo = I am alone)
 // Returns the number of rounds the CTA ran.
-template <int CELLS, int MODE, bool LC, bool WIDE = false>
+template <int CELLS, int MODE, bool LC, bool WIDE = false, class Lim>
 __device__ __forceinline__ uint32_t rl_replay_rounds(const RlBatch& B, bool write_out, unsigned long long* gsv,
                                                      unsigned long long* gse, uint32_t* gmin, uint32_t gstride,
-                                                     uint32_t* gdirty, const RlReq& acc, const RlMyLimits& L,
+                                                     uint32_t* gdirty, const RlReq& acc, const Lim& L,
                                                      const RlCellDesc* desc, const RlCellDesc* gdesc, bool multi,
                                                      bool like_rep, bool valid, unsigned peers, bool solo, int leader,
                                                      uint32_t lane, uint32_t ord, uint32_t cnt, bool& done, uint32_t& pos) {
@@ -1071,7 +1118,7 @@ __device__ __forceinline__ uint32_t rl_group_slot(uint32_t row, uint32_t weak) {
 // GEO = cells per row of the table layout (row bytes), CELLS = cells any row group actually
 // uses (<= GEO): loops, registers and shared memory are sized by the latter.
 template <int GEO, int CELLS, class Src, int MODE, int CH, bool LC>
-__global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTAS : 4)) * 128 / CH) k_main(RlDev D, RlBatch B, Src src, uint32_t weak) {
+__global__ void __launch_bounds__(CH, rl_main_ctas<CELLS, Src, MODE, CH, LC>() * 128 / CH) k_main(RlDev D, RlBatch B, Src src, uint32_t weak) {
     using Smem = RlMainSmem<CELLS, CH>;
     constexpr int GT = Smem::GT;
     constexpr int PW = Smem::PW;
@@ -1086,7 +1133,6 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
     const bool snapshot = Src::kCanBeMulti && (B.phase == RL_PHASE_SNAPSHOT);
 
     if (blockIdx.x == 0 && tid == 0) rl_trace(D.trace, D.trace_pos, RL_EV_MAIN, 0, D.seq);
-    const uint32_t n_items = *B.n_items;
     const uint32_t ntile = B.num_tiles;
     const uint32_t tsz = rl_tile_of(B, rl_batch_n(B));
     for (;;) {
@@ -1097,7 +1143,7 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
         for (uint32_t i = tid; i < GT * PW; i += CH) sm.g_packed[i] = 0ull;
         __syncthreads();
         const uint32_t item = sm.item;
-        if (item >= n_items) {
+        if (item >= *B.n_items) {
             // the last CTA to leave re-arms the ticket for the next launch over this workspace
             if (tid == 0 && atomicAdd(B.exit_ctr, 1u) == gridDim.x - 1) {
                 *B.exit_ctr = 0;
@@ -1106,7 +1152,7 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             }
             break;
         }
-        long long tph = D.kstats != nullptr ? clock64() : 0;
+        if (D.kstats != nullptr && tid == 0) sm.tph = clock64();
         const uint4 it = B.items[item];
         const uint32_t lo = it.y, hi = it.z;  // [lo, hi) of the partition's list
         // ---- the partition's list = its runs in the tiles' slices, tile after tile: merge on read --------
@@ -1161,8 +1207,11 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
         // earlier chunk may still have to read it).  With no ordered row the state this chunk saw
         // is the one sequential execution shows it and nobody before it can be disturbed by its
         // writes (a saturated hot key is read by every chunk and written by none): it commits at
-        // once.  Otherwise it waits for exactly the earlier chunks touching an ordered row,
-        // re-reads its rows and replays the keys whose state changed.  Earlier chunks hold lower
+        // once.  Otherwise it waits for exactly the earlier chunks touching an ordered row, re-reads
+        // the rows an earlier chunk declared it writes and replays their keys from the committed
+        // state.  (A row no earlier chunk declared is unchanged: a chunk becomes a writer of a row
+        // only by replaying it again, which takes an earlier declared writer.  Replaying a row whose
+        // state did not change after all reproduces the first replay.)  Earlier chunks hold lower
         // tickets, so they are running (or done) whenever a chunk waits for them.
         const bool chained = (it.w != RL_NONE_U32);
         // (access, row) pairs of the first chunk
@@ -1214,38 +1263,45 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
                 }
                 slot = __shfl_sync(peers, s, leader);
             }
-            uint8_t* row = nullptr;
-            RlRow<CELLS> st;
+            // the rep loads its row state while the records are in flight (the probe located or claimed the row,
+            // so its sectors are often still in L2) and stages it in shared memory at once: no copy of it, nor the
+            // row's address (recomputed at each use), is live across the replay
+            auto row_ptr = [&]() { return D.rows + (size_t)sm.g_row[slot] * RlGeom<GEO>::ROW_BYTES; };
             if (is_rep) {
-                // the row was located (or claimed) by the probe; its sectors are often still in L2
-                row = D.rows + (size_t)myrow * RlGeom<GEO>::ROW_BYTES;
-                rl_row_load<CELLS>(row, CELLS, st);
+                RlRow<CELLS> st;
+                rl_row_load<CELLS>(row_ptr(), CELLS, st);
+#pragma unroll
+                for (int c = 0; c < CELLS; c++) {
+                    sm.s_val[tid * CELLS + c] = st.value[c];
+                    sm.s_exp[tid * CELLS + c] = st.expiry[c];
+                }
+                if (snapshot) {
+                    B.log_row[mypos] = row_ptr();
+#pragma unroll
+                    for (int c = 0; c < CELLS; c++)
+                        B.log_state[(size_t)mypos * GEO + c] = make_ulonglong2(st.value[c], st.expiry[c]);
+                }
             }
-            __syncthreads();
-            if (valid) gid = sm.g_rep[slot];
-
             // ---- decode the record: limits of the cells I touch -----------------------------------
             RlReq acc;
-            acc.req = 0; acc.cells = 0; acc.group = 0; acc.posorig = 0; acc.delta = 0; acc.now = 0;
+            acc.req = 0; acc.cells = 0; acc.group = 0; acc.posorig = Src::kAccessIsRequest ? RL_IDENT_POSORIG : 0; acc.delta = 0; acc.now = 0;
             if (valid) src.decode(D, a, rawrec, acc);
             const uint64_t delta = acc.delta, now = acc.now;
             const RlCellDesc* gdesc = D.desc + (size_t)acc.group * 8;
             const uint32_t ncell = rl_cells_n(acc.cells);
             const bool multi = Src::kCanBeMulti && (MODE == 0) && rl_cells_multi(acc.cells);  // coupled to other rows
-            RlMyLimits L;
-            L.qmask = 0;
+            typename std::conditional<CELLS == 1, RlMyLimits, RlDescLimits>::type L;  // one cell: a copy is cheaper
+            L.template load<CELLS>(gdesc, acc.cells);
             constexpr bool kGeneric = LC || Src::kCanBeMulti;
             RlCellDesc mydesc[kGeneric ? CELLS : 1];  // generic variants: the limits of the cells I touch,
                                                       // indexed by cell, in local memory (L1) for the walks
+            if (kGeneric) {
 #pragma unroll
-            for (int k = 0; k < CELLS; k++) {
-                L.mx[k] = 0;
-                if (valid && (uint32_t)k < ncell) {
-                    const uint32_t c = rl_cells_at(acc.cells, k);
-                    const RlCellDesc d = gdesc[c];
-                    if (kGeneric) mydesc[kGeneric ? c : 0] = d;
-                    L.mx[k] = d.max_value;
-                    L.qmask |= (d.qualified ? 1u : 0u) << k;
+                for (int k = 0; k < CELLS; k++) {
+                    if (valid && (uint32_t)k < ncell) {
+                        const uint32_t c = rl_cells_at(acc.cells, k);
+                        mydesc[kGeneric ? c : 0] = gdesc[c];
+                    }
                 }
             }
             const RlCellDesc* desc = kGeneric ? mydesc : gdesc;
@@ -1255,27 +1311,14 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             sm.g_dirty[tid] = 0;
             sm.g_min[0][0][tid] = sm.g_min[0][1][tid] = 0xFFFFFFFFu;
             sm.g_min[1][0][tid] = sm.g_min[1][1][tid] = 0xFFFFFFFFu;
-            RL_PHASE_TICK(0)  // item fetch + gather + grouping
-
             // ---- 2. stable ordinal: one packed add per (warp, row), one barrier --------------------
             if (valid && (int)lane == leader)
                 atomicAdd(&sm.g_packed[slot * PW + (warp >> 3)], (unsigned long long)__popc(peers) << (8 * (warp & 7)));
-            const bool solo = (peers & (peers - 1)) == 0;  // my row's only lane in this warp
-            // ---- 3. the rep stages the row state -----------------------------------------------------
-            if (is_rep) {
-#pragma unroll
-                for (int c = 0; c < CELLS; c++) {
-                    sm.s_val[tid * CELLS + c] = st.value[c];
-                    sm.s_exp[tid * CELLS + c] = st.expiry[c];
-                }
-                if (snapshot) {
-                    B.log_row[mypos] = row;
-#pragma unroll
-                    for (int c = 0; c < CELLS; c++)
-                        B.log_state[(size_t)mypos * GEO + c] = make_ulonglong2(st.value[c], st.expiry[c]);
-                }
-            }
             __syncthreads();
+            if (valid) gid = sm.g_rep[slot];
+            const bool rep = valid && gid == tid;  // = is_rep, read back rather than kept across the replay
+            RL_PHASE_TICK(0)  // item fetch + gather + grouping + row state staged
+            const bool solo = (peers & (peers - 1)) == 0;  // my row's only lane in this warp
             uint32_t ord = 0, cnt = 0;
             if (valid) {
 #pragma unroll
@@ -1287,17 +1330,17 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
                 ord += __popc(peers & ((1u << lane) - 1));
             }
             // a row that dominates this chunk is a candidate for a partition of its own in the coming batches
-            if (is_rep && B.nhot && cnt >= RL_HOT_MIN) {
+            if (rep && B.nhot && cnt >= RL_HOT_MIN) {
                 const uint32_t k = atomicAdd(D.hot_cand_n, 1u);
-                if (k < RL_HOT_CAND) D.hot_cand[k] = myrow;
+                if (k < RL_HOT_CAND) D.hot_cand[k] = sm.g_row[slot];
             }
             // a run of allowed requests is closed-form only over members that carry the rep's delta and
             // cell list: a member that differs is never part of a run (it ends the run before it and is
             // applied alone), so the members of any run are mutually alike
             const bool like_rep = valid && sm.d_arr[gid] == delta && sm.cells_arr[gid] == acc.cells;
-            RL_PHASE_TICK(2)  // ordinals + row state staged
+            RL_PHASE_TICK(2)  // ordinals
 
-            // ---- 4. lock-step run-length replay -----------------------------------------------------
+            // ---- 3. lock-step run-length replay -----------------------------------------------------
             bool done = !valid || snapshot;
             uint32_t pos = 0;
             for (int attempt = 0;; attempt++) {
@@ -1318,10 +1361,10 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             for (uint32_t i = tid; i < 64; i += CH) sm.need_bits[i] = 0;
             if (tid == 0) sm.w_cnt = 0;
             __syncthreads();
-            if (is_rep) {
+            if (rep) {
                 // a row I WRITE is ordered too: no earlier chunk may still be reading it when I commit
                 if (sm.g_dirty[tid]) sm.rflag[slot] = 1;
-                B.chain_w[(size_t)item * CH + atomicAdd(&sm.w_cnt, 1u)] = (myrow << 1) | (sm.g_dirty[tid] ? 1u : 0u);
+                B.chain_w[(size_t)item * CH + atomicAdd(&sm.w_cnt, 1u)] = (sm.g_row[slot] << 1) | (sm.g_dirty[tid] ? 1u : 0u);
                 __threadfence();  // my entry is visible device-wide before the status word says so
             }
             __syncthreads();
@@ -1348,7 +1391,7 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             //     dependent round trip per earlier chunk).
             bool any_dep = false;
             for (int pass = 0; pass < 2; pass++) {
-                bool flagged = is_rep && sm.g_dirty[tid] != 0;
+                bool flagged = rep && sm.g_dirty[tid] != 0;
                 for (uint32_t blk = 0; blk < it.w; blk += CH) {
                     const uint32_t jn = min((uint32_t)CH, it.w - blk);  // chunks in this block
                     const uint32_t myc = (tid < jn) ? __ldcg(B.chain_wcnt + base_item + blk + tid) : 0;
@@ -1384,7 +1427,7 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
                             if (xs == w) {
                                 if (pass == 0) {
                                     if (e & 1u) {
-                                        sm.rflag[s2] = 1;
+                                        sm.rflag[s2] = 3;
                                         flagged = true;
                                     }
                                 } else if (sm.rflag[s2]) {
@@ -1419,25 +1462,19 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             }
             __threadfence();
             bool redo = false;
-            if (is_rep) {
-                RlRow<CELLS> cur;
-                rl_row_load<CELLS>(row, CELLS, cur);
-                bool same = true;
+            if (rep && (sm.rflag[slot] & 2u)) {  // an earlier chunk declared a write of this row: replay it
+                RlRow<CELLS> cur;                 // from the committed state
+                rl_row_load<CELLS>(row_ptr(), CELLS, cur);
 #pragma unroll
-                for (int c = 0; c < CELLS; c++) same = same && cur.value[c] == st.value[c] && cur.expiry[c] == st.expiry[c];
-                if (!same) {  // an earlier chunk changed this key: replay it from the committed state
-                    st = cur;
-#pragma unroll
-                    for (int c = 0; c < CELLS; c++) {
-                        sm.s_val[tid * CELLS + c] = cur.value[c];
-                        sm.s_exp[tid * CELLS + c] = cur.expiry[c];
-                    }
-                    sm.g_dirty[tid] = 0;
-                    sm.g_min[0][0][tid] = sm.g_min[0][1][tid] = 0xFFFFFFFFu;
-                    sm.g_min[1][0][tid] = sm.g_min[1][1][tid] = 0xFFFFFFFFu;
-                    sm.g_flags[tid] |= 4u;
-                    redo = true;
+                for (int c = 0; c < CELLS; c++) {
+                    sm.s_val[tid * CELLS + c] = cur.value[c];
+                    sm.s_exp[tid * CELLS + c] = cur.expiry[c];
                 }
+                sm.g_dirty[tid] = 0;
+                sm.g_min[0][0][tid] = sm.g_min[0][1][tid] = 0xFFFFFFFFu;
+                sm.g_min[1][0][tid] = sm.g_min[1][1][tid] = 0xFFFFFFFFu;
+                sm.g_flags[tid] |= 4u;
+                redo = true;
             }
             if (!__syncthreads_or(redo)) break;
             if (valid && (sm.g_flags[gid] & 4u)) {
@@ -1447,13 +1484,13 @@ __global__ void __launch_bounds__(CH, (CELLS <= 2 ? 8 : (CELLS <= 4 ? RL_MID_CTA
             }
 
             RL_PHASE_TICK(4)  // optimistic-commit protocol (chained chunks)
-            // ---- 5. write the dirty cells back -------------------------------------------------------
-            if (is_rep && !snapshot) {
+            // ---- 4. write the dirty cells back -------------------------------------------------------
+            if (rep && !snapshot) {
                 const uint32_t dirty = sm.g_dirty[tid];
 #pragma unroll
                 for (int c = 0; c < CELLS; c++)
                     if (dirty & (1u << c))
-                        rl_st_cg(row + 16 + 16 * c, sm.s_val[tid * CELLS + c], sm.s_exp[tid * CELLS + c]);
+                        rl_st_cg(row_ptr() + 16 + 16 * c, sm.s_val[tid * CELLS + c], sm.s_exp[tid * CELLS + c]);
                 if (chained && dirty) __threadfence();
             }
             __syncthreads();
@@ -1564,20 +1601,6 @@ __global__ void __launch_bounds__(RL_HOT_THREADS) k_hot(RlDev D, RlBatch B, Src 
     if (tid < 8) s_desc[tid] = D.desc[(size_t)s_head.group * 8 + tid];  // one row => one row group
     __syncthreads();
 
-    // limits of the cells request `acc` touches, in its own cell order (shared-memory copies)
-    auto limits_of = [&](const RlReq& acc, RlMyLimits& L) {
-        const uint32_t n = rl_cells_n(acc.cells);
-        L.qmask = 0;
-#pragma unroll
-        for (int k = 0; k < CELLS; k++) {
-            L.mx[k] = 0;
-            if ((uint32_t)k < n) {
-                const uint32_t c = rl_cells_at(acc.cells, k);
-                L.mx[k] = s_desc[c].max_value;
-                L.qmask |= (s_desc[c].qualified ? 1u : 0u) << k;
-            }
-        }
-    };
     auto write_first = [&](const RlReq& acc, uint32_t fl) {
         if (!B.out_first_limited) return;
         if (fl == RL_NONE_U32) {
@@ -1631,7 +1654,7 @@ __global__ void __launch_bounds__(RL_HOT_THREADS) k_hot(RlDev D, RlBatch B, Src 
                 RlReq acc;
                 src.decode(D, ai[u], wi[u], acc);
                 RlMyLimits L;
-                limits_of(acc, L);
+                L.load<CELLS>(s_desc, acc.cells);  // shared-memory copies of the descriptors
                 bool aok, bok;
                 uint32_t fl;
                 rl_eval_ab<CELLS>((const unsigned long long*)S.value, (const unsigned long long*)S.expiry, L, acc.cells, acc.posorig, acc.delta,
@@ -1676,7 +1699,7 @@ __global__ void __launch_bounds__(RL_HOT_THREADS) k_hot(RlDev D, RlBatch B, Src 
                     fl = rl_walk_check_single<CELLS>(loc, dirty, s_desc, acc.cells, acc.posorig, acc.delta, acc.now, true, rem, ttl);
                 } else {
                     RlMyLimits L;
-                    limits_of(acc, L);
+                    L.load<CELLS>(s_desc, acc.cells);
                     bool aok, bok;
                     rl_eval_ab<CELLS>((const unsigned long long*)S.value, (const unsigned long long*)S.expiry, L, acc.cells, acc.posorig, acc.delta,
                                       acc.delta, acc.now, false, true, aok, bok, fl);
