@@ -237,7 +237,8 @@ int rl_sweep(rl_engine *e, uint64_t now_us, uint64_t *out_invalidated);
  * tombstones reach min_tombstone_pct percent of its rows (0 = any region with a tombstone): the region's rows go to a
  * scratch slab (one table-sized device allocation for the call), the region is cleared and the rows that still hold a
  * counter are inserted again by the hot path's own probing rule.  Rows whose cells are all (0, 0) hold nothing and are
- * dropped as well.  Observable state is unchanged: rl_dump_table before == after.  Serialise with the request path. */
+ * dropped as well.  Observable state is unchanged: what rl_counters_export(..., now_us = 0) lists before == after.
+ * Serialise with the request path. */
 typedef struct rl_compact_stats {
     uint64_t regions;          /* table regions */
     uint64_t regions_rebuilt;
@@ -269,22 +270,17 @@ int rl_ns_metrics_read(rl_engine *e, uint32_t ns_cap, uint64_t *out_authorized_c
                        uint64_t *out_limited_calls, uint32_t limits_cap, uint64_t *out_limited_by_limit,
                        uint64_t *out_dropped, int reset);
 
-/* Parity aid: every present counter (limit_id, key, value, expiry_us), unordered. */
-int rl_dump_table(rl_engine *e, uint64_t cap, uint32_t *out_limit_id, uint64_t *out_key_lo,
-                  uint64_t *out_key_hi, uint64_t *out_value, uint64_t *out_expiry_us,
-                  uint64_t *out_count);
-
 /* ---- Counter snapshots: restart, resize or re-shard an engine without losing counters -----------------------------
- * A snapshot is the five arrays rl_dump_table returns.  Export it from one engine and import it into another (one with
- * another capacity, cells_per_row or region count, or another rank of a sharded store): the counters go on exactly
+ * A snapshot is the five arrays rl_counters_export returns.  Export it from one engine and import it into another (one
+ * with another capacity, cells_per_row or region count, or another rank of a sharded store): the counters go on exactly
  * where they were.  Limit ids are the caller's: the target must register the same limits under the same ids
  * (rl_limits_get lists them) before the import.  No reference function: the reference keeps counters across restarts
  * only in its disk store (limitador/src/storage/disk/rocksdb_storage.rs). */
-/* Every present counter of the selected namespaces (ns_ids == NULL: all), as rl_dump_table reports them.
- * now_us == 0: the exact state.  now_us > 0: qualified counters with 0 < expiry <= now_us are left out, i.e. the
- * state rl_sweep(now_us) would leave.  mem = RL_MEM_HOST or RL_MEM_DEVICE for the five outputs; unordered (the
- * counters of one row are adjacent), at most cap written, *out_count = number found (may exceed cap).  Does not
- * change the table. */
+/* Every present counter of the selected namespaces (ns_ids == NULL: all) as (limit_id, key, value, expiry_us); an
+ * unqualified counter whose row was never touched is (limit_id, 0, 0, 0, 0).  now_us == 0: the exact state.
+ * now_us > 0: qualified counters with 0 < expiry <= now_us are left out, i.e. the state rl_sweep(now_us) would leave.
+ * mem = RL_MEM_HOST or RL_MEM_DEVICE for the five outputs; unordered (the counters of one row are adjacent), at most
+ * cap written, *out_count = number found (may exceed cap).  Does not change the table. */
 int rl_counters_export(rl_engine *e, const uint32_t *ns_ids, uint32_t n_ns, uint64_t now_us, uint64_t cap, int mem,
                        uint32_t *out_limit_id, uint64_t *out_key_lo, uint64_t *out_key_hi,
                        uint64_t *out_value, uint64_t *out_expiry_us, uint64_t *out_count);

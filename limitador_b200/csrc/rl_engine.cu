@@ -1063,21 +1063,34 @@ int rl_limits_set(rl_engine* e, const rl_limit_desc* limits, uint32_t n) {
     return RL_OK;
 }
 
-static int reset_selected(rl_engine* e, const std::vector<uint8_t>& sel) {
+// One k_reset pass over the table, behind every pipelined call.  mode 0 resets the cells of the limits in `limit_sel`
+// (indexed by limit id), mode 1 sweeps the qualified cells expired at now_us.  *out_dropped (nullable) = cells reset.
+static int reset_table(rl_engine* e, int mode, uint64_t now_us, const std::vector<uint8_t>& limit_sel,
+                       uint64_t* out_dropped) {
     int r = pipe_fence(e);
     if (r) return r;
     r = upload_tables(e);
     if (r) return r;
     DevBuf<uint8_t> d_sel;
-    RL_CUDA(e, d_sel.reserve(std::max<size_t>(sel.size(), 1)));
-    RL_CUDA(e, cudaMemcpyAsync(d_sel.p, sel.data(), sel.size(), cudaMemcpyHostToDevice, e->stream));
+    DevBuf<unsigned long long> d_cnt;
+    if (!limit_sel.empty()) {
+        RL_CUDA(e, d_sel.reserve(limit_sel.size()));
+        RL_CUDA(e, cudaMemcpyAsync(d_sel.p, limit_sel.data(), limit_sel.size(), cudaMemcpyHostToDevice, e->stream));
+    }
+    if (out_dropped) {
+        RL_CUDA(e, d_cnt.reserve(1));
+        RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
+    }
     RlDev D = make_dev(e);
     const uint32_t blocks = ceil_div(e->capacity, 256);
     with_cells(e, [&](auto c) {
-        k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 0, 0, d_sel.p, nullptr);
+        k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, d_cnt.p);
     });
     RL_LAUNCH_CHECK(e);
+    unsigned long long cnt = 0;
+    if (out_dropped) RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
+    if (out_dropped) *out_dropped = cnt;
     return RL_OK;
 }
 
@@ -1093,7 +1106,7 @@ int rl_delete_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
         any = true;
         if (!e->limits[id].qualified) e->limits[id].simple_present = false;  // in_memory.rs:242-243
     }
-    return any ? reset_selected(e, sel) : RL_OK;
+    return any ? reset_table(e, 0, 0, sel, nullptr) : RL_OK;
 }
 
 int rl_limits_delete(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
@@ -1125,109 +1138,84 @@ int rl_clear(rl_engine* e) {
 int rl_sweep(rl_engine* e, uint64_t now_us, uint64_t* out_invalidated) {
     if (!e) return RL_FATAL;
     RL_CUDA(e, cudaSetDevice(e->device));
-    int r = pipe_fence(e);
-    if (r) return r;
-    r = upload_tables(e);
-    if (r) return r;
-    DevBuf<unsigned long long> d_cnt;
-    RL_CUDA(e, d_cnt.reserve(1));
-    RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
-    RlDev D = make_dev(e);
-    const uint32_t blocks = ceil_div(e->capacity, 256);
-    with_cells(e, [&](auto c) {
-        k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 1, now_us, nullptr, d_cnt.p);
-    });
-    RL_LAUNCH_CHECK(e);
-    unsigned long long cnt = 0;
-    RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
-    RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    if (out_invalidated) *out_invalidated = cnt;
-    return RL_OK;
+    return reset_table(e, 1, now_us, {}, out_invalidated);
 }
 
-// shared by rl_dump_table (mode 0) and rl_get_counters (mode 1)
-static int scan_table(rl_engine* e, int mode, uint64_t now_us, const std::vector<uint8_t>& ns_sel, uint64_t cap,
-                      uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_a,
+// The table reads behind rl_get_counters (live) and rl_counters_export: one k_scan pass over the rows of the
+// namespaces in ns_sel (empty: every namespace), restricted to the limits whose counters exist.  live: (remaining,
+// ttl) of the counters with ttl(now_us) > 0.  Otherwise (value, expiry), followed by the present unqualified limits
+// whose row was never touched, as (l, 0, 0, 0, 0).  mem = RL_MEM_HOST stages at most capacity x cells entries on the
+// device, RL_MEM_DEVICE writes the caller's arrays.  At most cap written; *out_count = number found.
+static int read_table(rl_engine* e, bool live, uint64_t now_us, const std::vector<uint8_t>& ns_sel, uint64_t cap,
+                      int mem, uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_a,
                       uint64_t* out_b, uint64_t* out_count) {
+    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE)
+        return fail(e, RL_FATAL, "mem must be RL_MEM_HOST or RL_MEM_DEVICE (got %d)", mem);
+    if (cap && (!out_limit_id || !out_key_lo || !out_key_hi || !out_a || !out_b))
+        return fail(e, RL_FATAL, "cap > 0 needs all five output arrays");
     int r = pipe_fence(e);
     if (r) return r;
     r = upload_tables(e);
     if (r) return r;
-    // device capacity: every live cell could match; bound by cap + unqualified fix-ups
-    const uint64_t dcap = std::max<uint64_t>(cap, 1);
-    DevBuf<uint32_t> d_lid;
-    DevBuf<uint64_t> d_lo, d_hi, d_a, d_b;
+    // present [L]: the limit's counters exist (unqualified ones while simple_present, in_memory.rs:14,38-44) | seen [L]
+    const uint32_t L = e->limits_cap;
+    std::vector<uint8_t> flags(2 * (size_t)L, 0);
+    for (size_t l = 0; l < e->limits.size(); l++)
+        flags[l] = e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
+    DevBuf<uint8_t> d_sel, d_flags;
     DevBuf<unsigned long long> d_cnt;
-    DevBuf<uint8_t> d_sel;
-    RL_CUDA(e, d_lid.reserve(dcap));
-    RL_CUDA(e, d_lo.reserve(dcap));
-    RL_CUDA(e, d_hi.reserve(dcap));
-    RL_CUDA(e, d_a.reserve(dcap));
-    RL_CUDA(e, d_b.reserve(dcap));
+    RL_CUDA(e, d_flags.reserve(flags.size()));
     RL_CUDA(e, d_cnt.reserve(1));
-    RL_CUDA(e, d_sel.reserve(std::max<size_t>(ns_sel.size(), 1)));
     RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
-    if (!ns_sel.empty())
+    RL_CUDA(e, cudaMemcpyAsync(d_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, e->stream));
+    if (!ns_sel.empty()) {
+        RL_CUDA(e, d_sel.reserve(ns_sel.size()));
         RL_CUDA(e, cudaMemcpyAsync(d_sel.p, ns_sel.data(), ns_sel.size(), cudaMemcpyHostToDevice, e->stream));
+    }
+    // outputs: the caller's device arrays, or staging no larger than the table's cells
+    uint64_t* out64[4] = {out_key_lo, out_key_hi, out_a, out_b};
+    DevBuf<uint32_t> s_lid;
+    DevBuf<uint64_t> s64[4];
+    RlScanOut O{out_limit_id, out_key_lo, out_key_hi, out_a, out_b, d_cnt.p, cap, d_flags.p, d_flags.p + L};
+    if (mem == RL_MEM_HOST) {
+        const uint64_t n = std::min<uint64_t>(cap, e->capacity * e->cells);
+        RL_CUDA(e, s_lid.reserve(n));
+        for (auto& s : s64) RL_CUDA(e, s.reserve(n));
+        O = RlScanOut{s_lid.p, s64[0].p, s64[1].p, s64[2].p, s64[3].p, d_cnt.p, n, d_flags.p, d_flags.p + L};
+    }
     RlDev D = make_dev(e);
-    RlScanOut O{d_lid.p, d_lo.p, d_hi.p, d_a.p, d_b.p, d_cnt.p, dcap, nullptr, nullptr};
     const uint32_t blocks = ceil_div(e->capacity, 256);
     with_cells(e, [&](auto c) {
-        k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, e->d_group_ns.p, O);
+        k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, live, now_us, d_sel.p, e->d_group_ns.p, O);
     });
     RL_LAUNCH_CHECK(e);
     unsigned long long cnt = 0;
     RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
+    if (!live) RL_CUDA(e, cudaMemcpyAsync(flags.data() + L, d_flags.p + L, L, cudaMemcpyDeviceToHost, e->stream));
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    const uint64_t got = std::min<uint64_t>(cnt, dcap);
-    std::vector<uint32_t> lid(got);
-    std::vector<uint64_t> lo(got), hi(got), a(got), b(got);
-    if (got) {
-        RL_CUDA(e, cudaMemcpy(lid.data(), d_lid.p, got * 4, cudaMemcpyDeviceToHost));
-        RL_CUDA(e, cudaMemcpy(lo.data(), d_lo.p, got * 8, cudaMemcpyDeviceToHost));
-        RL_CUDA(e, cudaMemcpy(hi.data(), d_hi.p, got * 8, cudaMemcpyDeviceToHost));
-        RL_CUDA(e, cudaMemcpy(a.data(), d_a.p, got * 8, cudaMemcpyDeviceToHost));
-        RL_CUDA(e, cudaMemcpy(b.data(), d_b.p, got * 8, cudaMemcpyDeviceToHost));
+    const uint64_t got = std::min<uint64_t>(cnt, O.cap);
+    if (mem == RL_MEM_HOST && got) {
+        RL_CUDA(e, cudaMemcpy(out_limit_id, s_lid.p, got * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        for (int k = 0; k < 4; k++)
+            RL_CUDA(e, cudaMemcpy(out64[k], s64[k].p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     }
-    // host fix-up of unqualified counters: present iff simple_present (in_memory.rs:14,38-44)
-    uint64_t w = 0, total = 0;
-    std::vector<uint8_t> seen(e->limits.size() + 1, 0);
-    auto emit = [&](uint32_t l, uint64_t klo, uint64_t khi, uint64_t va, uint64_t vb) {
-        if (w < cap) {
-            out_limit_id[w] = l;
-            out_key_lo[w] = klo;
-            out_key_hi[w] = khi;
-            out_a[w] = va;
-            out_b[w] = vb;
-            w++;
-        }
-        total++;
-    };
-    for (uint64_t i = 0; i < got; i++) {
-        const uint32_t l = lid[i];
-        if (l < e->limits.size() && e->limits[l].defined && !e->limits[l].qualified) {
-            if (!e->limits[l].simple_present) continue;
-            seen[l] = 1;
-        }
-        emit(l, lo[i], hi[i], a[i], b[i]);
+    // the export's present unqualified limits of the selected namespaces that no row showed, appended
+    std::vector<uint32_t> extra;
+    for (size_t l = 0; !live && l < e->limits.size(); l++)
+        if (flags[l] && !e->limits[l].qualified && !flags[L + l] && (ns_sel.empty() || ns_sel[e->limits[l].ns]))
+            extra.push_back((uint32_t)l);
+    const uint64_t fit = cnt < cap ? std::min<uint64_t>(extra.size(), cap - cnt) : 0;
+    if (fit && mem == RL_MEM_HOST) {
+        std::copy(extra.begin(), extra.begin() + fit, out_limit_id + cnt);
+        for (uint64_t* o : out64) std::fill(o + cnt, o + cnt + fit, 0);
+    } else if (fit) {
+        const std::vector<uint64_t> zero(fit, 0);
+        RL_CUDA(e, cudaMemcpy(out_limit_id + cnt, extra.data(), fit * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        for (uint64_t* o : out64)
+            RL_CUDA(e, cudaMemcpy(o + cnt, zero.data(), fit * sizeof(uint64_t), cudaMemcpyHostToDevice));
     }
-    if (mode == 0) {
-        // unqualified counters whose row was never touched are still present as (0, EPOCH)
-        for (size_t l = 0; l < e->limits.size(); l++)
-            if (e->limits[l].defined && !e->limits[l].qualified && e->limits[l].simple_present && !seen[l])
-                emit((uint32_t)l, 0, 0, 0, 0);
-    }
-    total += (cnt > dcap) ? (cnt - dcap) : 0;
-    if (out_count) *out_count = total;
+    if (out_count) *out_count = cnt + extra.size();
     return RL_OK;
-}
-
-int rl_dump_table(rl_engine* e, uint64_t cap, uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi,
-                  uint64_t* out_value, uint64_t* out_expiry_us, uint64_t* out_count) {
-    if (!e) return RL_FATAL;
-    RL_CUDA(e, cudaSetDevice(e->device));
-    std::vector<uint8_t> none;
-    return scan_table(e, 0, 0, none, cap, out_limit_id, out_key_lo, out_key_hi, out_value, out_expiry_us, out_count);
 }
 
 int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_t now_us, uint64_t cap,
@@ -1241,8 +1229,8 @@ int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_
         const uint32_t id = limit_ids[i];
         if (id < e->limits.size() && e->limits[id].defined) ns_sel[e->limits[id].ns] = 1;
     }
-    return scan_table(e, 1, now_us, ns_sel, cap, out_limit_id, out_key_lo, out_key_hi, out_remaining, out_ttl_us,
-                      out_count);
+    return read_table(e, true, now_us, ns_sel, cap, RL_MEM_HOST, out_limit_id, out_key_lo, out_key_hi, out_remaining,
+                      out_ttl_us, out_count);
 }
 
 int rl_counters_export(rl_engine* e, const uint32_t* ns_ids, uint32_t n_ns, uint64_t now_us, uint64_t cap, int mem,
@@ -1250,89 +1238,15 @@ int rl_counters_export(rl_engine* e, const uint32_t* ns_ids, uint32_t n_ns, uint
                        uint64_t* out_expiry_us, uint64_t* out_count) {
     if (!e) return RL_FATAL;
     RL_CUDA(e, cudaSetDevice(e->device));
-    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE)
-        return fail(e, RL_FATAL, "rl_counters_export: mem must be RL_MEM_HOST or RL_MEM_DEVICE (got %d)", mem);
-    if (cap && (!out_limit_id || !out_key_lo || !out_key_hi || !out_value || !out_expiry_us))
-        return fail(e, RL_FATAL, "rl_counters_export: cap > 0 needs all five output arrays");
     if (n_ns && !ns_ids) return fail(e, RL_FATAL, "rl_counters_export: n_ns > 0 with ns_ids == NULL");
-    int r = pipe_fence(e);
-    if (r) return r;
-    r = upload_tables(e);
-    if (r) return r;
-    // the namespace selection (empty = every namespace) and the limits whose counters exist
-    std::vector<uint8_t> ns_sel;
+    std::vector<uint8_t> ns_sel;  // empty: every namespace
     if (ns_ids) {
         ns_sel.assign(std::max<size_t>(e->ns_limits.size(), 1), 0);
         for (uint32_t i = 0; i < n_ns; i++)
             if (ns_ids[i] < ns_sel.size()) ns_sel[ns_ids[i]] = 1;
     }
-    const uint32_t L = e->limits_cap;
-    std::vector<uint8_t> flags(2 * (size_t)L, 0);  // present [L] | seen [L]
-    for (size_t l = 0; l < e->limits.size(); l++)
-        flags[l] = e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
-    DevBuf<uint8_t> d_sel, d_flags;
-    DevBuf<unsigned long long> d_cnt;
-    RL_CUDA(e, d_sel.reserve(std::max<size_t>(ns_sel.size(), 1)));
-    RL_CUDA(e, d_flags.reserve(flags.size()));
-    RL_CUDA(e, d_cnt.reserve(1));
-    // outputs: the caller's device arrays, or staging no larger than the table's cells
-    DevBuf<uint32_t> s_lid;
-    DevBuf<uint64_t> s_lo, s_hi, s_val, s_exp;
-    uint64_t dcap = cap;
-    RlScanOut O{out_limit_id, out_key_lo, out_key_hi, out_value, out_expiry_us, d_cnt.p, cap, d_flags.p, d_flags.p + L};
-    if (mem == RL_MEM_HOST) {
-        dcap = std::min<uint64_t>(cap, e->capacity * e->cells);
-        const size_t n = std::max<uint64_t>(dcap, 1);
-        RL_CUDA(e, s_lid.reserve(n));
-        RL_CUDA(e, s_lo.reserve(n));
-        RL_CUDA(e, s_hi.reserve(n));
-        RL_CUDA(e, s_val.reserve(n));
-        RL_CUDA(e, s_exp.reserve(n));
-        O = RlScanOut{s_lid.p, s_lo.p, s_hi.p, s_val.p, s_exp.p, d_cnt.p, dcap, d_flags.p, d_flags.p + L};
-    }
-    RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), e->stream));
-    if (!ns_sel.empty()) RL_CUDA(e, cudaMemcpyAsync(d_sel.p, ns_sel.data(), ns_sel.size(), cudaMemcpyHostToDevice, e->stream));
-    RL_CUDA(e, cudaMemcpyAsync(d_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, e->stream));
-    RlDev D = make_dev(e);
-    const uint32_t blocks = ceil_div(e->capacity, 256);
-    const uint8_t* sel = ns_sel.empty() ? nullptr : d_sel.p;
-    with_cells(e, [&](auto c) {
-        k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, 2, now_us, sel, e->d_group_ns.p, O);
-    });
-    RL_LAUNCH_CHECK(e);
-    unsigned long long cnt = 0;
-    RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, e->stream));
-    RL_CUDA(e, cudaMemcpyAsync(flags.data() + L, d_flags.p + L, L, cudaMemcpyDeviceToHost, e->stream));
-    RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    // present unqualified limits of the selected namespaces whose row was never touched: (l, 0, 0, 0, 0), appended
-    std::vector<uint32_t> extra;
-    for (size_t l = 0; l < e->limits.size(); l++) {
-        const HostLimit& h = e->limits[l];
-        if (h.defined && !h.qualified && h.simple_present && !flags[L + l] && (ns_sel.empty() || ns_sel[h.ns]))
-            extra.push_back((uint32_t)l);
-    }
-    const uint64_t fit = cnt < cap ? std::min<uint64_t>(extra.size(), cap - cnt) : 0;
-    if (mem == RL_MEM_HOST) {
-        const uint64_t got = std::min<uint64_t>(cnt, dcap);
-        if (got) {
-            RL_CUDA(e, cudaMemcpy(out_limit_id, s_lid.p, got * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-            RL_CUDA(e, cudaMemcpy(out_key_lo, s_lo.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-            RL_CUDA(e, cudaMemcpy(out_key_hi, s_hi.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-            RL_CUDA(e, cudaMemcpy(out_value, s_val.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-            RL_CUDA(e, cudaMemcpy(out_expiry_us, s_exp.p, got * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-        }
-        for (uint64_t k = 0; k < fit; k++) {
-            out_limit_id[cnt + k] = extra[k];
-            out_key_lo[cnt + k] = out_key_hi[cnt + k] = out_value[cnt + k] = out_expiry_us[cnt + k] = 0;
-        }
-    } else if (fit) {
-        const std::vector<uint64_t> zero(fit, 0);
-        RL_CUDA(e, cudaMemcpy(out_limit_id + cnt, extra.data(), fit * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        for (uint64_t* o : {out_key_lo, out_key_hi, out_value, out_expiry_us})
-            RL_CUDA(e, cudaMemcpy(o + cnt, zero.data(), fit * sizeof(uint64_t), cudaMemcpyHostToDevice));
-    }
-    if (out_count) *out_count = cnt + extra.size();
-    return RL_OK;
+    return read_table(e, false, now_us, ns_sel, cap, mem, out_limit_id, out_key_lo, out_key_hi, out_value,
+                      out_expiry_us, out_count);
 }
 
 int rl_limits_get(rl_engine* e, uint32_t cap, rl_limit_desc* out, uint32_t* out_n) {

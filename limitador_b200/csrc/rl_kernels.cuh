@@ -2035,19 +2035,20 @@ struct RlScanOut {
     uint32_t* limit_id;
     uint64_t* key_lo;
     uint64_t* key_hi;
-    uint64_t* a;  // dump / export: value      | get_counters: remaining
-    uint64_t* b;  // dump / export: expiry_us  | get_counters: ttl_us
+    uint64_t* a;  // export: value      | get_counters: remaining
+    uint64_t* b;  // export: expiry_us  | get_counters: ttl_us
     unsigned long long* count;
     uint64_t cap;
-    const uint8_t* present;  // export: [limits_cap] 1 = the limit's counters exist (unqualified: simple_present)
+    const uint8_t* present;  // [limits_cap] 1 = the limit's counters exist (unqualified: simple_present)
     uint8_t* seen;           // export: [limits_cap] set for every unqualified limit emitted from a row
 };
 
-// mode 0: dump every present cell; mode 1: get_counters (ns_sel[ns]!=0, ttl>0); mode 2: export = the dump restricted
-// to ns_sel (nullable = every namespace) and to present limits, without the qualified cells with 0 < expiry <= now
-// when now > 0 (what rl_sweep(now) would drop).  A row's cells take one position reservation and sit side by side.
+// The cells of present limits (O.present) in the rows of the namespaces in ns_sel (nullable = every namespace).
+// live (get_counters): the cells with ttl(now) > 0, as (remaining, ttl).  Otherwise (export): every such cell as
+// (value, expiry), without the qualified cells with 0 < expiry <= now when now > 0 (what rl_sweep(now) would drop).
+// A row's cells take one position reservation and sit side by side.
 template <int CELLS>
-__global__ void k_scan(RlDev D, uint64_t nrows, int mode, uint64_t now, const uint8_t* __restrict__ ns_sel,
+__global__ void k_scan(RlDev D, uint64_t nrows, bool live, uint64_t now, const uint8_t* __restrict__ ns_sel,
                        const uint32_t* __restrict__ group_ns, RlScanOut O) {
     constexpr uint32_t RB = RlGeom<CELLS>::ROW_BYTES;
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -2056,7 +2057,7 @@ __global__ void k_scan(RlDev D, uint64_t nrows, int mode, uint64_t now, const ui
     const ulonglong2 hdr = rl_ld_cg(row);
     if (hdr.y == 0 || hdr.y == RL_TOMB_HI) return;
     const uint32_t group = (uint32_t)(hdr.y >> 32);
-    if ((mode == 1 || (mode == 2 && ns_sel)) && !ns_sel[group_ns[group]]) return;
+    if (ns_sel && !ns_sel[group_ns[group]]) return;
     const RlCellDesc* desc = D.desc + (size_t)group * 8;
     uint64_t a[CELLS], b[CELLS];
     uint32_t emit = 0;
@@ -2068,15 +2069,15 @@ __global__ void k_scan(RlDev D, uint64_t nrows, int mode, uint64_t now, const ui
         if (d.limit_id == RL_NONE_U32) continue;
         const ulonglong2 cell = rl_ld_cg(row + 16 + 16 * c);
         if (d.qualified && cell.y == 0) continue;  // logically absent
+        if (!O.present[d.limit_id]) continue;
         a[c] = cell.x;
         b[c] = cell.y;
-        if (mode == 1) {
+        if (live) {
             const uint64_t ttl = rl_ttl(cell.y, now);
             if (ttl == 0) continue;                                  // in_memory.rs:167-169
             a[c] = d.max_value - rl_value_at(cell.x, cell.y, now);  // wrapping, :164-165
             b[c] = ttl;
-        } else if (mode == 2) {
-            if (!O.present[d.limit_id]) continue;
+        } else {
             if (d.qualified && now && cell.y <= now) continue;
             if (!d.qualified) O.seen[d.limit_id] = 1;
         }

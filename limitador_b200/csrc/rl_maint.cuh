@@ -8,7 +8,7 @@
 //                       rows that still hold a counter are inserted again by the rule the hot path probes by
 //                       (rl_kernels.cuh rl_probe: home = low hash bits, linear probing inside the region, 128-bit
 //                       CAS on the header).  No reference analog (moka evicts, in_memory.rs:205-212); observable
-//                       state is unchanged: rl_dump_table before == after.
+//                       state is unchanged: what rl_counters_export(..., now_us = 0) lists before == after.
 //   k_import_resolve /  counter import (rl_counters_import): set counters to exported (value, expiry) pairs in three
 //   k_import_claim /    passes — check every entry, find or claim every row by rl_probe's rule, then write the cells —
 //   k_import_write      so that a refused call has written no cell (DESIGN.md §9f).
@@ -185,8 +185,8 @@ __global__ void k_compact_reinsert(uint8_t* rows, const uint8_t* __restrict__ sc
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Counter import.  The entries are the five arrays rl_dump_table returns; every error is one word, (index << 8) |
-// reason, lowered with atomicMin so that the host learns the first bad index (~0 = no error).
+// Counter import.  The entries are the five arrays rl_counters_export returns; every error is one word,
+// (index << 8) | reason, lowered with atomicMin so that the host learns the first bad index (~0 = no error).
 enum : uint32_t {
     RLM_IMP_UNKNOWN_LIMIT = 1,  // limit id not registered in this engine
     RLM_IMP_KEY_RANGE = 2,      // qualified counter with key_hi >= 2^32

@@ -48,7 +48,7 @@ ABI_SYMBOLS = [
     "rl_sync", "rl_get_stats", "rl_limits_set", "rl_limits_delete", "rl_check_and_update_records",
     "rl_check_and_update_batch", "rl_is_within_limits_batch", "rl_is_within_limits_records",
     "rl_update_batch", "rl_update_records", "rl_get_counters", "rl_delete_counters", "rl_clear",
-    "rl_sweep", "rl_dump_table", "rl_bucket_by_owner", "rl_unpermute_u8", "rl_owner_of",
+    "rl_sweep", "rl_bucket_by_owner", "rl_unpermute_u8", "rl_owner_of",
     "rl_profile_begin", "rl_profile_end", "rl_bucket_by_owner_padded", "rl_gather_u8", "rl_record_lane_put", "rl_record_lane_gather", "rl_fence", "rl_fence_call",
     "rl_front_create", "rl_front_destroy", "rl_front_check_and_update", "rl_front_stats",
     "rl_shard_create", "rl_shard_destroy", "rl_shard_ipc_handle", "rl_shard_connect_ipc", "rl_shard_connect_ptrs",
@@ -132,7 +132,6 @@ def load_library(path: str | None = None):
     L.rl_ns_metrics_enable.argtypes = [vp, i32]
     L.rl_ns_metrics_accumulate.argtypes = [vp, u64, vp, u32, vp, vp, i32]
     L.rl_ns_metrics_read.argtypes = [vp, u32, vp, vp, vp, u32, vp, vp, i32]
-    L.rl_dump_table.argtypes = [vp, u64, vp, vp, vp, vp, vp, vp]
     L.rl_counters_export.argtypes = [vp, vp, u32, u64, u64, i32, vp, vp, vp, vp, vp, vp]
     L.rl_counters_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, i32]
     L.rl_limits_get.argtypes = [vp, u32, vp, vp]
@@ -386,18 +385,34 @@ class Engine:
         self._check(self._lib.rl_unpermute_u8(self._h, n, C.c_void_p(in_ptr), C.c_void_p(src_ptr), C.c_void_p(out_ptr)))
 
     # -- maintenance --
-    def get_counters(self, limit_ids, now_us, cap=1 << 20):
-        ids = np.ascontiguousarray(limit_ids, dtype=np.uint32)
-        lid = np.zeros(cap, dtype=np.uint32)
-        lo = np.zeros(cap, dtype=np.uint64)
-        hi = np.zeros(cap, dtype=np.uint64)
-        rem = np.zeros(cap, dtype=np.uint64)
-        ttl = np.zeros(cap, dtype=np.uint64)
+    def _read_table(self, call, cap, device=False):
+        """Count, then fetch (again if the table grew in between).  call(cap, five output pointers, count pointer) is
+        rl_get_counters or rl_counters_export with every other argument bound; the first call fetches `cap` rows.
+        Returns five numpy arrays (uint32, then uint64), or with device=True torch tensors on the engine's GPU
+        (int32 / int64 holding the same bits)."""
         cnt = C.c_uint64(0)
-        self._check(self._lib.rl_get_counters(self._h, _p(ids), len(ids), now_us, cap, _p(lid), _p(lo), _p(hi),
-                                              _p(rem), _p(ttl), C.byref(cnt)))
-        c = min(cnt.value, cap)
-        return sorted(zip(lid[:c].tolist(), lo[:c].tolist(), hi[:c].tolist(), rem[:c].tolist(), ttl[:c].tolist()))
+        while True:
+            if device:
+                import torch
+                dev = torch.device("cuda", self.device)
+                arrs = [torch.empty(max(cap, 1), dtype=torch.int32, device=dev)] + [
+                    torch.empty(max(cap, 1), dtype=torch.int64, device=dev) for _ in range(4)]
+                ptrs = [C.c_void_p(a.data_ptr()) for a in arrs]
+            else:
+                arrs = [np.zeros(cap, dtype=np.uint32)] + [np.zeros(cap, dtype=np.uint64) for _ in range(4)]
+                ptrs = [_p(a) for a in arrs]
+            self._check(call(cap, *ptrs, C.byref(cnt)))
+            if cnt.value <= cap:
+                return tuple(a[:cnt.value] for a in arrs)
+            cap = int(cnt.value)
+
+    def get_counters(self, limit_ids, now_us, cap=1 << 20):
+        """Sorted list of (limit_id, key_lo, key_hi, remaining, ttl_us) of every counter with ttl(now_us) > 0 in the
+        namespaces of the given limits.  cap: rows of the first fetch."""
+        ids = np.ascontiguousarray(limit_ids, dtype=np.uint32)
+        cols = self._read_table(
+            lambda cap, *out: self._lib.rl_get_counters(self._h, _p(ids), len(ids), now_us, cap, *out), cap)
+        return sorted(zip(*(c.tolist() for c in cols)))
 
     def delete_counters(self, limit_ids):
         ids = np.ascontiguousarray(limit_ids, dtype=np.uint32)
@@ -440,17 +455,9 @@ class Engine:
                 "limited_by_limit": bl[:limits_cap], "dropped": int(dropped.value)}
 
     def dump_arrays(self, cap=1 << 22):
-        lid = np.zeros(cap, dtype=np.uint32)
-        lo = np.zeros(cap, dtype=np.uint64)
-        hi = np.zeros(cap, dtype=np.uint64)
-        val = np.zeros(cap, dtype=np.uint64)
-        exp = np.zeros(cap, dtype=np.uint64)
-        cnt = C.c_uint64(0)
-        self._check(self._lib.rl_dump_table(self._h, cap, _p(lid), _p(lo), _p(hi), _p(val), _p(exp), C.byref(cnt)))
-        if cnt.value > cap:
-            return self.dump_arrays(cap=int(cnt.value) + 16)
-        c = cnt.value
-        return lid[:c], lo[:c], hi[:c], val[:c], exp[:c]
+        """export_counters() as numpy arrays, with a first fetch of `cap` rows."""
+        return self._read_table(
+            lambda cap, *out: self._lib.rl_counters_export(self._h, None, 0, 0, cap, MEM_HOST, *out), cap)
 
     def dump(self):
         """Sorted list of (limit_id, key_lo, key_hi, value, expiry_us) for every present counter."""
@@ -473,22 +480,9 @@ class Engine:
         would drop."""
         ids = None if ns_ids is None else np.ascontiguousarray(ns_ids, dtype=np.uint32)
         n_ids = 0 if ids is None else len(ids)
-        cnt, cap = C.c_uint64(0), 0
-        while True:  # count, then fetch (again if the table grew in between)
-            if device:
-                import torch
-                dev = torch.device("cuda", self.device)
-                arrs = [torch.empty(max(cap, 1), dtype=torch.int32, device=dev)] + [
-                    torch.empty(max(cap, 1), dtype=torch.int64, device=dev) for _ in range(4)]
-                ptrs = [C.c_void_p(a.data_ptr()) for a in arrs]
-            else:
-                arrs = [np.zeros(cap, dtype=np.uint32)] + [np.zeros(cap, dtype=np.uint64) for _ in range(4)]
-                ptrs = [_p(a) for a in arrs]
-            self._check(self._lib.rl_counters_export(self._h, _p(ids), n_ids, now_us, cap,
-                                                     MEM_DEVICE if device else MEM_HOST, *ptrs, C.byref(cnt)))
-            if cnt.value <= cap:
-                return tuple(a[:cnt.value] for a in arrs)
-            cap = int(cnt.value)
+        mem = MEM_DEVICE if device else MEM_HOST
+        return self._read_table(
+            lambda cap, *out: self._lib.rl_counters_export(self._h, _p(ids), n_ids, now_us, cap, mem, *out), 0, device)
 
     def import_counters(self, limit_id, key_lo, key_hi, value, expiry_us):
         """rl_counters_import: set each counter to exactly (value, expiry_us), all or nothing.  numpy arrays, or torch
