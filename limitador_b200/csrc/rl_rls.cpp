@@ -8,8 +8,9 @@
 // request is independent) —, the counters are laid out as one CSR, the store is called once for the whole batch, and
 // the responses are encoded by the worker pool.  No protobuf runtime: the four message types on the path have a
 // handful of fields, decoded by hand (rl_wire.h, shared with the device plan) and encoded below.
-// The HTTP API (include/rl_http.h) is served by the same stages over JSON bodies (rl_json.h): plan_range and plan_cpu
-// take either surface, the finish and the responses are its own, and it shares the RLS service's workers and metrics.
+// The HTTP API (include/rl_http.h) is served by the same stages over JSON bodies (rl_json.h): both surfaces are a
+// Batch and share the stage code around it; the decoding, how the store is called and the responses are each surface's
+// own, and the HTTP API shares the RLS service's workers and metrics.
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -40,14 +41,13 @@ extern "C" {
 __attribute__((weak)) int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, uint64_t n, const uint8_t* buf,
                                           const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
                                           const RlsDevReq** out_req);
-__attribute__((weak)) int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta);
+__attribute__((weak)) int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
 __attribute__((weak)) int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counters, uint8_t* limited,
                                             uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
                                             rl_counter* ctrs);
 __attribute__((weak)) int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
                                            const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
                                            const HttpDevReq** out_req, const HttpRun** out_runs, uint32_t* out_n_runs);
-__attribute__((weak)) int rl_http_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
 __attribute__((weak)) int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int endpoint, int* run_status, uint8_t* limited,
                                              uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
                                              rl_counter* ctrs);
@@ -242,64 +242,20 @@ struct WorkerOut {
     std::map<std::pair<std::string, std::string>, uint64_t> limited_by_name;
 };
 
-}  // namespace
-
-struct rl_rls {
-    rl_matcher* m = nullptr;
-    rl_engine* engine = nullptr;
-    int header_mode = RL_RLS_HEADERS_NONE;
-    bool use_limit_name = false;
-    Pool* pool = nullptr;
-    rl_rls_dev* dev = nullptr;  // the device plan's state (rl_rls_dev.cu), created by the first device plan
-    std::string last_error;
-
-    // the batch
-    int method = 0;
-    uint64_t n = 0;
-    const uint8_t* buf = nullptr;  // only dereferenced during plan
-    bool planned = false, finished = false;
-    std::vector<ReqPlan> plan;
-    std::vector<std::string> domains;  // copy of every request's domain (the metrics outlive the input buffer)
-    std::vector<WorkerOut> wout;
-    std::vector<uint32_t> store_index;
-    // store call
-    uint64_t n_store = 0;
-    std::vector<uint32_t> ctr_off;
-    RawBuf<rl_counter> ctrs;
-    std::vector<uint64_t> delta, now;
-    int load_counters = 0;
-    // engine outputs (serve)
-    std::vector<uint8_t> o_limited;
-    std::vector<uint32_t> o_first;
-    std::vector<uint64_t> o_rem, o_ttl;
-    // responses
-    RawBuf<uint8_t> resp;
-    std::vector<uint64_t> resp_off;
-    std::vector<uint8_t> grpc, code;
-    // metrics
-    std::map<std::string, NsCounts> by_ns;
-    std::map<std::pair<std::string, std::string>, uint64_t> limited_by_name;
-    double t_plan = 0, t_store = 0, t_finish = 0;
-    // rl_rls_configure outcomes (Status::config_success / config_failure)
-    uint64_t config_version = 0, config_err_since = 0;
-};
-
-// The HTTP API (include/rl_http.h) over an RLS service: its own batch, the service's matcher, engine, workers, device
-// state and metrics.  The member names are the RLS service's, so that the plan stages below serve both.
-struct rl_http {
-    rl_rls* rls = nullptr;
+// One batch of either surface as the stages below take it: the plan, the store call's CSR, the engine's outputs and the
+// stage times.  The RLS service and the HTTP API each derive from it and add what is their own.
+struct Batch {
     rl_matcher* m = nullptr;
     rl_engine* engine = nullptr;
     Pool* pool = nullptr;
     std::string last_error;
 
-    // the batch
-    int method = 0;  // the endpoint
+    int method = 0;  // RLS: the method; HTTP: the endpoint
     uint64_t n = 0;
     const uint8_t* buf = nullptr;  // only dereferenced during plan
     bool planned = false, finished = false;
     std::vector<ReqPlan> plan;
-    std::vector<std::string> domains;  // every body's namespace, unescaped
+    std::vector<std::string> domains;  // every request's domain / namespace (the metrics outlive the input buffer)
     std::vector<WorkerOut> wout;
     std::vector<uint32_t> store_index;
     // store requests
@@ -307,18 +263,42 @@ struct rl_http {
     std::vector<uint32_t> ctr_off;
     RawBuf<rl_counter> ctrs;
     std::vector<uint64_t> delta, now;
-    std::vector<uint8_t> load;
     // engine outputs (serve)
-    std::vector<int> run_status;
-    std::vector<int32_t> o_status;
     std::vector<uint8_t> o_limited;
     std::vector<uint32_t> o_first;
     std::vector<uint64_t> o_rem, o_ttl;
+    double t_plan = 0, t_store = 0, t_finish = 0;
+};
+
+}  // namespace
+
+struct rl_rls : Batch {
+    int header_mode = RL_RLS_HEADERS_NONE;
+    bool use_limit_name = false;
+    rl_rls_dev* dev = nullptr;  // the device plan's state (rl_rls_dev.cu), created by the first device plan
+    int load_counters = 0;
+    // responses
+    RawBuf<uint8_t> resp;
+    std::vector<uint64_t> resp_off;
+    std::vector<uint8_t> grpc, code;
+    // metrics
+    std::map<std::string, NsCounts> by_ns;
+    std::map<std::pair<std::string, std::string>, uint64_t> limited_by_name;
+    // rl_rls_configure outcomes (Status::config_success / config_failure)
+    uint64_t config_version = 0, config_err_since = 0;
+};
+
+// The HTTP API (include/rl_http.h) over an RLS service: its own batch, the service's matcher, engine, workers, device
+// state and metrics.
+struct rl_http : Batch {
+    rl_rls* rls = nullptr;
+    std::vector<uint8_t> load;  // one load_counters flag per store request
+    std::vector<int> run_status;
+    std::vector<int32_t> o_status;
     // responses
     std::vector<uint16_t> status;
     RawBuf<uint8_t> body, hval;
     std::vector<uint64_t> body_off, hval_off;
-    double t_plan = 0, t_store = 0, t_finish = 0;
     uint32_t store_calls = 0;
     // the last GET response
     uint16_t get_status = 0;
@@ -328,8 +308,8 @@ struct rl_http {
 
 namespace {
 
-template <class Svc, class... A>
-int sfail(Svc* s, const char* fmt, A... a) {
+template <class... A>
+int sfail(Batch* s, const char* fmt, A... a) {
     s->last_error = rl_format(fmt, a...);
     return RL_FATAL;
 }
@@ -517,40 +497,104 @@ void finish_scatter(rl_rls* s, uint32_t w, uint64_t byte_base) {
     }
 }
 
-void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uint32_t* first, const uint64_t* rem, const uint64_t* ttl,
-                  uint32_t w) {
-    uint64_t lo, hi;
+// Worker w's range [lo, hi) of the batch, with its finish outputs emptied.
+WorkerOut& finish_worker(Batch* s, uint32_t w, uint64_t& lo, uint64_t& hi) {
     range_of(s->n, s->pool->n, w, lo, hi);
     WorkerOut& W = s->wout[w];
     W.resp.clear();
     W.resp_len.assign(hi - lo, 0);
     W.by_ns.clear();
     W.limited_by_name.clear();
-    static const char* const kKeys[3] = {"X-RateLimit-Limit", "X-RateLimit-Remaining", "X-RateLimit-Reset"};  // sorted by key (server.rs:55)
-    // the store requests of the range are one run of store indices: their header values in ONE matcher call
-    const bool with_headers = store_status == RL_OK && s->method == RL_RLS_SHOULD_RATE_LIMIT && s->load_counters;
-    uint64_t j0 = RL_RLS_NO_STORE, j1 = 0;
+    return W;
+}
+
+// The header values of the store requests in [lo, hi), which are one run of store indices from j0: ONE matcher call into
+// W.hdr, made when `all` is set, or with `by_body` when one of the requests asks for draft-03 headers (HTTP).  Returns
+// whether the values are there.
+bool range_headers(const Batch* s, WorkerOut& W, uint64_t lo, uint64_t hi, bool all, bool by_body, const uint64_t* rem,
+                   const uint64_t* ttl, uint64_t& j0) {
+    j0 = RL_RLS_NO_STORE;
+    uint64_t j1 = 0;
+    bool want = all;
     for (uint64_t i = lo; i < hi; i++)
         if (s->plan[i].kind == REQ_STORE) {
             if (j0 == RL_RLS_NO_STORE) j0 = s->plan[i].store;
             j1 = (uint64_t)s->plan[i].store + 1;
+            want = want || (by_body && s->plan[i].hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03);
         }
-    bool headers_ok = false;
-    if (with_headers && j0 != RL_RLS_NO_STORE) {
-        W.hdr_off.assign(j1 - j0 + 1, 0);
-        uint64_t need = 0;
-        W.hdr.resize(std::max<size_t>(W.hdr.size(), (size_t)(j1 - j0) * 96));
-        int r = rl_matcher_response_headers_batch(s->m, j1 - j0, s->ctr_off.data() + j0, s->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
-                                                  W.hdr_off.data(), &need);
-        if (r != RL_OK && need > W.hdr.size()) {
-            W.hdr.resize(need);
-            r = rl_matcher_response_headers_batch(s->m, j1 - j0, s->ctr_off.data() + j0, s->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
-                                                  W.hdr_off.data(), &need);
-        }
-        headers_ok = r == RL_OK;
+    if (!want || j0 == RL_RLS_NO_STORE) return false;
+    W.hdr_off.assign(j1 - j0 + 1, 0);
+    uint64_t need = 0;
+    W.hdr.resize(std::max<size_t>(W.hdr.size(), (size_t)(j1 - j0) * 96));
+    int r = rl_matcher_response_headers_batch(s->m, j1 - j0, s->ctr_off.data() + j0, s->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
+                                              W.hdr_off.data(), &need);
+    if (r != RL_OK && need > W.hdr.size()) {
+        W.hdr.resize(need);
+        r = rl_matcher_response_headers_batch(s->m, j1 - j0, s->ctr_off.data() + j0, s->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
+                                              W.hdr_off.data(), &need);
     }
-    const std::string* last_ns = nullptr;  // consecutive requests of one namespace share the metrics entry
-    NsCounts* last_counts = nullptr;
+    return r == RL_OK;
+}
+
+// The three X-RateLimit-* values range_headers fetched for store request j.
+void header_values(const WorkerOut& W, uint64_t j, uint64_t j0, const char* vals[3]) {
+    vals[0] = W.hdr.data() + W.hdr_off[j - j0];
+    vals[1] = vals[0] + strlen(vals[0]) + 1;
+    vals[2] = vals[1] + strlen(vals[1]) + 1;
+}
+
+// The worker's metrics entry of the namespace last counted: consecutive requests of one namespace share it.
+struct NsCache {
+    const std::string* ns = nullptr;
+    NsCounts* counts = nullptr;
+};
+
+// Count decided request i into the worker's metrics: a limited one also under the name of its first limited limit when
+// the service labels by name; an authorized one with `calls` calls and `hits` hits.
+void count_decided(const Batch* s, WorkerOut& W, NsCache& at, uint64_t i, bool limited, bool by_name, const uint32_t* first,
+                   uint64_t calls, uint64_t hits) {
+    if (!at.ns || *at.ns != s->domains[i]) {
+        at.ns = &s->domains[i];
+        at.counts = &W.by_ns[s->domains[i]];
+    }
+    if (!limited) {
+        at.counts->authorized_calls += calls;
+        at.counts->authorized_hits += hits;
+        return;
+    }
+    at.counts->limited_calls++;
+    if (!by_name) return;
+    std::string name;
+    const uint32_t lid = first ? first[s->plan[i].store] : RL_NONE;
+    if (lid != RL_NONE) {
+        char nb[512];
+        int has = 0;
+        if (rl_matcher_limit_name_copy(s->m, lid, nb, sizeof nb, &has) == RL_OK && has) name = nb;
+    }
+    W.limited_by_name[{s->domains[i], name}]++;
+}
+
+// The workers' metrics into the RLS service's tables, which both surfaces count into.
+void merge_metrics(rl_rls* s, const std::vector<WorkerOut>& wout) {
+    for (const WorkerOut& W : wout) {
+        for (const auto& kv : W.by_ns) {
+            NsCounts& c = s->by_ns[kv.first];
+            c.authorized_calls += kv.second.authorized_calls;
+            c.authorized_hits += kv.second.authorized_hits;
+            c.limited_calls += kv.second.limited_calls;
+        }
+        for (const auto& kv : W.limited_by_name) s->limited_by_name[kv.first] += kv.second;
+    }
+}
+
+void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uint32_t* first, const uint64_t* rem, const uint64_t* ttl,
+                  uint32_t w) {
+    uint64_t lo, hi, j0;
+    WorkerOut& W = finish_worker(s, w, lo, hi);
+    static const char* const kKeys[3] = {"X-RateLimit-Limit", "X-RateLimit-Remaining", "X-RateLimit-Reset"};  // sorted by key (server.rs:55)
+    const bool with_headers = store_status == RL_OK && s->method == RL_RLS_SHOULD_RATE_LIMIT && s->load_counters;
+    const bool headers_ok = range_headers(s, W, lo, hi, with_headers, false, rem, ttl, j0);
+    NsCache at;
     for (uint64_t i = lo; i < hi; i++) {
         const ReqPlan& P = s->plan[i];
         uint8_t grpc = RL_GRPC_OK, code = RL_RLS_CODE_UNKNOWN;
@@ -581,9 +625,7 @@ void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uin
                         grpc = RL_GRPC_UNAVAILABLE;
                         break;
                     }
-                    vals[0] = W.hdr.data() + W.hdr_off[j - j0];
-                    vals[1] = vals[0] + strlen(vals[0]) + 1;
-                    vals[2] = vals[1] + strlen(vals[1]) + 1;
+                    header_values(W, j, j0, vals);
                     nh = 3;
                 }
                 break;
@@ -599,38 +641,101 @@ void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uin
         // metrics, once per request after the decision (server.rs:183-195, kuadrant_service.rs:81-92,173-174), into the
         // worker's own table (merged after the workers are done)
         if (P.kind == REQ_UNKNOWN_DOMAIN) continue;
-        if (!last_ns || *last_ns != s->domains[i]) {
-            last_ns = &s->domains[i];
-            last_counts = &W.by_ns[s->domains[i]];
-        }
-        NsCounts& c = *last_counts;
-        if (s->method == RL_RLS_REPORT) {
-            c.authorized_hits += P.hits;
-        } else if (code == RL_RLS_CODE_OVER_LIMIT) {
-            c.limited_calls++;
-            if (s->use_limit_name) {
-                std::string name;
-                const uint32_t lid = first ? first[P.store] : RL_NONE;
-                if (lid != RL_NONE) {
-                    char nb[512];
-                    int has = 0;
-                    if (rl_matcher_limit_name_copy(s->m, lid, nb, sizeof nb, &has) == RL_OK && has) name = nb;
-                }
-                W.limited_by_name[{s->domains[i], name}]++;
-            }
-        } else {
-            c.authorized_calls++;
-            if (s->method == RL_RLS_SHOULD_RATE_LIMIT) c.authorized_hits += P.hits;
-        }
+        const bool report = s->method == RL_RLS_REPORT;
+        count_decided(s, W, at, i, !report && code == RL_RLS_CODE_OVER_LIMIT, s->use_limit_name, first, report ? 0 : 1,
+                      s->method == RL_RLS_CHECK_RATE_LIMIT ? 0 : P.hits);
     }
+}
+
+// requests (RLS) or bodies (HTTP) are byte ranges [off[i], off[i + 1]) of the batch
+int check_offsets(Batch* s, const char* what, uint64_t n, const uint64_t* off) {
+    for (uint64_t i = 0; i < n; i++)
+        if (off[i + 1] < off[i]) return sfail(s, "%s offsets must be non-decreasing (%s %llu)", what, what, (unsigned long long)i);
+    return RL_OK;
 }
 
 int check_batch(rl_rls* s, int method, uint64_t n, const uint64_t* off) {
     if (method != RL_RLS_SHOULD_RATE_LIMIT && method != RL_RLS_CHECK_RATE_LIMIT && method != RL_RLS_REPORT)
         return sfail(s, "unknown method %d", method);
-    for (uint64_t i = 0; i < n; i++)
-        if (off[i + 1] < off[i]) return sfail(s, "request offsets must be non-decreasing (request %llu)", (unsigned long long)i);
+    return check_offsets(s, "request", n, off);
+}
+
+int check_batch(rl_http* h, int endpoint, uint64_t n, const uint64_t* off) {
+    if (endpoint != RL_HTTP_CHECK && endpoint != RL_HTTP_REPORT && endpoint != RL_HTTP_CHECK_AND_REPORT)
+        return sfail(h, "unknown endpoint %d", endpoint);
+    return check_offsets(h, "body", n, off);
+}
+
+// What a device plan of either surface starts with: the checks (rl_rls_dev.cu's plans are linked together or not at all)
+// and the new batch; now_us is set to the clock the plan runs at.
+template <class Svc>
+int device_plan_begin(Svc* s, int method, uint64_t n, const uint64_t* off, uint64_t& now_us) {
+    if (!s->engine) return sfail(s, "the device plan needs a service created with an engine");
+    if (!rl_rls_dev_plan) return sfail(s, "this build of the library has no device plan");
+    const int r = check_batch(s, method, n, off);
+    if (r) return r;
+    s->planned = s->finished = false;
+    s->method = method;
+    s->n = n;
+    if (!now_us) now_us = wall_us();
     return RL_OK;
+}
+
+// r, with the device state's reason in last_error when it is not RL_OK
+int dev_fail(Batch* s, rl_rls_dev* dev, int r) {
+    if (r) s->last_error = std::string("device plan: ") + rl_rls_dev_error(dev);
+    return r;
+}
+
+// What a device plan of either surface ends with, given the status r of its rl_*_dev_plan call: the store request count
+// and, with copy_csr, host copies of the CSR (and of HTTP's load flags, when `load` is given).
+int device_plan_end(Batch* s, rl_rls_dev* dev, int r, uint64_t n_store, uint64_t n_ctr, uint64_t now_us, bool copy_csr,
+                    std::vector<uint8_t>* load) {
+    s->n_store = n_store;
+    if (r || !copy_csr) return dev_fail(s, dev, r);
+    s->ctr_off.resize(n_store + 1);
+    s->ctrs.ensure(n_ctr);
+    s->delta.resize(n_store);
+    s->now.assign(n_store, now_us);
+    if (load) load->resize(n_store);
+    return dev_fail(s, dev,
+                    rl_rls_dev_copy_plan(dev, s->ctr_off.data(), s->ctrs.data(), s->delta.data(), load ? load->data() : nullptr));
+}
+
+// The host arrays a served batch's store calls return into: the verdicts, and with `load` the remaining / ttl of the
+// counters and the CSR their headers are formatted from.
+void size_outputs(Batch* s, bool load, uint64_t n_ctr) {
+    const uint64_t m = s->n_store;
+    s->o_limited.resize(m);
+    s->o_first.resize(m);
+    if (load) {
+        s->o_rem.resize(n_ctr);
+        s->o_ttl.resize(n_ctr);
+        s->ctr_off.resize(m + 1);
+        s->ctrs.ensure(n_ctr);
+    }
+}
+
+// rl_rls_plan_view / rl_http_plan_view but for load_counters, which each surface keeps its own way
+int plan_view(Batch* s, uint64_t* out_n_store, const uint32_t** out_ctr_off, const rl_counter** out_ctrs, const uint64_t** out_delta,
+              const uint64_t** out_now_us, const uint32_t** out_store_index) {
+    if (!s->planned) return sfail(s, "no planned batch");
+    if (out_n_store) *out_n_store = s->n_store;
+    if (out_ctr_off) *out_ctr_off = s->ctr_off.data();
+    if (out_ctrs) *out_ctrs = s->ctrs.data();
+    if (out_delta) *out_delta = s->delta.data();
+    if (out_now_us) *out_now_us = s->now.data();
+    if (out_store_index) *out_store_index = s->store_index.data();
+    return RL_OK;
+}
+
+// A served batch's stage times, from the clock at its start, after its plan, after its store calls and after the take of
+// its plan; the finish ends now.
+void stage_times(Batch* s, double t0, double t1, double t2, double t3) {
+    const double t4 = mono_us();
+    s->t_plan = (t1 - t0) + (t3 - t2);
+    s->t_store = t2 - t1;
+    s->t_finish = t4 - t3;
 }
 
 // Stage 1 on the engine's device (rl_rls_dev.cu).  Leaves the service as rl_rls_plan does, except for what the kernels
@@ -638,41 +743,25 @@ int check_batch(rl_rls* s, int method, uint64_t n, const uint64_t* off) {
 // (rl_rls_plan_device; rl_rls_serve keeps it on the device).
 int plan_on_device(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us, bool copy_csr,
                    const RlsDevReq*& req, uint64_t& n_ctr) {
-    if (!s->engine) return sfail(s, "the device plan needs a service created with an engine");
-    if (!rl_rls_dev_plan) return sfail(s, "this build of the library has no device plan");
-    int r = check_batch(s, method, n, off);
+    int r = device_plan_begin(s, method, n, off, now_us);
     if (r) return r;
-    s->planned = s->finished = false;
-    s->method = method;
-    s->n = n;
-    const uint64_t now = now_us ? now_us : wall_us();
     uint64_t n_store = 0;
-    r = rl_rls_dev_plan(&s->dev, s->engine, s->m, method, n, buf, off, now, &n_store, &n_ctr, &req);
-    if (r) {
-        s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
-        return r;
-    }
-    s->n_store = n_store;
+    r = rl_rls_dev_plan(&s->dev, s->engine, s->m, method, n, buf, off, now_us, &n_store, &n_ctr, &req);
     s->load_counters = (method == RL_RLS_SHOULD_RATE_LIMIT && s->header_mode != RL_RLS_HEADERS_NONE) ? 1 : 0;  // server.rs:146
-    if (copy_csr) {
-        s->ctr_off.resize(n_store + 1);
-        s->ctrs.ensure(n_ctr);
-        s->delta.resize(n_store);
-        s->now.assign(n_store, now);
-        if ((r = rl_rls_dev_copy_plan(s->dev, s->ctr_off.data(), s->ctrs.data(), s->delta.data()))) {
-            s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
-            return r;
-        }
-    }
-    return RL_OK;
+    return device_plan_end(s, s->dev, r, n_store, n_ctr, now_us, copy_csr, nullptr);
+}
+
+// What the take of a device plan starts with, for either surface: the plan, domains and store index sized for the batch.
+void size_plan(Batch* s) {
+    s->plan.resize(s->n);
+    s->domains.resize(s->n);
+    s->store_index.resize(s->n);
 }
 
 // The per-request outcomes of a device plan (in host memory once rl_rls_dev_copy_plan / _wait returned) into the
 // service's plan, store index and domains, on the worker pool.
 void take_device_plan(rl_rls* s, const RlsDevReq* req, const uint8_t* buf, const uint64_t* off) {
-    s->plan.resize(s->n);
-    s->domains.resize(s->n);
-    s->store_index.resize(s->n);
+    size_plan(s);
     s->pool->run([&](uint32_t w) {
         uint64_t lo, hi;
         range_of(s->n, s->pool->n, w, lo, hi);
@@ -725,54 +814,17 @@ int plan_cpu(Svc* s, int method, uint64_t n, const uint8_t* buf, const uint64_t*
 
 
 // ---- the HTTP API (include/rl_http.h) ------------------------------------------------------------------------------
-int check_http_batch(rl_http* h, int endpoint, uint64_t n, const uint64_t* off) {
-    if (endpoint != RL_HTTP_CHECK && endpoint != RL_HTTP_REPORT && endpoint != RL_HTTP_CHECK_AND_REPORT)
-        return sfail(h, "unknown endpoint %d", endpoint);
-    for (uint64_t i = 0; i < n; i++)
-        if (off[i + 1] < off[i]) return sfail(h, "body offsets must be non-decreasing (body %llu)", (unsigned long long)i);
-    return RL_OK;
-}
-
 // Responses [lo, hi) of worker w (server.rs:129-260): status, body, X-RateLimit-* values, and the metrics of
 // /check_and_report (server.rs:217-242).
 void finish_range_http(rl_http* h, const int32_t* store_status, const uint8_t* limited, const uint32_t* first, const uint64_t* rem,
                        const uint64_t* ttl, uint32_t w) {
-    uint64_t lo, hi;
-    range_of(h->n, h->pool->n, w, lo, hi);
-    WorkerOut& W = h->wout[w];
-    W.resp.clear();
-    W.resp_len.assign(hi - lo, 0);
+    uint64_t lo, hi, j0;
+    WorkerOut& W = finish_worker(h, w, lo, hi);
     W.hval.clear();
     W.hval_len.assign(3 * (hi - lo), 0);
-    W.by_ns.clear();
-    W.limited_by_name.clear();
     const bool car = h->method == RL_HTTP_CHECK_AND_REPORT;
-    // the store requests of the range are one run of store indices: their header values in ONE matcher call, when one of
-    // them asks for the headers
-    uint64_t j0 = RL_RLS_NO_STORE, j1 = 0;
-    bool want = false;
-    for (uint64_t i = lo; i < hi; i++)
-        if (h->plan[i].kind == REQ_STORE) {
-            if (j0 == RL_RLS_NO_STORE) j0 = h->plan[i].store;
-            j1 = (uint64_t)h->plan[i].store + 1;
-            want = want || (car && h->plan[i].hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03);
-        }
-    bool headers_ok = false;
-    if (want) {
-        W.hdr_off.assign(j1 - j0 + 1, 0);
-        uint64_t need = 0;
-        W.hdr.resize(std::max<size_t>(W.hdr.size(), (size_t)(j1 - j0) * 96));
-        int r = rl_matcher_response_headers_batch(h->m, j1 - j0, h->ctr_off.data() + j0, h->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
-                                                  W.hdr_off.data(), &need);
-        if (r != RL_OK && need > W.hdr.size()) {
-            W.hdr.resize(need);
-            r = rl_matcher_response_headers_batch(h->m, j1 - j0, h->ctr_off.data() + j0, h->ctrs.data(), rem, ttl, W.hdr.data(), W.hdr.size(),
-                                                  W.hdr_off.data(), &need);
-        }
-        headers_ok = r == RL_OK;
-    }
-    const std::string* last_ns = nullptr;
-    NsCounts* last_counts = nullptr;
+    const bool headers_ok = range_headers(h, W, lo, hi, false, car, rem, ttl, j0);
+    NsCache at;
     for (uint64_t i = lo; i < hi; i++) {
         const ReqPlan& P = h->plan[i];
         uint16_t status = 500;
@@ -794,9 +846,7 @@ void finish_range_http(rl_http* h, const int32_t* store_status, const uint8_t* l
                 decided = true;
                 if (car && P.hdr == RL_HTTP_HEADERS_DRAFT_VERSION_03) {  // server.rs:262-280
                     if (headers_ok) {
-                        vals[0] = W.hdr.data() + W.hdr_off[j - j0];
-                        vals[1] = vals[0] + strlen(vals[0]) + 1;
-                        vals[2] = vals[1] + strlen(vals[1]) + 1;
+                        header_values(W, j, j0, vals);
                     } else {
                         status = 500;
                         decided = false;
@@ -817,70 +867,25 @@ void finish_range_http(rl_http* h, const int32_t* store_status, const uint8_t* l
             W.hval.insert(W.hval.end(), (const uint8_t*)vals[k], (const uint8_t*)vals[k] + vl);
             W.hval_len[3 * (i - lo) + k] = vl;
         }
-        if (!car || !decided) continue;
-        if (!last_ns || *last_ns != h->domains[i]) {
-            last_ns = &h->domains[i];
-            last_counts = &W.by_ns[h->domains[i]];
-        }
-        NsCounts& c = *last_counts;
-        if (lim) {
-            c.limited_calls++;
-            if (h->rls->use_limit_name) {
-                std::string name;
-                const uint32_t lid = first ? first[P.store] : RL_NONE;
-                if (lid != RL_NONE) {
-                    char nb[512];
-                    int has = 0;
-                    if (rl_matcher_limit_name_copy(h->m, lid, nb, sizeof nb, &has) == RL_OK && has) name = nb;
-                }
-                W.limited_by_name[{h->domains[i], name}]++;
-            }
-        } else {
-            c.authorized_calls++;
-            c.authorized_hits += P.delta;
-        }
+        if (car && decided) count_decided(h, W, at, i, lim, h->rls->use_limit_name, first, 1, P.delta);
     }
 }
 
 // Stage 1 of an HTTP batch on the engine's device, through the RLS service's device state (rl_rls_dev.cu).
 int http_plan_on_device(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us, bool copy_csr,
                         const HttpDevReq*& req, uint64_t& n_ctr, const HttpRun*& runs, uint32_t& n_runs) {
-    if (!h->engine) return sfail(h, "the device plan needs a service created with an engine");
-    if (!rl_http_dev_plan) return sfail(h, "this build of the library has no device plan");
-    int r = check_http_batch(h, endpoint, n, off);
+    int r = device_plan_begin(h, endpoint, n, off, now_us);
     if (r) return r;
-    h->planned = h->finished = false;
-    h->method = endpoint;
-    h->n = n;
-    const uint64_t now = now_us ? now_us : wall_us();
     uint64_t n_store = 0;
     rl_rls* s = h->rls;
-    r = rl_http_dev_plan(&s->dev, h->engine, h->m, endpoint, n, buf, off, now, &n_store, &n_ctr, &req, &runs, &n_runs);
-    if (r) {
-        h->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
-        return r;
-    }
-    h->n_store = n_store;
-    if (copy_csr) {
-        h->ctr_off.resize(n_store + 1);
-        h->ctrs.ensure(n_ctr);
-        h->delta.resize(n_store);
-        h->load.resize(n_store);
-        h->now.assign(n_store, now);
-        if ((r = rl_http_dev_copy_plan(s->dev, h->ctr_off.data(), h->ctrs.data(), h->delta.data(), h->load.data()))) {
-            h->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
-            return r;
-        }
-    }
-    return RL_OK;
+    r = rl_http_dev_plan(&s->dev, h->engine, h->m, endpoint, n, buf, off, now_us, &n_store, &n_ctr, &req, &runs, &n_runs);
+    return device_plan_end(h, s->dev, r, n_store, n_ctr, now_us, copy_csr, &h->load);
 }
 
 // The per-body outcomes of a device plan into the service's plan, store index and namespaces.  The namespace comes from
 // the host's copy of the body, unescaped again (rl_json.h) when its source holds a backslash.
 void take_http_device_plan(rl_http* h, const HttpDevReq* req, const uint8_t* buf, const uint64_t* off) {
-    h->plan.resize(h->n);
-    h->domains.resize(h->n);
-    h->store_index.resize(h->n);
+    size_plan(h);
     h->pool->run([&](uint32_t w) {
         uint64_t lo, hi;
         range_of(h->n, h->pool->n, w, lo, hi);
@@ -1107,15 +1112,9 @@ int rl_rls_plan_view(rl_rls* s, uint64_t* out_n_store, const uint32_t** out_ctr_
                      const uint64_t** out_delta, const uint64_t** out_now_us, int* out_load_counters,
                      const uint32_t** out_store_index) {
     if (!s) return RL_FATAL;
-    if (!s->planned) return sfail(s, "no planned batch");
-    if (out_n_store) *out_n_store = s->n_store;
-    if (out_ctr_off) *out_ctr_off = s->ctr_off.data();
-    if (out_ctrs) *out_ctrs = s->ctrs.data();
-    if (out_delta) *out_delta = s->delta.data();
-    if (out_now_us) *out_now_us = s->now.data();
-    if (out_load_counters) *out_load_counters = s->load_counters;
-    if (out_store_index) *out_store_index = s->store_index.data();
-    return RL_OK;
+    const int r = plan_view(s, out_n_store, out_ctr_off, out_ctrs, out_delta, out_now_us, out_store_index);
+    if (r == RL_OK && out_load_counters) *out_load_counters = s->load_counters;
+    return r;
 }
 
 int rl_rls_finish(rl_rls* s, int store_status, const uint8_t* limited, const uint32_t* first_limited,
@@ -1136,16 +1135,7 @@ int rl_rls_finish(rl_rls* s, int store_status, const uint8_t* limited, const uin
     s->resp.ensure(byte_base[s->pool->n]);
     s->resp_off.assign(s->n + 1, 0);
     s->pool->run([&](uint32_t w) { finish_scatter(s, w, byte_base[w]); });
-    for (uint32_t w = 0; w < s->pool->n; w++) {
-        const WorkerOut& W = s->wout[w];
-        for (const auto& kv : W.by_ns) {
-            NsCounts& c = s->by_ns[kv.first];
-            c.authorized_calls += kv.second.authorized_calls;
-            c.authorized_hits += kv.second.authorized_hits;
-            c.limited_calls += kv.second.limited_calls;
-        }
-        for (const auto& kv : W.limited_by_name) s->limited_by_name[kv.first] += kv.second;
-    }
+    merge_metrics(s, s->wout);
     s->finished = true;
     s->planned = false;  // a batch is finished once: its metrics are counted once
     return RL_OK;
@@ -1174,30 +1164,16 @@ int rl_rls_serve(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const ui
     if (r) return r;
     const double t1 = mono_us();
     // the store call on the device arrays; only what the finish reads comes back
-    const uint64_t m = s->n_store;
-    s->o_limited.resize(m);
-    s->o_first.resize(m);
-    if (s->load_counters) {
-        s->o_rem.resize(n_ctr);
-        s->o_ttl.resize(n_ctr);
-        s->ctr_off.resize(m + 1);
-        s->ctrs.ensure(n_ctr);
-    }
+    size_outputs(s, s->load_counters, n_ctr);
     const int st = rl_rls_dev_decide(s->dev, s->engine, method, s->load_counters, s->o_limited.data(), s->o_first.data(),
                                      s->o_rem.data(), s->o_ttl.data(), s->ctr_off.data(), s->ctrs.data());
     if (st != RL_OK) s->last_error = std::string("store call failed: ") + rl_last_error(s->engine);
-    if ((r = rl_rls_dev_wait(s->dev))) {
-        s->last_error = std::string("device plan: ") + rl_rls_dev_error(s->dev);
-        return r;
-    }
+    if ((r = dev_fail(s, s->dev, rl_rls_dev_wait(s->dev)))) return r;
     const double t2 = mono_us();
     take_device_plan(s, req, buf, off);
     const double t3 = mono_us();
     r = rl_rls_finish(s, st, s->o_limited.data(), s->o_first.data(), s->o_rem.data(), s->o_ttl.data());
-    const double t4 = mono_us();
-    s->t_plan = (t1 - t0) + (t3 - t2);
-    s->t_store = t2 - t1;
-    s->t_finish = t4 - t3;
+    stage_times(s, t0, t1, t2, t3);
     return r;
 }
 
@@ -1351,7 +1327,7 @@ const char* rl_http_last_error(rl_http* h) { return h ? h->last_error.c_str() : 
 
 int rl_http_plan(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
     if (!h || (n && (!off || !buf))) return RL_FATAL;
-    int r = check_http_batch(h, endpoint, n, off);
+    int r = check_batch(h, endpoint, n, off);
     if (r) return r;
     if ((r = plan_cpu(h, endpoint, n, buf, off, now_us))) return r;
     h->load.assign(h->n_store, 0);
@@ -1377,15 +1353,9 @@ int rl_http_plan_view(rl_http* h, uint64_t* out_n_store, const uint32_t** out_ct
                       const uint64_t** out_delta, const uint64_t** out_now_us, const uint8_t** out_load_counters,
                       const uint32_t** out_store_index) {
     if (!h) return RL_FATAL;
-    if (!h->planned) return sfail(h, "no planned batch");
-    if (out_n_store) *out_n_store = h->n_store;
-    if (out_ctr_off) *out_ctr_off = h->ctr_off.data();
-    if (out_ctrs) *out_ctrs = h->ctrs.data();
-    if (out_delta) *out_delta = h->delta.data();
-    if (out_now_us) *out_now_us = h->now.data();
-    if (out_load_counters) *out_load_counters = h->load.data();
-    if (out_store_index) *out_store_index = h->store_index.data();
-    return RL_OK;
+    const int r = plan_view(h, out_n_store, out_ctr_off, out_ctrs, out_delta, out_now_us, out_store_index);
+    if (r == RL_OK && out_load_counters) *out_load_counters = h->load.data();
+    return r;
 }
 
 int rl_http_finish(rl_http* h, const int32_t* store_status, const uint8_t* limited, const uint32_t* first_limited,
@@ -1426,17 +1396,7 @@ int rl_http_finish(rl_http* h, const int32_t* store_status, const uint8_t* limit
             }
         }
     });
-    rl_rls* s = h->rls;
-    for (uint32_t w = 0; w < nw; w++) {
-        const WorkerOut& W = h->wout[w];
-        for (const auto& kv : W.by_ns) {
-            NsCounts& c = s->by_ns[kv.first];
-            c.authorized_calls += kv.second.authorized_calls;
-            c.authorized_hits += kv.second.authorized_hits;
-            c.limited_calls += kv.second.limited_calls;
-        }
-        for (const auto& kv : W.limited_by_name) s->limited_by_name[kv.first] += kv.second;
-    }
+    merge_metrics(h->rls, h->wout);
     h->finished = true;
     h->planned = false;  // a batch is finished once: its metrics are counted once
     return RL_OK;
@@ -1472,24 +1432,14 @@ int rl_http_serve(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, cons
     const uint64_t m = h->n_store;
     bool any_load = false;
     for (uint32_t k = 0; k < n_runs; k++) any_load = any_load || runs[k].load;
-    h->o_limited.resize(m);
-    h->o_first.resize(m);
-    if (any_load) {
-        h->o_rem.resize(n_ctr);
-        h->o_ttl.resize(n_ctr);
-        h->ctr_off.resize(m + 1);
-        h->ctrs.ensure(n_ctr);
-    }
+    size_outputs(h, any_load, n_ctr);
     h->run_status.assign(n_runs, RL_OK);
     const int st = rl_http_dev_decide(h->rls->dev, h->engine, endpoint, h->run_status.data(), h->o_limited.data(), h->o_first.data(),
                                       h->o_rem.data(), h->o_ttl.data(), h->ctr_off.data(), h->ctrs.data());
     if (st != RL_OK) h->run_status.assign(n_runs, st);
     for (uint32_t k = 0; k < n_runs; k++)
         if (h->run_status[k] != RL_OK) h->last_error = std::string("store call failed: ") + rl_last_error(h->engine);
-    if ((r = rl_rls_dev_wait(h->rls->dev))) {
-        h->last_error = std::string("device plan: ") + rl_rls_dev_error(h->rls->dev);
-        return r;
-    }
+    if ((r = dev_fail(h, h->rls->dev, rl_rls_dev_wait(h->rls->dev)))) return r;
     h->o_status.resize(m);
     for (uint32_t k = 0; k < n_runs; k++) {
         const uint64_t j1 = k + 1 < n_runs ? runs[k + 1].store : m;
@@ -1500,10 +1450,7 @@ int rl_http_serve(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, cons
     take_http_device_plan(h, req, buf, off);
     const double t3 = mono_us();
     r = rl_http_finish(h, h->o_status.data(), h->o_limited.data(), h->o_first.data(), h->o_rem.data(), h->o_ttl.data());
-    const double t4 = mono_us();
-    h->t_plan = (t1 - t0) + (t3 - t2);
-    h->t_store = t2 - t1;
-    h->t_finish = t4 - t3;
+    stage_times(h, t0, t1, t2, t3);
     return r;
 }
 

@@ -175,34 +175,83 @@ int reserve_outputs(rl_rls_dev* S, bool load_counters) {
     return RL_OK;
 }
 
+// The engine call a store request makes: RLS method or HTTP endpoint -> operation
+enum StoreOp { CHECK_AND_UPDATE, IS_WITHIN, UPDATE };
+StoreOp store_op(bool http, int method) {
+    if (http) return method == RL_HTTP_CHECK_AND_REPORT ? CHECK_AND_UPDATE : method == RL_HTTP_CHECK ? IS_WITHIN : UPDATE;
+    return method == RL_RLS_SHOULD_RATE_LIMIT ? CHECK_AND_UPDATE : method == RL_RLS_CHECK_RATE_LIMIT ? IS_WITHIN : UPDATE;
+}
+
+// One store call on the device arrays: the m store requests from j0, whose CSR offsets `off` count from counter c0.
+// Returns its status, with the device-memory call's deferred errors.
+int store_call(rl_rls_dev* S, rl_engine* e, StoreOp op, uint64_t j0, uint64_t m, const uint32_t* off, uint64_t c0, bool load) {
+    const rl_counter* c = S->d_ctrs.p + c0;
+    const uint64_t *d = S->d_delta.p + j0, *now = S->d_now.p + j0;
+    int st;
+    if (op == CHECK_AND_UPDATE)
+        st = rl_check_and_update_batch(e, m, off, c, d, now, load, RL_MEM_DEVICE, S->d_lim.p + j0, S->d_first.p + j0,
+                                       load ? S->d_rem.p + c0 : nullptr, load ? S->d_ttl.p + c0 : nullptr);
+    else if (op == IS_WITHIN)
+        st = rl_is_within_limits_batch(e, m, off, c, d, now, RL_MEM_DEVICE, S->d_lim.p + j0, S->d_first.p + j0);
+    else
+        st = rl_update_batch(e, m, off, c, d, now, RL_MEM_DEVICE);
+    return st == RL_OK ? rl_sync(e) : st;
+}
+
+// The store call's CSR on the device, once the plan read its size: ctr_off [n_store + 1], ctrs [n_ctr], delta and now
+// [n_store]
+int grow_csr(rl_rls_dev* S, uint64_t n_store, uint64_t n_ctr) {
+    RL_CUDA(S, S->d_ctr_off.grow(n_store + 1));
+    RL_CUDA(S, S->d_ctrs.grow(n_ctr + 1));
+    RL_CUDA(S, S->d_delta.grow(n_store + 1));
+    RL_CUDA(S, S->d_now.grow(n_store + 1));
+    return RL_OK;
+}
+
+// What both plans end with: the per-request array back into pinned memory (there once the stream is waited for), the
+// batch's sizes and the out-parameters.
+template <class Req>
+int close_plan(rl_rls_dev* S, uint64_t n, uint64_t n_store, uint64_t n_ctr, PinnedBuf<Req>& h_req, const DevBuf<Req>& d_req,
+               uint64_t* out_n_store, uint64_t* out_n_ctr, const Req** out_req) {
+    if (n) RL_CUDA(S, cudaMemcpyAsync(h_req.p, d_req.p, n * sizeof(Req), cudaMemcpyDeviceToHost, S->stream));
+    S->n = n;
+    S->n_store = n_store;
+    S->n_ctr = n_ctr;
+    *out_n_store = n_store;
+    *out_n_ctr = n_ctr;
+    *out_req = h_req.p;
+    return RL_OK;
+}
+
 CvDict cv_dict(rl_rls_dev* S) {
     return CvDict{S->d_cv_slots.p, S->cv_slots - 1, S->d_cv_arena.p, S->cv_arena_bytes, S->d_cv_ctl.p};
 }
 
-// k_counter_vars_record after a plan's scatter, when keeping is on: the plan's scratch is still the batch's.  Returns the
-// kernels launched (0 or 1).
+// k_counter_vars_record after a plan's scatter, when keeping is on: the plan's scratch is still the batch's.  Then the
+// plan's `launched` kernels and this one are counted.
 template <class Dec>
-int record_vars(rl_rls_dev* S, uint64_t n, uint32_t per_req, const unsigned long long* rls_count, const HttpScan* http_count,
-                uint32_t& launched) {
-    launched = 0;
-    if (!S->cv_slots || n == 0) return RL_OK;
-    CvRecordArgs a;
-    a.buf = S->d_buf.p;
-    a.off = S->d_off.p;
-    a.n = n;
-    a.img = rl_img_view(S->image.data(), S->d_image.p);
-    a.per_req = per_req;
-    a.ent = S->d_ent.p;
-    a.scratch = S->d_scratch.p;
-    a.rls_count = rls_count;
-    a.http_count = http_count;
-    a.txt = S->d_txt.p;
-    a.bits = S->d_bits.p;
-    a.dict = cv_dict(S);
-    const uint32_t threads = 128;
-    k_counter_vars_record<Dec><<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
-    RL_CUDA(S, cudaGetLastError());
-    launched = 1;
+int record_vars(rl_rls_dev* S, rl_engine* e, uint32_t launched, uint64_t n, uint32_t per_req, const unsigned long long* rls_count,
+                const HttpScan* http_count) {
+    if (S->cv_slots && n) {
+        CvRecordArgs a;
+        a.buf = S->d_buf.p;
+        a.off = S->d_off.p;
+        a.n = n;
+        a.img = rl_img_view(S->image.data(), S->d_image.p);
+        a.per_req = per_req;
+        a.ent = S->d_ent.p;
+        a.scratch = S->d_scratch.p;
+        a.rls_count = rls_count;
+        a.http_count = http_count;
+        a.txt = S->d_txt.p;
+        a.bits = S->d_bits.p;
+        a.dict = cv_dict(S);
+        const uint32_t threads = 128;
+        k_counter_vars_record<Dec><<<blocks_for(n, threads), threads, 0, S->stream>>>(a);
+        RL_CUDA(S, cudaGetLastError());
+        launched++;
+    }
+    rl_internal_launched(e, launched);
     return RL_OK;
 }
 
@@ -330,10 +379,7 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     // the one read before the store call: how many store requests and counters the batch has
     if ((r = read_totals(S, S->h_total.p, S->d_start.p + n, sizeof(unsigned long long)))) return r;
     const uint64_t n_store = S->h_total.p[0] >> 32, n_ctr = S->h_total.p[0] & 0xFFFFFFFFull;
-    RL_CUDA(S, S->d_ctr_off.grow(n_store + 1));
-    RL_CUDA(S, S->d_ctrs.grow(n_ctr + 1));
-    RL_CUDA(S, S->d_delta.grow(n_store + 1));
-    RL_CUDA(S, S->d_now.grow(n_store + 1));
+    if ((r = grow_csr(S, n_store, n_ctr))) return r;
     RlsScatterArgs b;
     b.req = S->d_req.p;
     b.scratch = S->d_scratch.p;
@@ -348,25 +394,19 @@ int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, ui
     b.now = S->d_now.p;
     k_rls_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
     RL_CUDA(S, cudaGetLastError());
-    uint32_t rec = 0;
-    if ((r = record_vars<CvWire>(S, n, per_req, S->d_count.p, nullptr, rec))) return r;
-    rl_internal_launched(e, 2 + rec);
-    if (n) RL_CUDA(S, cudaMemcpyAsync(S->h_req.p, S->d_req.p, n * sizeof(RlsDevReq), cudaMemcpyDeviceToHost, S->stream));
-    S->n = n;
-    S->n_store = n_store;
-    S->n_ctr = n_ctr;
-    *out_n_store = n_store;
-    *out_n_ctr = n_ctr;
-    *out_req = S->h_req.p;
-    return RL_OK;
+    if ((r = record_vars<CvWire>(S, e, 2, n, per_req, S->d_count.p, nullptr))) return r;
+    return close_plan(S, n, n_store, n_ctr, S->h_req, S->d_req, out_n_store, out_n_ctr, out_req);
 }
 
-int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta) {
+int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load) {
     if (!S) return RL_FATAL;
     RL_CUDA(S, cudaSetDevice(S->device));
     RL_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
     if (S->n_ctr) RL_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_store) RL_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+    if (S->n_store) {
+        RL_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
+        if (load) RL_CUDA(S, cudaMemcpyAsync(load, S->d_load.p, S->n_store, cudaMemcpyDeviceToHost, S->stream));
+    }
     RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
@@ -374,23 +414,13 @@ int rl_rls_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uin
 int rl_rls_dev_decide(rl_rls_dev* S, rl_engine* e, int method, int load_counters, uint8_t* limited, uint32_t* first_limited,
                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
     if (!S || !e) return RL_FATAL;
-    const uint64_t m = S->n_store;
-    if (m == 0) return RL_OK;
+    if (S->n_store == 0) return RL_OK;
     RL_CUDA(S, cudaSetDevice(S->device));
+    const StoreOp op = store_op(false, method);
     int st = reserve_outputs(S, load_counters != 0);
-    if (st) return st;
-    if (method == RL_RLS_SHOULD_RATE_LIMIT)
-        st = rl_check_and_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, load_counters, RL_MEM_DEVICE,
-                                       S->d_lim.p, S->d_first.p, load_counters ? S->d_rem.p : nullptr,
-                                       load_counters ? S->d_ttl.p : nullptr);
-    else if (method == RL_RLS_CHECK_RATE_LIMIT)
-        st = rl_is_within_limits_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, RL_MEM_DEVICE, S->d_lim.p,
-                                       S->d_first.p);
-    else
-        st = rl_update_batch(e, m, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, RL_MEM_DEVICE);
-    if (st == RL_OK) st = rl_sync(e);  // a device-memory call reports its deferred errors here
+    if (st == RL_OK) st = store_call(S, e, op, 0, S->n_store, S->d_ctr_off.p, 0, load_counters != 0);
     if (st != RL_OK) return st;
-    return copy_outputs(S, method != RL_RLS_REPORT, load_counters != 0, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
+    return copy_outputs(S, op != UPDATE, load_counters != 0, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
 }
 
 int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
@@ -446,11 +476,8 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
         (r = read_totals(S, S->h_runs.p + first_read, S->d_runs.p + first_read,
                          (RL_HTTP_RUNS_HEAD + 3 * n_runs - first_read) * sizeof(uint32_t))))
         return r;
-    RL_CUDA(S, S->d_ctr_off.grow(n_store + 1));
+    if ((r = grow_csr(S, n_store, n_ctr))) return r;
     RL_CUDA(S, S->d_ctr_run.grow(n_store + n_runs + 1));
-    RL_CUDA(S, S->d_ctrs.grow(n_ctr + 1));
-    RL_CUDA(S, S->d_delta.grow(n_store + 1));
-    RL_CUDA(S, S->d_now.grow(n_store + 1));
     RL_CUDA(S, S->d_load.grow(n_store + 1));
     HttpScatterArgs b;
     b.req = S->d_hreq.p;
@@ -469,32 +496,11 @@ int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint,
     b.load = S->d_load.p;
     k_http_scatter<<<blocks_for(n + 1, threads), threads, 0, S->stream>>>(b);
     RL_CUDA(S, cudaGetLastError());
-    uint32_t rec = 0;
-    if ((r = record_vars<CvJson>(S, n, per_req, nullptr, S->d_hcount.p, rec))) return r;
-    rl_internal_launched(e, 3 + rec);
-    if (n) RL_CUDA(S, cudaMemcpyAsync(S->h_hreq.p, S->d_hreq.p, n * sizeof(HttpDevReq), cudaMemcpyDeviceToHost, S->stream));
-    S->n = n;
-    S->n_store = n_store;
-    S->n_ctr = n_ctr;
+    if ((r = record_vars<CvJson>(S, e, 3, n, per_req, nullptr, S->d_hcount.p))) return r;
+    if ((r = close_plan(S, n, n_store, n_ctr, S->h_hreq, S->d_hreq, out_n_store, out_n_ctr, out_req))) return r;
     S->n_runs = (uint32_t)n_runs;
-    *out_n_store = n_store;
-    *out_n_ctr = n_ctr;
-    *out_req = S->h_hreq.p;
     *out_runs = reinterpret_cast<const HttpRun*>(S->h_runs.p + RL_HTTP_RUNS_HEAD);
     *out_n_runs = (uint32_t)n_runs;
-    return RL_OK;
-}
-
-int rl_http_dev_copy_plan(rl_rls_dev* S, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load) {
-    if (!S) return RL_FATAL;
-    RL_CUDA(S, cudaSetDevice(S->device));
-    RL_CUDA(S, cudaMemcpyAsync(ctr_off, S->d_ctr_off.p, (S->n_store + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_ctr) RL_CUDA(S, cudaMemcpyAsync(ctrs, S->d_ctrs.p, S->n_ctr * sizeof(rl_counter), cudaMemcpyDeviceToHost, S->stream));
-    if (S->n_store) {
-        RL_CUDA(S, cudaMemcpyAsync(delta, S->d_delta.p, S->n_store * sizeof(uint64_t), cudaMemcpyDeviceToHost, S->stream));
-        RL_CUDA(S, cudaMemcpyAsync(load, S->d_load.p, S->n_store, cudaMemcpyDeviceToHost, S->stream));
-    }
-    RL_CUDA(S, cudaStreamSynchronize(S->stream));
     return RL_OK;
 }
 
@@ -503,6 +509,7 @@ int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_statu
     if (!S || !e || !run_status) return RL_FATAL;
     if (S->n_store == 0) return RL_OK;
     RL_CUDA(S, cudaSetDevice(S->device));
+    const StoreOp op = store_op(true, endpoint);
     const HttpRun* runs = reinterpret_cast<const HttpRun*>(S->h_runs.p + RL_HTTP_RUNS_HEAD);
     bool any_load = false;
     for (uint32_t k = 0; k < S->n_runs; k++) any_load = any_load || runs[k].load;
@@ -511,23 +518,10 @@ int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_statu
     // one store call per run, in batch order: run k's CSR starts at ctr_run[runs[k].store + k] and counts from 0
     for (uint32_t k = 0; k < S->n_runs; k++) {
         const HttpRun& R = runs[k];
-        const uint64_t j1 = k + 1 < S->n_runs ? runs[k + 1].store : S->n_store, m = j1 - R.store;
-        const uint32_t* off = S->d_ctr_run.p + R.store + k;
-        const rl_counter* c = S->d_ctrs.p + R.ctr;
-        const uint64_t *d = S->d_delta.p + R.store, *now = S->d_now.p + R.store;
-        int st;
-        if (endpoint == RL_HTTP_CHECK_AND_REPORT)
-            st = rl_check_and_update_batch(e, m, off, c, d, now, (int)R.load, RL_MEM_DEVICE, S->d_lim.p + R.store,
-                                           S->d_first.p + R.store, R.load ? S->d_rem.p + R.ctr : nullptr,
-                                           R.load ? S->d_ttl.p + R.ctr : nullptr);
-        else if (endpoint == RL_HTTP_CHECK)
-            st = rl_is_within_limits_batch(e, m, off, c, d, now, RL_MEM_DEVICE, S->d_lim.p + R.store, S->d_first.p + R.store);
-        else
-            st = rl_update_batch(e, m, off, c, d, now, RL_MEM_DEVICE);
-        if (st == RL_OK) st = rl_sync(e);  // a device-memory call reports its deferred errors here
-        run_status[k] = st;
+        const uint64_t j1 = k + 1 < S->n_runs ? runs[k + 1].store : S->n_store;
+        run_status[k] = store_call(S, e, op, R.store, j1 - R.store, S->d_ctr_run.p + R.store + k, R.ctr, R.load != 0);
     }
-    return copy_outputs(S, endpoint != RL_HTTP_REPORT, any_load, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
+    return copy_outputs(S, op != UPDATE, any_load, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
 }
 
 int rl_rls_dev_wait(rl_rls_dev* S) {

@@ -38,8 +38,9 @@ extern "C" {
 int rl_rls_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int method, uint64_t n, const uint8_t* buf,
                     const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
                     const RlsDevReq** out_req);
-// Host copies of the planned store call: ctr_off [n_store + 1], ctrs [n_ctr], delta [n_store].
-int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta);
+// Host copies of the planned store requests of either plan: ctr_off [n_store + 1], ctrs [n_ctr], delta [n_store], and
+// unless load is NULL (an HTTP plan's) load_counters flags [n_store].
+int rl_rls_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
 // The store call of the planned batch from its device arrays (RL_MEM_DEVICE), then its outputs copied back: limited and
 // first_limited [n_store] (not for Report), and with load_counters remaining / ttl_us [n_ctr] together with ctr_off
 // [n_store + 1] and ctrs [n_ctr], which the headers are formatted from.  Returns the store call's status;
@@ -53,8 +54,6 @@ int rl_rls_dev_wait(rl_rls_dev* st);
 int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,
                      const uint64_t* off, uint64_t now_us, uint64_t* out_n_store, uint64_t* out_n_ctr,
                      const HttpDevReq** out_req, const HttpRun** out_runs, uint32_t* out_n_runs);
-// Host copies of the planned store requests: ctr_off [n_store + 1], ctrs [n_ctr], delta and load [n_store].
-int rl_http_dev_copy_plan(rl_rls_dev* st, uint32_t* ctr_off, rl_counter* ctrs, uint64_t* delta, uint8_t* load);
 // One store call per run from the device arrays, then the outputs back as rl_rls_dev_decide copies them (remaining / ttl,
 // ctr_off and ctrs when a run loads counters).  run_status[r] = the status of run r's call.
 int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int endpoint, int* run_status, uint8_t* limited, uint32_t* first_limited,

@@ -95,7 +95,7 @@ def decode_body(body: bytes, cap_entries: int = 64):
     return s(q.ns_off, q.ns_len), pairs, q.delta, q.response_headers
 
 
-_view = _rls._view
+_view, _ptr = _rls._view, _rls._ptr
 
 
 class HttpApi:
@@ -136,37 +136,16 @@ class HttpApi:
         return self._plan(self._lib.rl_http_plan_device, endpoint, buf, off, now_us)
 
     def _plan(self, fn, endpoint, buf, off, now_us):
-        buf = np.ascontiguousarray(buf, dtype=np.uint8)
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        n = len(off) - 1
-        self._keep, self._n = (buf, off), n
-        self._check(fn(self._h, endpoint, n, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
-        ns = C.c_uint64()
-        p_off, p_ctr, p_delta, p_now, p_load, p_idx = (C.c_void_p() for _ in range(6))
-        self._check(self._lib.rl_http_plan_view(self._h, C.byref(ns), C.byref(p_off), C.byref(p_ctr), C.byref(p_delta),
-                                                C.byref(p_now), C.byref(p_load), C.byref(p_idx)))
-        m = ns.value
-        ctr_off = _view(p_off.value, m + 1, np.uint32).copy()
-        return {
-            "n_store": m, "ctr_off": ctr_off,
-            "ctrs": _view(p_ctr.value, int(ctr_off[-1]) if m else 0, _eng.COUNTER_DTYPE).copy(),
-            "delta": _view(p_delta.value, m, np.uint64).copy(), "now_us": _view(p_now.value, m, np.uint64).copy(),
-            "load_counters": _view(p_load.value, m, np.uint8).copy(), "store_index": _view(p_idx.value, n, np.uint32).copy(),
-        }
+        self._n = n = len(off) - 1
+        _rls._batch_call(self, fn, endpoint, buf, off, now_us)
+        return _rls._read_plan(self._lib.rl_http_plan_view, self._h, self._check, n, True)
 
     def finish(self, limited=None, first_limited=None, remaining=None, ttl_us=None, store_status=None):
         """Stage 3.  store_status: one status per store request (None = all OK)."""
-        arrs = []
-
-        def ptr(a, dt):
-            if a is None:
-                return None
-            a = np.ascontiguousarray(a, dtype=dt)
-            arrs.append(a)
-            return a.ctypes.data if len(a) else None
-
-        self._check(self._lib.rl_http_finish(self._h, ptr(store_status, np.int32), ptr(limited, np.uint8),
-                                             ptr(first_limited, np.uint32), ptr(remaining, np.uint64), ptr(ttl_us, np.uint64)))
+        keep = []
+        self._check(self._lib.rl_http_finish(self._h, _ptr(store_status, np.int32, keep), _ptr(limited, np.uint8, keep),
+                                             _ptr(first_limited, np.uint32, keep), _ptr(remaining, np.uint64, keep),
+                                             _ptr(ttl_us, np.uint64, keep)))
         return self.responses()
 
     def responses(self) -> List[Tuple[int, bytes, Dict[str, str]]]:
@@ -191,11 +170,8 @@ class HttpApi:
 
     def serve(self, endpoint: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
         """plan_device -> the engine (one call per run) -> finish.  Needs an engine."""
-        buf = np.ascontiguousarray(buf, dtype=np.uint8)
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        self._keep, self._n = (buf, off), len(off) - 1
-        self._check(self._lib.rl_http_serve(self._h, endpoint, len(off) - 1, buf.ctypes.data if len(buf) else None,
-                                            off.ctypes.data, now_us))
+        self._n = len(off) - 1
+        _rls._batch_call(self, self._lib.rl_http_serve, endpoint, buf, off, now_us)
 
     def timings(self) -> Dict[str, float]:
         a, b, c, k = C.c_double(), C.c_double(), C.c_double(), C.c_uint32()

@@ -217,6 +217,45 @@ def _view(ptr, n, dtype):
     return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_uint8)), shape=(n * np.dtype(dtype).itemsize,)).view(dtype)
 
 
+def _batch_call(svc, fn, method: int, buf, off, now_us: int) -> int:
+    """fn(handle, method, n, buf, off, now_us), a plan or serve call, on svc's service; svc keeps the batch's arrays
+    alive -> n."""
+    buf = np.ascontiguousarray(buf, dtype=np.uint8)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    svc._keep = (buf, off)
+    svc._check(fn(svc._h, method, len(off) - 1, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
+    return len(off) - 1
+
+
+def _read_plan(view_fn, h, check, n: int, load_per_request: bool):
+    """The planned batch of n requests through rl_rls_plan_view / rl_http_plan_view -> dict(n_store, ctr_off, ctrs, delta,
+    now_us, load_counters, store_index), copies of its arrays.  load_counters is one bool for the batch, or with
+    load_per_request one flag per store request."""
+    ns = C.c_uint64()
+    p_off, p_ctr, p_delta, p_now, p_idx = (C.c_void_p() for _ in range(5))
+    lc = C.c_void_p() if load_per_request else C.c_int()
+    check(view_fn(h, C.byref(ns), C.byref(p_off), C.byref(p_ctr), C.byref(p_delta), C.byref(p_now), C.byref(lc), C.byref(p_idx)))
+    m = ns.value
+    ctr_off = _view(p_off.value, m + 1, np.uint32).copy()
+    return {
+        "n_store": m, "ctr_off": ctr_off,
+        "ctrs": _view(p_ctr.value, int(ctr_off[-1]) if m else 0, _eng.COUNTER_DTYPE).copy(),
+        "delta": _view(p_delta.value, m, np.uint64).copy(), "now_us": _view(p_now.value, m, np.uint64).copy(),
+        "load_counters": _view(lc.value, m, np.uint8).copy() if load_per_request else bool(lc.value),
+        "store_index": _view(p_idx.value, n, np.uint32).copy(),
+    }
+
+
+def _ptr(a, dtype, keep: list):
+    """a's address as a contiguous dtype array for a C call (None for None or an empty array); the array is appended to
+    keep, which the caller holds until the call returns."""
+    if a is None:
+        return None
+    a = np.ascontiguousarray(a, dtype=dtype)
+    keep.append(a)
+    return a.ctypes.data if len(a) else None
+
+
 class RlsService:
     """One RLS front over a Matcher and (optionally) an Engine.  Not thread-safe: one batch at a time."""
 
@@ -255,37 +294,14 @@ class RlsService:
         return self._plan(self._lib.rl_rls_plan_device, method, buf, off, now_us)
 
     def _plan(self, fn, method, buf, off, now_us):
-        buf = np.ascontiguousarray(buf, dtype=np.uint8)
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        n = len(off) - 1
-        self._keep = (buf, off)
-        self._check(fn(self._h, method, n, buf.ctypes.data if len(buf) else None, off.ctypes.data, now_us))
-        ns = C.c_uint64()
-        p_off, p_ctr, p_delta, p_now, p_idx = (C.c_void_p() for _ in range(5))
-        lc = C.c_int()
-        self._check(self._lib.rl_rls_plan_view(self._h, C.byref(ns), C.byref(p_off), C.byref(p_ctr), C.byref(p_delta),
-                                               C.byref(p_now), C.byref(lc), C.byref(p_idx)))
-        m = ns.value
-        ctr_off = _view(p_off.value, m + 1, np.uint32).copy()
-        return {
-            "n_store": m, "ctr_off": ctr_off,
-            "ctrs": _view(p_ctr.value, int(ctr_off[-1]) if m else 0, _eng.COUNTER_DTYPE).copy(),
-            "delta": _view(p_delta.value, m, np.uint64).copy(), "now_us": _view(p_now.value, m, np.uint64).copy(),
-            "load_counters": bool(lc.value), "store_index": _view(p_idx.value, n, np.uint32).copy(),
-        }
+        n = _batch_call(self, fn, method, buf, off, now_us)
+        return _read_plan(self._lib.rl_rls_plan_view, self._h, self._check, n, False)
 
     def finish(self, limited=None, first_limited=None, remaining=None, ttl_us=None, store_status: int = 0):
-        arrs = []
-
-        def ptr(a, dt):
-            if a is None:
-                return None
-            a = np.ascontiguousarray(a, dtype=dt)
-            arrs.append(a)
-            return a.ctypes.data if len(a) else None
-
-        self._check(self._lib.rl_rls_finish(self._h, store_status, ptr(limited, np.uint8), ptr(first_limited, np.uint32),
-                                            ptr(remaining, np.uint64), ptr(ttl_us, np.uint64)))
+        keep = []
+        self._check(self._lib.rl_rls_finish(self._h, store_status, _ptr(limited, np.uint8, keep),
+                                            _ptr(first_limited, np.uint32, keep), _ptr(remaining, np.uint64, keep),
+                                            _ptr(ttl_us, np.uint64, keep)))
         return self.responses()
 
     def responses(self) -> List[Tuple[int, bytes]]:
@@ -311,11 +327,7 @@ class RlsService:
 
     def serve(self, method: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
         """plan -> ONE engine call -> finish.  Needs an engine (no CPU store exists in the product)."""
-        buf = np.ascontiguousarray(buf, dtype=np.uint8)
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        self._keep = (buf, off)
-        self._check(self._lib.rl_rls_serve(self._h, method, len(off) - 1, buf.ctypes.data if len(buf) else None,
-                                           off.ctypes.data, now_us))
+        _batch_call(self, self._lib.rl_rls_serve, method, buf, off, now_us)
 
     def timings(self) -> Dict[str, float]:
         a, b, c = C.c_double(), C.c_double(), C.c_double()
