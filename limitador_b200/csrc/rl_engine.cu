@@ -360,14 +360,10 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     B.scan_ctr = w.small.p + 0;
     B.ticket = w.small.p + 2;
     B.exit_ctr = w.small.p + 3;
-    uint32_t tile = ceil_div(n_acc, kMaxTiles);
-    tile = std::max<uint32_t>(512, ((tile + 255) / 256) * 256);
-    B.tile = tile;
-    B.num_tiles = std::max<uint32_t>(1, ceil_div(n_acc, tile));
-    // n_hint (sharded steps): n_acc is only the upper bound of a device-side count; partitions are sized for
-    // the expected count, and the kernels derive the tile from the actual one (rl_tile_of)
-    const uint32_t n_size = n_hint ? std::min(n_hint, n_acc) : n_acc;
-    if (n_hint) B.num_tiles = std::min<uint32_t>(256, std::max<uint32_t>(1, ceil_div(n_acc, 256)));
+    // n_hint (sharded steps): n_acc is only the upper bound of a device-side count (rl_batch_geom)
+    const RlBatchGeom g = rl_batch_geom(n_acc, n_hint, e->log2P, e->part_target, e->chunk, e->heavy_mult);
+    B.tile = g.tile;
+    B.num_tiles = g.num_tiles;
     B.out_limited = o.limited;
     B.out_first_limited = o.first;
     B.out_remaining = o.rem;
@@ -384,17 +380,11 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     B.chain_wcnt = w.chain_wcnt.p;
     B.chain_w = w.chain_w.p;
     B.chunk = e->chunk;
-    // a region is split into chained chunks only when it is far heavier than the average one
-    // partition granularity: about one k_main chunk per partition, never finer than the table's regions
-    {
-        uint32_t want = std::max<uint32_t>(64, ceil_div(n_size, e->part_target));
-        uint32_t lp = 0;
-        while ((1u << (lp + 1)) <= want) lp++;
-        lp = std::min<uint32_t>(lp, e->log2P);
-        B.part_shift = e->log2P - lp;
-        B.nparts = 1u << lp;
-    }
-    B.heavy_len = e->heavy_mult ? std::max<uint32_t>(2 * e->chunk, e->heavy_mult * ceil_div(n_size, B.nparts)) : 0xFFFFFFFFu;
+    // a region is split into chained chunks only when it is far heavier than the average one; partition
+    // granularity: about one k_main chunk per partition, never finer than the table's regions
+    B.part_shift = g.part_shift;
+    B.nparts = g.nparts;
+    B.heavy_len = g.heavy_len;
     B.log_row = nullptr;
     B.log_state = nullptr;
     return B;
@@ -414,16 +404,14 @@ auto with_cells(const rl_engine* e, F&& f) {
 template <class Src>
 int launch_front(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st = nullptr) {
     if (!st) st = e->stream;
-    const uint32_t P1 = B.nparts + B.nhot + 1;
-    const size_t smem = ((size_t)RL_PART_WARPS * P1 + P1 + 1) * sizeof(uint32_t);
+    const size_t smem = rl_front_smem_bytes(B.nparts, B.nhot);
     return with_cells(e, [&](auto c) -> int {
         auto kern = k_front<decltype(c)::value, Src>;
         static int smem_limit[64] = {};  // per instantiation and device: raised as engines with more regions appear
         const int dv = e->device & 63;
         // (k_front also has ~8 KB of static shared memory: opt in well before the 48 KB default is reached)
         if (smem > 32 * 1024 && (int)smem > smem_limit[dv]) {
-            const uint32_t maxP1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;
-            const int max_smem = (int)(((size_t)RL_PART_WARPS * maxP1 + maxP1 + 1) * sizeof(uint32_t));
+            const int max_smem = (int)rl_front_smem_bytes(1u << e->log2P, RL_HOT_SLOTS);
             RL_CUDA(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
             smem_limit[dv] = max_smem;
         }
@@ -447,7 +435,7 @@ int launch_main_ch(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& sr
     // items from a ticket, so a smaller grid only means that some CTAs take several
     // (capping the grid at one resident wave was tried: the CTAs that then take a second item make the kernel last
     // two chunk latencies instead of one)
-    const uint32_t grid = std::min<uint32_t>(B.nparts + ceil_div(B.n_acc, CH), e->main_grid_cap);
+    const uint32_t grid = rl_main_grid(B.nparts, B.n_acc, CH, e->main_grid_cap);
     kern<<<grid, CH, rl_main_smem_bytes<CELLS, CH>(B.num_tiles), st>>>(D, B, src, e->weak_slots);
     return RL_OK;
 }

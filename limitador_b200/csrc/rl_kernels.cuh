@@ -13,13 +13,23 @@
 // one group, so counter values need no atomics at all; the only atomic on the table is the
 // 128-bit CAS that claims an empty row for a new key.
 #pragma once
+#ifndef RL_SIMT
 #include <cuda_runtime.h>
+#endif
 #include <stdint.h>
 
 #include <type_traits>
 
 #include "../../include/rl_engine.h"
 #include "rl_core.h"
+
+// A kernel's dynamic shared memory, declared as an array `name` of T.  Under tests/emu/cuda_simt.h (RL_SIMT) it is a
+// pointer to the running block's own dynamic shared memory, sized at launch.
+#ifndef RL_SIMT
+#define RL_DYN_SMEM(T, name) extern __shared__ T name[]
+#else
+#define RL_DYN_SMEM(T, name) T* const name = reinterpret_cast<T*>(simt_dyn_smem())
+#endif
 
 #define RL_PART_THREADS 256
 #define RL_MAX_TILES 1024  // tiles (CTAs of k_front) per batch: a 1 M-request batch gives every warp one 4-deep probe iteration
@@ -70,7 +80,11 @@ enum { RL_EV_FRONT = 1, RL_EV_MAIN = 2, RL_EV_XCOUNT = 3, RL_EV_XSCATTER = 4, RL
 __device__ __forceinline__ void rl_trace(uint4* trace, uint32_t* pos, uint32_t ev, uint32_t end, uint32_t seq) {
     if (trace == nullptr) return;
     unsigned long long t;
+#ifndef RL_SIMT
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+#else
+    t = clock64();
+#endif
     const uint32_t i = atomicAdd(pos, 1u) & (RL_TRACE_CAP - 1);
     trace[i] = make_uint4(ev | (end << 8), seq, (uint32_t)t, (uint32_t)(t >> 32));
 }
@@ -125,6 +139,51 @@ struct RlBatch {
     ulonglong2* log_state; // [n_acc][CELLS]
 };
 
+// The geometry of a batch of n_acc accesses (host code: make_batch in rl_engine.cu, and the host driver of the kernels in
+// tests/emu/emu_engine.cpp).  Tiles of at least 512 accesses, at most RL_MAX_TILES of them; n_hint != 0 (sharded
+// steps): n_acc is only the upper bound of a device-side count, the kernels derive the tile from the actual one
+// (rl_tile_of) over at most 256 tiles, and the partitions are sized for the expected count n_hint.  Partitions:
+// about one k_main chunk each (part_target accesses), never finer than the table's regions.  A partition longer than
+// heavy_len (heavy_mult x the average one, at least two chunks) is chained (heavy_mult = 0: never).
+struct RlBatchGeom {
+    uint32_t tile, num_tiles, nparts, part_shift, heavy_len;
+};
+inline uint32_t rl_ceil_div(uint64_t a, uint64_t b) { return (uint32_t)((a + b - 1) / b); }
+inline RlBatchGeom rl_batch_geom(uint32_t n_acc, uint32_t n_hint, uint32_t log2P, uint32_t part_target, uint32_t chunk,
+                                 uint32_t heavy_mult) {
+    RlBatchGeom g;
+    const uint32_t t = rl_ceil_div(n_acc, RL_MAX_TILES);
+    g.tile = ((t + 255) / 256) * 256 > 512 ? ((t + 255) / 256) * 256 : 512;
+    const uint32_t nt = rl_ceil_div(n_acc, g.tile);
+    g.num_tiles = nt > 1 ? nt : 1;
+    const uint32_t n_size = (n_hint && n_hint < n_acc) ? n_hint : n_acc;
+    if (n_hint) {
+        const uint32_t ns = rl_ceil_div(n_acc, 256);
+        g.num_tiles = ns < 1 ? 1 : (ns > 256 ? 256 : ns);
+    }
+    const uint32_t pt = rl_ceil_div(n_size, part_target);
+    const uint32_t want = pt > 64 ? pt : 64;
+    uint32_t lp = 0;
+    while ((1u << (lp + 1)) <= want) lp++;
+    if (lp > log2P) lp = log2P;
+    g.part_shift = log2P - lp;
+    g.nparts = 1u << lp;
+    const uint32_t hl = heavy_mult * rl_ceil_div(n_size, g.nparts);
+    g.heavy_len = heavy_mult ? (hl > 2 * chunk ? hl : 2 * chunk) : 0xFFFFFFFFu;
+    return g;
+}
+// k_front's dynamic shared memory: per-warp counts of every partition (cold, hot, the no-row bucket), then loc[]
+inline size_t rl_front_smem_bytes(uint32_t nparts, uint32_t nhot) {
+    const size_t P1 = (size_t)nparts + nhot + 1;
+    return ((size_t)RL_PART_WARPS * P1 + P1 + 1) * sizeof(uint32_t);
+}
+// k_main's grid: one CTA per partition + one per chunk of a heavy partition bounds the work items; CTAs take items
+// from a ticket, so a smaller grid (cap) only means that some CTAs take several
+inline uint32_t rl_main_grid(uint32_t nparts, uint32_t n_acc, uint32_t ch, uint32_t cap) {
+    const uint32_t g = nparts + rl_ceil_div(n_acc, ch);
+    return g < cap ? g : cap;
+}
+
 __device__ __forceinline__ void rl_store_verdict(const RlBatch& B, uint32_t req, uint8_t v) {
     if (B.omap_prefix == nullptr) {
         B.out_limited[req] = v;
@@ -154,6 +213,13 @@ __device__ __forceinline__ void rl_st_cg(void* p, unsigned long long a, unsigned
 }
 // 128-bit compare-and-swap (PTX atom.cas.b128, sm_90+): claims a row header atomically.
 __device__ __forceinline__ ulonglong2 rl_cas128(void* addr, ulonglong2 cmp, ulonglong2 val) {
+#ifdef RL_SIMT
+    RLM_EMU_SWITCH();  // a switch point of the emulator's interleaving mode, like every global atomic
+    ulonglong2* p = reinterpret_cast<ulonglong2*>(addr);
+    const ulonglong2 old = *p;
+    if (old.x == cmp.x && old.y == cmp.y) *p = val;
+    return old;
+#else
     ulonglong2 old;
     asm volatile(
         "{\n\t"
@@ -167,6 +233,7 @@ __device__ __forceinline__ ulonglong2 rl_cas128(void* addr, ulonglong2 cmp, ulon
         : "l"(addr), "l"(cmp.x), "l"(cmp.y), "l"(val.x), "l"(val.y)
         : "memory");
     return old;
+#endif
 }
 // streaming (read-once) loads of request data: keep them out of L1
 __device__ __forceinline__ ulonglong2 rl_ld_stream(const void* p) {
@@ -427,7 +494,11 @@ __device__ __forceinline__ uint32_t rl_block_excl_scan(uint32_t v, uint32_t* s_w
 
 __device__ __forceinline__ unsigned long long rl_globaltimer_ns() {
     unsigned long long t;
+#ifndef RL_SIMT
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+#else
+    t = clock64();
+#endif
     return t;
 }
 
@@ -444,7 +515,7 @@ __device__ __forceinline__ uint32_t rl_batch_n(const RlBatch& B) {
 
 template <int CELLS, class Src>
 __global__ void __launch_bounds__(RL_PART_THREADS, Src::kAccessIsRequest ? 4 : 3) k_front(RlDev D, RlBatch B, Src src) {
-    extern __shared__ uint32_t wcnt[];  // [RL_PART_WARPS][P+1] per-warp counts -> positions, then loc[P+2]
+    RL_DYN_SMEM(uint32_t, wcnt);  // [RL_PART_WARPS][P+1] per-warp counts -> positions, then loc[P+2]
     __shared__ uint32_t s_warp[RL_PART_WARPS], s_warp2[RL_PART_WARPS];
     __shared__ uint32_t s_last;
     constexpr uint32_t RB = RlGeom<CELLS>::ROW_BYTES;
@@ -1122,7 +1193,7 @@ __global__ void __launch_bounds__(CH, rl_main_ctas<CELLS, Src, MODE, CH, LC>() *
     using Smem = RlMainSmem<CELLS, CH>;
     constexpr int GT = Smem::GT;
     constexpr int PW = Smem::PW;
-    extern __shared__ __align__(16) unsigned char rl_smem_raw[];
+    RL_DYN_SMEM(__align__(16) unsigned char, rl_smem_raw);
     Smem& sm = *reinterpret_cast<Smem*>(rl_smem_raw);
     uint32_t* const sm_t_pfx = reinterpret_cast<uint32_t*>(rl_smem_raw + sizeof(Smem));
     uint32_t* const sm_t_loc = sm_t_pfx + B.num_tiles + 1;

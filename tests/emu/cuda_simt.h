@@ -1,5 +1,5 @@
 // cuda_simt.h — TEST-ONLY: a small SIMT emulator, one step up from cuda_shim.h.  Every CUDA thread of a block is a fiber
-// (ucontext) scheduled cooperatively on the calling OS thread; warp-level intrinsics (__match_any_sync, __ballot_sync,
+// (its own stack, switched by a few instructions of x86-64 assembly) scheduled cooperatively on the calling OS thread; warp-level intrinsics (__match_any_sync, __ballot_sync,
 // __reduce_*_sync, __shfl_sync, __syncwarp) are rendezvous points of the lanes named in their mask, and __syncthreads is
 // a block barrier.  With it the DEVICE branches of the maintenance kernels — the warp-aggregated fast paths that
 // cuda_shim.h compiles out (`#ifndef RL_SHIM`) — run on the host, without a GPU, against the same
@@ -14,16 +14,27 @@
 // memory helpers of rl_devmem.cuh (rlm_ld, rlm_ld64, rlm_cas128, rlm_or) first hand control back to the scheduler with
 // probability p, and every pass of the scheduler visits the block's fibers in a seeded random order; p = 1 switches at
 // every one of them.  A kernel whose threads claim and then write shared words thus runs under many interleavings of
-// those steps, deterministically for one seed.  Blocks still run one after the other: only the threads of one block
-// interleave, so a test puts the work that must collide inside one block.
+// those steps, deterministically for one seed.  Global loads and stores (__ldcg, __ldcs, __ldg, __stcg) and
+// __threadfence are switch points too.
+//
+// Resident blocks (simt_launch_ex): a launch keeps up to R blocks live at once, as an SM keeps several CTAs, and
+// dispatches the next block when one exits.  Every pass of the scheduler visits the fibers of all resident blocks (in
+// a seeded random order in the interleaving mode); barriers and warp rendezvous stay per block.  With R = 1 (and in
+// simt_launch) the blocks run one after the other.  A block's dynamic shared memory (simt_dyn_smem) is its own,
+// filled with a poison pattern at its start, as the GPU leaves it uninitialised; statically declared __shared__
+// variables are `static`, one copy for all blocks, so a kernel that has any may only run with R = 1.
+//
+// Wait loops: __nanosleep gives way.  A pass in which every block that did anything also slept is a pass of waiting;
+// after kSpinPasses of them in a row the launch is reported (block and thread of a sleeper) and aborts: a block that
+// waits for a flag that no resident block will set hangs a GPU.
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
-#include <ucontext.h>
 
 #include <functional>
 #include <memory>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -34,6 +45,8 @@
 #define __forceinline__ inline
 #define __restrict__
 #define __launch_bounds__(...)
+#define __shared__ static
+#define __align__(n) __attribute__((aligned(n)))
 
 struct simt_dim3 {
     unsigned x = 0, y = 0, z = 0;
@@ -44,10 +57,54 @@ struct ulonglong2 {
     unsigned long long x, y;
 };
 static inline ulonglong2 make_ulonglong2(unsigned long long x, unsigned long long y) { return ulonglong2{x, y}; }
+struct uint4 {
+    unsigned x, y, z, w;
+};
+static inline uint4 make_uint4(unsigned x, unsigned y, unsigned z, unsigned w) { return uint4{x, y, z, w}; }
+// the device's min / max take mixed integer types
+template <class A, class B>
+static inline typename std::common_type<A, B>::type min(A a, B b) {
+    return a < b ? a : b;
+}
+template <class A, class B>
+static inline typename std::common_type<A, B>::type max(A a, B b) {
+    return a < b ? b : a;
+}
 
 namespace simt {
 static void interleave_point();
 }
+
+#if !defined(__x86_64__)
+#error "cuda_simt.h switches fibers with x86-64 assembly"
+#endif
+// simt_fiber_switch(&from_sp, to_sp): saves the callee-saved registers on the current stack, stores the stack pointer
+// in *from_sp and resumes the fiber whose stack pointer is to_sp (the system's swapcontext would also save the signal
+// mask, a system call per switch).  Hidden: every library built from this header has its own copy.
+extern "C" void simt_fiber_switch(void** from_sp, void* to_sp);
+asm(R"(
+    .text
+    .globl simt_fiber_switch
+    .hidden simt_fiber_switch
+    .type simt_fiber_switch, @function
+simt_fiber_switch:
+    pushq %rbp
+    pushq %rbx
+    pushq %r12
+    pushq %r13
+    pushq %r14
+    pushq %r15
+    movq %rsp, (%rdi)
+    movq %rsi, %rsp
+    popq %r15
+    popq %r14
+    popq %r13
+    popq %r12
+    popq %rbx
+    popq %rbp
+    ret
+    .size simt_fiber_switch, .-simt_fiber_switch
+)");
 #define RLM_EMU_SWITCH() simt::interleave_point()  // rl_devmem.cuh's memory helpers are switch points too
 
 template <class T>
@@ -86,12 +143,41 @@ static inline T atomicExch(T* p, T v) {
     *p = v;
     return o;
 }
+template <class T>
+static inline T atomicOr(T* p, T v) {
+    simt::interleave_point();
+    const T o = *p;
+    *p = o | v;
+    return o;
+}
+// global memory through the caches (the emulator has one memory: only the switch point differs from a plain access)
+template <class T>
+static inline T __ldcg(const T* p) {
+    simt::interleave_point();
+    return *p;
+}
+template <class T>
+static inline T __ldcs(const T* p) {
+    simt::interleave_point();
+    return *p;
+}
+template <class T>
+static inline T __ldg(const T* p) {
+    simt::interleave_point();
+    return *p;
+}
+template <class T>
+static inline void __stcg(T* p, T v) {
+    simt::interleave_point();
+    *p = v;
+}
+static inline void __threadfence() { simt::interleave_point(); }
 static inline int __ffs(unsigned v) { return v ? __builtin_ctz(v) + 1 : 0; }
 static inline int __popc(unsigned v) { return __builtin_popcount(v); }
 
 namespace simt {
 
-enum Op { OP_MATCH_ANY = 1, OP_BALLOT, OP_REDUCE_ADD, OP_REDUCE_MIN, OP_REDUCE_MAX, OP_SHFL, OP_SYNCWARP };
+enum Op { OP_MATCH_ANY = 1, OP_BALLOT, OP_REDUCE_ADD, OP_REDUCE_MIN, OP_REDUCE_MAX, OP_SHFL, OP_SYNCWARP, OP_SHFL_UP };
 
 struct Warp {
     unsigned pending = 0;
@@ -103,23 +189,28 @@ struct Warp {
 };
 
 struct Fiber {
-    ucontext_t ctx;
-    std::unique_ptr<char[]> stack;  // uninitialised: a block of 256 threads would otherwise zero 16 MB per launch
+    void* sp = nullptr;  // saved stack pointer (simt_fiber_switch)
+    char* stack = nullptr;  // from the stack pool, uninitialised: a block of 256 threads would otherwise zero 16 MB
     bool done = false;
     unsigned tid = 0;
 };
 
 struct Block {
+    unsigned idx = 0;  // blockIdx.x
     std::vector<Fiber> fibers;
     std::vector<Warp> warps;
-    ucontext_t sched;
     unsigned current = 0;
     unsigned long long progress = 0;  // bumped by every arrival, completion and exit: a pass without a bump is a deadlock
+    unsigned long long naps = 0;      // __nanosleep calls: a block that only naps is waiting for another one
     unsigned bar_arrived = 0, bar_gen = 0, live = 0;
+    int bar_or = 0, bar_and = 1, bar_result = 0;  // __syncthreads_or / _and of the barrier being filled, and of the last one
+    std::vector<unsigned char> smem;              // dynamic shared memory
     std::function<void()> body;
 };
 
 static Block* g_block = nullptr;
+static void* g_sched = nullptr;  // the scheduler's saved stack pointer
+static unsigned long long g_clock = 0;  // clock64(): a counter, monotonic per process
 
 // the interleaving mode (see the header comment)
 struct Interleave {
@@ -143,7 +234,7 @@ static uint64_t next_random() {  // splitmix64
 
 static void yield() {
     Block* b = g_block;
-    swapcontext(&b->fibers[b->current].ctx, &b->sched);
+    simt_fiber_switch(&b->fibers[b->current].sp, g_sched);
 }
 
 // A switch point: with the interleaving mode on, inside a launch, give way to the other fibers with probability p.  A
@@ -156,16 +247,24 @@ static void interleave_point() {
     yield();
 }
 
+static void nap() {
+    Block* b = g_block;
+    if (!b) return;
+    b->naps++;
+    yield();
+}
+
 static void trampoline() {
     Block* b = g_block;
     b->body();
+    b = g_block;
     Fiber& f = b->fibers[b->current];
     f.done = true;
     b->live--;
     b->progress++;
     const unsigned lane = f.tid & 31u;
     if (b->warps[f.tid >> 5].pending & (1u << lane)) die("a thread exited inside a warp rendezvous");
-    swapcontext(&f.ctx, &b->sched);
+    simt_fiber_switch(&f.sp, g_sched);  // never resumed
 }
 
 static unsigned long long compute(const Warp& w, int op, unsigned lane, unsigned mask) {
@@ -199,6 +298,10 @@ static unsigned long long compute(const Warp& w, int op, unsigned lane, unsigned
             const unsigned src = w.aux[lane] & 31u;
             return (mask >> src & 1u) ? w.val[src] : w.val[lane];
         }
+        case OP_SHFL_UP: {  // lanes below delta keep their own value
+            const unsigned d = w.aux[lane];
+            return (lane >= d && (mask >> (lane - d) & 1u)) ? w.val[lane - d] : w.val[lane];
+        }
         default: return 0;
     }
 }
@@ -231,16 +334,23 @@ static unsigned long long rendezvous(int op, unsigned mask, unsigned long long v
     return w.res[lane];
 }
 
-static void syncthreads() {
+// a block barrier; op 1 / 2 also reduces pred over the block (__syncthreads_or / __syncthreads_and)
+static int syncthreads(int op = 0, int pred = 0) {
     Block* b = g_block;
     const unsigned gen = b->bar_gen;
     b->progress++;
+    if (pred) b->bar_or = 1;
+    else b->bar_and = 0;
     if (++b->bar_arrived == b->live) {
+        b->bar_result = op == 1 ? b->bar_or : b->bar_and;
         b->bar_arrived = 0;
+        b->bar_or = 0;
+        b->bar_and = 1;
         b->bar_gen++;
     } else {
         while (b->bar_gen == gen) yield();
     }
+    return op ? g_block->bar_result : 0;
 }
 
 }  // namespace simt
@@ -252,7 +362,16 @@ static inline unsigned __reduce_min_sync(unsigned mask, unsigned v) { return (un
 static inline unsigned __reduce_max_sync(unsigned mask, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_REDUCE_MAX, mask, v); }
 static inline unsigned __shfl_sync(unsigned mask, unsigned v, int src) { return (unsigned)simt::rendezvous(simt::OP_SHFL, mask, v, (unsigned)src); }
 static inline void __syncwarp(unsigned mask = 0xFFFFFFFFu) { simt::rendezvous(simt::OP_SYNCWARP, mask, 0); }
+static inline unsigned __shfl_up_sync(unsigned mask, unsigned v, unsigned delta) {
+    return (unsigned)simt::rendezvous(simt::OP_SHFL_UP, mask, v, delta);
+}
 static inline void __syncthreads() { simt::syncthreads(); }
+static inline int __syncthreads_or(int pred) { return simt::syncthreads(1, pred); }
+static inline int __syncthreads_and(int pred) { return simt::syncthreads(2, pred); }
+static inline void __nanosleep(unsigned) { simt::nap(); }
+static inline long long clock64() { return (long long)++simt::g_clock; }
+// the running block's dynamic shared memory
+static inline void* simt_dyn_smem() { return simt::g_block->smem.data(); }
 
 // Turn the interleaving mode on (seed, switch probability p in (0, 1]) or off.
 static inline void simt_interleave(bool on, uint64_t seed = 0, double p = 1.0) {
@@ -261,48 +380,120 @@ static inline void simt_interleave(bool on, uint64_t seed = 0, double p = 1.0) {
     simt::g_interleave.state = seed;
 }
 
+namespace simt {
+constexpr size_t kStack = 128 * 1024;
+constexpr unsigned kSpinPasses = 256;  // passes of nothing but waiting before a launch is reported as hung
+static std::vector<char*> g_stacks;    // free stacks, reused across blocks and launches
+
+static std::unique_ptr<Block> start_block(unsigned bx, unsigned block, size_t smem, const std::function<void()>& body) {
+    std::unique_ptr<Block> B(new Block());
+    B->idx = bx;
+    B->body = body;
+    B->fibers.resize(block);
+    B->warps.resize((block + 31) / 32);
+    B->live = block;
+    B->smem.assign(smem, 0xA5);  // poison: the GPU does not zero shared memory
+    for (unsigned t = 0; t < block; t++) {
+        Fiber& f = B->fibers[t];
+        f.tid = t;
+        if (g_stacks.empty()) {
+            f.stack = new char[kStack];
+        } else {
+            f.stack = g_stacks.back();
+            g_stacks.pop_back();
+        }
+        // the first switch to the fiber pops six zero registers and "returns" into trampoline with the stack
+        // aligned as after a call
+        uintptr_t top = ((uintptr_t)(f.stack + kStack)) & ~(uintptr_t)15;
+        void** sp = reinterpret_cast<void**>(top - 16);
+        sp[0] = reinterpret_cast<void*>(&trampoline);
+        sp[1] = nullptr;
+        sp -= 6;
+        for (int k = 0; k < 6; k++) sp[k] = nullptr;
+        f.sp = sp;
+    }
+    return B;
+}
+static void end_block(Block& B) {
+    for (Fiber& f : B.fibers) g_stacks.push_back(f.stack);
+    B.fibers.clear();
+}
+}  // namespace simt
+
+// run body() once per thread of a <<<grid, block, smem>>> launch with up to `resident` blocks live at a time (see the
+// header comment); each block gets `smem` bytes of dynamic shared memory
+template <class F>
+static void simt_launch_ex(unsigned grid, unsigned block, size_t smem, unsigned resident, F&& body) {
+    gridDim.x = grid;
+    blockDim.x = block;
+    if (resident < 1) resident = 1;
+    const std::function<void()> fn = body;
+    std::vector<std::unique_ptr<simt::Block>> slots;
+    unsigned next = 0, spin = 0;
+    std::vector<std::pair<unsigned, unsigned>> order;
+    std::vector<unsigned long long> before, naps_before;
+    for (;;) {
+        // dispatch: an exited block's place goes to the next block of the grid
+        for (auto it = slots.begin(); it != slots.end();) {
+            if ((*it)->live == 0) {
+                simt::end_block(**it);
+                it = slots.erase(it);
+            } else {
+                ++it;
+            }
+        }
+        while (slots.size() < resident && next < grid) slots.push_back(simt::start_block(next++, block, smem, fn));
+        if (slots.empty()) break;
+        // one pass: every live fiber of every resident block gets a turn; the threads of a block start from a thread
+        // that depends on the block (no lane is always first); in the interleaving mode the pass takes all the
+        // fibers in a fresh random order
+        order.clear();
+        for (unsigned s = 0; s < slots.size(); s++)
+            for (unsigned k = 0; k < block; k++) order.emplace_back(s, (k + slots[s]->idx) % block);
+        if (simt::g_interleave.on)
+            for (size_t k = order.size(); k > 1; k--) std::swap(order[k - 1], order[simt::next_random() % k]);
+        before.resize(slots.size());
+        naps_before.resize(slots.size());
+        for (unsigned s = 0; s < slots.size(); s++) {
+            before[s] = slots[s]->progress;
+            naps_before[s] = slots[s]->naps;
+        }
+        for (const auto& o : order) {
+            simt::Block& B = *slots[o.first];
+            simt::Fiber& f = B.fibers[o.second];
+            if (f.done) continue;
+            B.current = o.second;
+            simt::g_block = &B;
+            blockIdx.x = B.idx;
+            threadIdx.x = o.second;
+            simt_fiber_switch(&simt::g_sched, f.sp);
+        }
+        simt::g_block = nullptr;
+        bool worked = false, napped = false;
+        for (unsigned s = 0; s < slots.size(); s++) {
+            simt::Block& B = *slots[s];
+            const bool moved = B.progress != before[s], slept = B.naps != naps_before[s];
+            blockIdx.x = B.idx;
+            threadIdx.x = B.current;
+            if (B.live && !moved && !slept) simt::die("no thread of the block can make progress (a barrier or a *_sync some threads never reach)");
+            if (slept) napped = true;
+            else if (moved) worked = true;
+        }
+        spin = (napped && !worked) ? spin + 1 : 0;
+        if (spin > simt::kSpinPasses) {
+            for (auto& b : slots)
+                if (b->naps) {
+                    blockIdx.x = b->idx;
+                    threadIdx.x = b->current;
+                    break;
+                }
+            simt::die("a block waits in a __nanosleep loop that no resident block makes progress towards (a hang on a GPU)");
+        }
+    }
+}
+
 // run body() once per thread of a <<<grid, block>>> launch: blocks one after the other, the threads of a block as fibers
 template <class F>
 static void simt_launch(unsigned grid, unsigned block, F&& body) {
-    gridDim.x = grid;
-    blockDim.x = block;
-    for (unsigned bx = 0; bx < grid; bx++) {
-        simt::Block B;
-        B.body = body;
-        B.fibers.resize(block);
-        B.warps.resize((block + 31) / 32);
-        B.live = block;
-        simt::g_block = &B;
-        for (unsigned t = 0; t < block; t++) {
-            simt::Fiber& f = B.fibers[t];
-            f.tid = t;
-            constexpr size_t kStack = 64 * 1024;
-            f.stack.reset(new char[kStack]);
-            getcontext(&f.ctx);
-            f.ctx.uc_stack.ss_sp = f.stack.get();
-            f.ctx.uc_stack.ss_size = kStack;
-            f.ctx.uc_link = nullptr;
-            makecontext(&f.ctx, simt::trampoline, 0);
-        }
-        std::vector<unsigned> order(block);
-        while (B.live) {
-            const unsigned long long before = B.progress;
-            // the threads take turns, starting from a thread that depends on the block: no lane is always first; in the
-            // interleaving mode every pass takes them in a fresh random order
-            for (unsigned k = 0; k < block; k++) order[k] = (k + bx) % block;
-            if (simt::g_interleave.on)
-                for (unsigned k = block; k > 1; k--) std::swap(order[k - 1], order[simt::next_random() % k]);
-            for (unsigned k = 0; k < block; k++) {
-                const unsigned t = order[k];
-                simt::Fiber& f = B.fibers[t];
-                if (f.done) continue;
-                B.current = t;
-                blockIdx.x = bx;
-                threadIdx.x = t;
-                swapcontext(&B.sched, &f.ctx);
-            }
-            if (B.live && B.progress == before) simt::die("no thread of the block can make progress (a barrier or a *_sync some threads never reach)");
-        }
-        simt::g_block = nullptr;
-    }
+    simt_launch_ex(grid, block, 0, 1, body);
 }

@@ -2,8 +2,8 @@
 // fallback).  It runs the same rl_core.h functions the sm_90a kernels run — request
 // resolution into row accesses, per-row stream-order replay, and the fixed-point rounds
 // for multi-row requests — so the algorithm can be checked against the oracle on a
-// machine without a GPU.  GPU-only mechanics (partition, smem grouping, CAS inserts) are
-// covered by the -m gpu tests.  Both position encodings of rl_core.h run through the one
+// machine without a GPU.  The kernels' own mechanics (partition, smem grouping, CAS inserts,
+// the chained commit) run on the host in emu_engine.cpp, and on the GPU in the -m gpu tests.  Both position encodings of rl_core.h run through the one
 // driver: narrow (up to 16 counters per request) and wide (up to 64).
 #include <cstdint>
 #include <cstring>

@@ -1,0 +1,558 @@
+// emu_engine.cpp — TEST-ONLY host driver of the decision kernels (limitador_b200/csrc/rl_kernels.cuh: k_front, k_hot,
+// k_main, the resolve kernels, k_restore, k_fl_step, k_wide_scatter, k_scan) under tests/emu/cuda_simt.h: the SAME
+// kernel source the GPU runs, every CUDA thread a fiber, warp intrinsics as rendezvous, up to R k_main blocks resident at
+// once.  Not shipped, not a fallback.  The call sequences follow rl_engine.cu (run_record_pipeline without the pipeline,
+// run_acc_pipeline), the batch geometry is rl_batch_geom itself, and every call reports the geometry it reached.
+#include "cuda_simt.h"
+// (the emulator must come first: it defines __global__ & co. away)
+#include <algorithm>
+#include <array>
+#include <cstring>
+#include <map>
+#include <vector>
+
+#include "../../limitador_b200/csrc/rl_kernels.cuh"
+
+namespace {
+
+struct Limit {
+    bool defined = false;
+    uint32_t ns = 0, varset = 0, qualified = 0, group = 0, cell = 0;
+    uint64_t max_value = 0, window_us = 0;
+};
+
+// what the report says about a call (indices of emu_engine's report array)
+enum {
+    G_TILES, G_TILE, G_MERGE_MAIN, G_MERGE_HOT, G_NPARTS, G_ITEMS, G_HEAVY_ITEMS, G_MAX_W, G_HOT_IN_USE, G_HOT_CAND,
+    G_HOT_MAX_LIST, G_HOT_SWEEPS, G_FP_ROUNDS, G_CHUNKS, G_ROUNDS, G_CHAINED, G_ORDERED, G_HOT_AFTER, G_MAX_PART,
+    G_CH, G_REARMED, G_N
+};
+
+}  // namespace
+
+struct emu_engine {
+    uint32_t cells = 1, log2P = 0, log2R = 0, row_bytes = 32;
+    std::vector<uint8_t> rows;
+    // registry and device tables (rl_limits_set / upload_tables)
+    std::vector<Limit> limits;
+    std::vector<std::array<uint32_t, RL_MAX_CELLS>> groups{std::array<uint32_t, RL_MAX_CELLS>{}};
+    std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> groups_by_key;
+    std::vector<std::vector<uint32_t>> ns_limits;
+    std::vector<RlCellDesc> desc;
+    std::vector<RlLimitDev> lim;
+    std::vector<RlNsDev> ns;
+    std::vector<uint32_t> ns_ids, group_ns;
+    uint32_t max_cells_used = 1, max_ns_limits = 0;
+    bool any_multi_ns = false;
+    // knobs
+    uint32_t chunk = 128, part_target = 128, heavy_mult = 2, main_grid_cap = 132 * 16, weak = 0, hot_on = 0, resident = 1;
+    uint32_t n_dev = 0;  // sharded geometry: the access count lives on the device, the tile is derived there
+    bool interleave = false;
+    uint64_t seed = 0;
+    double p = 1.0;
+    // device state that lives across calls
+    std::vector<uint32_t> hot;  // hot_rows [RL_HOT_SLOTS] | hot_cand [RL_HOT_CAND] | hot_cand_n | pad
+    std::vector<uint32_t> region_total, small;
+    uint32_t err = 0, flags = 0, changed = 0;
+    unsigned long long kstats[32] = {};
+    unsigned long long report[G_N] = {};
+};
+
+namespace {
+
+// rl_limits_set (rl_engine.cu:1004-1064): limits of one (namespace, variable set) share a row group with a free cell
+int limits_set(emu_engine* e, const rl_limit_desc* d, uint32_t n) {
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t q = d[i].qualified ? 1 : 0, varset = q ? d[i].varset_id : 0;
+        if (d[i].limit_id >= e->limits.size()) e->limits.resize(d[i].limit_id + 1);
+        Limit& l = e->limits[d[i].limit_id];
+        if (l.defined) {  // identity fixed, max_value swapped
+            l.max_value = d[i].max_value;
+            continue;
+        }
+        auto& glist = e->groups_by_key[{d[i].ns_id, varset}];
+        uint32_t g = 0, c = 0;
+        for (uint32_t cand : glist) {
+            for (uint32_t k = 0; k < e->cells; k++)
+                if (e->groups[cand][k] == RL_NONE_U32) {
+                    g = cand;
+                    c = k;
+                    break;
+                }
+            if (g) break;
+        }
+        if (!g) {
+            g = (uint32_t)e->groups.size();
+            std::array<uint32_t, RL_MAX_CELLS> none;
+            none.fill(RL_NONE_U32);
+            e->groups.push_back(none);
+            glist.push_back(g);
+        }
+        e->groups[g][c] = d[i].limit_id;
+        l = Limit{true, d[i].ns_id, varset, q, g, c, d[i].max_value, d[i].window_us};
+        if (d[i].ns_id >= e->ns_limits.size()) e->ns_limits.resize(d[i].ns_id + 1);
+        e->ns_limits[d[i].ns_id].push_back(d[i].limit_id);
+    }
+    return 0;
+}
+
+// upload_tables (rl_engine.cu:203-287): cell descriptors per row group, limits, namespaces (single-row namespaces
+// get mode 1 and their packed cell list, the others mode 2)
+void upload_tables(emu_engine* e) {
+    const size_t ngroups = e->groups.size();
+    e->desc.assign(ngroups * 8, RlCellDesc{0, 0, RL_NONE_U32, 0});
+    e->group_ns.assign(ngroups, 0);
+    e->max_cells_used = 1;
+    for (size_t g = 1; g < ngroups; g++) {
+        for (uint32_t c = 0; c < RL_MAX_CELLS; c++) {
+            const uint32_t lid = e->groups[g][c];
+            if (lid == RL_NONE_U32) continue;
+            e->max_cells_used = std::max(e->max_cells_used, c + 1);
+            const Limit& l = e->limits[lid];
+            e->group_ns[g] = l.ns;
+            e->desc[g * 8 + c] = RlCellDesc{l.max_value, l.window_us, lid, l.qualified};
+        }
+    }
+    e->lim.assign(std::max<size_t>(e->limits.size(), 1), RlLimitDev{0, 0, 0, 0});
+    for (size_t i = 0; i < e->limits.size(); i++)
+        if (e->limits[i].defined) e->lim[i] = RlLimitDev{e->limits[i].group, e->limits[i].cell, e->limits[i].ns, e->limits[i].qualified};
+    e->ns.assign(std::max<size_t>(e->ns_limits.size(), 1), RlNsDev{});
+    e->ns_ids.clear();
+    e->any_multi_ns = false;
+    e->max_ns_limits = 0;
+    for (size_t n = 0; n < e->ns_limits.size(); n++) {
+        memset(&e->ns[n], 0, sizeof(RlNsDev));
+        const auto& L = e->ns_limits[n];
+        if (L.empty()) continue;
+        e->ns[n].lim_off = (uint32_t)e->ns_ids.size();
+        e->ns[n].lim_cnt = (uint32_t)L.size();
+        e->max_ns_limits = std::max<uint32_t>(e->max_ns_limits, (uint32_t)L.size());
+        bool single = L.size() <= RL_MAX_CELLS;
+        for (uint32_t lid : L) {
+            e->ns_ids.push_back(lid);
+            if (e->limits[lid].group != e->limits[L[0]].group) single = false;
+        }
+        if (single) {
+            e->ns[n].mode = 1;
+            e->ns[n].group = e->limits[L[0]].group;
+            e->ns[n].qualified_row = e->limits[L[0]].qualified;
+            uint32_t cells = 0;
+            for (size_t k = 0; k < L.size(); k++) cells |= e->limits[L[k]].cell << (4 * k);
+            e->ns[n].cells = cells | ((uint32_t)L.size() << 28);
+        } else {
+            e->ns[n].mode = 2;
+            e->any_multi_ns = true;
+        }
+    }
+    if (e->ns_ids.empty()) e->ns_ids.push_back(0);
+}
+
+RlDev make_dev(emu_engine* e) {
+    RlDev D;
+    D.rows = e->rows.data();
+    D.log2P = e->log2P;
+    D.log2R = e->log2R;
+    D.desc = e->desc.data();
+    D.limits = e->lim.data();
+    D.limits_cap = (uint32_t)e->lim.size();
+    D.ns = e->ns.data();
+    D.ns_cap = (uint32_t)e->ns.size();
+    D.ns_limit_ids = e->ns_ids.data();
+    D.err = &e->err;
+    D.flags = &e->flags;
+    D.kstats = e->kstats;
+    D.hot_rows = e->hot.data();
+    D.hot_cand = e->hot.data() + RL_HOT_SLOTS;
+    D.hot_cand_n = e->hot.data() + RL_HOT_SLOTS + RL_HOT_CAND;
+    D.trace = nullptr;
+    D.trace_pos = nullptr;
+    D.seq = 0;
+    return D;
+}
+
+// the per-batch workspace: poisoned where the GPU's would hold the previous batch's data; region totals and the
+// counters of `small` persist, as the kernels re-arm them
+struct Work {
+    std::vector<uint32_t> tile_loc, part_idx, part_row, row_of, chain_status, chain_wcnt, chain_w, fl_prev, fl_next;
+    std::vector<uint4> items;
+    std::vector<uint8_t*> log_row;
+    std::vector<ulonglong2> log_state;
+    uint32_t n_dev = 0;
+};
+
+RlBatch make_batch(emu_engine* e, Work& w, uint32_t n_acc, uint32_t n_req, uint8_t* lim, uint32_t* first, uint64_t* rem,
+                   uint64_t* ttl, const uint32_t* off, uint32_t stride, int lc, bool hot_ok) {
+    RlBatch B;
+    memset(&B, 0, sizeof B);
+    B.nhot = (hot_ok && e->hot_on) ? RL_HOT_SLOTS : 0;
+    B.n_acc = n_acc;
+    B.n_req = n_req;
+    const RlBatchGeom g = rl_batch_geom(n_acc, e->n_dev ? n_acc : 0, e->log2P, e->part_target, e->chunk, e->heavy_mult);
+    B.tile = g.tile;
+    B.num_tiles = g.num_tiles;
+    B.nparts = g.nparts;
+    B.part_shift = g.part_shift;
+    B.heavy_len = g.heavy_len;
+    if (e->n_dev) {
+        w.n_dev = n_acc;
+        B.n_dev = &w.n_dev;
+    }
+    const uint32_t P1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;
+    const uint32_t tsz = e->n_dev ? std::max<uint32_t>(256, ((rl_ceil_div(n_acc, g.num_tiles) + 255) / 256) * 256) : g.tile;
+    const size_t buf = (size_t)g.num_tiles * tsz;
+    const size_t max_items = (size_t)(1u << e->log2P) + n_acc / 128 + 2 + g.nparts;
+    w.tile_loc.assign((size_t)(g.num_tiles + 1) * (P1 + 1), 0xA5A5A5A5u);
+    w.part_idx.assign(buf, 0xA5A5A5A5u);
+    w.part_row.assign(buf, 0xA5A5A5A5u);
+    w.row_of.assign(std::max<uint32_t>(n_acc, 1), 0xA5A5A5A5u);
+    w.items.assign(max_items, uint4{0xA5A5A5A5u, 0xA5A5A5A5u, 0xA5A5A5A5u, 0xA5A5A5A5u});
+    w.chain_status.assign(max_items, 0xA5A5A5A5u);
+    w.chain_wcnt.assign(max_items, 0xA5A5A5A5u);
+    w.chain_w.assign(max_items * 256, 0xA5A5A5A5u);
+    w.fl_prev.assign(std::max<uint32_t>(n_req, 1), RL_NONE_U32);
+    w.fl_next.assign(std::max<uint32_t>(n_req, 1), RL_NONE_U32);
+    B.tile_loc = w.tile_loc.data();
+    B.region_total = e->region_total.data();
+    B.row_of = w.row_of.data();
+    B.part_idx = w.part_idx.data();
+    B.part_row = w.part_row.data();
+    B.scan_ctr = e->small.data() + 0;
+    B.n_items = e->small.data() + 1;
+    B.ticket = e->small.data() + 2;
+    B.exit_ctr = e->small.data() + 3;
+    B.out_limited = lim;
+    B.out_first_limited = first;
+    B.out_remaining = rem;
+    B.out_ttl = ttl;
+    B.out_off = off;
+    B.out_stride = stride;
+    B.fl_prev = w.fl_prev.data();
+    B.fl_next = w.fl_next.data();
+    B.phase = RL_PHASE_COMMIT;
+    B.load_counters = lc;
+    B.items = w.items.data();
+    B.chain_status = w.chain_status.data();
+    B.chain_wcnt = w.chain_wcnt.data();
+    B.chain_w = w.chain_w.data();
+    B.chunk = e->chunk;
+    return B;
+}
+
+void interleave_on(emu_engine* e, uint64_t salt) {
+    if (e->interleave) simt_interleave(true, e->seed * 0x9E3779B97F4A7C15ull + salt, e->p);
+}
+void interleave_off() { simt_interleave(false); }
+
+template <int CELLS, class Src>
+void front(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
+    interleave_on(e, 1);
+    simt_launch_ex(B.num_tiles, RL_PART_THREADS, rl_front_smem_bytes(B.nparts, B.nhot), 1, [&] { k_front<CELLS, Src>(D, B, src); });
+    interleave_off();
+}
+template <class Src>
+void launch_front(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
+    if (e->cells == 1) front<1>(e, D, B, src);
+    else if (e->cells == 3) front<3>(e, D, B, src);
+    else front<7>(e, D, B, src);
+}
+
+// what k_front's last block built: the work items, and the hot lists (partitions nparts ..)
+void report_front(emu_engine* e, const RlBatch& B, const Work& w) {
+    unsigned long long* g = e->report;
+    g[G_TILES] = B.num_tiles;
+    g[G_TILE] = B.n_dev ? std::max<uint32_t>(256, ((rl_ceil_div(*B.n_dev, B.num_tiles) + 255) / 256) * 256) : B.tile;
+    g[G_NPARTS] = B.nparts;
+    const uint32_t n_items = *B.n_items;
+    g[G_ITEMS] = n_items;
+    uint64_t heavy = 0, maxw = 0, maxpart = 0;
+    for (uint32_t i = 0; i < n_items; i++) {
+        const uint4 it = w.items[i];
+        if (it.w != RL_NONE_U32) {
+            heavy++;
+            maxw = std::max<uint64_t>(maxw, it.w);
+        }
+    }
+    const uint32_t TL = B.nparts + B.nhot + 2;
+    std::vector<uint64_t> len(B.nparts + B.nhot, 0);
+    for (uint32_t t = 0; t < B.num_tiles; t++)
+        for (uint32_t q = 0; q < B.nparts + B.nhot; q++) len[q] += w.tile_loc[(size_t)t * TL + q + 1] - w.tile_loc[(size_t)t * TL + q];
+    uint64_t hmax = 0, sweeps = 0;
+    for (uint32_t q = 0; q < B.nparts; q++) maxpart = std::max(maxpart, len[q]);
+    for (uint32_t h = 0; h < B.nhot; h++) {
+        hmax = std::max(hmax, len[B.nparts + h]);
+        sweeps = std::max<uint64_t>(sweeps, rl_ceil_div(len[B.nparts + h], RL_HOT_SWEEP));
+    }
+    g[G_HEAVY_ITEMS] = heavy;
+    g[G_MAX_W] = maxw;
+    g[G_HOT_MAX_LIST] = hmax;
+    g[G_HOT_SWEEPS] = sweeps;  // at least: the longest list's whole-list sweeps
+    g[G_MAX_PART] = maxpart;
+    g[G_MERGE_HOT] = B.nhot ? rl_ceil_div(B.num_tiles, RL_HOT_THREADS) : 0;
+}
+
+template <int GEO, int CELLS, class Src, int MODE, bool LC, int CH>
+void main_ch(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
+    const uint32_t grid = rl_main_grid(B.nparts, B.n_acc, CH, e->main_grid_cap);
+    e->report[G_CH] = CH;
+    e->report[G_MERGE_MAIN] = rl_ceil_div(B.num_tiles, CH);
+    interleave_on(e, 3 + (uint64_t)B.phase);
+    simt_launch_ex(grid, CH, rl_main_smem_bytes<CELLS, CH>(B.num_tiles), e->resident,
+                   [&] { k_main<GEO, CELLS, Src, MODE, CH, LC>(D, B, src, e->weak); });
+    interleave_off();
+}
+
+template <int GEO, int CELLS, class Src, int MODE, bool LC>
+void main_lc(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
+    if constexpr (Src::kWide) {
+        main_ch<GEO, CELLS, Src, MODE, LC, 128>(e, D, B, src);  // wide batches: no hot rows, 128-access chunks
+    } else {
+        if (B.nhot && B.phase == RL_PHASE_COMMIT) {
+            // k_hot has static shared memory: one block at a time
+            interleave_on(e, 2);
+            simt_launch_ex(B.nhot, RL_HOT_THREADS, 0, 1, [&] { k_hot<GEO, CELLS, Src, MODE, LC>(D, B, src); });
+            interleave_off();
+        }
+        if (e->chunk == 128) main_ch<GEO, CELLS, Src, MODE, LC, 128>(e, D, B, src);
+        else main_ch<GEO, CELLS, Src, MODE, LC, 256>(e, D, B, src);
+    }
+}
+
+// launch_main (rl_engine.cu:472-496): 1/1, 3/3, then 7/4 while at most 4 cells of a 7-cell row are in use, else 7/7
+template <class Src, int MODE>
+void launch_main(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
+    const bool lc = MODE == 0 && B.load_counters;
+#define EMU_MAIN_CASE(G, A) \
+    (lc ? main_lc<G, A, Src, MODE, MODE == 0>(e, D, B, src) : main_lc<G, A, Src, MODE, false>(e, D, B, src))
+    if (e->cells == 1) EMU_MAIN_CASE(1, 1);
+    else if (e->cells == 3) EMU_MAIN_CASE(3, 3);
+    else if (e->max_cells_used <= 4) EMU_MAIN_CASE(7, 4);
+    else EMU_MAIN_CASE(7, 7);
+#undef EMU_MAIN_CASE
+}
+
+void begin_call(emu_engine* e) {
+    memset(e->report, 0, sizeof e->report);
+    memset(e->kstats, 0, sizeof e->kstats);
+    e->err = 0;
+    e->flags = 0;
+    for (uint32_t h = 0; h < RL_HOT_SLOTS; h++) e->report[G_HOT_IN_USE] += e->hot[h] != 0xFFFFFFFFu;
+}
+int end_call(emu_engine* e) {
+    unsigned long long* g = e->report;
+    g[G_CHUNKS] = e->kstats[0];
+    g[G_ROUNDS] = e->kstats[1];
+    g[G_CHAINED] = e->kstats[2];
+    g[G_ORDERED] = e->kstats[3];
+    g[G_HOT_CAND] = e->hot[RL_HOT_SLOTS + RL_HOT_CAND];  // reported by this call's k_main, read by the next front
+    for (uint32_t h = 0; h < RL_HOT_SLOTS; h++) g[G_HOT_AFTER] += e->hot[h] != 0xFFFFFFFFu;
+    // the counters the kernels re-arm for the next batch
+    bool rearmed = e->small[0] == 0 && e->small[2] == 0 && e->small[3] == 0;
+    for (uint32_t v : e->region_total) rearmed = rearmed && v == 0;
+    g[G_REARMED] = rearmed;
+    return (int)e->err;
+}
+
+// run_acc_pipeline (rl_engine.cu:514-587): accesses that may hold coupled (multi-row) requests.  check_and_update with
+// coupled requests: SNAPSHOT, SPEC rounds (k_restore, k_fl_step) until the first-limited positions settle, COMMIT.
+int acc_pipeline(emu_engine* e, RlDev& D, std::vector<RlAccess>& acc, uint32_t n_req, const uint64_t* delta,
+                 const uint64_t* now, int mode, int lc, uint8_t* lim, uint32_t* first, uint64_t* rem, uint64_t* ttl,
+                 const uint32_t* off, uint32_t stride, bool wide, const std::vector<uint8_t>& perm, uint32_t acc_stride) {
+    const uint32_t n_acc = (uint32_t)acc.size();
+    const bool scatter = wide && mode == 0 && lc && (rem || ttl);
+    std::vector<uint64_t> wrem(scatter ? n_acc + 1 : 0), wttl(scatter ? n_acc + 1 : 0);
+    Work w;
+    RlBatch B = make_batch(e, w, n_acc, n_req, lim, first, scatter && rem ? wrem.data() : rem, scatter && ttl ? wttl.data() : ttl,
+                           off, scatter && !off ? acc_stride : stride, lc, mode != 0);
+    if (mode == 0) B.heavy_len = 0xFFFFFFFFu;
+    AccSrc src{acc.data(), delta, now};
+    launch_front(e, D, B, src);
+    report_front(e, B, w);
+    if (mode == 2) {
+        launch_main<AccSrc, 2>(e, D, B, src);
+        return 0;
+    }
+    auto main0 = [&]() {
+        if (wide) launch_main<AccSrcWide, 0>(e, D, B, AccSrcWide{src});
+        else launch_main<AccSrc, 0>(e, D, B, src);
+    };
+    if (e->flags & 1u) {
+        e->flags = 0;
+        const uint32_t buf_len = B.num_tiles * B.tile;
+        w.log_row.assign(buf_len, nullptr);
+        w.log_state.assign((size_t)buf_len * e->cells, ulonglong2{0xA5A5A5A5A5A5A5A5ull, 0xA5A5A5A5A5A5A5A5ull});
+        B.log_row = w.log_row.data();
+        B.log_state = w.log_state.data();
+        B.phase = RL_PHASE_SNAPSHOT;
+        main0();
+        for (uint32_t round = 0;; round++) {
+            if (round > n_req + 2) return -1;  // did not converge
+            e->changed = 0;
+            B.phase = RL_PHASE_SPEC;
+            main0();
+            const uint32_t act = e->cells == 7 && e->max_cells_used <= 4 ? 4 : e->cells;
+            const uint32_t blocks = rl_ceil_div(buf_len, 256);
+            if (e->cells == 1) simt_launch(blocks, 256, [&] { k_restore<1>(buf_len, act, B.log_row, B.log_state); });
+            else if (e->cells == 3) simt_launch(blocks, 256, [&] { k_restore<3>(buf_len, act, B.log_row, B.log_state); });
+            else simt_launch(blocks, 256, [&] { k_restore<7>(buf_len, act, B.log_row, B.log_state); });
+            simt_launch(rl_ceil_div(n_req, 256), 256, [&] { k_fl_step(n_req, B.fl_prev, B.fl_next, &e->changed); });
+            e->report[G_FP_ROUNDS] = round + 1;
+            if (!(e->changed & 1u)) break;
+        }
+    }
+    B.phase = RL_PHASE_COMMIT;
+    main0();
+    if (scatter)
+        simt_launch(rl_ceil_div(n_req, 128), 128, [&] {
+            k_wide_scatter(n_req, off, acc_stride, stride, perm.data(), rem ? wrem.data() : nullptr, ttl ? wttl.data() : nullptr, rem, ttl);
+        });
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+// capacity = 2^(log2P + log2R) rows of cells (1, 3 or 7) cells
+emu_engine* emu_engine_create(uint32_t cells, uint32_t log2P, uint32_t log2R) {
+    emu_engine* e = new emu_engine();
+    e->cells = cells;
+    e->log2P = log2P;
+    e->log2R = log2R;
+    e->row_bytes = 16 * (1 + cells);
+    e->rows.assign(((size_t)1 << (log2P + log2R)) * e->row_bytes, 0);
+    e->hot.assign(RL_HOT_SLOTS + RL_HOT_CAND + 4, 0xFFFFFFFFu);  // rl_internal_reset_hot_rows
+    for (uint32_t i = RL_HOT_SLOTS + RL_HOT_CAND; i < e->hot.size(); i++) e->hot[i] = 0;
+    e->region_total.assign((1u << log2P) + RL_HOT_SLOTS + 2, 0);
+    e->small.assign(8, 0);
+    return e;
+}
+void emu_engine_destroy(emu_engine* e) { delete e; }
+
+int emu_engine_limits_set(emu_engine* e, const rl_limit_desc* d, uint32_t n) {
+    const int r = limits_set(e, d, n);
+    upload_tables(e);
+    return r;
+}
+
+// knobs: chunk (128/256), heavy_mult, part_target, hot rows, weak tags, sharded geometry, resident k_main blocks, grid cap
+void emu_engine_knobs(emu_engine* e, uint32_t chunk, uint32_t heavy_mult, uint32_t part_target, uint32_t hot, uint32_t weak,
+                      uint32_t n_dev, uint32_t resident, uint32_t main_grid_cap) {
+    e->chunk = chunk;
+    e->heavy_mult = heavy_mult;
+    e->part_target = part_target;
+    e->hot_on = hot;
+    e->weak = weak;
+    e->n_dev = n_dev;
+    e->resident = resident;
+    e->main_grid_cap = main_grid_cap;
+}
+// cuda_simt.h's interleaving mode for every launch of the calls that follow (the n-th launch of a call salts the seed)
+void emu_engine_interleave(emu_engine* e, int on, uint64_t seed, double p) {
+    e->interleave = on != 0;
+    e->seed = seed;
+    e->p = p;
+}
+const unsigned long long* emu_engine_report(emu_engine* e) { return e->report; }
+uint32_t emu_engine_max_cells_used(emu_engine* e) { return e->max_cells_used; }
+// the table region of record r's row (single-row namespaces), or -1 when the record has no row
+int64_t emu_engine_record_region(emu_engine* e, const rl_record* r) {
+    if (r->ns_id >= e->ns.size() || e->ns[r->ns_id].mode != 1) return -1;
+    const RlNsDev& ns = e->ns[r->ns_id];
+    const uint64_t klo = ns.qualified_row ? r->key_lo : 0;
+    const uint64_t hhi = ((uint64_t)ns.group << 32) | (ns.qualified_row ? (r->key_hi & 0xFFFFFFFFull) : 0);
+    const uint64_t h = rl_row_hash(klo, hhi);
+    return e->log2P ? (int64_t)(h >> (64 - e->log2P)) : 0;
+}
+// remaining / ttl slots per record: the most limits of a namespace when some namespace spans several rows, else the
+// cells of a row (what rl_check_and_update_records' callers pass by default)
+uint32_t emu_engine_record_stride(emu_engine* e) { return e->any_multi_ns ? std::max<uint32_t>(1, e->max_ns_limits) : e->cells; }
+
+// check_and_update (mode 0) / update_counters (mode 2) over 32-byte records: run_record_pipeline (rl_engine.cu:600-677)
+// without the pipeline — k_front, k_hot when hot rows are on, k_main — or, when some namespace spans several rows, the
+// records resolved into accesses (k_resolve_records, narrow or wide) and run_acc_pipeline.  rem / ttl: [n * stride]
+// with stride = emu_engine_record_stride.  Returns the device error code.
+int emu_engine_records(emu_engine* e, int mode, uint32_t n, const rl_record* recs, int lc, uint8_t* lim, uint32_t* first,
+                       uint64_t* rem, uint64_t* ttl) {
+    begin_call(e);
+    RlDev D = make_dev(e);
+    if (e->any_multi_ns) {
+        const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
+        const bool wide = stride > RL_MAX_CTRS_PER_REQ;
+        std::vector<RlAccess> acc((size_t)n * stride);
+        std::vector<uint64_t> delta(std::max<uint32_t>(n, 1)), now(std::max<uint32_t>(n, 1));
+        std::vector<uint8_t> perm(wide ? acc.size() + 1 : 0);
+        RlResolveOut O{acc.data(), delta.data(), now.data(), lim, first};
+        const uint32_t blocks = rl_ceil_div(n, 128);
+        if (wide) simt_launch(blocks, 128, [&] { k_resolve_records_wide(D, n, recs, stride, O, mode == 0, perm.data(), RL_MAX_CTRS_PER_REQ_WIDE); });
+        else simt_launch(blocks, 128, [&] { k_resolve_records(D, n, recs, stride, O, mode == 0); });
+        if (e->err) return (int)e->err;
+        if (acc_pipeline(e, D, acc, n, delta.data(), now.data(), mode, lc, lim, first, rem, ttl, nullptr, stride, wide, perm, stride))
+            return -1;
+        return end_call(e);
+    }
+    Work w;
+    RlBatch B = make_batch(e, w, n, n, lim, first, rem, ttl, nullptr, e->cells, lc, true);
+    RecordSrc src{recs, nullptr, 0, 0, 0, 0};
+    launch_front(e, D, B, src);
+    report_front(e, B, w);
+    if (mode == 2) launch_main<RecordSrc, 2>(e, D, B, src);
+    else launch_main<RecordSrc, 0>(e, D, B, src);
+    return end_call(e);
+}
+
+// check_and_update / update_counters in the general (CSR) form: k_resolve_csr (or _wide when a request has more than 16
+// counters) and run_acc_pipeline.  rem / ttl: [off[n]].
+int emu_engine_csr(emu_engine* e, int mode, uint32_t n, const uint32_t* off, const rl_counter* ctrs, const uint64_t* delta,
+                   const uint64_t* now, int lc, uint8_t* lim, uint32_t* first, uint64_t* rem, uint64_t* ttl) {
+    begin_call(e);
+    RlDev D = make_dev(e);
+    uint32_t maxm = 0;
+    for (uint32_t i = 0; i < n; i++) maxm = std::max(maxm, off[i + 1] - off[i]);
+    const bool wide = maxm > RL_MAX_CTRS_PER_REQ;
+    std::vector<RlAccess> acc(off[n]);
+    std::vector<uint8_t> perm(wide ? off[n] + 1 : 0);
+    RlResolveOut O{acc.data(), nullptr, nullptr, lim, first};
+    const uint32_t blocks = rl_ceil_div(n, 128);
+    if (wide) simt_launch(blocks, 128, [&] { k_resolve_csr_wide(D, n, off, ctrs, O, mode == 0, perm.data(), RL_MAX_CTRS_PER_REQ_WIDE); });
+    else simt_launch(blocks, 128, [&] { k_resolve_csr(D, n, off, ctrs, O, mode == 0); });
+    if (e->err) return (int)e->err;
+    if (acc.empty()) return end_call(e);
+    if (acc_pipeline(e, D, acc, n, delta, now, mode, lc, lim, first, rem, ttl, off, 0, wide, perm, 0)) return -1;
+    return end_call(e);
+}
+
+// is_within_limits over records (k_query_records): read-only
+int emu_engine_query_records(emu_engine* e, uint32_t n, const rl_record* recs, uint8_t* lim, uint32_t* first) {
+    begin_call(e);
+    RlDev D = make_dev(e);
+    auto run = [&](auto c) {
+        constexpr int C = decltype(c)::value;
+        simt_launch(rl_ceil_div(n, 128), 128, [&] { k_query_records<C>(D, n, recs, lim, first); });
+    };
+    if (e->cells == 1) run(std::integral_constant<int, 1>{});
+    else if (e->cells == 3) run(std::integral_constant<int, 3>{});
+    else run(std::integral_constant<int, 7>{});
+    return (int)e->err;
+}
+
+// the table through k_scan in export mode (read_table, rl_engine.cu:1149-1219, now = 0: every present cell as
+// (value, expiry)); the present unqualified limits no row showed are left out, as a never-touched counter.
+uint64_t emu_engine_export(emu_engine* e, uint64_t cap, uint32_t* lid, uint64_t* lo, uint64_t* hi, uint64_t* val, uint64_t* exp) {
+    RlDev D = make_dev(e);
+    const uint32_t L = (uint32_t)e->lim.size();
+    std::vector<uint8_t> flags(2 * (size_t)L, 0);
+    for (size_t l = 0; l < e->limits.size(); l++) flags[l] = e->limits[l].defined;
+    unsigned long long cnt = 0;
+    RlScanOut O{lid, lo, hi, val, exp, &cnt, cap, flags.data(), flags.data() + L};
+    const uint64_t nrows = e->rows.size() / e->row_bytes;
+    auto run = [&](auto c) {
+        constexpr int C = decltype(c)::value;
+        simt_launch(rl_ceil_div(nrows, 256), 256, [&] { k_scan<C>(D, nrows, false, 0, nullptr, e->group_ns.data(), O); });
+    };
+    if (e->cells == 1) run(std::integral_constant<int, 1>{});
+    else if (e->cells == 3) run(std::integral_constant<int, 3>{});
+    else run(std::integral_constant<int, 7>{});
+    return cnt;
+}
+
+}  // extern "C"

@@ -2,7 +2,10 @@
 // barrier against closed forms, and — run with an argument — the three mistakes it must refuse (they are hangs or undefined
 // behaviour on a GPU): a *_sync mask naming an exited lane, lanes disagreeing on the mask, a barrier not every thread reaches.
 // Also the interleaving mode: a read-modify-write made of a plain load and store with a switch point between them must lose
-// updates under it, and the same update as an atomic must not — the mode can show a race at all.
+// updates under it, and the same update as an atomic must not — the mode can show a race at all.  And what the decision
+// kernels need: __shfl_up_sync scans, the reducing barriers, atomicOr, min / max on mixed types, uint4, static
+// __shared__ arrays, per-block dynamic shared memory that starts poisoned, and resident blocks: block 0 waits in a
+// __nanosleep loop for a flag block 1 sets, which finishes with two resident blocks and is reported as a hang with one.
 #include "cuda_simt.h"
 
 #include <cstdio>
@@ -64,8 +67,66 @@ __global__ void k_missed_barrier() {
     if (threadIdx.x & 1) __syncthreads();
 }
 
+// inclusive scan of the lane ids with __shfl_up_sync, the reducing barriers, atomicOr, static __shared__, uint4, min/max
+__global__ void k_scan_reduce(unsigned* out_scan, int* out_or, int* out_and, unsigned* out_bits, uint4* out_q) {
+    __shared__ unsigned s_bits;
+    const unsigned t = threadIdx.x, lane = t & 31u;
+    if (t == 0) s_bits = 0;
+    __syncthreads();
+    unsigned x = lane + 1;
+    for (unsigned o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+        if (lane >= o) x += y;
+    }
+    out_scan[blockIdx.x * blockDim.x + t] = x;
+    out_or[blockIdx.x * 2 + 0] = __syncthreads_or(t == 77);    // one thread true
+    out_or[blockIdx.x * 2 + 1] = __syncthreads_or(0);          // none
+    out_and[blockIdx.x * 2 + 0] = __syncthreads_and(t != 77);  // one thread false
+    out_and[blockIdx.x * 2 + 1] = __syncthreads_and(1);        // all
+    atomicOr(&s_bits, 1u << (t & 31u));
+    __syncthreads();
+    if (t == 0) {
+        *out_bits = s_bits;
+        const uint64_t big = 1ull << 40;
+        *out_q = make_uint4(min(3u, big), (unsigned)(max(2u, big) >> 32), min(blockDim.x, 7u), max(1, -1));
+    }
+}
+
+// dynamic shared memory: every block must find it poisoned (not the previous block's values), then owns it
+__global__ void k_dyn_smem(unsigned* out_fresh) {
+    unsigned* s = reinterpret_cast<unsigned*>(simt_dyn_smem());
+    const unsigned t = threadIdx.x;
+    const bool poisoned = s[t] == 0xA5A5A5A5u;
+    __syncthreads();
+    s[t] = blockIdx.x + 1;  // what a block that saw its predecessor's memory would read
+    __syncthreads();
+    if (s[(t + 1) % blockDim.x] != blockIdx.x + 1) out_fresh[blockIdx.x] = 2;
+    if (!__syncthreads_and(poisoned) && t == 0) out_fresh[blockIdx.x] = 3;
+}
+
+// block 0 waits for a flag that block 1 sets: finishes only if both are resident at once
+__global__ void k_flag_wait(volatile unsigned* flag, unsigned* seen) {
+    if (blockIdx.x == 1) {
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence();
+            atomicExch(const_cast<unsigned*>(flag), 1u);
+        }
+        return;
+    }
+    for (;;) {
+        if (__syncthreads_or(*flag != 0)) break;
+        __nanosleep(100);
+    }
+    if (threadIdx.x == 0) *seen = 1;
+}
+
 int main(int argc, char** argv) {
     if (argc > 1) {
+        if (!strcmp(argv[1], "spin")) {  // the flag wait with one resident block: the detector must report it
+            unsigned flag = 0, seen = 0;
+            simt_launch_ex(2, 64, 0, 1, [&] { k_flag_wait(&flag, &seen); });
+        }
         if (!strcmp(argv[1], "exited")) simt_launch(1, 64, [] { k_exited_lane(); });
         if (!strcmp(argv[1], "mask")) simt_launch(1, 32, [] { k_mask_mismatch(); });
         if (!strcmp(argv[1], "barrier")) simt_launch(1, 32, [] { k_missed_barrier(); });
@@ -99,6 +160,45 @@ int main(int argc, char** argv) {
     const unsigned long long lost_p1 = 256 - racy;
     race(2, 0.5, &racy, &atomic);
     if (racy >= 256 || atomic != 256) return 6;
+    // shfl_up scan, reducing barriers, atomicOr, static __shared__, uint4, mixed min / max
+    {
+        const unsigned g2 = 2, b2 = 128;
+        std::vector<unsigned> scan(g2 * b2);
+        int ors[4], ands[4];
+        unsigned bits = 0;
+        uint4 q{};
+        simt_launch(g2, b2, [&] { k_scan_reduce(scan.data(), ors, ands, &bits, &q); });
+        for (unsigned i = 0; i < g2 * b2; i++) {
+            const unsigned lane = i % 32;
+            if (scan[i] != (lane + 1) * (lane + 2) / 2) return 7;
+        }
+        for (unsigned g = 0; g < g2; g++)
+            if (ors[2 * g] != 1 || ors[2 * g + 1] != 0 || ands[2 * g] != 0 || ands[2 * g + 1] != 1) return 8;
+        if (bits != 0xFFFFFFFFu || q.x != 3 || q.y != 256 || q.z != 7 || q.w != 1) return 9;
+    }
+    // dynamic shared memory: poisoned at every block start, one copy per resident block, with one or four resident
+    for (unsigned R : {1u, 4u}) {
+        std::vector<unsigned> fresh(9, 0);
+        simt_launch_ex(9, 64, 64 * sizeof(unsigned), R, [&] { k_dyn_smem(fresh.data()); });
+        for (unsigned v : fresh)
+            if (v) return 10;
+        simt_interleave(true, 7, 1.0);
+        simt_launch_ex(9, 64, 64 * sizeof(unsigned), R, [&] { k_dyn_smem(fresh.data()); });
+        simt_interleave(false);
+        for (unsigned v : fresh)
+            if (v) return 11;
+    }
+    // resident blocks: the flag wait finishes with two of them, in either mode
+    {
+        unsigned flag = 0, seen = 0;
+        simt_launch_ex(2, 64, 0, 2, [&] { k_flag_wait(&flag, &seen); });
+        if (!seen) return 12;
+        flag = seen = 0;
+        simt_interleave(true, 3, 0.5);
+        simt_launch_ex(2, 64, 0, 2, [&] { k_flag_wait(&flag, &seen); });
+        simt_interleave(false);
+        if (!seen) return 13;
+    }
     printf("ok simt (racy update lost %llu and %llu of 256 increments)\n", lost_p1, 256 - racy);
     return 0;
 }

@@ -898,3 +898,123 @@ def run_edge_kat(kat, layer, batched, lc):
             assert got is None or got == step[2], "get_counters"
         else:
             layer.set_max(step[1])
+
+
+@functools.cache
+def emu_engine_lib():
+    """tests/emu/emu_engine.cpp: the decision kernels (k_front, k_hot, k_main, the resolve kernels, k_restore,
+    k_fl_step, k_wide_scatter, k_query_records, k_scan) compiled for the host under tests/emu/cuda_simt.h, driven
+    through the engine's call sequences."""
+    L = host_lib("emu_engine.cpp", "librl_emu_engine.so")
+    vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
+    L.emu_engine_create.restype = vp
+    L.emu_engine_create.argtypes = [u32, u32, u32]
+    L.emu_engine_destroy.argtypes = [vp]
+    L.emu_engine_limits_set.argtypes = [vp, vp, u32]
+    L.emu_engine_knobs.argtypes = [vp, u32, u32, u32, u32, u32, u32, u32, u32]
+    L.emu_engine_knobs.restype = None
+    L.emu_engine_interleave.argtypes = [vp, C.c_int, u64, C.c_double]
+    L.emu_engine_interleave.restype = None
+    L.emu_engine_report.restype = C.POINTER(C.c_ulonglong)
+    L.emu_engine_report.argtypes = [vp]
+    L.emu_engine_max_cells_used.restype = u32
+    L.emu_engine_max_cells_used.argtypes = [vp]
+    L.emu_engine_record_stride.restype = u32
+    L.emu_engine_record_stride.argtypes = [vp]
+    L.emu_engine_record_region.restype = C.c_int64
+    L.emu_engine_record_region.argtypes = [vp, vp]
+    L.emu_engine_records.argtypes = [vp, C.c_int, u32, vp, C.c_int, vp, vp, vp, vp]
+    L.emu_engine_csr.argtypes = [vp, C.c_int, u32, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]
+    L.emu_engine_query_records.argtypes = [vp, u32, vp, vp, vp]
+    L.emu_engine_export.restype = u64
+    L.emu_engine_export.argtypes = [vp, u64, vp, vp, vp, vp, vp]
+    return L
+
+
+# what EmuEngine.geometry reports about the last call, in emu_engine.cpp's order
+EMU_GEOMETRY = ("tiles", "tile", "merge_passes_main", "merge_passes_hot", "nparts", "items", "heavy_items", "max_w",
+                "hot_in_use", "hot_candidates", "hot_max_list", "hot_sweeps", "fixed_point_rounds", "chunks", "rounds",
+                "chained_chunks", "ordered_chunks", "hot_after", "max_partition", "ch", "rearmed")
+
+
+class EmuEngine:
+    """The engine's decision calls on the host (tests/emu/emu_engine.cpp): the same kernels the GPU runs, under the
+    fiber emulator.  Knobs: chunk (128 / 256), heavy_mult, part_target, hot rows, weak grouping tags, the sharded
+    geometry (tile derived from a device-side count), resident k_main blocks and the grid cap; interleave=(seed, p)
+    turns cuda_simt.h's interleaving mode on.  After every call `geometry` says what the call reached."""
+
+    def __init__(self, descs, cells, log2P, log2R, chunk=128, heavy_mult=2, part_target=128, hot=False, weak=False,
+                 sharded=False, resident=1, grid_cap=132 * 16, interleave=None):
+        self.L = emu_engine_lib()
+        self.h = self.L.emu_engine_create(cells, log2P, log2R)
+        self.cells = cells
+        self.L.emu_engine_knobs(self.h, chunk, heavy_mult, part_target, int(hot), int(weak), int(sharded), resident, grid_cap)
+        if interleave is not None:
+            self.L.emu_engine_interleave(self.h, 1, interleave[0], interleave[1])
+        self.set_limits(descs)
+        self.geometry = {}
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.L.emu_engine_destroy(self.h)
+
+    def set_limits(self, descs):
+        d = np.ascontiguousarray(descs, dtype=LIMIT_DESC_DTYPE)
+        assert self.L.emu_engine_limits_set(self.h, _p(d), len(d)) == 0
+
+    @property
+    def max_cells_used(self):
+        return int(self.L.emu_engine_max_cells_used(self.h))
+
+    def _report(self):
+        r = self.L.emu_engine_report(self.h)
+        self.geometry = {k: int(r[i]) for i, k in enumerate(EMU_GEOMETRY)}
+
+    def region_of(self, rec):
+        """The table region of a record's row (single-row namespaces), or -1."""
+        r = np.ascontiguousarray(np.array([rec], dtype=RECORD_DTYPE))
+        return int(self.L.emu_engine_record_region(self.h, _p(r)))
+
+    def records(self, mode, recs, load_counters=False):
+        """check_and_update (mode 0) / update_counters (mode 2) over records: limited, first-limited, remaining, ttl
+        ([n * stride]) and the device error code."""
+        recs = np.ascontiguousarray(recs, dtype=RECORD_DTYPE)
+        n = len(recs)
+        stride = int(self.L.emu_engine_record_stride(self.h))
+        lim = np.full(n, 0xA5, dtype=np.uint8)
+        fl = np.full(n, 0xA5A5A5A5, dtype=np.uint32)
+        rem = np.zeros(n * stride, dtype=np.uint64)
+        ttl = np.zeros(n * stride, dtype=np.uint64)
+        err = self.L.emu_engine_records(self.h, mode, n, _p(recs), int(load_counters), _p(lim), _p(fl), _p(rem), _p(ttl))
+        self._report()
+        return lim, fl, rem, ttl, err
+
+    def csr(self, mode, off, ctrs, delta, now_us, load_counters=False):
+        off = np.ascontiguousarray(off, dtype=np.uint32)
+        ctrs = np.ascontiguousarray(ctrs, dtype=COUNTER_DTYPE)
+        delta = np.ascontiguousarray(delta, dtype=np.uint64)
+        now_us = np.ascontiguousarray(now_us, dtype=np.uint64)
+        n = len(delta)
+        lim = np.full(n, 0xA5, dtype=np.uint8)
+        fl = np.full(n, 0xA5A5A5A5, dtype=np.uint32)
+        rem = np.zeros(max(len(ctrs), 1), dtype=np.uint64)
+        ttl = np.zeros(max(len(ctrs), 1), dtype=np.uint64)
+        err = self.L.emu_engine_csr(self.h, mode, n, _p(off), _p(ctrs), _p(delta), _p(now_us), int(load_counters),
+                                    _p(lim), _p(fl), _p(rem), _p(ttl))
+        self._report()
+        return lim, fl, rem[:len(ctrs)], ttl[:len(ctrs)], err
+
+    def query_records(self, recs):
+        recs = np.ascontiguousarray(recs, dtype=RECORD_DTYPE)
+        lim = np.zeros(len(recs), dtype=np.uint8)
+        fl = np.zeros(len(recs), dtype=np.uint32)
+        err = self.L.emu_engine_query_records(self.h, len(recs), _p(recs), _p(lim), _p(fl))
+        return lim, fl, err
+
+    def dump(self, cap=1 << 20):
+        """The table read through k_scan's export: sorted (limit_id, key_lo, key_hi, value, expiry_us)."""
+        lid = np.zeros(cap, dtype=np.uint32)
+        lo, hi, val, exp = (np.zeros(cap, dtype=np.uint64) for _ in range(4))
+        c = int(self.L.emu_engine_export(self.h, cap, _p(lid), _p(lo), _p(hi), _p(val), _p(exp)))
+        assert c <= cap
+        return sorted(zip(lid[:c].tolist(), lo[:c].tolist(), hi[:c].tolist(), val[:c].tolist(), exp[:c].tolist()))

@@ -183,7 +183,9 @@ def test_threshold_selects_regions_by_their_tombstone_share():
 
 def test_the_fiber_emulator_computes_the_intrinsics_and_refuses_what_would_hang_a_gpu(tmp_path):
     """tests/emu/cuda_simt.h on its own (tests/emu/simt_selftest.cpp): __match_any_sync groups reducing over their own
-    masks, ballots, shuffles and a __syncthreads tree reduction against closed forms; then the mistakes it must abort on."""
+    masks, ballots, shuffles, __shfl_up_sync scans, the reducing barriers, poisoned per-block dynamic shared memory and a flag
+    wait across two resident blocks against closed forms; then the mistakes it must abort on, the same flag wait with one
+    resident block among them."""
     import os
     import subprocess
     here = os.path.dirname(os.path.abspath(__file__))
@@ -192,6 +194,7 @@ def test_the_fiber_emulator_computes_the_intrinsics_and_refuses_what_would_hang_
     r = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0 and r.stdout.startswith("ok simt"), r.stdout + r.stderr
     for case, message in (("exited", "names a thread that has exited"), ("mask", "cuda_simt: "),
-                          ("barrier", "no thread of the block can make progress")):
+                          ("barrier", "no thread of the block can make progress"),
+                          ("spin", "waits in a __nanosleep loop")):
         r = subprocess.run([exe, case], capture_output=True, text=True, timeout=120)
         assert r.returncode != 0 and message in r.stderr and "not refused" not in r.stdout, (case, r.stdout, r.stderr)
