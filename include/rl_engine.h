@@ -298,6 +298,32 @@ int rl_counters_import(rl_engine *e, uint64_t n, const uint32_t *limit_id, const
  * *out_n = number registered. */
 int rl_limits_get(rl_engine *e, uint32_t cap, rl_limit_desc *out, uint32_t *out_n);
 
+/* ---- Change tracking: the counters changed since the last drain (DESIGN.md §9k) ------------------------------------
+ * What a journal on disk needs to bring a service's counters back after a crash, without moving the whole table each
+ * time.  The decision kernels do not take part: a drain compares the table with a shadow copy in one pass of its own,
+ * so an engine that never drains pays nothing.  No reference function: the reference's disk store writes every update
+ * through RocksDB's write-ahead log (limitador/src/storage/disk/rocksdb_storage.rs).
+ *   rl_counters_track  on = 1: allocate the shadow, capacity_rows x row bytes of device memory (RL_TRANSIENT when there
+ *                      is no room), and make the next drain full.  on = 0: free it.
+ *   rl_counters_drain  full drain (*out_full = 1): exactly rl_counters_export(e, NULL, 0, 0, cap, mem, ...).  It is the
+ *                      first drain after rl_counters_track, and the first after any call that can move rows or re-map
+ *                      cells: rl_limits_set, rl_limits_delete, rl_delete_counters, rl_clear, rl_compact and
+ *                      rl_counters_import (rl_rls_configure runs through them).
+ *                      delta drain (*out_full = 0): every counter whose (value, expiry) differs from what the previous
+ *                      drain saw, as (limit_id, key, value, expiry_us); a counter that is no longer listed is
+ *                      (limit_id, key, 0, 0).  One row position can go from key A to a tombstone to key B between two
+ *                      drains: then A's counters come out absent and B's present, so apply a delta's absents before its
+ *                      presents.  Replaying the full drain and then every delta in order gives exactly what
+ *                      rl_counters_export(e, NULL, 0, 0, ...) lists at the last drain.
+ *                      Both: mem = RL_MEM_HOST or RL_MEM_DEVICE for the five outputs, unordered, *out_count = entries
+ *                      found, at most cap written.  When *out_count > cap the drain is not consumed (the shadow stays
+ *                      as it was): the same drain can be repeated with a larger cap.  Needs tracking on.  Serialise with the request path (as rl_compact);
+ *                      pipelined record calls are fenced first. */
+int rl_counters_track(rl_engine *e, int on);
+int rl_counters_drain(rl_engine *e, uint64_t cap, int mem, uint32_t *out_limit_id, uint64_t *out_key_lo,
+                      uint64_t *out_key_hi, uint64_t *out_value, uint64_t *out_expiry_us, uint64_t *out_count,
+                      int *out_full);
+
 /* Measurement aid (bench.py roofline leg): between begin and end the engine brackets every
  * launch of its dominant kernel (k_main) with CUDA events on the launching stream;
  * end() synchronises and returns the summed device time and the launch count. */

@@ -159,6 +159,17 @@ int rl_rls_counter_vars_export(rl_rls *s, const uint32_t *ns_ids, uint32_t n_ns,
 int rl_rls_counter_vars_import(rl_rls *s, uint64_t n, const uint32_t *varset, const uint64_t *key_lo,
                                const uint64_t *key_hi, const uint64_t *blob_off, const uint8_t *blobs,
                                uint64_t *out_added);
+/* The entries recorded since the last drain, in rl_rls_counter_vars_export's layout, beside rl_counters_drain (a
+ * journal on disk keeps both).  The arena is append-only between a GC and an import, so those are the slots whose blob
+ * starts at or past the arena cursor the previous drain read.  *out_full = 1 (and no entry) on the first drain after
+ * rl_rls_keep_counter_vars, rl_rls_counter_vars_gc or rl_rls_counter_vars_import: take a full
+ * rl_rls_counter_vars_export then; the next drain starts from this one.  When *out_count > cap or *out_bytes >
+ * bytes_cap nothing is written and the drain is not consumed (repeat it with larger caps).  With keeping off the
+ * count is 0.  Serialise with serve, as rl_compact. */
+int rl_rls_counter_vars_drain(rl_rls *s, uint64_t cap, uint64_t bytes_cap,
+                              uint32_t *out_varset, uint64_t *out_key_lo, uint64_t *out_key_hi,
+                              uint64_t *out_blob_off, uint8_t *out_blobs,
+                              uint64_t *out_count, uint64_t *out_bytes, int *out_full);
 
 /* ---- configuration (RateLimiter::configure_with, limitador/src/lib.rs:475-505) -----------------------------------
  * rl_rls_configure makes the service's matcher and engine hold exactly the limits of `limits`, as limitador-server does

@@ -20,6 +20,8 @@
 //   k_counter_vars_export / _check / _import   snapshots: the GC's mark, then the marked entries laid out for the host;
 //                       an import checks every entry against the image (rl_cv_check_entry), then copies the dictionary
 //                       into a fresh table (_occupied, _kept, _rebuild) and claims the new entries there
+//   k_counter_vars_since   drains (rl_rls_counter_vars_drain): the entries recorded since the last drain, laid out by
+//                       the export's kernels
 // Written, like rl_rls_dev.cuh, so that the same source runs under tests/emu/cuda_shim.h: per-thread code and global
 // atomics only.
 #pragma once
@@ -416,4 +418,11 @@ __global__ void k_counter_vars_import(CvImportArgs a) {
 __global__ void k_counter_vars_occupied(CvDict d, uint8_t* mark) {
     const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p <= d.mask) mark[p] = d.slots[p].fp != 0;
+}
+
+// Drains: the arena is append-only between a GC or an import (its cursor is an atomic add), so the entries recorded
+// since a drain that read the cursor as `since` are exactly the slots whose blob starts at or past it.
+__global__ void k_counter_vars_since(CvDict d, uint64_t since, uint8_t* mark) {
+    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p <= d.mask) mark[p] = d.slots[p].fp != 0 && d.slots[p].off >= since;
 }

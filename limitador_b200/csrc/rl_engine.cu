@@ -74,6 +74,7 @@ struct rl_engine {
     std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> groups_by_key;
     std::vector<std::vector<uint32_t>> ns_limits;  // registration order
     bool tables_dirty = true;
+    uint64_t structure_epoch = 0;  // calls that can move rows or re-map cells (rl_counters_drain: the next drain is full)
     bool any_multi_ns = false;
     uint32_t max_ns_limits = 0;
     uint32_t max_cells_used = 1;  // highest cell index + 1 over all row groups
@@ -991,6 +992,7 @@ int rl_get_stats(rl_engine* e, rl_stats* out) {
 
 int rl_limits_set(rl_engine* e, const rl_limit_desc* limits, uint32_t n) {
     if (!e || (!limits && n)) return RL_FATAL;
+    e->structure_epoch++;
     for (uint32_t i = 0; i < n; i++) {
         const rl_limit_desc& d = limits[i];
         if (d.limit_id == RL_NONE_U32) return fail(e, RL_FATAL, "limit_id 0xFFFFFFFF is reserved");
@@ -1085,6 +1087,7 @@ static int reset_table(rl_engine* e, int mode, uint64_t now_us, const std::vecto
 int rl_delete_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
     if (!e) return RL_FATAL;
     RL_CUDA(e, cudaSetDevice(e->device));
+    e->structure_epoch++;
     std::vector<uint8_t> sel(std::max<size_t>(e->limits.size(), 1), 0);
     bool any = false;
     for (uint32_t i = 0; i < n; i++) {
@@ -1099,6 +1102,7 @@ int rl_delete_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
 
 int rl_limits_delete(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
     if (!e) return RL_FATAL;
+    e->structure_epoch++;
     int r = rl_delete_counters(e, limit_ids, n);  // storage/mod.rs:104 — counters first
     if (r) return r;
     for (uint32_t i = 0; i < n; i++) {
@@ -1662,6 +1666,8 @@ int rl_internal_view(rl_engine* e, RlTableView* out) {
     out->ns_cap = e->ns_cap;
     out->limits_cap = e->limits_cap;
     out->limits = e->d_limits.p;
+    out->desc = e->d_desc.p;
+    out->structure_epoch = e->structure_epoch;
     out->stream = e->stream;
     out->device = e->device;
     return RL_OK;
@@ -1680,6 +1686,11 @@ int rl_internal_reset_hot_rows(rl_engine* e) {
     RL_CUDA(e, cudaMemsetAsync(e->d_hot.p, 0xFF, (RL_HOT_SLOTS + RL_HOT_CAND) * sizeof(uint32_t), e->stream));
     RL_CUDA(e, cudaMemsetAsync(e->d_hot.p + RL_HOT_SLOTS + RL_HOT_CAND, 0, 4 * sizeof(uint32_t), e->stream));
     return RL_OK;
+}
+void rl_internal_structure_changed(rl_engine* e) { e->structure_epoch++; }
+void rl_internal_present(rl_engine* e, uint8_t* present, uint32_t n) {
+    for (uint32_t l = 0; l < n; l++)
+        present[l] = l < e->limits.size() && e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
 }
 void rl_internal_mark_present(rl_engine* e, const uint8_t* flags, uint32_t n) {
     for (uint32_t l = 0; l < n && l < e->limits.size(); l++)

@@ -12,6 +12,8 @@ struct RlTableView {
     uint64_t capacity;  // rows
     uint32_t ns_cap, limits_cap;
     const RlLimitDev* limits;  // [limits_cap] device limit table: group (0 = not registered), cell, qualified
+    const RlCellDesc* desc;    // [row groups][8] the limit of every (row group, cell)
+    uint64_t structure_epoch;  // calls so far that can move rows or re-map cells (rl_internal_structure_changed)
     cudaStream_t stream;
     int device;
 };
@@ -30,5 +32,10 @@ void** rl_internal_ext(rl_engine* e, void (*ext_free)(void*));  // slot for rl_m
 void rl_internal_set_ns_hook(rl_engine* e, rl_ns_hook_fn fn);
 // forget the hot-row table (rows move when a region is rebuilt); enqueued on the engine's stream
 int rl_internal_reset_hot_rows(rl_engine* e);
+// a call that can move rows or re-map cells ran (limits set or deleted, counters deleted, compaction, import): the next
+// rl_counters_drain is a full one
+void rl_internal_structure_changed(rl_engine* e);
+// present[l] = the counters of limit l exist, as rl_counters_export lists them (l < n; n >= limits_cap)
+void rl_internal_present(rl_engine* e, uint8_t* present, uint32_t n);
 // the unqualified limits l with flags[l] != 0 (l < n) have a counter again (as after add_counter): host registry only
 void rl_internal_mark_present(rl_engine* e, const uint8_t* flags, uint32_t n);

@@ -1,5 +1,5 @@
-// rl_maint.cu — host side of the maintenance kernels (rl_maint.cuh): tombstone reclamation (rl_compact) and the
-// per-namespace metrics reduction (rl_ns_metrics_*).  A translation unit of its own: it sees an engine only through
+// rl_maint.cu — host side of the maintenance kernels (rl_maint.cuh): tombstone reclamation (rl_compact), the
+// per-namespace metrics reduction (rl_ns_metrics_*), counter import and change tracking (rl_counters_track / _drain).  A translation unit of its own: it sees an engine only through
 // rl_internal.h.
 #include <cuda_runtime.h>
 
@@ -20,6 +20,10 @@ struct MaintState {
     DevBuf<unsigned long long> d_metrics;
     uint32_t ns_cap = 0, limits_cap = 0;
     bool metrics_on = false;
+    // change tracking: the table as the last drain saw it; the next drain is full until one ran at epoch_seen
+    DevBuf<uint8_t> d_shadow;
+    bool full_next = true;
+    uint64_t epoch_seen = 0;
 };
 
 void maint_free(void* p) {
@@ -228,6 +232,7 @@ int rl_compact(rl_engine* e, uint32_t min_tombstone_pct, rl_compact_stats* out) 
     k_compact_reinsert<<<blocks, threads, 0, v.stream>>>(v.rows, d_scratch.p, v.row_bytes, v.log2P, v.log2R, v.capacity, d_sel.p, d_counts.p);
     RL_CUDA(e, cudaGetLastError());
     rl_internal_launched(e, 2);
+    rl_internal_structure_changed(e);
     r = rl_internal_reset_hot_rows(e);  // table row indices changed
     unsigned long long counts[3] = {0, 0, 0};
     RL_CUDA(e, cudaMemcpyAsync(counts, d_counts.p, sizeof counts, cudaMemcpyDeviceToHost, v.stream));
@@ -252,6 +257,7 @@ int rl_counters_import(rl_engine* e, uint64_t n, const uint32_t* limit_id, const
         return rl_internal_fail(e, RL_FATAL, "rl_counters_import: n > 0 needs all five input arrays");
     if (n >= (1ull << 48)) return rl_internal_fail(e, RL_FATAL, "rl_counters_import: n must stay below 2^48");
     if (n == 0) return RL_OK;
+    rl_internal_structure_changed(e);
     // inputs on the device: the caller's arrays, or staged for the call
     In<uint32_t> lid;
     In<uint64_t> lo, hi, val, exp;
@@ -317,6 +323,95 @@ int rl_counters_import(rl_engine* e, uint64_t n, const uint32_t* limit_id, const
     RL_CUDA(e, cudaMemcpyAsync(unq.data(), d_unq.p, unq.size(), cudaMemcpyDeviceToHost, v.stream));
     RL_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staged inputs are freed
     rl_internal_mark_present(e, unq.data(), v.limits_cap);
+    return RL_OK;
+}
+
+int rl_counters_track(rl_engine* e, int on) {
+    RlTableView v;
+    int r = rl_internal_view(e, &v);
+    if (r) return r;
+    MaintState* s = state_of(e, v.device);
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));
+    if (!on) {
+        RL_CUDA(e, s->d_shadow.exact(0));
+        return RL_OK;
+    }
+    if (!s->d_shadow.p && s->d_shadow.exact((size_t)v.capacity * v.row_bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return rl_internal_fail(e, RL_TRANSIENT, "rl_counters_track: no device memory for the shadow (one copy of the table)");
+    }
+    s->full_next = true;
+    return RL_OK;
+}
+
+int rl_counters_drain(rl_engine* e, uint64_t cap, int mem, uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi,
+                      uint64_t* out_value, uint64_t* out_expiry_us, uint64_t* out_count, int* out_full) {
+    RlTableView v;
+    int r = rl_internal_view(e, &v);
+    if (r) return r;
+    if (!out_count || !out_full) return rl_internal_fail(e, RL_FATAL, "rl_counters_drain: out_count and out_full are needed");
+    *out_count = 0;
+    *out_full = 0;
+    MaintState* s = state_of(e, v.device);
+    if (!s->d_shadow.p) return rl_internal_fail(e, RL_FATAL, "rl_counters_drain: change tracking is off (rl_counters_track)");
+    if (mem != RL_MEM_HOST && mem != RL_MEM_DEVICE)
+        return rl_internal_fail(e, RL_FATAL, "rl_counters_drain: mem must be RL_MEM_HOST or RL_MEM_DEVICE");
+    if (cap && (!out_limit_id || !out_key_lo || !out_key_hi || !out_value || !out_expiry_us))
+        return rl_internal_fail(e, RL_FATAL, "rl_counters_drain: cap > 0 needs all five output arrays");
+    const size_t table_bytes = (size_t)v.capacity * v.row_bytes;
+    if (s->full_next || s->epoch_seen != v.structure_epoch) {
+        // full: the export itself, and the table into the shadow only when the caller got all of it
+        *out_full = 1;
+        if ((r = rl_counters_export(e, nullptr, 0, 0, cap, mem, out_limit_id, out_key_lo, out_key_hi, out_value, out_expiry_us,
+                                    out_count)))
+            return r;
+        if (*out_count > cap) return RL_OK;
+        RL_CUDA(e, cudaMemcpyAsync(s->d_shadow.p, v.rows, table_bytes, cudaMemcpyDeviceToDevice, v.stream));
+        RL_CUDA(e, cudaStreamSynchronize(v.stream));
+        s->full_next = false;
+        s->epoch_seen = v.structure_epoch;
+        return RL_OK;
+    }
+    std::vector<uint8_t> present(std::max<uint32_t>(v.limits_cap, 1));
+    rl_internal_present(e, present.data(), (uint32_t)present.size());
+    DevBuf<uint8_t> d_present;
+    DevBuf<unsigned long long> d_cnt;
+    RL_CUDA(e, d_present.alloc(present.size()));
+    RL_CUDA(e, d_cnt.alloc(1));
+    RL_CUDA(e, cudaMemcpyAsync(d_present.p, present.data(), present.size(), cudaMemcpyHostToDevice, v.stream));
+    RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), v.stream));
+    const RlChangeTab T{v.rows, s->d_shadow.p, v.row_bytes, v.cells, v.capacity, v.desc, d_present.p};
+    const uint32_t threads = 256;
+    const uint32_t blocks = (uint32_t)((v.capacity + threads - 1) / threads);
+    // count first: a drain that does not fit leaves the shadow as it was, so the call can be repeated with a larger cap
+    RlChangeOut O{nullptr, nullptr, nullptr, nullptr, nullptr, d_cnt.p};
+    k_changes<<<blocks, threads, 0, v.stream>>>(T, O, 0);
+    RL_CUDA(e, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    unsigned long long cnt = 0;
+    RL_CUDA(e, cudaMemcpyAsync(&cnt, d_cnt.p, sizeof cnt, cudaMemcpyDeviceToHost, v.stream));
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));
+    *out_count = cnt;
+    if (cnt > cap) return RL_OK;
+    // then emit, into the caller's device arrays or staging of exactly the count
+    DevBuf<uint32_t> s_lid;
+    DevBuf<uint64_t> s64[4];
+    O = RlChangeOut{out_limit_id, out_key_lo, out_key_hi, out_value, out_expiry_us, d_cnt.p};
+    if (mem == RL_MEM_HOST) {
+        RL_CUDA(e, s_lid.alloc(cnt));
+        for (auto& b : s64) RL_CUDA(e, b.alloc(cnt));
+        O = RlChangeOut{s_lid.p, s64[0].p, s64[1].p, s64[2].p, s64[3].p, d_cnt.p};
+    }
+    RL_CUDA(e, cudaMemsetAsync(d_cnt.p, 0, sizeof(unsigned long long), v.stream));
+    k_changes<<<blocks, threads, 0, v.stream>>>(T, O, 1);
+    RL_CUDA(e, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    if (mem == RL_MEM_HOST && cnt) {
+        RL_CUDA(e, cudaMemcpyAsync(out_limit_id, s_lid.p, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream));
+        uint64_t* out64[4] = {out_key_lo, out_key_hi, out_value, out_expiry_us};
+        for (int k = 0; k < 4; k++) RL_CUDA(e, cudaMemcpyAsync(out64[k], s64[k].p, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, v.stream));
+    }
+    RL_CUDA(e, cudaStreamSynchronize(v.stream));  // before the staging is freed
     return RL_OK;
 }
 

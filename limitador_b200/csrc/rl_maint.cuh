@@ -337,3 +337,109 @@ __global__ void k_import_write(RlImportTab T, RlImportIn I, const unsigned long 
     const uint32_t cell = T.limits[I.limit_id[i]].cell;
     rlm_st(T.rows + RLM_ROW_INDEX(row_of[i]) * T.row_bytes + 16 + 16 * cell, I.value[i], I.expiry[i]);
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Change tracking (rl_counters_drain): the table against its shadow, a copy taken at the previous drain.  Between two
+// calls that move rows or re-map cells only the decision calls and rl_sweep change the table, and neither moves a row,
+// so row r of the shadow and row r of the table are read with the same (row group, cell) -> limit mapping.
+struct RlChangeTab {
+    const uint8_t* rows;
+    uint8_t* shadow;             // [nrows * row_bytes]
+    uint32_t row_bytes, cells;
+    uint64_t nrows;
+    const RlCellDesc* desc;      // [row groups][8]
+    const uint8_t* present;      // [limits] 1 = the limit's counters exist (rl_counters_export's rule)
+};
+
+struct RlChangeOut {
+    uint32_t* limit_id;
+    uint64_t* key_lo;
+    uint64_t* key_hi;
+    uint64_t* value;
+    uint64_t* expiry;
+    unsigned long long* count;
+};
+
+// The cells of a row that rl_counters_export(now_us = 0) lists, as a bit mask; cell[c] = (value, expiry) of cell c.
+__device__ __forceinline__ uint32_t rlm_listed(const RlChangeTab& T, const uint8_t* row, ulonglong2& hdr, ulonglong2* cell) {
+    hdr = rlm_ld(row);
+    if (hdr.y == 0 || hdr.y == RLM_TOMB_HI) return 0;
+    const RlCellDesc* d = T.desc + (size_t)(hdr.y >> 32) * 8;
+    uint32_t m = 0;
+    for (uint32_t c = 0; c < T.cells; c++) {
+        cell[c] = rlm_ld(row + 16 + 16 * c);
+        const uint32_t lid = d[c].limit_id;
+        if (lid == RL_NONE_U32 || !T.present[lid]) continue;
+        if (d[c].qualified && cell[c].y == 0) continue;  // logically absent
+        m |= 1u << c;
+    }
+    return m;
+}
+
+// One thread per row.  A row whose bytes equal the shadow's is skipped.  Otherwise the counters it lists now and
+// listed then are compared: the same key in both keeps the cells whose (value, expiry) moved, and a listed cell that
+// is gone is absent, (limit, key, 0, 0).  A row that holds another key than its shadow (empty, tombstone, key A then
+// key B) lists every old counter as absent and every new one as present: a journal applies a drain's absents before
+// its presents.  emit = 0: *O.count += the entries.  emit = 1: the entries are written at reserved positions (the
+// count pass found them to fit) and the row is copied into the shadow.
+__global__ void k_changes(RlChangeTab T, RlChangeOut O, int emit) {
+    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= T.nrows) return;
+    const uint8_t* row = T.rows + r * T.row_bytes;
+    uint8_t* old = T.shadow + r * T.row_bytes;
+    bool same = true;
+    for (uint32_t q = 0; q < T.row_bytes && same; q += 16) {
+        const ulonglong2 a = rlm_ld(row + q), b = rlm_ld(old + q);
+        same = a.x == b.x && a.y == b.y;
+    }
+    if (same) return;
+    ulonglong2 hn, ho, cn[RL_MAX_CELLS], co[RL_MAX_CELLS];
+    const uint32_t mn = rlm_listed(T, row, hn, cn), mo = rlm_listed(T, old, ho, co);
+    const bool same_key = mn && mo && hn.x == ho.x && hn.y == ho.y;
+    const RlCellDesc* dn = mn ? T.desc + (size_t)(hn.y >> 32) * 8 : T.desc;
+    const RlCellDesc* d_o = mo ? T.desc + (size_t)(ho.y >> 32) * 8 : T.desc;
+    uint32_t gone = 0, now = 0;  // cells emitted as absent (old key) / as present (new key)
+    if (same_key) {
+        for (uint32_t c = 0; c < T.cells; c++) {
+            if (mn >> c & 1u) {
+                if (!(mo >> c & 1u) || cn[c].x != co[c].x || cn[c].y != co[c].y) now |= 1u << c;
+            } else if (mo >> c & 1u) {
+                gone |= 1u << c;
+            }
+        }
+    } else {
+        gone = mo;
+        now = mn;
+    }
+    uint32_t n = 0;
+    for (uint32_t c = 0; c < T.cells; c++) n += (gone >> c & 1u) + (now >> c & 1u);
+    if (!emit) {
+        if (n) atomicAdd(O.count, (unsigned long long)n);
+        return;
+    }
+    if (n) {
+        unsigned long long pos = atomicAdd(O.count, (unsigned long long)n);
+        for (uint32_t c = 0; c < T.cells; c++) {
+            if (!(gone >> c & 1u)) continue;
+            O.limit_id[pos] = d_o[c].limit_id;
+            O.key_lo[pos] = ho.x;
+            O.key_hi[pos] = ho.y & 0xFFFFFFFFull;
+            O.value[pos] = 0;
+            O.expiry[pos] = 0;
+            pos++;
+        }
+        for (uint32_t c = 0; c < T.cells; c++) {
+            if (!(now >> c & 1u)) continue;
+            O.limit_id[pos] = dn[c].limit_id;
+            O.key_lo[pos] = hn.x;
+            O.key_hi[pos] = hn.y & 0xFFFFFFFFull;
+            O.value[pos] = cn[c].x;
+            O.expiry[pos] = cn[c].y;
+            pos++;
+        }
+    }
+    for (uint32_t q = 0; q < T.row_bytes; q += 16) {
+        const ulonglong2 a = rlm_ld(row + q);
+        rlm_st(old + q, a.x, a.y);
+    }
+}

@@ -67,6 +67,9 @@ __attribute__((weak)) int rl_cv_dev_export(rl_rls_dev** st, rl_engine* e, rl_mat
 __attribute__((weak)) int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* varset,
                                            const uint64_t* key_lo, const uint64_t* key_hi, const uint64_t* blob_off,
                                            const uint8_t* blobs, uint64_t* out_added);
+__attribute__((weak)) int rl_cv_dev_drain(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t cap, uint64_t bytes_cap,
+                                          uint32_t* out_varset, uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_blob_off,
+                                          uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes, int* out_full);
 __attribute__((weak)) int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_t now_us, uint64_t cap,
                                           uint32_t* out_limit_id, uint64_t* out_key_lo, uint64_t* out_key_hi,
                                           uint64_t* out_remaining, uint64_t* out_ttl_us, uint64_t* out_count);
@@ -1508,6 +1511,18 @@ int rl_rls_counter_vars_import(rl_rls* s, uint64_t n, const uint32_t* varset, co
     if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
     if (!rl_cv_dev_import) return sfail(s, "this build of the library has no device plan");
     const int r = rl_cv_dev_import(&s->dev, s->engine, s->m, n, varset, key_lo, key_hi, blob_off, blobs, out_added);
+    if (r) s->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
+    return r;
+}
+
+int rl_rls_counter_vars_drain(rl_rls* s, uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset, uint64_t* out_key_lo,
+                              uint64_t* out_key_hi, uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count,
+                              uint64_t* out_bytes, int* out_full) {
+    if (!s || !out_count || !out_bytes || !out_full) return RL_FATAL;
+    if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
+    if (!rl_cv_dev_drain) return sfail(s, "this build of the library has no device plan");
+    const int r = rl_cv_dev_drain(&s->dev, s->engine, s->m, cap, bytes_cap, out_varset, out_key_lo, out_key_hi, out_blob_off,
+                                  out_blobs, out_count, out_bytes, out_full);
     if (r) s->last_error = std::string("counter variables: ") + rl_rls_dev_error(s->dev);
     return r;
 }

@@ -62,6 +62,9 @@ struct rl_rls_dev {
     DevBuf<CvSlot> d_cv_slots;
     DevBuf<uint8_t> d_cv_arena;
     DevBuf<unsigned long long> d_cv_ctl;
+    // drains: the arena cursor the last drain read; the next drain is full after keeping is set, a GC or an import
+    uint64_t cv_since = 0;
+    bool cv_full_next = true;
     // lookup and GC scratch
     DevBuf<uint32_t> d_cv_lid;
     DevBuf<uint64_t> d_cv_lo, d_cv_hi, d_cv_val, d_cv_exp, d_cv_src;
@@ -320,6 +323,56 @@ int rebuild_fresh(rl_rls_dev* S, DevBuf<CvSlot>& slots2, DevBuf<uint8_t>& arena2
     return RL_OK;
 }
 
+// The second half of the export and of the drains: the slots marked in d_cv_mark [slots + 1] laid out for the host.
+// *out_count / *out_bytes = what the marks select; written only when cap and bytes_cap hold it all.
+int export_marked(rl_rls_dev* S, rl_engine* e, uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset, uint64_t* out_key_lo,
+                  uint64_t* out_key_hi, uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes) {
+    int r;
+    if ((r = kept_positions(S))) return r;
+    // each entry's index: a scan over the marks
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, S->d_cv_idx.grow(slots + 1));
+    size_t tmp = 0;
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull, (int64_t)(slots + 1),
+                                               S->stream));
+    RL_CUDA(S, S->d_cub.grow(tmp + 1));
+    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull,
+                                               (int64_t)(slots + 1), S->stream));
+    unsigned long long tot[2] = {0, 0};
+    RL_CUDA(S, cudaMemcpyAsync(&tot[0], S->d_cv_idx.p + slots, sizeof tot[0], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaMemcpyAsync(&tot[1], S->d_cv_pos.p + slots, sizeof tot[1], cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    rl_internal_launched(e, 1);
+    const uint64_t count = tot[0], bytes = tot[1];
+    *out_count = count;
+    *out_bytes = bytes;
+    if (cap == 0 || cap < count || bytes_cap < bytes) return RL_OK;
+    if (!out_varset || !out_key_lo || !out_key_hi || !out_blob_off || (bytes && !out_blobs))
+        return fail(S, RL_FATAL, "exporting counter variables: cap > 0 needs every output array");
+    // one packed array on the device, one copy to the host: varset (padded to 8 bytes), key_lo, key_hi, blob_off, blobs
+    const uint64_t o_lo = (4 * count + 7) / 8 * 8, o_hi = o_lo + 8 * count, o_off = o_hi + 8 * count, o_blob = o_off + 8 * (count + 1);
+    RL_CUDA(S, S->d_cv_out.grow(o_blob + bytes));
+    uint8_t* P = S->d_cv_out.p;
+    CvExportArgs a{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, S->d_cv_idx.p, reinterpret_cast<uint32_t*>(P),
+                   reinterpret_cast<uint64_t*>(P + o_lo), reinterpret_cast<uint64_t*>(P + o_hi),
+                   reinterpret_cast<uint64_t*>(P + o_off), P + o_blob};
+    const uint32_t threads = 256;
+    k_counter_vars_export<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(a);
+    RL_CUDA(S, cudaGetLastError());
+    rl_internal_launched(e, 1);
+    S->h_cv_out.resize(o_blob + bytes);
+    RL_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), P, o_blob + bytes, cudaMemcpyDeviceToHost, S->stream));
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    const uint8_t* h = S->h_cv_out.data();
+    memcpy(out_varset, h, 4 * count);
+    memcpy(out_key_lo, h + o_lo, 8 * count);
+    memcpy(out_key_hi, h + o_hi, 8 * count);
+    memcpy(out_blob_off, h + o_off, 8 * (count + 1));
+    if (bytes) memcpy(out_blobs, h + o_blob, bytes);
+    return RL_OK;
+}
+
+
 const char* cv_reason(uint64_t why) {
     switch (why) {
         case RL_CV_BAD_VARSET: return "not the variable set of a qualified limit";
@@ -539,6 +592,7 @@ int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64
     if (r) return r;
     RL_CUDA(S, cudaStreamSynchronize(S->stream));  // no batch may still write the old dictionary
     S->cv_slots = S->cv_arena_bytes = 0;
+    S->cv_full_next = true;
     RL_CUDA(S, S->d_cv_slots.exact(0));
     RL_CUDA(S, S->d_cv_arena.exact(0));
     RL_CUDA(S, S->d_cv_ctl.exact(0));
@@ -649,6 +703,7 @@ int rl_cv_dev_gc(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t now_us, 
     S->d_cv_slots.swap(slots2);
     S->d_cv_arena.swap(arena2);
     S->d_cv_ctl.swap(ctl2);
+    S->cv_full_next = true;
     uint64_t after[RL_CV_CTL_WORDS];
     RL_CUDA(S, cudaMemcpy(after, S->d_cv_ctl.p, sizeof after, cudaMemcpyDeviceToHost));
     if (out_kept) *out_kept = after[RL_CV_KEYS];
@@ -667,47 +722,40 @@ int rl_cv_dev_export(rl_rls_dev** st, rl_engine* e, rl_matcher* m, const uint32_
     if (r) return r;
     uint32_t launched = 0;
     if ((r = mark_live(S, e, ns_ids, n_ns, now_us, launched))) return r;
-    if ((r = kept_positions(S))) return r;
-    // each entry's index: a scan over the marks
-    const uint64_t slots = S->cv_slots;
-    RL_CUDA(S, S->d_cv_idx.grow(slots + 1));
-    size_t tmp = 0;
-    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(nullptr, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull, (int64_t)(slots + 1),
-                                               S->stream));
-    RL_CUDA(S, S->d_cub.grow(tmp + 1));
-    RL_CUDA(S, cub::DeviceScan::ExclusiveScan(S->d_cub.p, tmp, S->d_cv_mark.p, S->d_cv_idx.p, cuda::std::plus<>(), 0ull,
-                                               (int64_t)(slots + 1), S->stream));
-    unsigned long long tot[2] = {0, 0};
-    RL_CUDA(S, cudaMemcpyAsync(&tot[0], S->d_cv_idx.p + slots, sizeof tot[0], cudaMemcpyDeviceToHost, S->stream));
-    RL_CUDA(S, cudaMemcpyAsync(&tot[1], S->d_cv_pos.p + slots, sizeof tot[1], cudaMemcpyDeviceToHost, S->stream));
+    rl_internal_launched(e, launched);
+    return export_marked(S, e, cap, bytes_cap, out_varset, out_key_lo, out_key_hi, out_blob_off, out_blobs, out_count, out_bytes);
+}
+
+int rl_cv_dev_drain(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset,
+                    uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count,
+                    uint64_t* out_bytes, int* out_full) {
+    if (!st || !e || !m || !out_count || !out_bytes || !out_full) return RL_FATAL;
+    *out_count = *out_bytes = 0;
+    *out_full = 0;
+    if (!*st || !(*st)->cv_slots) return RL_OK;
+    rl_rls_dev* S = *st;
+    int r = bind_engine(S, e, m);
+    if (r) return r;
+    unsigned long long cursor = 0;
+    RL_CUDA(S, cudaMemcpyAsync(&cursor, S->d_cv_ctl.p + RL_CV_CURSOR, sizeof cursor, cudaMemcpyDeviceToHost, S->stream));
     RL_CUDA(S, cudaStreamSynchronize(S->stream));
-    rl_internal_launched(e, launched + 1);
-    const uint64_t count = tot[0], bytes = tot[1];
-    *out_count = count;
-    *out_bytes = bytes;
-    if (cap == 0 || cap < count || bytes_cap < bytes) return RL_OK;
-    if (!out_varset || !out_key_lo || !out_key_hi || !out_blob_off || (bytes && !out_blobs))
-        return fail(S, RL_FATAL, "exporting counter variables: cap > 0 needs every output array");
-    // one packed array on the device, one copy to the host: varset (padded to 8 bytes), key_lo, key_hi, blob_off, blobs
-    const uint64_t o_lo = (4 * count + 7) / 8 * 8, o_hi = o_lo + 8 * count, o_off = o_hi + 8 * count, o_blob = o_off + 8 * (count + 1);
-    RL_CUDA(S, S->d_cv_out.grow(o_blob + bytes));
-    uint8_t* P = S->d_cv_out.p;
-    CvExportArgs a{cv_dict(S), S->d_cv_mark.p, S->d_cv_pos.p, S->d_cv_idx.p, reinterpret_cast<uint32_t*>(P),
-                   reinterpret_cast<uint64_t*>(P + o_lo), reinterpret_cast<uint64_t*>(P + o_hi),
-                   reinterpret_cast<uint64_t*>(P + o_off), P + o_blob};
-    const uint32_t threads = 256;
-    k_counter_vars_export<<<blocks_for(slots + 1, threads), threads, 0, S->stream>>>(a);
+    if (S->cv_full_next) {  // the caller takes a full export; the next drain starts from here
+        *out_full = 1;
+        S->cv_since = cursor;
+        S->cv_full_next = false;
+        return RL_OK;
+    }
+    const uint64_t slots = S->cv_slots;
+    RL_CUDA(S, S->d_cv_mark.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_len.grow(slots + 1));
+    RL_CUDA(S, S->d_cv_pos.grow(slots + 1));
+    RL_CUDA(S, cudaMemsetAsync(S->d_cv_mark.p + slots, 0, 1, S->stream));
+    k_counter_vars_since<<<blocks_for(slots, 256), 256, 0, S->stream>>>(cv_dict(S), S->cv_since, S->d_cv_mark.p);
     RL_CUDA(S, cudaGetLastError());
     rl_internal_launched(e, 1);
-    S->h_cv_out.resize(o_blob + bytes);
-    RL_CUDA(S, cudaMemcpyAsync(S->h_cv_out.data(), P, o_blob + bytes, cudaMemcpyDeviceToHost, S->stream));
-    RL_CUDA(S, cudaStreamSynchronize(S->stream));
-    const uint8_t* h = S->h_cv_out.data();
-    memcpy(out_varset, h, 4 * count);
-    memcpy(out_key_lo, h + o_lo, 8 * count);
-    memcpy(out_key_hi, h + o_hi, 8 * count);
-    memcpy(out_blob_off, h + o_off, 8 * (count + 1));
-    if (bytes) memcpy(out_blobs, h + o_blob, bytes);
+    if ((r = export_marked(S, e, cap, bytes_cap, out_varset, out_key_lo, out_key_hi, out_blob_off, out_blobs, out_count, out_bytes)))
+        return r;
+    if (*out_count <= cap && *out_bytes <= bytes_cap) S->cv_since = cursor;  // consumed only when it was handed over
     return RL_OK;
 }
 
@@ -815,6 +863,7 @@ int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, c
     S->d_cv_slots.swap(slots2);
     S->d_cv_arena.swap(arena2);
     S->d_cv_ctl.swap(ctl2);
+    S->cv_full_next = true;
     if (out_added) *out_added = after[RL_CV_KEYS] - before[RL_CV_KEYS];
     return RL_OK;
 }

@@ -79,6 +79,10 @@ int rl_cv_dev_export(rl_rls_dev** st, rl_engine* e, rl_matcher* m, const uint32_
                      uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes);
 int rl_cv_dev_import(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t n, const uint32_t* varset, const uint64_t* key_lo,
                      const uint64_t* key_hi, const uint64_t* blob_off, const uint8_t* blobs, uint64_t* out_added);
+// Drains (include/rl_rls.h: rl_rls_counter_vars_drain): the entries recorded since the last drain, in the export's layout.
+int rl_cv_dev_drain(rl_rls_dev** st, rl_engine* e, rl_matcher* m, uint64_t cap, uint64_t bytes_cap, uint32_t* out_varset,
+                    uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count,
+                    uint64_t* out_bytes, int* out_full);
 const char* rl_rls_dev_error(rl_rls_dev* st);
 void rl_rls_dev_destroy(rl_rls_dev* st);
 }

@@ -55,7 +55,7 @@ ABI_SYMBOLS = [
     "rl_shard_slab", "rl_shard_slab_bytes", "rl_shard_send", "rl_shard_decide", "rl_shard_collect", "rl_shard_step",
     "rl_shard_flush", "rl_shard_debug", "rl_trace_dump", "rl_check_and_update_compact", "rl_shard_fence",
     "rl_compact", "rl_ns_metrics_enable", "rl_ns_metrics_accumulate", "rl_ns_metrics_read",
-    "rl_counters_export", "rl_counters_import", "rl_limits_get",
+    "rl_counters_export", "rl_counters_import", "rl_limits_get", "rl_counters_track", "rl_counters_drain",
 ]
 
 SNAPSHOT_VERSION = 1  # format of Engine.save_counters files
@@ -135,6 +135,8 @@ def load_library(path: str | None = None):
     L.rl_counters_export.argtypes = [vp, vp, u32, u64, u64, i32, vp, vp, vp, vp, vp, vp]
     L.rl_counters_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, i32]
     L.rl_limits_get.argtypes = [vp, u32, vp, vp]
+    L.rl_counters_track.argtypes = [vp, i32]
+    L.rl_counters_drain.argtypes = [vp, u64, i32, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int)]
     L.rl_bucket_by_owner.argtypes = [vp, u64, vp, u32, vp, vp, vp]
     L.rl_unpermute_u8.argtypes = [vp, u64, vp, vp, vp]
     L.rl_bucket_by_owner_padded.argtypes = [vp, u64, vp, u32, u32, vp, vp, vp]
@@ -529,13 +531,35 @@ class Engine:
                 raise ValueError(f"{path}: snapshot format {int(z['version'])}, this build reads {SNAPSHOT_VERSION}")
             limits = z["limits"]
             cols = [z[k] for k in ("limit_id", "key_lo", "key_hi", "value", "expiry_us")]
+        self.import_snapshot(limits, cols, path)
+
+    def import_snapshot(self, limits, cols, source: str = "snapshot"):
+        """load_counters on arrays: the limits the counters were saved under (LIMIT_DESC_DTYPE) and the five counter
+        columns.  Refused before any counter changes if a limit the counters use is registered here with another
+        namespace, window or qualified flag."""
         mine = {int(d["limit_id"]): d for d in self.limits_get()}
         used = set(np.unique(cols[0]).tolist())
         bad = sorted(int(d["limit_id"]) for d in limits if int(d["limit_id"]) in used and int(d["limit_id"]) in mine
                      and any(int(d[k]) != int(mine[int(d["limit_id"])][k]) for k in ("ns_id", "window_us", "qualified")))
         if bad:
-            raise ValueError(f"{path}: limits {bad} are registered here with another namespace, window or qualified flag")
+            raise ValueError(f"{source}: limits {bad} are registered here with another namespace, window or qualified flag")
         self.import_counters(*cols)
+
+    # -- change tracking: what a journal on disk drains (limitador_b200.journal) --
+    def track_changes(self, on: bool = True):
+        """rl_counters_track: keep a device shadow of the table (one more copy of it in HBM) so that drain_changes can
+        list what changed; the next drain is full.  on=False frees the shadow."""
+        self._check(self._lib.rl_counters_track(self._h, int(on)))
+
+    def drain_changes(self, cap: int = 1 << 16):
+        """rl_counters_drain -> (full, (limit_id, key_lo, key_hi, value, expiry_us)).  full: every counter, exactly
+        export_counters().  Otherwise the counters changed since the last drain, an absent one as value = expiry = 0
+        (apply those before the others).  cap: rows of the first fetch; a drain that does not fit is fetched again,
+        whole.  Serialise with the decision calls."""
+        full = C.c_int(0)
+        cols = self._read_table(
+            lambda cap, *out: self._lib.rl_counters_drain(self._h, cap, MEM_HOST, *out, C.byref(full)), cap)
+        return bool(full.value), cols
 
 
 def owner_of(ns_id: int, world: int) -> int:

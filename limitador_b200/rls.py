@@ -29,7 +29,7 @@ RLS_SYMBOLS = (
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
     "rl_rls_last_timings", "rl_rls_plan_device", "rl_rls_keep_counter_vars", "rl_rls_counter_vars_stats",
     "rl_rls_counter_vars_gc", "rl_rls_counter_vars_export", "rl_rls_counter_vars_import", "rl_rls_configure",
-    "rl_rls_config_status",
+    "rl_rls_config_status", "rl_rls_counter_vars_drain",
 )
 
 ENTRY_DTYPE = np.dtype([("descriptor", "<u4"), ("key_off", "<u4"), ("key_len", "<u4"), ("val_off", "<u4"), ("val_len", "<u4")])
@@ -95,6 +95,7 @@ def _lib():
     L.rl_rls_counter_vars_gc.argtypes = [vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.rl_rls_counter_vars_export.argtypes = [vp, vp, u32, u64, u64, u64, vp, vp, vp, vp, vp, C.POINTER(u64), C.POINTER(u64)]
     L.rl_rls_counter_vars_import.argtypes = [vp, u64, vp, vp, vp, vp, vp, C.POINTER(u64)]
+    L.rl_rls_counter_vars_drain.argtypes = [vp, u64, u64, vp, vp, vp, vp, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(i32)]
     L.rl_rls_configure.argtypes = [vp, C.POINTER(LimitSpec), u32, i32, C.POINTER(ConfigureReport)]
     L.rl_rls_config_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L._rl_rls_ready = True
@@ -389,6 +390,22 @@ class RlsService:
         self._check(self._lib.rl_rls_counter_vars_import(self._h, n, vs.ctypes.data, lo.ctypes.data, hi.ctypes.data,
                                                          off.ctypes.data, b.ctypes.data if len(b) else None, C.byref(added)))
         return added.value
+
+    def drain_counter_vars(self):
+        """rl_rls_counter_vars_drain -> (full, (varset, key_lo, key_hi, blob_off, blobs)): the dictionary entries recorded
+        since the last drain, in export_counter_vars' layout.  full = True (and no entries) after keep_counter_vars,
+        counter_vars_gc or import_counter_vars: take export_counter_vars() then.  Serialise with serve."""
+        cnt, nb, full, cap, bcap = C.c_uint64(0), C.c_uint64(0), C.c_int(0), 0, 0
+        while True:  # count, then fetch: a drain that does not fit is not consumed
+            vs, lo, hi = np.zeros(max(cap, 1), np.uint32), np.zeros(max(cap, 1), np.uint64), np.zeros(max(cap, 1), np.uint64)
+            off, blobs = np.zeros(cap + 1, np.uint64), np.zeros(max(bcap, 1), np.uint8)
+            self._check(self._lib.rl_rls_counter_vars_drain(self._h, cap, bcap, vs.ctypes.data, lo.ctypes.data, hi.ctypes.data,
+                                                            off.ctypes.data, blobs.ctypes.data, C.byref(cnt), C.byref(nb),
+                                                            C.byref(full)))
+            if full.value or (cnt.value <= cap and nb.value <= bcap):
+                n = 0 if full.value else cnt.value
+                return bool(full.value), (vs[:n], lo[:n], hi[:n], off[:n + 1], blobs[:int(off[n])])
+            cap, bcap = int(cnt.value), int(nb.value)
 
     def save_counters(self, path: str, now_us: int = 0):
         """Engine.save_counters(path, now_us) of the service's engine, plus the dictionary entries those counters refer
