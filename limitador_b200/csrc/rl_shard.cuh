@@ -11,6 +11,9 @@
 // (source, owner, step) written with release and polled with acquire semantics at system scope.
 #pragma once
 #include "rl_kernels.cuh"
+#ifdef RL_SIMT
+#include <chrono>
+#endif
 
 #define RL_XCHG_MAX_WORLD 32
 #ifndef RL_XCHG_TIMEOUT_NS
@@ -41,18 +44,35 @@ struct RlXchg {
     }
 };
 
+// Under tests/emu/cuda_simt.h (RL_SIMT) the flag accesses are switch points of the emulator's interleaving mode around a
+// plain access (it has one memory and runs one fiber at a time), and the timer is the host's steady clock.
 __device__ __forceinline__ uint32_t rl_ld_acquire_sys(const uint32_t* p) {
+#ifdef RL_SIMT
+    RLM_EMU_SWITCH();
+    return *(volatile const uint32_t*)p;
+#else
     uint32_t v;
     asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
+#endif
 }
 __device__ __forceinline__ void rl_st_release_sys(uint32_t* p, uint32_t v) {
+#ifdef RL_SIMT
+    RLM_EMU_SWITCH();
+    *(volatile uint32_t*)p = v;
+#else
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+#endif
 }
 __device__ __forceinline__ unsigned long long rl_globaltimer() {
+#ifdef RL_SIMT
+    return (unsigned long long)std::chrono::duration_cast<std::chrono::nanoseconds>(
+               std::chrono::steady_clock::now().time_since_epoch()).count();
+#else
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
+#endif
 }
 // spin until *p has reached `want` (step flags only grow); false on time-out
 __device__ __forceinline__ bool rl_wait_flag(const uint32_t* p, uint32_t want) {

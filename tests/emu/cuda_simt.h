@@ -14,8 +14,8 @@
 // memory helpers of rl_devmem.cuh (rlm_ld, rlm_ld64, rlm_cas128, rlm_or) first hand control back to the scheduler with
 // probability p, and every pass of the scheduler visits the block's fibers in a seeded random order; p = 1 switches at
 // every one of them.  A kernel whose threads claim and then write shared words thus runs under many interleavings of
-// those steps, deterministically for one seed.  Global loads and stores (__ldcg, __ldcs, __ldg, __stcg) and
-// __threadfence are switch points too.
+// those steps, deterministically for one seed.  Global loads and stores (__ldcg, __ldcs, __ldg, __stcg),
+// __threadfence and __threadfence_system are switch points too.
 //
 // Resident blocks (simt_launch_ex): a launch keeps up to R blocks live at once, as an SM keeps several CTAs, and
 // dispatches the next block when one exits.  Every pass of the scheduler visits the fibers of all resident blocks (in
@@ -172,6 +172,7 @@ static inline void __stcg(T* p, T v) {
     *p = v;
 }
 static inline void __threadfence() { simt::interleave_point(); }
+static inline void __threadfence_system() { simt::interleave_point(); }
 static inline int __ffs(unsigned v) { return v ? __builtin_ctz(v) + 1 : 0; }
 static inline int __popc(unsigned v) { return __builtin_popcount(v); }
 

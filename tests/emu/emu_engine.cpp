@@ -1,8 +1,10 @@
 // emu_engine.cpp — TEST-ONLY host driver of the decision kernels (limitador_b200/csrc/rl_kernels.cuh: k_front, k_hot,
-// k_main, the resolve kernels, k_restore, k_fl_step, k_wide_scatter, k_scan) under tests/emu/cuda_simt.h: the SAME
-// kernel source the GPU runs, every CUDA thread a fiber, warp intrinsics as rendezvous, up to R k_main blocks resident at
-// once.  Not shipped, not a fallback.  The call sequences follow rl_engine.cu (run_record_pipeline without the pipeline,
-// run_acc_pipeline), the batch geometry is rl_batch_geom itself, and every call reports the geometry it reached.
+// k_main, the resolve kernels, k_restore, k_fl_step, k_wide_scatter, k_scan) and of the peer exchange
+// (limitador_b200/csrc/rl_shard.cuh: k_xcount .. k_xgather) under tests/emu/cuda_simt.h: the SAME kernel source the GPU
+// runs, every CUDA thread a fiber, warp intrinsics as rendezvous, up to R k_main blocks resident at once.  Not shipped,
+// not a fallback.  The call sequences follow rl_engine.cu (run_record_pipeline without the pipeline, run_acc_pipeline)
+// and rl_shard_host.inc (rl_shard_send / _decide / _collect over `world` emulated engines and their slabs), the batch
+// geometry is rl_batch_geom itself, and every call reports the geometry it reached.
 #include "cuda_simt.h"
 // (the emulator must come first: it defines __global__ & co. away)
 #include <algorithm>
@@ -11,7 +13,7 @@
 #include <map>
 #include <vector>
 
-#include "../../limitador_b200/csrc/rl_kernels.cuh"
+#include "../../limitador_b200/csrc/rl_shard.cuh"
 
 namespace {
 
@@ -46,14 +48,14 @@ struct emu_engine {
     bool any_multi_ns = false;
     // knobs
     uint32_t chunk = 128, part_target = 128, heavy_mult = 2, main_grid_cap = 132 * 16, weak = 0, hot_on = 0, resident = 1;
-    uint32_t n_dev = 0;  // sharded geometry: the access count lives on the device, the tile is derived there
+    uint32_t n_dev = 0;  // sharded geometry on a plain call: the access count lives on the device, the tile is derived there
     bool interleave = false;
     uint64_t seed = 0;
     double p = 1.0;
     // device state that lives across calls
     std::vector<uint32_t> hot;  // hot_rows [RL_HOT_SLOTS] | hot_cand [RL_HOT_CAND] | hot_cand_n | pad
     std::vector<uint32_t> region_total, small;
-    uint32_t err = 0, flags = 0, changed = 0;
+    uint32_t err[8] = {}, flags = 0, changed = 0;  // err: sticky RL_DEV_* code; err[7]: the exchange's detail word
     unsigned long long kstats[32] = {};
     unsigned long long report[G_N] = {};
 };
@@ -158,7 +160,7 @@ RlDev make_dev(emu_engine* e) {
     D.ns = e->ns.data();
     D.ns_cap = (uint32_t)e->ns.size();
     D.ns_limit_ids = e->ns_ids.data();
-    D.err = &e->err;
+    D.err = e->err;
     D.flags = &e->flags;
     D.kstats = e->kstats;
     D.hot_rows = e->hot.data();
@@ -180,25 +182,25 @@ struct Work {
     uint32_t n_dev = 0;
 };
 
+// n_hint / n_dev (sharded steps, rl_shard_decide): n_acc is only the upper bound of the device-side count *n_dev, the
+// partitions are sized for n_hint and the kernels derive the tile from *n_dev
 RlBatch make_batch(emu_engine* e, Work& w, uint32_t n_acc, uint32_t n_req, uint8_t* lim, uint32_t* first, uint64_t* rem,
-                   uint64_t* ttl, const uint32_t* off, uint32_t stride, int lc, bool hot_ok) {
+                   uint64_t* ttl, const uint32_t* off, uint32_t stride, int lc, bool hot_ok, uint32_t n_hint = 0,
+                   const uint32_t* n_dev = nullptr) {
     RlBatch B;
     memset(&B, 0, sizeof B);
     B.nhot = (hot_ok && e->hot_on) ? RL_HOT_SLOTS : 0;
     B.n_acc = n_acc;
     B.n_req = n_req;
-    const RlBatchGeom g = rl_batch_geom(n_acc, e->n_dev ? n_acc : 0, e->log2P, e->part_target, e->chunk, e->heavy_mult);
+    const RlBatchGeom g = rl_batch_geom(n_acc, n_hint, e->log2P, e->part_target, e->chunk, e->heavy_mult);
     B.tile = g.tile;
     B.num_tiles = g.num_tiles;
     B.nparts = g.nparts;
     B.part_shift = g.part_shift;
     B.heavy_len = g.heavy_len;
-    if (e->n_dev) {
-        w.n_dev = n_acc;
-        B.n_dev = &w.n_dev;
-    }
+    B.n_dev = n_dev;
     const uint32_t P1 = (1u << e->log2P) + RL_HOT_SLOTS + 1;
-    const uint32_t tsz = e->n_dev ? std::max<uint32_t>(256, ((rl_ceil_div(n_acc, g.num_tiles) + 255) / 256) * 256) : g.tile;
+    const uint32_t tsz = n_dev ? std::max<uint32_t>(256, ((rl_ceil_div(n_acc, g.num_tiles) + 255) / 256) * 256) : g.tile;
     const size_t buf = (size_t)g.num_tiles * tsz;
     const size_t max_items = (size_t)(1u << e->log2P) + n_acc / 128 + 2 + g.nparts;
     w.tile_loc.assign((size_t)(g.num_tiles + 1) * (P1 + 1), 0xA5A5A5A5u);
@@ -333,7 +335,7 @@ void launch_main(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src
 void begin_call(emu_engine* e) {
     memset(e->report, 0, sizeof e->report);
     memset(e->kstats, 0, sizeof e->kstats);
-    e->err = 0;
+    memset(e->err, 0, sizeof e->err);
     e->flags = 0;
     for (uint32_t h = 0; h < RL_HOT_SLOTS; h++) e->report[G_HOT_IN_USE] += e->hot[h] != 0xFFFFFFFFu;
 }
@@ -349,7 +351,7 @@ int end_call(emu_engine* e) {
     bool rearmed = e->small[0] == 0 && e->small[2] == 0 && e->small[3] == 0;
     for (uint32_t v : e->region_total) rearmed = rearmed && v == 0;
     g[G_REARMED] = rearmed;
-    return (int)e->err;
+    return (int)e->err[0];
 }
 
 // run_acc_pipeline (rl_engine.cu:514-587): accesses that may hold coupled (multi-row) requests.  check_and_update with
@@ -470,12 +472,14 @@ uint32_t emu_engine_record_stride(emu_engine* e) { return e->any_multi_ns ? std:
 // check_and_update (mode 0) / update_counters (mode 2) over 32-byte records: run_record_pipeline (rl_engine.cu:600-677)
 // without the pipeline — k_front, k_hot when hot rows are on, k_main — or, when some namespace spans several rows, the
 // records resolved into accesses (k_resolve_records, narrow or wide) and run_acc_pipeline.  rem / ttl: [n * stride]
-// with stride = emu_engine_record_stride.  Returns the device error code.
+// with stride = emu_engine_record_stride.  compact_now != 0: recs points at n 16-byte rl_record16 stamped with that one
+// clock reading (rl_check_and_update_compact; single-row namespaces only).  Returns the device error code.
 int emu_engine_records(emu_engine* e, int mode, uint32_t n, const rl_record* recs, int lc, uint8_t* lim, uint32_t* first,
-                       uint64_t* rem, uint64_t* ttl) {
+                       uint64_t* rem, uint64_t* ttl, uint64_t compact_now) {
     begin_call(e);
     RlDev D = make_dev(e);
     if (e->any_multi_ns) {
+        if (compact_now) return -1;  // run_record_pipeline refuses it
         const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
         const bool wide = stride > RL_MAX_CTRS_PER_REQ;
         std::vector<RlAccess> acc((size_t)n * stride);
@@ -485,14 +489,17 @@ int emu_engine_records(emu_engine* e, int mode, uint32_t n, const rl_record* rec
         const uint32_t blocks = rl_ceil_div(n, 128);
         if (wide) simt_launch(blocks, 128, [&] { k_resolve_records_wide(D, n, recs, stride, O, mode == 0, perm.data(), RL_MAX_CTRS_PER_REQ_WIDE); });
         else simt_launch(blocks, 128, [&] { k_resolve_records(D, n, recs, stride, O, mode == 0); });
-        if (e->err) return (int)e->err;
+        if (e->err[0]) return (int)e->err[0];
         if (acc_pipeline(e, D, acc, n, delta.data(), now.data(), mode, lc, lim, first, rem, ttl, nullptr, stride, wide, perm, stride))
             return -1;
         return end_call(e);
     }
     Work w;
-    RlBatch B = make_batch(e, w, n, n, lim, first, rem, ttl, nullptr, e->cells, lc, true);
-    RecordSrc src{recs, nullptr, 0, 0, 0, 0};
+    // the sharded knob: the count handed over on the device (n_hint = n_dev = n), the tile derived from it there
+    w.n_dev = n;
+    RlBatch B = make_batch(e, w, n, n, lim, first, rem, ttl, nullptr, e->cells, lc, true, e->n_dev ? n : 0,
+                           e->n_dev ? &w.n_dev : nullptr);
+    RecordSrc src{recs, nullptr, 0, 0, compact_now ? 1u : 0u, compact_now};
     launch_front(e, D, B, src);
     report_front(e, B, w);
     if (mode == 2) launch_main<RecordSrc, 2>(e, D, B, src);
@@ -515,7 +522,7 @@ int emu_engine_csr(emu_engine* e, int mode, uint32_t n, const uint32_t* off, con
     const uint32_t blocks = rl_ceil_div(n, 128);
     if (wide) simt_launch(blocks, 128, [&] { k_resolve_csr_wide(D, n, off, ctrs, O, mode == 0, perm.data(), RL_MAX_CTRS_PER_REQ_WIDE); });
     else simt_launch(blocks, 128, [&] { k_resolve_csr(D, n, off, ctrs, O, mode == 0); });
-    if (e->err) return (int)e->err;
+    if (e->err[0]) return (int)e->err[0];
     if (acc.empty()) return end_call(e);
     if (acc_pipeline(e, D, acc, n, delta, now, mode, lc, lim, first, rem, ttl, off, 0, wide, perm, 0)) return -1;
     return end_call(e);
@@ -532,7 +539,7 @@ int emu_engine_query_records(emu_engine* e, uint32_t n, const rl_record* recs, u
     if (e->cells == 1) run(std::integral_constant<int, 1>{});
     else if (e->cells == 3) run(std::integral_constant<int, 3>{});
     else run(std::integral_constant<int, 7>{});
-    return (int)e->err;
+    return (int)e->err[0];
 }
 
 // the table through k_scan in export mode (read_table, rl_engine.cu:1149-1219, now = 0: every present cell as
@@ -554,5 +561,188 @@ uint64_t emu_engine_export(emu_engine* e, uint64_t cap, uint32_t* lid, uint64_t*
     else run(std::integral_constant<int, 7>{});
     return cnt;
 }
+
+}  // extern "C"
+
+// ---- the namespace-sharded peer exchange (rl_shard_host.inc) over `world` emulated engines -------------------------
+// Every rank has a host "slab" laid out as rl_shard_create lays out the device one (records | verdict inboxes | control
+// words, depth = lag + 2 buffers) and its own exchange workspace; X.base[] of every rank names all the slabs, as
+// rl_shard_connect_ptrs does.  The launches run in the caller's issue order, one at a time: a wait kernel issued before
+// the kernels it waits for is reported by cuda_simt.h as a hang.
+struct emu_shard_rank {
+    emu_engine* e = nullptr;
+    std::vector<uint8_t> slab;
+    RlXchg X{};
+    std::vector<uint32_t> tile_cnt, totals, ctrs, dest, seg;
+    std::vector<uint8_t> verdict;  // the decide call's local mirror of the sources' verdict blocks [world][cap]
+    uint64_t sent = 0, decided = 0, collected = 0;
+    static constexpr int kRingN = 8;
+    uint32_t n_of[kRingN] = {};
+    uint8_t* out_of[kRingN] = {};
+};
+struct emu_shard {
+    uint32_t world = 1, cap = 0, lag = 0, depth = 2, max_batch = 0;
+    size_t recs_bytes = 0, vin_bytes = 0, ctl_bytes = 0;
+    std::vector<emu_shard_rank> r;
+};
+
+namespace {
+constexpr uint8_t kPoison = 0xA5;
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+}  // namespace
+
+extern "C" {
+
+// world engines (one per rank, each with its limits set), cap records per source batch (a multiple of 16), lag 0..4,
+// max_batch of every engine (an owner's inbox larger than min(world x cap, max_batch) fails the step).  NULL on bad input.
+emu_shard* emu_shard_create(emu_engine** engines, uint32_t world, uint32_t cap, uint32_t lag, uint32_t max_batch) {
+    if (world == 0 || world > RL_XCHG_MAX_WORLD || cap == 0 || (cap & 15u) || lag > 4) return nullptr;
+    emu_shard* S = new emu_shard();
+    S->world = world;
+    S->cap = cap;
+    S->lag = lag;
+    S->depth = lag + 2;
+    S->max_batch = max_batch;
+    S->recs_bytes = align256((size_t)S->depth * world * cap * sizeof(rl_record));
+    S->vin_bytes = align256((size_t)S->depth * world * cap);
+    S->ctl_bytes = align256((size_t)S->depth * world * sizeof(RlXCtl));
+    S->r.resize(world);
+    for (uint32_t k = 0; k < world; k++) {
+        emu_shard_rank& R = S->r[k];
+        R.e = engines[k];
+        R.slab.assign(S->recs_bytes + S->vin_bytes + S->ctl_bytes, 0);  // rl_shard_create zeroes the slab
+        R.tile_cnt.assign((size_t)(RL_MAX_TILES + 1) * 32, 0);
+        R.totals.assign(32, 0);
+        R.ctrs.assign(4, 0);
+        R.dest.assign((size_t)S->depth * cap, 0);
+        R.seg.assign(40, 0);
+        R.verdict.assign((size_t)world * cap, 0);
+    }
+    for (uint32_t k = 0; k < world; k++) {
+        RlXchg& X = S->r[k].X;
+        X.trace = nullptr;
+        X.trace_pos = nullptr;
+        for (auto& b : X.base) b = nullptr;
+        for (uint32_t j = 0; j < world; j++) X.base[j] = S->r[j].slab.data();
+        X.off_recs = 0;
+        X.off_vin = S->recs_bytes;
+        X.off_ctl = S->recs_bytes + S->vin_bytes;
+        X.world = world;
+        X.rank = k;
+        X.cap = cap;
+        X.depth = S->depth;
+    }
+    return S;
+}
+void emu_shard_destroy(emu_shard* S) { delete S; }
+
+// rl_shard_send: bucket rank's n records by owner (k_xcount) and store them into the owners' inboxes (k_xscatter).  The
+// blocks this step writes, the verdict blocks it will read and dest are poisoned first, so that a read past a fill or a
+// missing verdict shows as a wrong result, not as a stale correct one.  out: n verdict bytes, filled by the collection.
+int emu_shard_send(emu_shard* S, uint32_t rank, uint32_t n, const rl_record* recs, uint8_t* out) {
+    emu_shard_rank& R = S->r[rank];
+    if (n > S->cap || R.sent - R.collected > S->lag || (n && (!recs || !out))) return -1;
+    const uint32_t step = (uint32_t)R.sent, buf = (uint32_t)(R.sent % S->depth), world = S->world;
+    for (uint32_t o = 0; o < world; o++) {
+        memset(R.X.inbox(o, buf, rank), kPoison, (size_t)S->cap * sizeof(rl_record));
+        memset(R.X.vin(rank, buf, o), kPoison, S->cap);
+    }
+    std::fill(R.dest.begin() + (size_t)buf * S->cap, R.dest.begin() + (size_t)(buf + 1) * S->cap, 0xA5A5A5A5u);
+    std::fill(R.tile_cnt.begin(), R.tile_cnt.end(), 0xA5A5A5A5u);
+    std::fill(R.totals.begin(), R.totals.end(), 0xA5A5A5A5u);
+    uint32_t tile = rl_ceil_div(std::max<uint64_t>(n, 1), RL_MAX_TILES);
+    tile = std::max<uint32_t>(256, ((tile + 255) / 256) * 256);
+    const uint32_t num_tiles = std::max<uint32_t>(1, rl_ceil_div(n, tile));
+    // static __shared__ arrays: one copy for all blocks, so one block at a time
+    simt_launch(num_tiles, RL_PART_THREADS, [&] {
+        k_xcount(recs, n, world, tile, R.tile_cnt.data(), R.totals.data(), R.ctrs.data() + 0, nullptr, nullptr, step);
+    });
+    simt_launch(num_tiles, RL_PART_THREADS, [&] {
+        k_xscatter(R.X, recs, n, tile, R.tile_cnt.data(), R.totals.data(), buf, step, R.dest.data() + (size_t)buf * S->cap,
+                   R.ctrs.data() + 1);
+    });
+    R.n_of[R.sent % emu_shard_rank::kRingN] = n;
+    R.out_of[R.sent % emu_shard_rank::kRingN] = out;
+    R.sent++;
+    return 0;
+}
+
+// rl_shard_decide: k_xwait, then the record path over the segmented inbox (n_acc = min(world x cap, max_batch), partitions
+// sized for one source batch, the tile derived from the inbox fill on the device), the verdicts into the local mirror
+// (poisoned first), then k_xreturn.  The engine's report holds the call's geometry; returns the device error code.
+int emu_shard_decide(emu_shard* S, uint32_t rank) {
+    emu_shard_rank& R = S->r[rank];
+    emu_engine* e = R.e;
+    if (R.decided >= R.sent || e->any_multi_ns) return -1;
+    const uint32_t step = (uint32_t)R.decided, buf = (uint32_t)(R.decided % S->depth), world = S->world, cap = S->cap;
+    const uint32_t n_max = (uint32_t)std::min<uint64_t>((uint64_t)world * cap, S->max_batch);
+    begin_call(e);
+    RlDev D = make_dev(e);
+    std::fill(R.seg.begin(), R.seg.end(), 0xA5A5A5A5u);
+    std::fill(R.verdict.begin(), R.verdict.end(), kPoison);
+    uint32_t* segp = R.seg.data();
+    simt_launch(1, 32, [&] { k_xwait(R.X, buf, step, segp, segp + 36, n_max, e->err); });
+    const RecordSrc src{R.X.inbox(rank, buf, 0), segp, world, cap, 0, 0};
+    Work w;
+    RlBatch B = make_batch(e, w, n_max, n_max, R.verdict.data(), nullptr, nullptr, nullptr, nullptr, 0, 0, true, cap, segp + 36);
+    B.omap_prefix = segp;
+    B.omap_n = world;
+    B.omap_stride = cap;
+    launch_front(e, D, B, src);
+    report_front(e, B, w);
+    launch_main<RecordSrc, 0>(e, D, B, src);
+    simt_launch(world * RL_XRET_SLICES, 256, [&] { k_xreturn(R.X, R.verdict.data(), segp, buf, step, R.ctrs.data() + 2); });
+    R.decided++;
+    return end_call(e);
+}
+
+// rl_shard_collect (all = 0: only once more than `lag` decided steps are outstanding) / rl_shard_flush (all = 1): k_xwaitv,
+// then k_xgather into the step's output.  Returns the steps collected.
+int emu_shard_collect(emu_shard* S, uint32_t rank, int all) {
+    emu_shard_rank& R = S->r[rank];
+    emu_engine* e = R.e;
+    int done = 0;
+    while (R.collected < R.decided && (all || R.decided - R.collected > S->lag)) {
+        const uint32_t step = (uint32_t)R.collected, buf = (uint32_t)(R.collected % S->depth);
+        const uint32_t n = R.n_of[R.collected % emu_shard_rank::kRingN];
+        uint8_t* out = R.out_of[R.collected % emu_shard_rank::kRingN];
+        simt_launch(1, 32, [&] { k_xwaitv(R.X, buf, step, e->err); });
+        if (n) {
+            const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>(rl_ceil_div(n, 256), e->main_grid_cap / 8));
+            simt_launch(grid, 256, [&] { k_xgather(R.X, n, R.dest.data() + (size_t)buf * S->cap, buf, out); });
+        }
+        R.collected++;
+        done++;
+    }
+    return done;
+}
+
+// k_xwait alone on rank's control words of (buf, step) (set them first with emu_shard_set_ctl, so that nothing waits):
+// seg_out [40] = the exclusive prefix seg_prefix[0..world] and, at [36], n_dev; err_out [8] = the error words
+void emu_shard_xwait(emu_shard* S, uint32_t rank, uint32_t buf, uint32_t step, uint32_t n_max, uint32_t* seg_out,
+                     uint32_t* err_out) {
+    emu_shard_rank& R = S->r[rank];
+    std::fill(seg_out, seg_out + 40, 0xA5A5A5A5u);
+    memset(err_out, 0, 8 * sizeof(uint32_t));
+    simt_launch(1, 32, [&] { k_xwait(R.X, buf, step, seg_out, seg_out + 36, n_max, err_out); });
+}
+
+// rank's control words: [(buf * world + peer) * 4 + {0 cnt, 1 rflag, 2 vflag, 3 pad}], depth * world * 4 of them
+void emu_shard_ctl(emu_shard* S, uint32_t rank, uint32_t* out) {
+    memcpy(out, S->r[rank].slab.data() + S->recs_bytes + S->vin_bytes, (size_t)S->depth * S->world * sizeof(RlXCtl));
+}
+void emu_shard_set_ctl(emu_shard* S, uint32_t rank, const uint32_t* in) {
+    memcpy(S->r[rank].slab.data() + S->recs_bytes + S->vin_bytes, in, (size_t)S->depth * S->world * sizeof(RlXCtl));
+}
+// block `src` of owner's inbox `buf` (cap records), rank's dest of `buf` (cap words), its blocks-done counters (4 words:
+// k_xcount, k_xscatter, k_xreturn, unused) and its error words of the last decide / collect (8 words)
+void emu_shard_inbox(emu_shard* S, uint32_t owner, uint32_t buf, uint32_t src, rl_record* out) {
+    memcpy(out, S->r[owner].X.inbox(owner, buf, src), (size_t)S->cap * sizeof(rl_record));
+}
+void emu_shard_dest(emu_shard* S, uint32_t rank, uint32_t buf, uint32_t* out) {
+    memcpy(out, S->r[rank].dest.data() + (size_t)buf * S->cap, (size_t)S->cap * sizeof(uint32_t));
+}
+void emu_shard_ctrs(emu_shard* S, uint32_t rank, uint32_t* out) { memcpy(out, S->r[rank].ctrs.data(), 4 * sizeof(uint32_t)); }
+void emu_shard_err(emu_shard* S, uint32_t rank, uint32_t* out) { memcpy(out, S->r[rank].e->err, 8 * sizeof(uint32_t)); }
 
 }  // extern "C"

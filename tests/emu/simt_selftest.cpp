@@ -110,6 +110,7 @@ __global__ void k_flag_wait(volatile unsigned* flag, unsigned* seen) {
         __syncthreads();
         if (threadIdx.x == 0) {
             __threadfence();
+            __threadfence_system();  // a switch point like __threadfence (the peer exchange's kernels fence at system scope)
             atomicExch(const_cast<unsigned*>(flag), 1u);
         }
         return;

@@ -903,8 +903,8 @@ def run_edge_kat(kat, layer, batched, lc):
 @functools.cache
 def emu_engine_lib():
     """tests/emu/emu_engine.cpp: the decision kernels (k_front, k_hot, k_main, the resolve kernels, k_restore,
-    k_fl_step, k_wide_scatter, k_query_records, k_scan) compiled for the host under tests/emu/cuda_simt.h, driven
-    through the engine's call sequences."""
+    k_fl_step, k_wide_scatter, k_query_records, k_scan) and the peer exchange's (k_xcount .. k_xgather) compiled for
+    the host under tests/emu/cuda_simt.h, driven through the engine's and the shard's call sequences."""
     L = host_lib("emu_engine.cpp", "librl_emu_engine.so")
     vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
     L.emu_engine_create.restype = vp
@@ -923,11 +923,26 @@ def emu_engine_lib():
     L.emu_engine_record_stride.argtypes = [vp]
     L.emu_engine_record_region.restype = C.c_int64
     L.emu_engine_record_region.argtypes = [vp, vp]
-    L.emu_engine_records.argtypes = [vp, C.c_int, u32, vp, C.c_int, vp, vp, vp, vp]
+    L.emu_engine_records.argtypes = [vp, C.c_int, u32, vp, C.c_int, vp, vp, vp, vp, u64]
     L.emu_engine_csr.argtypes = [vp, C.c_int, u32, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]
     L.emu_engine_query_records.argtypes = [vp, u32, vp, vp, vp]
     L.emu_engine_export.restype = u64
     L.emu_engine_export.argtypes = [vp, u64, vp, vp, vp, vp, vp]
+    L.emu_shard_create.restype = vp
+    L.emu_shard_create.argtypes = [vp, u32, u32, u32, u32]
+    L.emu_shard_destroy.argtypes = [vp]
+    L.emu_shard_send.argtypes = [vp, u32, u32, vp, vp]
+    L.emu_shard_decide.argtypes = [vp, u32]
+    L.emu_shard_collect.argtypes = [vp, u32, C.c_int]
+    L.emu_shard_xwait.argtypes = [vp, u32, u32, u32, u32, vp, vp]
+    L.emu_shard_xwait.restype = None
+    for f in ("ctl", "set_ctl", "ctrs", "err"):
+        getattr(L, f"emu_shard_{f}").argtypes = [vp, u32, vp]
+        getattr(L, f"emu_shard_{f}").restype = None
+    L.emu_shard_inbox.argtypes = [vp, u32, u32, u32, vp]
+    L.emu_shard_inbox.restype = None
+    L.emu_shard_dest.argtypes = [vp, u32, u32, vp]
+    L.emu_shard_dest.restype = None
     return L
 
 
@@ -985,9 +1000,22 @@ class EmuEngine:
         fl = np.full(n, 0xA5A5A5A5, dtype=np.uint32)
         rem = np.zeros(n * stride, dtype=np.uint64)
         ttl = np.zeros(n * stride, dtype=np.uint64)
-        err = self.L.emu_engine_records(self.h, mode, n, _p(recs), int(load_counters), _p(lim), _p(fl), _p(rem), _p(ttl))
+        err = self.L.emu_engine_records(self.h, mode, n, _p(recs), int(load_counters), _p(lim), _p(fl), _p(rem), _p(ttl), 0)
         self._report()
         return lim, fl, rem, ttl, err
+
+    def records16(self, recs16, now_us):
+        """check_and_update over 16-byte records (rl_record16) stamped with one clock reading: limited, first-limited
+        and the device error code."""
+        from limitador_b200.engine import RECORD16_DTYPE
+        recs16 = np.ascontiguousarray(recs16, dtype=RECORD16_DTYPE)
+        n = len(recs16)
+        lim = np.full(n, 0xA5, dtype=np.uint8)
+        fl = np.full(n, 0xA5A5A5A5, dtype=np.uint32)
+        assert now_us != 0  # 0 selects the 32-byte form
+        err = self.L.emu_engine_records(self.h, 0, n, _p(recs16), 0, _p(lim), _p(fl), None, None, int(now_us))
+        self._report()
+        return lim, fl, err
 
     def csr(self, mode, off, ctrs, delta, now_us, load_counters=False):
         off = np.ascontiguousarray(off, dtype=np.uint32)
@@ -1018,3 +1046,81 @@ class EmuEngine:
         c = int(self.L.emu_engine_export(self.h, cap, _p(lid), _p(lo), _p(hi), _p(val), _p(exp)))
         assert c <= cap
         return sorted(zip(lid[:c].tolist(), lo[:c].tolist(), hi[:c].tolist(), val[:c].tolist(), exp[:c].tolist()))
+
+
+class EmuShard:
+    """The namespace-sharded peer exchange on the host (tests/emu/emu_engine.cpp's emu_shard_*): one EmuEngine per rank
+    and host slabs laid out as rl_shard_create lays out the device ones; send / decide / collect follow rl_shard_send,
+    rl_shard_decide and rl_shard_collect launch for launch.  The caller issues them in an order in which every wait
+    kernel runs after the kernels it waits for (every rank sends, then every rank decides, then every rank collects)."""
+
+    def __init__(self, engines, cap, lag, max_batch=None):
+        self.L = emu_engine_lib()
+        self.engines = list(engines)
+        self.world, self.cap, self.lag, self.depth = len(engines), cap, lag, lag + 2
+        arr = (C.c_void_p * self.world)(*[e.h for e in self.engines])
+        mb = self.world * cap if max_batch is None else max_batch
+        self.h = self.L.emu_shard_create(arr, self.world, cap, lag, mb)
+        assert self.h, "emu_shard_create refused its arguments"
+        self._keep = {}  # (rank, step) -> (records, verdict output): the slab and the collection point at them
+        self._sent = [0] * self.world
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.L.emu_shard_destroy(self.h)
+
+    def send(self, rank, recs):
+        """Returns the verdict array the step's collection fills (poisoned until then)."""
+        recs = np.ascontiguousarray(recs, dtype=RECORD_DTYPE)
+        out = np.full(max(len(recs), 1), 0xA5, dtype=np.uint8)
+        assert self.L.emu_shard_send(self.h, rank, len(recs), _p(recs), _p(out)) == 0
+        self._keep[(rank, self._sent[rank])] = (recs, out)
+        self._sent[rank] += 1
+        return out[:len(recs)]
+
+    def decide(self, rank):
+        """The device error code of the call; the engine's `geometry` says what it reached."""
+        err = self.L.emu_shard_decide(self.h, rank)
+        self.engines[rank]._report()
+        return err
+
+    def collect(self, rank, flush=False):
+        return int(self.L.emu_shard_collect(self.h, rank, int(flush)))
+
+    def ctl(self, rank):
+        """Control words as [buffer, peer, (cnt, rflag, vflag, pad)]."""
+        out = np.zeros(self.depth * self.world * 4, dtype=np.uint32)
+        self.L.emu_shard_ctl(self.h, rank, _p(out))
+        return out.reshape(self.depth, self.world, 4)
+
+    def set_ctl(self, rank, words):
+        w = np.ascontiguousarray(words, dtype=np.uint32).reshape(-1)
+        assert len(w) == self.depth * self.world * 4
+        self.L.emu_shard_set_ctl(self.h, rank, _p(w))
+
+    def xwait(self, rank, buf, step, n_max):
+        """k_xwait alone: (seg_prefix[0..world], n_dev, error words)."""
+        seg = np.zeros(40, dtype=np.uint32)
+        err = np.zeros(8, dtype=np.uint32)
+        self.L.emu_shard_xwait(self.h, rank, buf, step, n_max, _p(seg), _p(err))
+        return seg[:self.world + 1], int(seg[36]), err
+
+    def inbox(self, owner, buf, src):
+        out = np.zeros(self.cap, dtype=RECORD_DTYPE)
+        self.L.emu_shard_inbox(self.h, owner, buf, src, _p(out))
+        return out
+
+    def dest(self, rank, buf):
+        out = np.zeros(self.cap, dtype=np.uint32)
+        self.L.emu_shard_dest(self.h, rank, buf, _p(out))
+        return out
+
+    def ctrs(self, rank):
+        out = np.zeros(4, dtype=np.uint32)
+        self.L.emu_shard_ctrs(self.h, rank, _p(out))
+        return out
+
+    def err(self, rank):
+        out = np.zeros(8, dtype=np.uint32)
+        self.L.emu_shard_err(self.h, rank, _p(out))
+        return out
