@@ -1,4 +1,4 @@
-// rl_engine.cu — host side of librl_engine.so: limit registry, device tables, workspace,
+// rl_engine.cu — host side of librl_engine.so: the device tables of the limit registry (rl_registry.h), workspace,
 // kernel launches and the C-ABI declared in include/rl_engine.h.
 //
 // There is NO CPU fallback: every entry point either runs the sm_90a kernels or returns
@@ -11,9 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
-#include <map>
 #include <string>
-#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -21,6 +19,7 @@
 #include "rl_kernels.cuh"
 #include "rl_shard.cuh"
 #include "rl_internal.h"
+#include "rl_registry.h"
 
 #ifndef RL_SETS
 #define RL_SETS 3  // RL_FLAG_PIPELINE: calls in flight on the device (>= 3: one per pipeline stage)
@@ -33,21 +32,6 @@ namespace {
 
 constexpr uint32_t kMaxTiles = RL_MAX_TILES;
 constexpr uint32_t kMaxRegions = 4096;
-
-struct HostLimit {
-    bool defined = false;
-    uint32_t ns = 0, varset = 0, qualified = 0;
-    uint64_t max_value = 0, window_us = 0;
-    uint32_t group = 0, cell = 0;
-    bool simple_present = false;  // unqualified: entry exists in simple_limits (in_memory.rs:14)
-};
-struct HostGroup {
-    uint32_t ns = 0, varset = 0, qualified = 0;
-    uint32_t limit_of_cell[RL_MAX_CELLS];
-    HostGroup() {
-        for (auto& l : limit_of_cell) l = RL_NONE_U32;
-    }
-};
 
 }  // namespace
 
@@ -68,16 +52,9 @@ struct rl_engine {
     uint32_t max_ctrs_req = RL_MAX_CTRS_PER_REQ;  // rl_config.max_counters_per_request (16: narrow encoding only)
     DevBuf<uint8_t> d_rows;
 
-    // registry
-    std::vector<HostLimit> limits;
-    std::vector<HostGroup> groups;  // [0] unused
-    std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> groups_by_key;
-    std::vector<std::vector<uint32_t>> ns_limits;  // registration order
-    bool tables_dirty = true;
+    RlRegistry reg;
     uint64_t structure_epoch = 0;  // calls that can move rows or re-map cells (rl_counters_drain: the next drain is full)
-    bool any_multi_ns = false;
-    uint32_t max_ns_limits = 0;
-    uint32_t max_cells_used = 1;  // highest cell index + 1 over all row groups
+    RlTableShape shape;            // of the uploaded tables
 
     // device tables
     DevBuf<RlCellDesc> d_desc;
@@ -202,88 +179,24 @@ RlDev make_dev(rl_engine* e) {
 
 // Rebuild and upload the limit / group / namespace tables.
 int upload_tables(rl_engine* e) {
-    if (!e->tables_dirty) return RL_OK;
-    const size_t ngroups = e->groups.size();
-    std::vector<RlCellDesc> desc(ngroups * 8);
-    std::vector<uint32_t> group_ns(ngroups, 0);
-    for (auto& d : desc) {
-        d.max_value = 0;
-        d.window_us = 0;
-        d.limit_id = RL_NONE_U32;
-        d.qualified = 0;
-    }
-    e->max_cells_used = 1;
-    for (size_t g = 1; g < ngroups; g++) {
-        group_ns[g] = e->groups[g].ns;
-        for (uint32_t c = 0; c < RL_MAX_CELLS; c++) {
-            const uint32_t lid = e->groups[g].limit_of_cell[c];
-            if (lid == RL_NONE_U32) continue;
-            e->max_cells_used = std::max(e->max_cells_used, c + 1);
-            const HostLimit& l = e->limits[lid];
-            RlCellDesc& d = desc[g * 8 + c];
-            d.max_value = l.max_value;
-            d.window_us = l.window_us;
-            d.limit_id = lid;
-            d.qualified = l.qualified;
-        }
-    }
-    std::vector<RlLimitDev> lim(std::max<size_t>(e->limits.size(), 1));
-    for (size_t i = 0; i < lim.size(); i++) {
-        lim[i].group = 0;
-        lim[i].cell = 0;
-        lim[i].ns_id = 0;
-        lim[i].qualified = 0;
-        if (i < e->limits.size() && e->limits[i].defined) {
-            lim[i].group = e->limits[i].group;
-            lim[i].cell = e->limits[i].cell;
-            lim[i].ns_id = e->limits[i].ns;
-            lim[i].qualified = e->limits[i].qualified;
-        }
-    }
-    std::vector<RlNsDev> ns(std::max<size_t>(e->ns_limits.size(), 1));
-    std::vector<uint32_t> ns_ids;
-    e->any_multi_ns = false;
-    e->max_ns_limits = 0;
-    for (size_t n = 0; n < ns.size(); n++) {
-        memset(&ns[n], 0, sizeof(RlNsDev));
-        if (n >= e->ns_limits.size() || e->ns_limits[n].empty()) continue;
-        const auto& L = e->ns_limits[n];
-        ns[n].lim_off = (uint32_t)ns_ids.size();
-        ns[n].lim_cnt = (uint32_t)L.size();
-        e->max_ns_limits = std::max<uint32_t>(e->max_ns_limits, (uint32_t)L.size());
-        bool single = L.size() <= RL_MAX_CELLS;
-        for (uint32_t lid : L) {
-            ns_ids.push_back(lid);
-            if (e->limits[lid].group != e->limits[L[0]].group) single = false;
-        }
-        if (single) {
-            ns[n].mode = 1;
-            ns[n].group = e->limits[L[0]].group;
-            ns[n].qualified_row = e->limits[L[0]].qualified;
-            uint32_t cells = 0;
-            for (size_t k = 0; k < L.size(); k++) cells |= e->limits[L[k]].cell << (4 * k);
-            ns[n].cells = cells | ((uint32_t)L.size() << 28);
-        } else {
-            ns[n].mode = 2;
-            e->any_multi_ns = true;
-        }
-    }
-    if (ns_ids.empty()) ns_ids.push_back(0);
-    RL_CUDA(e, e->d_desc.reserve(desc.size()));
-    RL_CUDA(e, e->d_limits.reserve(lim.size()));
-    RL_CUDA(e, e->d_ns.reserve(ns.size()));
-    RL_CUDA(e, e->d_ns_limit_ids.reserve(ns_ids.size()));
-    RL_CUDA(e, e->d_group_ns.reserve(group_ns.size()));
+    if (!e->reg.dirty) return RL_OK;
+    const RlTableImage t = e->reg.image();
+    e->shape = t.shape;
+    RL_CUDA(e, e->d_desc.reserve(t.desc.size()));
+    RL_CUDA(e, e->d_limits.reserve(t.lim.size()));
+    RL_CUDA(e, e->d_ns.reserve(t.ns.size()));
+    RL_CUDA(e, e->d_ns_limit_ids.reserve(t.ns_ids.size()));
+    RL_CUDA(e, e->d_group_ns.reserve(t.group_ns.size()));
     // synchronous copies: the host vectors die at scope exit
     RL_CUDA(e, cudaStreamSynchronize(e->stream));
-    RL_CUDA(e, cudaMemcpy(e->d_desc.p, desc.data(), desc.size() * sizeof(RlCellDesc), cudaMemcpyHostToDevice));
-    RL_CUDA(e, cudaMemcpy(e->d_limits.p, lim.data(), lim.size() * sizeof(RlLimitDev), cudaMemcpyHostToDevice));
-    RL_CUDA(e, cudaMemcpy(e->d_ns.p, ns.data(), ns.size() * sizeof(RlNsDev), cudaMemcpyHostToDevice));
-    RL_CUDA(e, cudaMemcpy(e->d_ns_limit_ids.p, ns_ids.data(), ns_ids.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    RL_CUDA(e, cudaMemcpy(e->d_group_ns.p, group_ns.data(), group_ns.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    e->limits_cap = (uint32_t)lim.size();
-    e->ns_cap = (uint32_t)ns.size();
-    e->tables_dirty = false;
+    RL_CUDA(e, cudaMemcpy(e->d_desc.p, t.desc.data(), t.desc.size() * sizeof(RlCellDesc), cudaMemcpyHostToDevice));
+    RL_CUDA(e, cudaMemcpy(e->d_limits.p, t.lim.data(), t.lim.size() * sizeof(RlLimitDev), cudaMemcpyHostToDevice));
+    RL_CUDA(e, cudaMemcpy(e->d_ns.p, t.ns.data(), t.ns.size() * sizeof(RlNsDev), cudaMemcpyHostToDevice));
+    RL_CUDA(e, cudaMemcpy(e->d_ns_limit_ids.p, t.ns_ids.data(), t.ns_ids.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    RL_CUDA(e, cudaMemcpy(e->d_group_ns.p, t.group_ns.data(), t.group_ns.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    e->limits_cap = (uint32_t)t.lim.size();
+    e->ns_cap = (uint32_t)t.ns.size();
+    e->reg.dirty = false;
     return RL_OK;
 }
 
@@ -391,22 +304,12 @@ RlBatch make_batch(rl_engine* e, uint32_t n_acc, uint32_t n_req, const Outs& o, 
     return B;
 }
 
-// Calls f(std::integral_constant<int, CELLS>{}) for the engine's row geometry: 1, 3 or 7 cells per row.
-template <class F>
-auto with_cells(const rl_engine* e, F&& f) {
-    switch (e->cells) {
-        case 1: return f(std::integral_constant<int, 1>{});
-        case 3: return f(std::integral_constant<int, 3>{});
-        default: return f(std::integral_constant<int, 7>{});
-    }
-}
-
 // probe + stable partition by table region (one launch)
 template <class Src>
 int launch_front(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, cudaStream_t st = nullptr) {
     if (!st) st = e->stream;
     const size_t smem = rl_front_smem_bytes(B.nparts, B.nhot);
-    return with_cells(e, [&](auto c) -> int {
+    return rl_with_cells(e->cells, [&](auto c) -> int {
         auto kern = k_front<decltype(c)::value, Src>;
         static int smem_limit[64] = {};  // per instantiation and device: raised as engines with more regions appear
         const int dv = e->device & 63;
@@ -466,15 +369,12 @@ int launch_main(rl_engine* e, const RlDev& D, const RlBatch& B, const Src& src, 
         RL_CUDA(e, cudaEventCreate(&ev1));
         RL_CUDA(e, cudaEventRecord(ev0, st));
     }
-    int r;
     const bool lc = (MODE == 0) && B.load_counters;
-#define RL_MAIN_CASE(G, A) \
-    r = lc ? launch_main_cells<G, A, Src, MODE, MODE == 0>(e, D, B, src, st) : launch_main_cells<G, A, Src, MODE, false>(e, D, B, src, st)
-    if (e->cells == 1) RL_MAIN_CASE(1, 1);
-    else if (e->cells == 3) RL_MAIN_CASE(3, 3);
-    else if (e->max_cells_used <= 4) RL_MAIN_CASE(7, 4);  // 128-B rows of which at most 4 cells are in use
-    else RL_MAIN_CASE(7, 7);
-#undef RL_MAIN_CASE
+    const int r = rl_with_main_cells(e->cells, e->shape.max_cells_used, [&](auto g, auto c) {
+        constexpr int G = decltype(g)::value, A = decltype(c)::value;
+        return lc ? launch_main_cells<G, A, Src, MODE, MODE == 0>(e, D, B, src, st)
+                  : launch_main_cells<G, A, Src, MODE, false>(e, D, B, src, st);
+    });
     if (r) return r;
     RL_LAUNCH_CHECK(e);
     if (e->profiling) {
@@ -551,10 +451,9 @@ int run_acc_pipeline(rl_engine* e, uint32_t n_acc, uint32_t n_req, const uint64_
             B.phase = RL_PHASE_SPEC;
             r = main0();
             if (r) return r;
-            with_cells(e, [&](auto c) {
-                constexpr int C = decltype(c)::value;
-                const uint32_t act = C == 7 && e->max_cells_used <= 4 ? 4 : C;
-                k_restore<C><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, act, B.log_row, B.log_state);
+            rl_with_main_cells(e->cells, e->shape.max_cells_used, [&](auto g, auto c) {
+                k_restore<decltype(g)::value><<<ceil_div(buf_len, 256), 256, 0, e->stream>>>(buf_len, decltype(c)::value,
+                                                                                            B.log_row, B.log_state);
             });
             RL_LAUNCH_CHECK(e);
             k_fl_step<<<ceil_div(n_req, 256), 256, 0, e->stream>>>(n_req, B.fl_prev, B.fl_next,
@@ -590,14 +489,14 @@ int run_record_pipeline(rl_engine* e, uint32_t n, const rl_record* d_recs, int m
                         bool may_pipeline = false, const PipeHooks* hooks = nullptr, uint32_t n_hint = 0,
                         uint64_t compact_now = 0) {
     RlDev D = make_dev(e);
-    const bool pipelined = may_pipeline && e->pipeline && !e->any_multi_ns;
+    const bool pipelined = may_pipeline && e->pipeline && !e->shape.any_multi_ns;
     if (hooks && !pipelined) return fail(e, RL_FATAL, "sharded steps need RL_FLAG_PIPELINE and single-row namespaces");
     int r = pipelined ? RL_OK : pipe_fence(e);
     if (r) return r;
-    if (e->any_multi_ns) {
+    if (e->shape.any_multi_ns) {
         if (compact_now) return fail(e, RL_FATAL, "16-byte records need single-row namespaces (use the 32-byte form)");
         // some namespace spans several rows: materialise accesses (stride = max limits per ns)
-        const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
+        const uint32_t stride = e->shape.record_stride(e->cells);
         if (stride > e->max_ctrs_req)
             return fail(e, RL_FATAL, "a namespace has more than %u limits", e->max_ctrs_req);
         const uint64_t n_acc = (uint64_t)n * stride;
@@ -673,7 +572,7 @@ int ensure_ready(rl_engine* e, uint64_t n, bool fence = true) {
     }
     if (n > e->max_batch) return fail(e, RL_FATAL, "batch of %llu exceeds max_batch=%u", (unsigned long long)n, e->max_batch);
     RL_CUDA(e, cudaSetDevice(e->device));
-    if (e->tables_dirty && e->pipeline) {
+    if (e->reg.dirty && e->pipeline) {
         int r = pipe_fence(e);
         if (r) return r;
         RL_CUDA(e, cudaStreamSynchronize(e->sp));
@@ -702,14 +601,16 @@ int preload_main(rl_engine* e) {
 int preload_record_kernels(rl_engine* e) {
     int r = upload_tables(e);  // max_cells_used selects the k_main instantiation
     if (r) return r;
-    return with_cells(e, [&](auto c) -> int {
-        constexpr int C = decltype(c)::value;
-        cudaFuncAttributes fa;
-        RL_CUDA(e, cudaFuncGetAttributes(&fa, k_front<C, RecordSrc>));
-        if (C != 7) return preload_main<C, C>(e);
-        if ((r = preload_main<7, 4>(e))) return r;
-        return preload_main<7, 7>(e);
-    });
+    cudaFuncAttributes fa;
+    RL_CUDA(e, rl_with_cells(e->cells, [&](auto c) {
+                return cudaFuncGetAttributes(&fa, k_front<decltype(c)::value, RecordSrc>);
+            }));
+    // k_main for the fewest and the most cells in use: every instantiation the limits set later can select
+    for (const uint32_t used : {1u, (uint32_t)RL_MAX_CELLS})
+        if ((r = rl_with_main_cells(e->cells, used,
+                                    [&](auto g, auto c) { return preload_main<decltype(g)::value, decltype(c)::value>(e); })))
+            return r;
+    return RL_OK;
 }
 
 // Allocates one workspace set for batches of up to max_counters accesses.
@@ -798,7 +699,7 @@ int rl_engine_create(const rl_config* cfg, rl_engine** out) {
     e->max_batch = std::max<uint32_t>(cfg->max_batch, 1);
     e->max_counters = cfg->max_counters ? cfg->max_counters : 4 * e->max_batch;
     e->max_counters = std::max(e->max_counters, e->max_batch);
-    e->groups.resize(1);
+    e->reg.cells = e->cells;
     if (const char* v = getenv("RL_CHUNK")) e->chunk = (atoi(v) == 128) ? 128 : 256;
     if (const char* v = getenv("RL_HEAVY_MULT")) e->heavy_mult = (uint32_t)atoi(v);
     if (const char* v = getenv("RL_PART_TARGET")) e->part_target = std::max(16, atoi(v));
@@ -993,64 +894,8 @@ int rl_get_stats(rl_engine* e, rl_stats* out) {
 int rl_limits_set(rl_engine* e, const rl_limit_desc* limits, uint32_t n) {
     if (!e || (!limits && n)) return RL_FATAL;
     e->structure_epoch++;
-    for (uint32_t i = 0; i < n; i++) {
-        const rl_limit_desc& d = limits[i];
-        if (d.limit_id == RL_NONE_U32) return fail(e, RL_FATAL, "limit_id 0xFFFFFFFF is reserved");
-        if (d.limit_id > (1u << 26) || d.ns_id > (1u << 26))
-            return fail(e, RL_FATAL, "limit_id / ns_id must be dense (<= 2^26)");
-        const uint32_t q = d.qualified ? 1 : 0;
-        const uint32_t varset = q ? d.varset_id : 0;
-        if (q && d.varset_id == 0) return fail(e, RL_FATAL, "qualified limits need varset_id != 0");
-        if (d.limit_id >= e->limits.size()) e->limits.resize(d.limit_id + 1);
-        HostLimit& l = e->limits[d.limit_id];
-        if (l.defined) {
-            // Storage::update_limit (storage/mod.rs:67-83): identity fixed, max_value swapped
-            if (l.ns != d.ns_id || l.window_us != d.window_us || l.qualified != q || l.varset != varset)
-                return fail(e, RL_FATAL, "limit %u: namespace/window/variables are part of a limit's identity", d.limit_id);
-            if (l.max_value != d.max_value) {
-                l.max_value = d.max_value;
-                e->tables_dirty = true;
-            }
-            if (!q) l.simple_present = true;  // add_counter: entry().or_default() (in_memory.rs:38-44)
-            continue;
-        }
-        // pick a row group with a free cell
-        auto& glist = e->groups_by_key[{d.ns_id, varset}];
-        uint32_t g = 0, c = 0;
-        for (uint32_t cand : glist) {
-            for (uint32_t k = 0; k < e->cells; k++)
-                if (e->groups[cand].limit_of_cell[k] == RL_NONE_U32) {
-                    g = cand;
-                    c = k;
-                    break;
-                }
-            if (g) break;
-        }
-        if (!g) {
-            if (e->groups.size() >= 0xFFFFFFF0u) return fail(e, RL_FATAL, "too many row groups");
-            g = (uint32_t)e->groups.size();
-            e->groups.emplace_back();
-            e->groups[g].ns = d.ns_id;
-            e->groups[g].varset = varset;
-            e->groups[g].qualified = q;
-            glist.push_back(g);
-            c = 0;
-        }
-        e->groups[g].limit_of_cell[c] = d.limit_id;
-        l.defined = true;
-        l.ns = d.ns_id;
-        l.varset = varset;
-        l.qualified = q;
-        l.max_value = d.max_value;
-        l.window_us = d.window_us;
-        l.group = g;
-        l.cell = c;
-        l.simple_present = !q;
-        if (d.ns_id >= e->ns_limits.size()) e->ns_limits.resize(d.ns_id + 1);
-        e->ns_limits[d.ns_id].push_back(d.limit_id);
-        e->tables_dirty = true;
-    }
-    return RL_OK;
+    std::string err;
+    return e->reg.set(limits, n, &err) == RL_OK ? RL_OK : fail(e, RL_FATAL, "%s", err.c_str());
 }
 
 // One k_reset pass over the table, behind every pipelined call.  mode 0 resets the cells of the limits in `limit_sel`
@@ -1073,7 +918,7 @@ static int reset_table(rl_engine* e, int mode, uint64_t now_us, const std::vecto
     }
     RlDev D = make_dev(e);
     const uint32_t blocks = ceil_div(e->capacity, 256);
-    with_cells(e, [&](auto c) {
+    rl_with_cells(e->cells, [&](auto c) {
         k_reset<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, mode, now_us, d_sel.p, d_cnt.p);
     });
     RL_LAUNCH_CHECK(e);
@@ -1088,14 +933,14 @@ int rl_delete_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
     if (!e) return RL_FATAL;
     RL_CUDA(e, cudaSetDevice(e->device));
     e->structure_epoch++;
-    std::vector<uint8_t> sel(std::max<size_t>(e->limits.size(), 1), 0);
+    std::vector<uint8_t> sel(std::max<size_t>(e->reg.limits.size(), 1), 0);
     bool any = false;
     for (uint32_t i = 0; i < n; i++) {
         const uint32_t id = limit_ids[i];
-        if (id >= e->limits.size() || !e->limits[id].defined) continue;
+        if (!e->reg.find(id)) continue;
         sel[id] = 1;
         any = true;
-        if (!e->limits[id].qualified) e->limits[id].simple_present = false;  // in_memory.rs:242-243
+        e->reg.set_simple_present(id, false);  // in_memory.rs:242-243
     }
     return any ? reset_table(e, 0, 0, sel, nullptr) : RL_OK;
 }
@@ -1105,16 +950,7 @@ int rl_limits_delete(rl_engine* e, const uint32_t* limit_ids, uint32_t n) {
     e->structure_epoch++;
     int r = rl_delete_counters(e, limit_ids, n);  // storage/mod.rs:104 — counters first
     if (r) return r;
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t id = limit_ids[i];
-        if (id >= e->limits.size() || !e->limits[id].defined) continue;
-        HostLimit& l = e->limits[id];
-        e->groups[l.group].limit_of_cell[l.cell] = RL_NONE_U32;
-        auto& v = e->ns_limits[l.ns];
-        v.erase(std::remove(v.begin(), v.end(), id), v.end());
-        l = HostLimit();
-        e->tables_dirty = true;
-    }
+    e->reg.remove(limit_ids, n);
     return RL_OK;
 }
 
@@ -1122,8 +958,9 @@ int rl_clear(rl_engine* e) {
     if (!e) return RL_FATAL;
     // in_memory.rs:197-201 — only simple_limits is cleared
     std::vector<uint32_t> ids;
-    for (size_t id = 0; id < e->limits.size(); id++)
-        if (e->limits[id].defined && !e->limits[id].qualified) ids.push_back((uint32_t)id);
+    e->reg.each([&](uint32_t id, const HostLimit& l) {
+        if (!l.qualified) ids.push_back(id);
+    });
     return rl_delete_counters(e, ids.data(), (uint32_t)ids.size());
 }
 
@@ -1149,11 +986,10 @@ static int read_table(rl_engine* e, bool live, uint64_t now_us, const std::vecto
     if (r) return r;
     r = upload_tables(e);
     if (r) return r;
-    // present [L]: the limit's counters exist (unqualified ones while simple_present, in_memory.rs:14,38-44) | seen [L]
+    // present [L]: the limit's counters exist (RlRegistry::present) | seen [L]
     const uint32_t L = e->limits_cap;
     std::vector<uint8_t> flags(2 * (size_t)L, 0);
-    for (size_t l = 0; l < e->limits.size(); l++)
-        flags[l] = e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
+    for (uint32_t l = 0; l < L; l++) flags[l] = e->reg.present(l);
     DevBuf<uint8_t> d_sel, d_flags;
     DevBuf<unsigned long long> d_cnt;
     RL_CUDA(e, d_flags.reserve(flags.size()));
@@ -1177,7 +1013,7 @@ static int read_table(rl_engine* e, bool live, uint64_t now_us, const std::vecto
     }
     RlDev D = make_dev(e);
     const uint32_t blocks = ceil_div(e->capacity, 256);
-    with_cells(e, [&](auto c) {
+    rl_with_cells(e->cells, [&](auto c) {
         k_scan<decltype(c)::value><<<blocks, 256, 0, e->stream>>>(D, e->capacity, live, now_us, d_sel.p, e->d_group_ns.p, O);
     });
     RL_LAUNCH_CHECK(e);
@@ -1193,9 +1029,10 @@ static int read_table(rl_engine* e, bool live, uint64_t now_us, const std::vecto
     }
     // the export's present unqualified limits of the selected namespaces that no row showed, appended
     std::vector<uint32_t> extra;
-    for (size_t l = 0; !live && l < e->limits.size(); l++)
-        if (flags[l] && !e->limits[l].qualified && !flags[L + l] && (ns_sel.empty() || ns_sel[e->limits[l].ns]))
-            extra.push_back((uint32_t)l);
+    if (!live)
+        e->reg.each([&](uint32_t l, const HostLimit& h) {
+            if (flags[l] && !h.qualified && !flags[L + l] && (ns_sel.empty() || ns_sel[h.ns])) extra.push_back(l);
+        });
     const uint64_t fit = cnt < cap ? std::min<uint64_t>(extra.size(), cap - cnt) : 0;
     if (fit && mem == RL_MEM_HOST) {
         std::copy(extra.begin(), extra.begin() + fit, out_limit_id + cnt);
@@ -1216,11 +1053,9 @@ int rl_get_counters(rl_engine* e, const uint32_t* limit_ids, uint32_t n, uint64_
     if (!e) return RL_FATAL;
     RL_CUDA(e, cudaSetDevice(e->device));
     // in_memory.rs:161-171: counters_in_namespace(limit.namespace()) for every given limit
-    std::vector<uint8_t> ns_sel(std::max<size_t>(e->ns_limits.size(), 1), 0);
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t id = limit_ids[i];
-        if (id < e->limits.size() && e->limits[id].defined) ns_sel[e->limits[id].ns] = 1;
-    }
+    std::vector<uint8_t> ns_sel(std::max<size_t>(e->reg.ns_limits.size(), 1), 0);
+    for (uint32_t i = 0; i < n; i++)
+        if (const HostLimit* l = e->reg.find(limit_ids[i])) ns_sel[l->ns] = 1;
     return read_table(e, true, now_us, ns_sel, cap, RL_MEM_HOST, out_limit_id, out_key_lo, out_key_hi, out_remaining,
                       out_ttl_us, out_count);
 }
@@ -1233,7 +1068,7 @@ int rl_counters_export(rl_engine* e, const uint32_t* ns_ids, uint32_t n_ns, uint
     if (n_ns && !ns_ids) return fail(e, RL_FATAL, "rl_counters_export: n_ns > 0 with ns_ids == NULL");
     std::vector<uint8_t> ns_sel;  // empty: every namespace
     if (ns_ids) {
-        ns_sel.assign(std::max<size_t>(e->ns_limits.size(), 1), 0);
+        ns_sel.assign(std::max<size_t>(e->reg.ns_limits.size(), 1), 0);
         for (uint32_t i = 0; i < n_ns; i++)
             if (ns_ids[i] < ns_sel.size()) ns_sel[ns_ids[i]] = 1;
     }
@@ -1245,19 +1080,10 @@ int rl_limits_get(rl_engine* e, uint32_t cap, rl_limit_desc* out, uint32_t* out_
     if (!e) return RL_FATAL;
     if (cap && !out) return fail(e, RL_FATAL, "rl_limits_get: cap > 0 with out == NULL");
     uint32_t n = 0;
-    for (size_t id = 0; id < e->limits.size(); id++) {
-        const HostLimit& l = e->limits[id];
-        if (!l.defined) continue;
-        if (n < cap) {
-            out[n].limit_id = (uint32_t)id;
-            out[n].ns_id = l.ns;
-            out[n].varset_id = l.varset;
-            out[n].qualified = l.qualified;
-            out[n].max_value = l.max_value;
-            out[n].window_us = l.window_us;
-        }
+    e->reg.each([&](uint32_t id, const HostLimit& l) {
+        if (n < cap) out[n] = rl_limit_desc{id, l.ns, l.varset, l.qualified, l.max_value, l.window_us};
         n++;
-    }
+    });
     if (out_n) *out_n = n;
     return RL_OK;
 }
@@ -1342,13 +1168,13 @@ int rl_check_and_update_records(rl_engine* e, uint64_t n, const rl_record* recs,
                                 uint8_t* out_limited, uint32_t* out_first_limited, uint64_t* out_remaining,
                                 uint64_t* out_ttl_us, uint32_t out_stride) {
     const bool lc = load_counters && (out_remaining || out_ttl_us);
-    int r = normalise_mem(e, mem, e && e->pipeline && !e->any_multi_ns && !lc);
+    int r = normalise_mem(e, mem, e && e->pipeline && !e->shape.any_multi_ns && !lc);
     if (r) return r;
     if ((r = ensure_ready(e, n, mem == RL_MEM_HOST))) return r;
     if (n == 0) return RL_OK;
     if (!recs || !out_limited) return fail(e, RL_FATAL, "null recs/out_limited");
-    if (lc && out_stride < e->max_ns_limits)
-        return fail(e, RL_FATAL, "out_stride %u < limits per namespace %u", out_stride, e->max_ns_limits);
+    if (lc && out_stride < e->shape.max_ns_limits)
+        return fail(e, RL_FATAL, "out_stride %u < limits per namespace %u", out_stride, e->shape.max_ns_limits);
     e->stats.batches++;
     e->stats.requests += n;
     e->trace_seq = (uint32_t)e->stats.batches;
@@ -1369,7 +1195,7 @@ int rl_check_and_update_records(rl_engine* e, uint64_t n, const rl_record* recs,
 
 int rl_check_and_update_compact(rl_engine* e, uint64_t n, const rl_record16* recs, uint64_t now_us, int mem,
                                 uint8_t* out_limited, uint32_t* out_first_limited) {
-    int r = normalise_mem(e, mem, e && e->pipeline && !e->any_multi_ns);
+    int r = normalise_mem(e, mem, e && e->pipeline && !e->shape.any_multi_ns);
     if (r) return r;
     if ((r = ensure_ready(e, n, mem == RL_MEM_HOST))) return r;
     if (n == 0) return RL_OK;
@@ -1523,7 +1349,7 @@ int rl_is_within_limits_batch(rl_engine* e, uint64_t n, const uint32_t* ctr_off,
     Outs o;
     if ((r = bind_outs(e, mem, user, 0, o))) return r;
     RlDev D = make_dev(e);
-    with_cells(e, [&](auto cl) {
+    rl_with_cells(e->cells, [&](auto cl) {
         k_query_csr<decltype(cl)::value><<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, c.off, c.ctrs, c.delta,
                                                                                    c.now, o.limited, o.first);
     });
@@ -1543,7 +1369,7 @@ int rl_is_within_limits_records(rl_engine* e, uint64_t n, const rl_record* recs,
     Outs o;
     if ((r = stage_records(e, mem, n, recs, sizeof(rl_record), d_recs)) || (r = bind_outs(e, mem, user, 0, o))) return r;
     RlDev D = make_dev(e);
-    with_cells(e, [&](auto c) {
+    rl_with_cells(e->cells, [&](auto c) {
         k_query_records<decltype(c)::value><<<ceil_div(n, 128), 128, 0, e->stream>>>(D, (uint32_t)n, d_recs, o.limited,
                                                                                      o.first);
     });
@@ -1689,10 +1515,9 @@ int rl_internal_reset_hot_rows(rl_engine* e) {
 }
 void rl_internal_structure_changed(rl_engine* e) { e->structure_epoch++; }
 void rl_internal_present(rl_engine* e, uint8_t* present, uint32_t n) {
-    for (uint32_t l = 0; l < n; l++)
-        present[l] = l < e->limits.size() && e->limits[l].defined && (e->limits[l].qualified || e->limits[l].simple_present);
+    for (uint32_t l = 0; l < n; l++) present[l] = e->reg.present(l);
 }
 void rl_internal_mark_present(rl_engine* e, const uint8_t* flags, uint32_t n) {
-    for (uint32_t l = 0; l < n && l < e->limits.size(); l++)
-        if (flags[l] && e->limits[l].defined && !e->limits[l].qualified) e->limits[l].simple_present = true;
+    for (uint32_t l = 0; l < n; l++)
+        if (flags[l]) e->reg.set_simple_present(l, true);
 }

@@ -914,6 +914,25 @@ constexpr int rl_main_ctas() {
     if (CELLS > 4) return 4;
     return (CELLS == 4 && Src::kAccessIsRequest && MODE == 0 && CH == 128 && !LC) ? RL_RECORD_MID_CTAS : RL_MID_CTAS;
 }
+
+// Calls f(std::integral_constant<int, CELLS>{}) for a table of `cells` cells per row: 1, 3 or 7.
+template <class F>
+auto rl_with_cells(uint32_t cells, F&& f) {
+    switch (cells) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        default: return f(std::integral_constant<int, 7>{});
+    }
+}
+// The k_main instantiation <GEO, CELLS> for a table of `cells` cells per row whose row groups use max_cells_used of
+// them: f(integral_constant GEO, integral_constant CELLS).  1/1, 3/3, then 7/4 while at most 4 cells of a 128-B row are
+// in use, else 7/7.  CELLS is also the count of cells per row that k_restore copies.
+template <class F>
+auto rl_with_main_cells(uint32_t cells, uint32_t max_cells_used, F&& f) {
+    using G7 = std::integral_constant<int, 7>;
+    if (cells != 7) return rl_with_cells(cells, [&](auto c) { return f(c, c); });
+    return max_cells_used <= 4 ? f(G7{}, std::integral_constant<int, 4>{}) : f(G7{}, G7{});
+}
 #ifndef RL_WAIT_NS
 #define RL_WAIT_NS 100  // back-off of the chained-commit wait loops
 #endif

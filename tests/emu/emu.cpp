@@ -6,12 +6,15 @@
 // the chained commit) run on the host in emu_engine.cpp, and on the GPU in the -m gpu tests.  Both position encodings of rl_core.h run through the one
 // driver: narrow (up to 16 counters per request) and wide (up to 64).
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <map>
+#include <string>
 #include <utility>
 #include <vector>
 
 #include "../../limitador_b200/csrc/rl_core.h"
+#include "../../limitador_b200/csrc/rl_registry.h"
 
 struct emu_counter {
     uint32_t limit_id, _pad;
@@ -20,8 +23,9 @@ struct emu_counter {
 
 struct emu {
     int cells;
-    std::vector<RlLimitDev> limits;
-    std::vector<RlCellDesc> desc;  // [groups][8]
+    RlRegistry reg;
+    std::vector<RlLimitDev> limits;  // reg's device tables
+    std::vector<RlCellDesc> desc;    // [groups][8]
     std::map<std::pair<uint64_t, uint64_t>, RlRow<RL_MAX_CELLS>> table;
     uint64_t steps = 0;  // replay steps (one run or one request alone each) of the last batch's committing pass
 };
@@ -218,13 +222,26 @@ extern "C" {
 emu* emu_create(int cells) {
     emu* e = new emu();
     e->cells = cells;
+    e->reg.cells = cells;
     return e;
 }
 void emu_destroy(emu* e) { delete e; }
 
-void emu_set_tables(emu* e, const RlLimitDev* limits, uint32_t n_limits, const RlCellDesc* desc, uint32_t n_groups) {
-    e->limits.assign(limits, limits + n_limits);
-    e->desc.assign(desc, desc + (size_t)n_groups * 8);
+// rl_limits_set: RL_OK, or RL_FATAL and the refusal in err[err_cap] (the limits before the refused one stay set)
+int emu_limits_set(emu* e, const rl_limit_desc* d, uint32_t n, char* err, uint32_t err_cap) {
+    std::string msg;
+    const int r = e->reg.set(d, n, &msg);
+    RlTableImage t = e->reg.image();
+    e->limits = std::move(t.lim);
+    e->desc = std::move(t.desc);
+    if (err_cap) snprintf(err, err_cap, "%s", msg.c_str());
+    return r;
+}
+
+// the row group of a limit (0: not defined)
+uint32_t emu_limit_group(emu* e, uint32_t limit_id) {
+    const HostLimit* l = e->reg.find(limit_id);
+    return l ? l->group : 0;
 }
 
 // batch_csr in the narrow (wide = 0) or the wide position encoding.

@@ -8,20 +8,13 @@
 #include "cuda_simt.h"
 // (the emulator must come first: it defines __global__ & co. away)
 #include <algorithm>
-#include <array>
 #include <cstring>
-#include <map>
 #include <vector>
 
+#include "../../limitador_b200/csrc/rl_registry.h"
 #include "../../limitador_b200/csrc/rl_shard.cuh"
 
 namespace {
-
-struct Limit {
-    bool defined = false;
-    uint32_t ns = 0, varset = 0, qualified = 0, group = 0, cell = 0;
-    uint64_t max_value = 0, window_us = 0;
-};
 
 // what the report says about a call (indices of emu_engine's report array)
 enum {
@@ -35,17 +28,8 @@ enum {
 struct emu_engine {
     uint32_t cells = 1, log2P = 0, log2R = 0, row_bytes = 32;
     std::vector<uint8_t> rows;
-    // registry and device tables (rl_limits_set / upload_tables)
-    std::vector<Limit> limits;
-    std::vector<std::array<uint32_t, RL_MAX_CELLS>> groups{std::array<uint32_t, RL_MAX_CELLS>{}};
-    std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> groups_by_key;
-    std::vector<std::vector<uint32_t>> ns_limits;
-    std::vector<RlCellDesc> desc;
-    std::vector<RlLimitDev> lim;
-    std::vector<RlNsDev> ns;
-    std::vector<uint32_t> ns_ids, group_ns;
-    uint32_t max_cells_used = 1, max_ns_limits = 0;
-    bool any_multi_ns = false;
+    RlRegistry reg;
+    RlTableImage t;  // the device tables of reg
     // knobs
     uint32_t chunk = 128, part_target = 128, heavy_mult = 2, main_grid_cap = 132 * 16, weak = 0, hot_on = 0, resident = 1;
     uint32_t n_dev = 0;  // sharded geometry on a plain call: the access count lives on the device, the tile is derived there
@@ -62,104 +46,17 @@ struct emu_engine {
 
 namespace {
 
-// rl_limits_set (rl_engine.cu:1004-1064): limits of one (namespace, variable set) share a row group with a free cell
-int limits_set(emu_engine* e, const rl_limit_desc* d, uint32_t n) {
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t q = d[i].qualified ? 1 : 0, varset = q ? d[i].varset_id : 0;
-        if (d[i].limit_id >= e->limits.size()) e->limits.resize(d[i].limit_id + 1);
-        Limit& l = e->limits[d[i].limit_id];
-        if (l.defined) {  // identity fixed, max_value swapped
-            l.max_value = d[i].max_value;
-            continue;
-        }
-        auto& glist = e->groups_by_key[{d[i].ns_id, varset}];
-        uint32_t g = 0, c = 0;
-        for (uint32_t cand : glist) {
-            for (uint32_t k = 0; k < e->cells; k++)
-                if (e->groups[cand][k] == RL_NONE_U32) {
-                    g = cand;
-                    c = k;
-                    break;
-                }
-            if (g) break;
-        }
-        if (!g) {
-            g = (uint32_t)e->groups.size();
-            std::array<uint32_t, RL_MAX_CELLS> none;
-            none.fill(RL_NONE_U32);
-            e->groups.push_back(none);
-            glist.push_back(g);
-        }
-        e->groups[g][c] = d[i].limit_id;
-        l = Limit{true, d[i].ns_id, varset, q, g, c, d[i].max_value, d[i].window_us};
-        if (d[i].ns_id >= e->ns_limits.size()) e->ns_limits.resize(d[i].ns_id + 1);
-        e->ns_limits[d[i].ns_id].push_back(d[i].limit_id);
-    }
-    return 0;
-}
-
-// upload_tables (rl_engine.cu:203-287): cell descriptors per row group, limits, namespaces (single-row namespaces
-// get mode 1 and their packed cell list, the others mode 2)
-void upload_tables(emu_engine* e) {
-    const size_t ngroups = e->groups.size();
-    e->desc.assign(ngroups * 8, RlCellDesc{0, 0, RL_NONE_U32, 0});
-    e->group_ns.assign(ngroups, 0);
-    e->max_cells_used = 1;
-    for (size_t g = 1; g < ngroups; g++) {
-        for (uint32_t c = 0; c < RL_MAX_CELLS; c++) {
-            const uint32_t lid = e->groups[g][c];
-            if (lid == RL_NONE_U32) continue;
-            e->max_cells_used = std::max(e->max_cells_used, c + 1);
-            const Limit& l = e->limits[lid];
-            e->group_ns[g] = l.ns;
-            e->desc[g * 8 + c] = RlCellDesc{l.max_value, l.window_us, lid, l.qualified};
-        }
-    }
-    e->lim.assign(std::max<size_t>(e->limits.size(), 1), RlLimitDev{0, 0, 0, 0});
-    for (size_t i = 0; i < e->limits.size(); i++)
-        if (e->limits[i].defined) e->lim[i] = RlLimitDev{e->limits[i].group, e->limits[i].cell, e->limits[i].ns, e->limits[i].qualified};
-    e->ns.assign(std::max<size_t>(e->ns_limits.size(), 1), RlNsDev{});
-    e->ns_ids.clear();
-    e->any_multi_ns = false;
-    e->max_ns_limits = 0;
-    for (size_t n = 0; n < e->ns_limits.size(); n++) {
-        memset(&e->ns[n], 0, sizeof(RlNsDev));
-        const auto& L = e->ns_limits[n];
-        if (L.empty()) continue;
-        e->ns[n].lim_off = (uint32_t)e->ns_ids.size();
-        e->ns[n].lim_cnt = (uint32_t)L.size();
-        e->max_ns_limits = std::max<uint32_t>(e->max_ns_limits, (uint32_t)L.size());
-        bool single = L.size() <= RL_MAX_CELLS;
-        for (uint32_t lid : L) {
-            e->ns_ids.push_back(lid);
-            if (e->limits[lid].group != e->limits[L[0]].group) single = false;
-        }
-        if (single) {
-            e->ns[n].mode = 1;
-            e->ns[n].group = e->limits[L[0]].group;
-            e->ns[n].qualified_row = e->limits[L[0]].qualified;
-            uint32_t cells = 0;
-            for (size_t k = 0; k < L.size(); k++) cells |= e->limits[L[k]].cell << (4 * k);
-            e->ns[n].cells = cells | ((uint32_t)L.size() << 28);
-        } else {
-            e->ns[n].mode = 2;
-            e->any_multi_ns = true;
-        }
-    }
-    if (e->ns_ids.empty()) e->ns_ids.push_back(0);
-}
-
 RlDev make_dev(emu_engine* e) {
     RlDev D;
     D.rows = e->rows.data();
     D.log2P = e->log2P;
     D.log2R = e->log2R;
-    D.desc = e->desc.data();
-    D.limits = e->lim.data();
-    D.limits_cap = (uint32_t)e->lim.size();
-    D.ns = e->ns.data();
-    D.ns_cap = (uint32_t)e->ns.size();
-    D.ns_limit_ids = e->ns_ids.data();
+    D.desc = e->t.desc.data();
+    D.limits = e->t.lim.data();
+    D.limits_cap = (uint32_t)e->t.lim.size();
+    D.ns = e->t.ns.data();
+    D.ns_cap = (uint32_t)e->t.ns.size();
+    D.ns_limit_ids = e->t.ns_ids.data();
     D.err = e->err;
     D.flags = &e->flags;
     D.kstats = e->kstats;
@@ -245,17 +142,14 @@ void interleave_on(emu_engine* e, uint64_t salt) {
 }
 void interleave_off() { simt_interleave(false); }
 
-template <int CELLS, class Src>
-void front(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
-    interleave_on(e, 1);
-    simt_launch_ex(B.num_tiles, RL_PART_THREADS, rl_front_smem_bytes(B.nparts, B.nhot), 1, [&] { k_front<CELLS, Src>(D, B, src); });
-    interleave_off();
-}
 template <class Src>
 void launch_front(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
-    if (e->cells == 1) front<1>(e, D, B, src);
-    else if (e->cells == 3) front<3>(e, D, B, src);
-    else front<7>(e, D, B, src);
+    interleave_on(e, 1);
+    rl_with_cells(e->cells, [&](auto c) {
+        simt_launch_ex(B.num_tiles, RL_PART_THREADS, rl_front_smem_bytes(B.nparts, B.nhot), 1,
+                       [&] { k_front<decltype(c)::value, Src>(D, B, src); });
+    });
+    interleave_off();
 }
 
 // what k_front's last block built: the work items, and the hot lists (partitions nparts ..)
@@ -319,17 +213,14 @@ void main_lc(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
     }
 }
 
-// launch_main (rl_engine.cu:472-496): 1/1, 3/3, then 7/4 while at most 4 cells of a 7-cell row are in use, else 7/7
+// launch_main: the instantiation rl_with_main_cells selects
 template <class Src, int MODE>
 void launch_main(emu_engine* e, const RlDev& D, const RlBatch& B, const Src& src) {
     const bool lc = MODE == 0 && B.load_counters;
-#define EMU_MAIN_CASE(G, A) \
-    (lc ? main_lc<G, A, Src, MODE, MODE == 0>(e, D, B, src) : main_lc<G, A, Src, MODE, false>(e, D, B, src))
-    if (e->cells == 1) EMU_MAIN_CASE(1, 1);
-    else if (e->cells == 3) EMU_MAIN_CASE(3, 3);
-    else if (e->max_cells_used <= 4) EMU_MAIN_CASE(7, 4);
-    else EMU_MAIN_CASE(7, 7);
-#undef EMU_MAIN_CASE
+    rl_with_main_cells(e->cells, e->t.shape.max_cells_used, [&](auto g, auto c) {
+        constexpr int G = decltype(g)::value, A = decltype(c)::value;
+        lc ? main_lc<G, A, Src, MODE, MODE == 0>(e, D, B, src) : main_lc<G, A, Src, MODE, false>(e, D, B, src);
+    });
 }
 
 void begin_call(emu_engine* e) {
@@ -354,7 +245,7 @@ int end_call(emu_engine* e) {
     return (int)e->err[0];
 }
 
-// run_acc_pipeline (rl_engine.cu:514-587): accesses that may hold coupled (multi-row) requests.  check_and_update with
+// run_acc_pipeline (rl_engine.cu): accesses that may hold coupled (multi-row) requests.  check_and_update with
 // coupled requests: SNAPSHOT, SPEC rounds (k_restore, k_fl_step) until the first-limited positions settle, COMMIT.
 int acc_pipeline(emu_engine* e, RlDev& D, std::vector<RlAccess>& acc, uint32_t n_req, const uint64_t* delta,
                  const uint64_t* now, int mode, int lc, uint8_t* lim, uint32_t* first, uint64_t* rem, uint64_t* ttl,
@@ -391,11 +282,10 @@ int acc_pipeline(emu_engine* e, RlDev& D, std::vector<RlAccess>& acc, uint32_t n
             e->changed = 0;
             B.phase = RL_PHASE_SPEC;
             main0();
-            const uint32_t act = e->cells == 7 && e->max_cells_used <= 4 ? 4 : e->cells;
-            const uint32_t blocks = rl_ceil_div(buf_len, 256);
-            if (e->cells == 1) simt_launch(blocks, 256, [&] { k_restore<1>(buf_len, act, B.log_row, B.log_state); });
-            else if (e->cells == 3) simt_launch(blocks, 256, [&] { k_restore<3>(buf_len, act, B.log_row, B.log_state); });
-            else simt_launch(blocks, 256, [&] { k_restore<7>(buf_len, act, B.log_row, B.log_state); });
+            rl_with_main_cells(e->cells, e->t.shape.max_cells_used, [&](auto g, auto c) {
+                simt_launch(rl_ceil_div(buf_len, 256), 256,
+                            [&] { k_restore<decltype(g)::value>(buf_len, decltype(c)::value, B.log_row, B.log_state); });
+            });
             simt_launch(rl_ceil_div(n_req, 256), 256, [&] { k_fl_step(n_req, B.fl_prev, B.fl_next, &e->changed); });
             e->report[G_FP_ROUNDS] = round + 1;
             if (!(e->changed & 1u)) break;
@@ -421,6 +311,7 @@ emu_engine* emu_engine_create(uint32_t cells, uint32_t log2P, uint32_t log2R) {
     e->log2P = log2P;
     e->log2R = log2R;
     e->row_bytes = 16 * (1 + cells);
+    e->reg.cells = cells;
     e->rows.assign(((size_t)1 << (log2P + log2R)) * e->row_bytes, 0);
     e->hot.assign(RL_HOT_SLOTS + RL_HOT_CAND + 4, 0xFFFFFFFFu);  // rl_internal_reset_hot_rows
     for (uint32_t i = RL_HOT_SLOTS + RL_HOT_CAND; i < e->hot.size(); i++) e->hot[i] = 0;
@@ -430,9 +321,11 @@ emu_engine* emu_engine_create(uint32_t cells, uint32_t log2P, uint32_t log2R) {
 }
 void emu_engine_destroy(emu_engine* e) { delete e; }
 
+// rl_limits_set and the upload of the tables
 int emu_engine_limits_set(emu_engine* e, const rl_limit_desc* d, uint32_t n) {
-    const int r = limits_set(e, d, n);
-    upload_tables(e);
+    std::string err;
+    const int r = e->reg.set(d, n, &err);
+    e->t = e->reg.image();
     return r;
 }
 
@@ -455,21 +348,20 @@ void emu_engine_interleave(emu_engine* e, int on, uint64_t seed, double p) {
     e->p = p;
 }
 const unsigned long long* emu_engine_report(emu_engine* e) { return e->report; }
-uint32_t emu_engine_max_cells_used(emu_engine* e) { return e->max_cells_used; }
+uint32_t emu_engine_max_cells_used(emu_engine* e) { return e->t.shape.max_cells_used; }
 // the table region of record r's row (single-row namespaces), or -1 when the record has no row
 int64_t emu_engine_record_region(emu_engine* e, const rl_record* r) {
-    if (r->ns_id >= e->ns.size() || e->ns[r->ns_id].mode != 1) return -1;
-    const RlNsDev& ns = e->ns[r->ns_id];
+    if (r->ns_id >= e->t.ns.size() || e->t.ns[r->ns_id].mode != 1) return -1;
+    const RlNsDev& ns = e->t.ns[r->ns_id];
     const uint64_t klo = ns.qualified_row ? r->key_lo : 0;
     const uint64_t hhi = ((uint64_t)ns.group << 32) | (ns.qualified_row ? (r->key_hi & 0xFFFFFFFFull) : 0);
     const uint64_t h = rl_row_hash(klo, hhi);
     return e->log2P ? (int64_t)(h >> (64 - e->log2P)) : 0;
 }
-// remaining / ttl slots per record: the most limits of a namespace when some namespace spans several rows, else the
-// cells of a row (what rl_check_and_update_records' callers pass by default)
-uint32_t emu_engine_record_stride(emu_engine* e) { return e->any_multi_ns ? std::max<uint32_t>(1, e->max_ns_limits) : e->cells; }
+// remaining / ttl slots per record (RlTableShape::record_stride)
+uint32_t emu_engine_record_stride(emu_engine* e) { return e->t.shape.record_stride(e->cells); }
 
-// check_and_update (mode 0) / update_counters (mode 2) over 32-byte records: run_record_pipeline (rl_engine.cu:600-677)
+// check_and_update (mode 0) / update_counters (mode 2) over 32-byte records: run_record_pipeline (rl_engine.cu)
 // without the pipeline — k_front, k_hot when hot rows are on, k_main — or, when some namespace spans several rows, the
 // records resolved into accesses (k_resolve_records, narrow or wide) and run_acc_pipeline.  rem / ttl: [n * stride]
 // with stride = emu_engine_record_stride.  compact_now != 0: recs points at n 16-byte rl_record16 stamped with that one
@@ -478,9 +370,9 @@ int emu_engine_records(emu_engine* e, int mode, uint32_t n, const rl_record* rec
                        uint64_t* rem, uint64_t* ttl, uint64_t compact_now) {
     begin_call(e);
     RlDev D = make_dev(e);
-    if (e->any_multi_ns) {
+    if (e->t.shape.any_multi_ns) {
         if (compact_now) return -1;  // run_record_pipeline refuses it
-        const uint32_t stride = std::max<uint32_t>(1, e->max_ns_limits);
+        const uint32_t stride = e->t.shape.record_stride(e->cells);
         const bool wide = stride > RL_MAX_CTRS_PER_REQ;
         std::vector<RlAccess> acc((size_t)n * stride);
         std::vector<uint64_t> delta(std::max<uint32_t>(n, 1)), now(std::max<uint32_t>(n, 1));
@@ -532,33 +424,26 @@ int emu_engine_csr(emu_engine* e, int mode, uint32_t n, const uint32_t* off, con
 int emu_engine_query_records(emu_engine* e, uint32_t n, const rl_record* recs, uint8_t* lim, uint32_t* first) {
     begin_call(e);
     RlDev D = make_dev(e);
-    auto run = [&](auto c) {
-        constexpr int C = decltype(c)::value;
-        simt_launch(rl_ceil_div(n, 128), 128, [&] { k_query_records<C>(D, n, recs, lim, first); });
-    };
-    if (e->cells == 1) run(std::integral_constant<int, 1>{});
-    else if (e->cells == 3) run(std::integral_constant<int, 3>{});
-    else run(std::integral_constant<int, 7>{});
+    rl_with_cells(e->cells, [&](auto c) {
+        simt_launch(rl_ceil_div(n, 128), 128, [&] { k_query_records<decltype(c)::value>(D, n, recs, lim, first); });
+    });
     return (int)e->err[0];
 }
 
-// the table through k_scan in export mode (read_table, rl_engine.cu:1149-1219, now = 0: every present cell as
+// the table through k_scan in export mode (read_table in rl_engine.cu, now = 0: every present cell as
 // (value, expiry)); the present unqualified limits no row showed are left out, as a never-touched counter.
 uint64_t emu_engine_export(emu_engine* e, uint64_t cap, uint32_t* lid, uint64_t* lo, uint64_t* hi, uint64_t* val, uint64_t* exp) {
     RlDev D = make_dev(e);
-    const uint32_t L = (uint32_t)e->lim.size();
+    const uint32_t L = (uint32_t)e->t.lim.size();
     std::vector<uint8_t> flags(2 * (size_t)L, 0);
-    for (size_t l = 0; l < e->limits.size(); l++) flags[l] = e->limits[l].defined;
+    for (uint32_t l = 0; l < L; l++) flags[l] = e->reg.present(l);
     unsigned long long cnt = 0;
     RlScanOut O{lid, lo, hi, val, exp, &cnt, cap, flags.data(), flags.data() + L};
     const uint64_t nrows = e->rows.size() / e->row_bytes;
-    auto run = [&](auto c) {
-        constexpr int C = decltype(c)::value;
-        simt_launch(rl_ceil_div(nrows, 256), 256, [&] { k_scan<C>(D, nrows, false, 0, nullptr, e->group_ns.data(), O); });
-    };
-    if (e->cells == 1) run(std::integral_constant<int, 1>{});
-    else if (e->cells == 3) run(std::integral_constant<int, 3>{});
-    else run(std::integral_constant<int, 7>{});
+    rl_with_cells(e->cells, [&](auto c) {
+        simt_launch(rl_ceil_div(nrows, 256), 256,
+                    [&] { k_scan<decltype(c)::value>(D, nrows, false, 0, nullptr, e->t.group_ns.data(), O); });
+    });
     return cnt;
 }
 
@@ -673,7 +558,7 @@ int emu_shard_send(emu_shard* S, uint32_t rank, uint32_t n, const rl_record* rec
 int emu_shard_decide(emu_shard* S, uint32_t rank) {
     emu_shard_rank& R = S->r[rank];
     emu_engine* e = R.e;
-    if (R.decided >= R.sent || e->any_multi_ns) return -1;
+    if (R.decided >= R.sent || e->t.shape.any_multi_ns) return -1;
     const uint32_t step = (uint32_t)R.decided, buf = (uint32_t)(R.decided % S->depth), world = S->world, cap = S->cap;
     const uint32_t n_max = (uint32_t)std::min<uint64_t>((uint64_t)world * cap, S->max_batch);
     begin_call(e);

@@ -1,7 +1,6 @@
-"""Shared test helpers: oracle-backed CounterStorage, table assignment mirroring the
-engine's row-group logic, the host emulator binding, random stream builders, the edge-domain
-streams and known answers of the counter arithmetic, and oracle_restore (an import applied to the
-CPU oracle)."""
+"""Shared test helpers: oracle-backed CounterStorage, the host emulator binding, random stream
+builders, the edge-domain streams and known answers of the counter arithmetic, and oracle_restore
+(an import applied to the CPU oracle)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -19,41 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 T0 = 1_700_000_000_000_000
 
-LIMITDEV_DTYPE = np.dtype([("group", "<u4"), ("cell", "<u4"), ("ns_id", "<u4"), ("qualified", "<u4")])
 CELLDESC_DTYPE = np.dtype([("max_value", "<u8"), ("window_us", "<u8"), ("limit_id", "<u4"), ("qualified", "<u4")])
-
-
-def assign_tables(descs: np.ndarray, cells: int):
-    """Mirror of rl_limits_set's row-group assignment (rl_engine.cu): limits of one
-    (namespace, varset) share a row group, `cells` limits per group."""
-    n_lim = int(descs["limit_id"].max()) + 1 if len(descs) else 1
-    limits = np.zeros(n_lim, dtype=LIMITDEV_DTYPE)
-    groups = [None]  # index 0 unused
-    by_key = {}
-    for d in descs:
-        q = 1 if d["qualified"] else 0
-        varset = int(d["varset_id"]) if q else 0
-        key = (int(d["ns_id"]), varset)
-        g = None
-        for cand in by_key.get(key, []):
-            if len(groups[cand]) < cells:
-                g = cand
-                break
-        if g is None:
-            g = len(groups)
-            groups.append([])
-            by_key.setdefault(key, []).append(g)
-        cell = len(groups[g])
-        groups[g].append(int(d["limit_id"]))
-        limits[int(d["limit_id"])] = (g, cell, int(d["ns_id"]), q)
-    desc = np.zeros(len(groups) * 8, dtype=CELLDESC_DTYPE)
-    desc["limit_id"] = NONE
-    by_id = {int(d["limit_id"]): d for d in descs}
-    for g in range(1, len(groups)):
-        for c, lid in enumerate(groups[g]):
-            d = by_id[lid]
-            desc[g * 8 + c] = (int(d["max_value"]), int(d["window_us"]), lid, 1 if d["qualified"] else 0)
-    return limits, desc, len(groups)
 
 
 def host_lib(src, name, defines=()):
@@ -79,7 +44,10 @@ def emu_lib():
     L.emu_create.restype = vp
     L.emu_create.argtypes = [C.c_int]
     L.emu_destroy.argtypes = [vp]
-    L.emu_set_tables.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32]
+    L.emu_limits_set.argtypes = [vp, vp, C.c_uint32, C.c_char_p, C.c_uint32]
+    L.emu_limits_set.restype = C.c_int
+    L.emu_limit_group.argtypes = [vp, C.c_uint32]
+    L.emu_limit_group.restype = C.c_uint32
     L.emu_batch_csr.argtypes = [vp, C.c_int, C.c_int, C.c_uint32, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     L.emu_resolve.argtypes = [vp, C.c_int, C.c_uint32, C.c_uint32, vp, C.c_uint32, vp, vp]
     L.emu_resolve.restype = C.c_int
@@ -111,9 +79,16 @@ class Emu:
         self.rounds = self.steps = 0
 
     def set_limits(self, descs):
-        """The limits again, e.g. with another max_value (rl_limits_set on live ids); the counters stay."""
-        limits, desc, ngroups = assign_tables(descs, self.cells)
-        self.L.emu_set_tables(self.h, _p(limits), len(limits), _p(desc), ngroups)
+        """rl_limits_set through the engine's registry (new ids, or live ids with another max_value; the counters
+        stay).  Raises ValueError with the engine's message when the registry refuses a limit."""
+        d = np.ascontiguousarray(descs, dtype=LIMIT_DESC_DTYPE)
+        err = C.create_string_buffer(512)
+        if self.L.emu_limits_set(self.h, _p(d), len(d), err, len(err)) != 0:
+            raise ValueError(err.value.decode())
+
+    def group_of(self, limit_id):
+        """The row group the registry gave a limit (0: not defined)."""
+        return int(self.L.emu_limit_group(self.h, limit_id))
 
     def __del__(self):
         if getattr(self, "h", None):

@@ -52,3 +52,28 @@ def test_wide_key_space_streams_match_oracle(cells, load_counters, seed):
     descs = H.mixed_limits(n_ns=12, seed=seed)
     batches = [H.random_csr_stream(descs, 2500, seed * 100 + b, n_keys=120, monotone=bool(b & 1)) for b in range(4)]
     H.emu_vs_oracle(descs, cells, batches, load_counters)
+
+
+def test_limit_registry_refusals():
+    """rl_limits_set's refusals, through the registry the engine runs (rl_registry.h): the message of each, and a call
+    that stops at its first refused limit with the earlier ones set."""
+    identity = "limit 0: namespace/window/variables are part of a limit's identity"
+    refused = {
+        (0xFFFFFFFF, 0, 1, 1, 5, 1): "limit_id 0xFFFFFFFF is reserved",
+        ((1 << 26) + 1, 0, 1, 1, 5, 1): "limit_id / ns_id must be dense (<= 2^26)",
+        (5, (1 << 26) + 1, 1, 1, 5, 1): "limit_id / ns_id must be dense (<= 2^26)",
+        (5, 0, 0, 1, 5, 1): "qualified limits need varset_id != 0",
+        (0, 1, 1, 1, 10, 1_000_000): identity,
+        (0, 0, 2, 1, 10, 1_000_000): identity,
+        (0, 0, 1, 1, 10, 2_000_000): identity,
+        (0, 0, 0, 0, 10, 1_000_000): identity,
+    }
+    emu = H.Emu(np.array([(0, 0, 1, 1, 10, 1_000_000)], dtype=H.LIMIT_DESC_DTYPE), 3)
+    for desc, msg in refused.items():
+        with pytest.raises(ValueError) as e:
+            emu.set_limits(np.array([desc], dtype=H.LIMIT_DESC_DTYPE))
+        assert str(e.value) == msg
+    with pytest.raises(ValueError):
+        emu.set_limits(np.array([(1, 0, 1, 1, 7, 1_000_000), (0, 1, 1, 1, 10, 1_000_000), (2, 0, 1, 1, 7, 1_000_000)],
+                                dtype=H.LIMIT_DESC_DTYPE))
+    assert emu.group_of(1) == emu.group_of(0) != 0 and emu.group_of(2) == 0

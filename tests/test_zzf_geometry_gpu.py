@@ -133,7 +133,7 @@ def test_chained_partition_with_chunk_indices_past_2048():
     e = Engine(capacity_rows=1 << 20, cells_per_row=3, max_batch=n, regions=1 << log2P, flags=KERNEL_STATS)
     e.limits_set(descs)
     o = H.oracle_with_limits(descs)
-    group = int(H.assign_tables(descs, 3)[0][0]["group"])
+    group = H.Emu(descs, 3).group_of(0)  # the row group the engine's registry gives limit 0
     rng = np.random.default_rng(5)
     keys = np.arange(1, 400_001, dtype=np.uint64)
     reg = region_of(keys, np.zeros_like(keys), group, log2P)
