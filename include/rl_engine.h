@@ -399,6 +399,56 @@ int rl_shard_flush(rl_shard *s);
  * 2 verdict flag}] for buf < lag+2, then the steps sent, decided, collected; out holds (lag+2)*world*4 + 3 words */
 int rl_shard_debug(rl_shard *s, uint32_t *out);
 
+/* ---- The general (CSR) form of the sharded exchange: served requests on a namespace-sharded store ----------------
+ * What rl_rls_serve and rl_http_serve hand their engine: request i owns counters ctrs[ctr_off[i] .. ctr_off[i+1]), with
+ * its own delta and now_us.  Its owner is rl_owner_of(ns of its first counter's limit, world): every counter of a request
+ * belongs to the request's namespace (lib.rs:512).  A step:
+ *   send    : bucket the batch by owner (stable) and STORE each request (a header: counter count, delta, now_us, op and
+ *             load flag; then its counters in their order) into its owner's inbox block, then publish the block (request
+ *             and counter fill, the digest of this rank's limit registry) and the step flag;
+ *   decide  : wait (on the device) for every source's block, lay the inbox out as one CSR in (source rank, index at the
+ *             source) order -- the canonical order -- and run one general-form engine call per run of equal (op, load)
+ *             (one read of the sizes and runs to the host); the outputs go back to every source;
+ *   collect : wait (on the device) for every owner and put verdicts, first_limited and, for requests with load_counters,
+ *             remaining / ttl back in request and counter order.  Synchronises the engine's stream.
+ * Results are those of the ranks' batches applied one after another, in rank order, to one engine.  Every rank issues
+ * the same calls (a rank without traffic sends n = 0), one step at a time (no lag).
+ * Guards, each for whole steps so that no peer is ever left waiting:
+ *   - cap_requests / cap_counters per source and step (multiples of 16); create refuses world x cap beyond the engine's
+ *     max_batch / max_counters.  A batch over its caps sends empty blocks; its requests get RL_VERDICT_ERROR and collect
+ *     returns RL_TRANSIENT.
+ *   - a source whose registry digest (limit ids, ns, varset, qualified, window, max_value) differs from the owner's: its
+ *     requests get RL_VERDICT_ERROR and the owner's decide returns RL_FATAL naming both ranks.
+ *   - a failed engine call (a full region, ...): its run's requests get RL_VERDICT_ERROR at their sources, decide returns
+ *     RL_TRANSIENT with the call's message; other runs and owners are unaffected.
+ * Only a call refused for its own arguments sends nothing (no peers connected, the previous step not collected, an
+ * unknown op, decide before send): that is a broken protocol and leaves the group out of step.  Any other failure on
+ * a rank (null or over-cap arrays, an engine that cannot run, a failed engine call) still sends and returns its step,
+ * with error verdicts, so that no peer is left waiting.
+ * All d_* pointers are device memory of the engine's device and stay valid until collect returns; d_load (nullable) =
+ * one load_counters flag per request, else load_all for every request; load_counters applies to
+ * RL_SHARD_CHECK_AND_UPDATE only.  Nullable outputs: d_first_limited, d_remaining / d_ttl_us (indexed like ctrs). */
+enum { RL_SHARD_CHECK_AND_UPDATE = 0, RL_SHARD_IS_WITHIN = 1, RL_SHARD_UPDATE = 2 };
+typedef struct rl_shard_batch rl_shard_batch;
+int rl_shard_batch_create(rl_engine *e, uint32_t rank, uint32_t world, uint32_t cap_requests, uint32_t cap_counters,
+                          rl_shard_batch **out);
+void rl_shard_batch_destroy(rl_shard_batch *s);
+void *rl_shard_batch_slab(rl_shard_batch *s);
+rl_engine *rl_shard_batch_engine(rl_shard_batch *s); /* the engine it was created on */
+/* as rl_shard_ipc_handle / rl_shard_connect_ipc / rl_shard_connect_ptrs */
+int rl_shard_batch_ipc_handle(rl_shard_batch *s, void *out64);
+int rl_shard_batch_connect_ipc(rl_shard_batch *s, const void *handles64);
+int rl_shard_batch_connect_ptrs(rl_shard_batch *s, void *const *slabs);
+int rl_shard_batch_send(rl_shard_batch *s, uint64_t n, uint64_t n_ctr, const uint32_t *d_ctr_off, const rl_counter *d_ctrs,
+                        const uint64_t *d_delta, const uint64_t *d_now_us, int op, const uint8_t *d_load, int load_all);
+int rl_shard_batch_decide(rl_shard_batch *s);
+int rl_shard_batch_collect(rl_shard_batch *s, uint8_t *d_limited, uint32_t *d_first_limited, uint64_t *d_remaining,
+                           uint64_t *d_ttl_us);
+/* send + decide + collect: the one call of the one-process-per-GPU deployment (returns the worse status) */
+int rl_shard_batch_step(rl_shard_batch *s, uint64_t n, uint64_t n_ctr, const uint32_t *d_ctr_off, const rl_counter *d_ctrs,
+                        const uint64_t *d_delta, const uint64_t *d_now_us, int op, const uint8_t *d_load, int load_all,
+                        uint8_t *d_limited, uint32_t *d_first_limited, uint64_t *d_remaining, uint64_t *d_ttl_us);
+
 /* ---- Batching front (SURVEY §8b threading row) ---------------------------------------------
  * Thread-safe, blocking, one request per call: concurrent callers are coalesced by a dispatcher
  * thread into batches of at most max_batch requests (waiting at most max_delay_us for company)

@@ -92,6 +92,12 @@ int rl_http_responses(rl_http *h, const uint16_t **out_status, const uint8_t **o
                       const uint8_t **out_hdr, const uint64_t **out_hdr_off);
 /* rl_http_plan_device -> the engine (RL_MEM_DEVICE, one call per run of equal load_counters flags) -> finish. */
 int rl_http_serve(rl_http *h, int endpoint, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+/* Over the RLS service's sharded store (rl_rls_attach_shard; rl_http_serve runs rl_http_serve_sharded then): one step
+ * covers the whole batch, however many load_counters runs it has.  Phases as rl_rls_send / _decide / _collect. */
+int rl_http_serve_sharded(rl_http *h, int endpoint, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+int rl_http_send(rl_http *h, int endpoint, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+int rl_http_decide(rl_http *h);
+int rl_http_collect(rl_http *h);
 /* Stage timings of the last serve call in microseconds, and the store calls it made. */
 int rl_http_last_timings(rl_http *h, double *out_plan_us, double *out_store_us, double *out_finish_us,
                          uint32_t *out_store_calls);

@@ -114,6 +114,28 @@ int rl_rls_responses(rl_rls *s, const uint8_t **out_buf, const uint64_t **out_of
  * finish. */
 int rl_rls_serve(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
 
+/* ---- serving on a namespace-sharded store (rl_shard_batch, include/rl_engine.h) --------------------------------------
+ * Every rank runs its own service (matcher and engine, configured with the same limits) and attaches its rank's
+ * rl_shard_batch; all ranks issue the same sequence of serve calls (a rank without traffic serves an empty batch).  Each
+ * rank plans its batch on its own GPU, ships every store request to the owner of its namespace and finishes its own
+ * responses and metrics from the outputs that come back.  The responses, metrics and the union of the owners' tables are
+ * those of serving the ranks' batches one after another, in rank order, through one service on one engine.  A store
+ * request that was not decided (a batch over the exchange's caps, a source whose limits differ from the owner's, a failed
+ * engine call on its owner) is answered UNAVAILABLE (gRPC 14), never allowed.
+ *   rl_rls_attach_shard   from now on rl_rls_serve runs rl_rls_serve_sharded (NULL detaches).  A sharded service does
+ *                         not keep counter variables: rl_rls_keep_counter_vars, the counter variable export, import and
+ *                         drain and GET /counters are refused (RL_FATAL).
+ *   rl_rls_serve_sharded  send, decide, collect.  RL_FATAL (after the responses are finished) when the owner found a
+ *                         source with other limits: rl_rls_last_error names both ranks.
+ *   rl_rls_send           plan on the device and send (buf / off are not read after it returns); rl_rls_decide: decide
+ *                         the owner's inbox; rl_rls_collect: collect and finish.  A one-process driver of several ranks
+ *                         calls every rank's send, then every decide, then every collect. */
+int rl_rls_attach_shard(rl_rls *s, rl_shard_batch *shard);
+int rl_rls_serve_sharded(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+int rl_rls_send(rl_rls *s, int method, uint64_t n, const uint8_t *buf, const uint64_t *off, uint64_t now_us);
+int rl_rls_decide(rl_rls *s);
+int rl_rls_collect(rl_rls *s);
+
 /* ---- counter variables (GET /counters, include/rl_http.h) ------------------------------------------------------
  * The store keeps a counter's 96-bit key digest only.  With keeping on, every device plan (rl_rls_serve,
  * rl_rls_plan_device and their HTTP counterparts on the same service) records the variable values behind the keys it

@@ -18,6 +18,7 @@
 #include "rl_cuda_host.h"
 #include "rl_kernels.cuh"
 #include "rl_shard.cuh"
+#include "rl_shard_csr.cuh"
 #include "rl_internal.h"
 #include "rl_registry.h"
 

@@ -52,6 +52,13 @@ __attribute__((weak)) int rl_http_dev_decide(rl_rls_dev* st, rl_engine* e, int e
                                              uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
                                              rl_counter* ctrs);
 __attribute__((weak)) int rl_rls_dev_wait(rl_rls_dev* st);
+__attribute__((weak)) int rl_rls_dev_shard_send(rl_rls_dev* st, rl_shard_batch* sb, int empty, int http, int method, int load_counters,
+                                                int* out_failed);
+__attribute__((weak)) int rl_rls_dev_shard_collect(rl_rls_dev* st, rl_shard_batch* sb, int load_counters, uint8_t* limited,
+                                                   uint32_t* first_limited, uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off,
+                                                   rl_counter* ctrs);
+__attribute__((weak)) int rl_shard_batch_decide(rl_shard_batch* s);
+__attribute__((weak)) rl_engine* rl_shard_batch_engine(rl_shard_batch* s);
 __attribute__((weak)) int rl_cv_dev_configure(rl_rls_dev** st, rl_engine* e, uint64_t max_keys, uint64_t arena_bytes);
 __attribute__((weak)) int rl_cv_dev_stats(rl_rls_dev* st, uint64_t* out_slots, uint64_t* out_keys, uint64_t* out_arena_used,
                                           uint64_t* out_dropped);
@@ -271,6 +278,12 @@ struct Batch {
     std::vector<uint32_t> o_first;
     std::vector<uint64_t> o_rem, o_ttl;
     double t_plan = 0, t_store = 0, t_finish = 0;
+    // a sharded step between its send and its collect: the plan's status, the collect's load flag, the send's and the
+    // decide's status and message, the stage clocks
+    bool sh_pending = false, sh_load = false;
+    int sh_plan = RL_OK, sh_status = RL_OK;
+    std::string sh_error;
+    double sh_t0 = 0, sh_t1 = 0;
 };
 
 }  // namespace
@@ -280,6 +293,8 @@ struct rl_rls : Batch {
     bool use_limit_name = false;
     rl_rls_dev* dev = nullptr;  // the device plan's state (rl_rls_dev.cu), created by the first device plan
     int load_counters = 0;
+    rl_shard_batch* shard = nullptr;          // rl_rls_attach_shard: store calls go through the sharded exchange
+    const uint8_t* report_verdicts = nullptr;  // sharded Report: error verdicts mark the requests that were not decided
     // responses
     RawBuf<uint8_t> resp;
     std::vector<uint64_t> resp_off;
@@ -615,7 +630,8 @@ void finish_range(rl_rls* s, int store_status, const uint8_t* limited, const uin
                 }
                 const uint32_t j = P.store;
                 if (s->method == RL_RLS_REPORT) {
-                    code = RL_RLS_CODE_OK;  // kuadrant_service.rs:176-178
+                    if (s->report_verdicts && s->report_verdicts[j] == RL_VERDICT_ERROR) grpc = RL_GRPC_UNAVAILABLE;
+                    else code = RL_RLS_CODE_OK;  // kuadrant_service.rs:176-178
                     break;
                 }
                 if (limited[j] == RL_VERDICT_ERROR) {
@@ -1157,6 +1173,7 @@ int rl_rls_responses(rl_rls* s, const uint8_t** out_buf, const uint64_t** out_of
 
 int rl_rls_serve(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
     if (!s) return RL_FATAL;
+    if (s->shard) return rl_rls_serve_sharded(s, method, n, buf, off, now_us);
     if (!s->engine) return sfail(s, "the service was created without an engine: there is no CPU store to fall back to");
     if (n && (!off || !buf)) return RL_FATAL;
     // plan on the device: the store call's CSR stays there
@@ -1421,6 +1438,7 @@ int rl_http_responses(rl_http* h, const uint16_t** out_status, const uint8_t** o
 
 int rl_http_serve(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
     if (!h) return RL_FATAL;
+    if (h->rls->shard) return rl_http_serve_sharded(h, endpoint, n, buf, off, now_us);
     if (!h->engine) return sfail(h, "the service was created without an engine: there is no CPU store to fall back to");
     if (n && (!off || !buf)) return RL_FATAL;
     const double t0 = mono_us();
@@ -1466,9 +1484,196 @@ int rl_http_last_timings(rl_http* h, double* out_plan_us, double* out_store_us, 
     return RL_OK;
 }
 
+// ---- serving on a namespace-sharded store (rl_shard_batch, include/rl_engine.h) ------------------------------------
+static const char* const kShardedNoCvars =
+    "counter variables are kept by one engine's service: a service with a sharded store does not keep, export, import or drain them";
+
+namespace {
+
+// The send half of a sharded step for either surface, after its device plan returned r: the plan's store requests (or,
+// when the plan failed, an empty batch: every rank takes part in every step) go to their owners.
+int sharded_send(Batch* s, rl_rls_dev* dev, rl_shard_batch* sb, bool http, int method, int r, bool load, double t0) {
+    s->sh_plan = r;
+    s->sh_load = load;
+    s->sh_status = RL_OK;
+    s->sh_error.clear();
+    s->sh_t0 = t0;
+    int failed = RL_OK;
+    const int st = rl_rls_dev_shard_send(r ? nullptr : dev, sb, r != 0, http, method, load, &failed);
+    if (st) {  // refused before anything went out (a protocol error of the caller): there is nothing to collect
+        s->sh_pending = false;
+        if (!r) s->last_error = std::string("sharded store: ") + rl_last_error(s->engine);
+        return r ? r : st;
+    }
+    if (failed) s->sh_plan = dev_fail(s, dev, failed);  // the batch went out empty
+    s->sh_pending = true;
+    s->sh_t1 = mono_us();
+    return RL_OK;
+}
+
+int sharded_decide(Batch* s, rl_shard_batch* sb) {
+    if (!s->sh_pending) return sfail(s, "no sharded step sent");
+    const int st = rl_shard_batch_decide(sb);
+    if (st != RL_OK && s->sh_status == RL_OK) {
+        s->sh_error = std::string("sharded store: ") + rl_last_error(s->engine);
+        s->sh_status = st;
+    }
+    return RL_OK;
+}
+
+// The collect of a sharded step into the batch's output arrays; its status, or the plan's when that failed
+int sharded_collect(Batch* s, rl_rls_dev* dev, rl_shard_batch* sb, int& store_status) {
+    if (!s->sh_pending) return sfail(s, "no sharded step sent");
+    s->sh_pending = false;
+    store_status = rl_rls_dev_shard_collect(s->sh_plan ? nullptr : dev, sb, s->sh_load, s->o_limited.data(), s->o_first.data(),
+                                            s->o_rem.data(), s->o_ttl.data(), s->ctr_off.data(), s->ctrs.data());
+    if (store_status != RL_OK && store_status != RL_TRANSIENT) s->last_error = std::string("store call failed: ") + rl_last_error(s->engine);
+    return s->sh_plan;
+}
+
+// the step's status once the batch is finished: a failed finish, else what the decide reported (the digest check)
+int sharded_status(Batch* s, int r) {
+    if (r) return r;
+    if (s->sh_status == RL_FATAL) {
+        s->last_error = s->sh_error;
+        return RL_FATAL;
+    }
+    return RL_OK;
+}
+
+}  // namespace
+
+int rl_rls_attach_shard(rl_rls* s, rl_shard_batch* shard) {
+    if (!s) return RL_FATAL;
+    if (shard) {
+        if (!s->engine) return sfail(s, "a sharded store needs a service created with an engine");
+        if (!rl_rls_dev_shard_send) return sfail(s, "this build of the library has no device plan");
+        if (rl_shard_batch_engine(shard) != s->engine) return sfail(s, "the sharded store was created on another engine than the service's");
+        uint64_t slots = 0;
+        if (s->dev && rl_cv_dev_stats && rl_cv_dev_stats(s->dev, &slots, nullptr, nullptr, nullptr) == RL_OK && slots)
+            return sfail(s, "%s (turn keeping off first)", kShardedNoCvars);
+    }
+    s->shard = shard;
+    return RL_OK;
+}
+
+int rl_rls_send(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!s) return RL_FATAL;
+    if (!s->shard) return sfail(s, "no sharded store attached (rl_rls_attach_shard)");
+    if (s->sh_pending) return sfail(s, "the previous sharded step is not collected");
+    const double t0 = mono_us();
+    const RlsDevReq* req = nullptr;
+    uint64_t n_ctr = 0;
+    int r = n && (!off || !buf) ? sfail(s, "null request buffer or offsets") : plan_on_device(s, method, n, buf, off, now_us, false, req, n_ctr);
+    if (r == RL_OK) size_outputs(s, s->load_counters, n_ctr);
+    if ((r = sharded_send(s, s->dev, s->shard, false, method, r, r == RL_OK && s->load_counters, t0))) return r;
+    if (s->sh_plan) return RL_OK;
+    // the per-request outcomes now (the wire bytes need not outlive this call)
+    if ((r = dev_fail(s, s->dev, rl_rls_dev_wait(s->dev)))) {
+        s->sh_plan = r;
+        return RL_OK;
+    }
+    take_device_plan(s, req, buf, off);
+    return RL_OK;
+}
+
+int rl_rls_decide(rl_rls* s) {
+    if (!s) return RL_FATAL;
+    return sharded_decide(s, s->shard);
+}
+
+int rl_rls_collect(rl_rls* s) {
+    if (!s) return RL_FATAL;
+    int st = RL_OK;
+    const std::string plan_error = s->last_error;
+    int r = sharded_collect(s, s->dev, s->shard, st);
+    if (r) {
+        s->last_error = plan_error;
+        return r;
+    }
+    const double t2 = mono_us();
+    s->report_verdicts = s->method == RL_RLS_REPORT ? s->o_limited.data() : nullptr;
+    r = rl_rls_finish(s, st == RL_TRANSIENT && s->n_store ? RL_OK : st, s->o_limited.data(), s->o_first.data(), s->o_rem.data(),
+                      s->o_ttl.data());
+    s->report_verdicts = nullptr;
+    s->t_plan = s->sh_t1 - s->sh_t0;
+    s->t_store = t2 - s->sh_t1;
+    s->t_finish = mono_us() - t2;
+    return sharded_status(s, r);
+}
+
+int rl_rls_serve_sharded(rl_rls* s, int method, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    int r = rl_rls_send(s, method, n, buf, off, now_us);
+    if (r) return r;
+    rl_rls_decide(s);
+    return rl_rls_collect(s);
+}
+
+int rl_http_send(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    if (!h) return RL_FATAL;
+    rl_shard_batch* sb = h->rls->shard;
+    if (!sb) return sfail(h, "no sharded store attached to the RLS service (rl_rls_attach_shard)");
+    if (h->sh_pending) return sfail(h, "the previous sharded step is not collected");
+    const double t0 = mono_us();
+    const HttpDevReq* req = nullptr;
+    const HttpRun* runs = nullptr;
+    uint64_t n_ctr = 0;
+    uint32_t n_runs = 0;
+    int r = n && (!off || !buf) ? sfail(h, "null body buffer or offsets")
+                                : http_plan_on_device(h, endpoint, n, buf, off, now_us, false, req, n_ctr, runs, n_runs);
+    bool any_load = false;
+    if (r == RL_OK) {
+        for (uint32_t k = 0; k < n_runs; k++) any_load = any_load || runs[k].load;
+        size_outputs(h, any_load, n_ctr);
+        h->store_calls = n_runs ? 1 : 0;  // one step, however many load_counters runs
+    }
+    if ((r = sharded_send(h, h->rls->dev, sb, true, endpoint, r, any_load, t0))) return r;
+    if (h->sh_plan) return RL_OK;
+    if ((r = dev_fail(h, h->rls->dev, rl_rls_dev_wait(h->rls->dev)))) {
+        h->sh_plan = r;
+        return RL_OK;
+    }
+    take_http_device_plan(h, req, buf, off);
+    return RL_OK;
+}
+
+int rl_http_decide(rl_http* h) {
+    if (!h) return RL_FATAL;
+    return sharded_decide(h, h->rls->shard);
+}
+
+int rl_http_collect(rl_http* h) {
+    if (!h) return RL_FATAL;
+    int st = RL_OK;
+    const std::string plan_error = h->last_error;
+    int r = sharded_collect(h, h->rls->dev, h->rls->shard, st);
+    if (r) {
+        h->last_error = plan_error;
+        return r;
+    }
+    const double t2 = mono_us();
+    // per store request: the collect's status, or the error verdict of a request that was not decided
+    h->o_status.resize(h->n_store);
+    for (uint64_t j = 0; j < h->n_store; j++)
+        h->o_status[j] = (st != RL_OK && st != RL_TRANSIENT) ? st : h->o_limited[j] == RL_VERDICT_ERROR ? RL_TRANSIENT : RL_OK;
+    r = rl_http_finish(h, h->o_status.data(), h->o_limited.data(), h->o_first.data(), h->o_rem.data(), h->o_ttl.data());
+    h->t_plan = h->sh_t1 - h->sh_t0;
+    h->t_store = t2 - h->sh_t1;
+    h->t_finish = mono_us() - t2;
+    return sharded_status(h, r);
+}
+
+int rl_http_serve_sharded(rl_http* h, int endpoint, uint64_t n, const uint8_t* buf, const uint64_t* off, uint64_t now_us) {
+    int r = rl_http_send(h, endpoint, n, buf, off, now_us);
+    if (r) return r;
+    rl_http_decide(h);
+    return rl_http_collect(h);
+}
+
 // ---- counter variables and the GET endpoints -------------------------------------------------------------------
 int rl_rls_keep_counter_vars(rl_rls* s, uint64_t max_keys, uint64_t arena_bytes) {
     if (!s) return RL_FATAL;
+    if (s->shard) return sfail(s, "%s", kShardedNoCvars);
     if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
     if (!rl_cv_dev_configure) return sfail(s, "this build of the library has no device plan");
     const int r = rl_cv_dev_configure(&s->dev, s->engine, max_keys, arena_bytes);
@@ -1497,6 +1702,7 @@ int rl_rls_counter_vars_export(rl_rls* s, const uint32_t* ns_ids, uint32_t n_ns,
                                uint32_t* out_varset, uint64_t* out_key_lo, uint64_t* out_key_hi, uint64_t* out_blob_off,
                                uint8_t* out_blobs, uint64_t* out_count, uint64_t* out_bytes) {
     if (!s || !out_count || !out_bytes) return RL_FATAL;
+    if (s->shard) return sfail(s, "%s", kShardedNoCvars);
     if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
     if (!rl_cv_dev_export) return sfail(s, "this build of the library has no device plan");
     const int r = rl_cv_dev_export(&s->dev, s->engine, s->m, ns_ids, n_ns, now_us, cap, bytes_cap, out_varset, out_key_lo, out_key_hi,
@@ -1508,6 +1714,7 @@ int rl_rls_counter_vars_export(rl_rls* s, const uint32_t* ns_ids, uint32_t n_ns,
 int rl_rls_counter_vars_import(rl_rls* s, uint64_t n, const uint32_t* varset, const uint64_t* key_lo, const uint64_t* key_hi,
                                const uint64_t* blob_off, const uint8_t* blobs, uint64_t* out_added) {
     if (!s) return RL_FATAL;
+    if (s->shard) return sfail(s, "%s", kShardedNoCvars);
     if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
     if (!rl_cv_dev_import) return sfail(s, "this build of the library has no device plan");
     const int r = rl_cv_dev_import(&s->dev, s->engine, s->m, n, varset, key_lo, key_hi, blob_off, blobs, out_added);
@@ -1519,6 +1726,7 @@ int rl_rls_counter_vars_drain(rl_rls* s, uint64_t cap, uint64_t bytes_cap, uint3
                               uint64_t* out_key_hi, uint64_t* out_blob_off, uint8_t* out_blobs, uint64_t* out_count,
                               uint64_t* out_bytes, int* out_full) {
     if (!s || !out_count || !out_bytes || !out_full) return RL_FATAL;
+    if (s->shard) return sfail(s, "%s", kShardedNoCvars);
     if (!s->engine) return sfail(s, "keeping counter variables needs a service created with an engine");
     if (!rl_cv_dev_drain) return sfail(s, "this build of the library has no device plan");
     const int r = rl_cv_dev_drain(&s->dev, s->engine, s->m, cap, bytes_cap, out_varset, out_key_lo, out_key_hi, out_blob_off,
@@ -1544,6 +1752,7 @@ int rl_http_get_limits(rl_http* h, const char* ns, uint32_t ns_len) {
 
 int rl_http_get_counters(rl_http* h, const char* ns, uint32_t ns_len, uint64_t now_us) {
     if (!h || (ns_len && !ns)) return RL_FATAL;
+    if (h->rls->shard) return sfail(h, "GET /counters reads one engine's table: a sharded service does not serve it");
     if (!h->engine || !rl_get_counters || !rl_cv_dev_lookup) return sfail(h, "GET /counters needs a service created with an engine");
     const std::string name(ns ? ns : "", ns_len);
     std::vector<RlLimitRecord> lims;

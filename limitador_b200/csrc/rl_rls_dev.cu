@@ -577,6 +577,35 @@ int rl_http_dev_decide(rl_rls_dev* S, rl_engine* e, int endpoint, int* run_statu
     return copy_outputs(S, op != UPDATE, any_load, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
 }
 
+int rl_rls_dev_shard_send(rl_rls_dev* S, rl_shard_batch* sb, int empty, int http, int method, int load_counters, int* out_failed) {
+    if (!sb || !out_failed) return RL_FATAL;
+    *out_failed = RL_OK;
+    const int op = store_op(http != 0, method);
+    if (!empty && S && S->n_store) {
+        RL_CUDA(S, cudaSetDevice(S->device));
+        const int r = reserve_outputs(S, load_counters != 0);
+        if (r == RL_OK)
+            return rl_shard_batch_send(sb, S->n_store, S->n_ctr, S->d_ctr_off.p, S->d_ctrs.p, S->d_delta.p, S->d_now.p, op,
+                                       http ? S->d_load.p : nullptr, http ? 0 : load_counters);
+        *out_failed = r;  // the step still goes out, empty: no peer waits for it
+    }
+    return rl_shard_batch_send(sb, 0, 0, nullptr, nullptr, nullptr, nullptr, op, nullptr, 0);
+}
+
+int rl_rls_dev_shard_collect(rl_rls_dev* S, rl_shard_batch* sb, int load_counters, uint8_t* limited, uint32_t* first_limited,
+                             uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs) {
+    if (!sb) return RL_FATAL;
+    const bool any = S && S->n_store;
+    const bool lc = any && load_counters;
+    const int st = rl_shard_batch_collect(sb, any ? S->d_lim.p : nullptr, any ? S->d_first.p : nullptr, lc ? S->d_rem.p : nullptr,
+                                          lc ? S->d_ttl.p : nullptr);
+    if (!any) return st;
+    const int r = copy_outputs(S, true, lc, limited, first_limited, remaining, ttl_us, ctr_off, ctrs);
+    if (r) return r;
+    RL_CUDA(S, cudaStreamSynchronize(S->stream));
+    return st;
+}
+
 int rl_rls_dev_wait(rl_rls_dev* S) {
     if (!S) return RL_FATAL;
     RL_CUDA(S, cudaSetDevice(S->device));

@@ -49,6 +49,15 @@ int rl_rls_dev_decide(rl_rls_dev* st, rl_engine* e, int method, int load_counter
                       uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
 // Wait for everything the plan and the store call enqueued (the per-request array and the outputs are then on the host).
 int rl_rls_dev_wait(rl_rls_dev* st);
+/* The planned batch's store requests through the sharded exchange (rl_shard_batch_send): method / endpoint -> op, with the
+ * HTTP plan's per-request load flags or load_counters for all.  empty != 0 (or no planned state): an empty batch, so that
+ * a rank whose plan failed still takes part in the step; *out_failed = the status that made a planned batch go out empty.  _collect: rl_shard_batch_collect into the plan's output arrays,
+ * then the verdicts (always: error verdicts mark the requests that were not decided) and, with load_counters, remaining /
+ * ttl and the CSR to the host.  Returns the collect's status. */
+int rl_rls_dev_shard_send(rl_rls_dev* st, rl_shard_batch* sb, int empty, int http, int method, int load_counters,
+                          int* out_failed);
+int rl_rls_dev_shard_collect(rl_rls_dev* st, rl_shard_batch* sb, int load_counters, uint8_t* limited, uint32_t* first_limited,
+                             uint64_t* remaining, uint64_t* ttl_us, uint32_t* ctr_off, rl_counter* ctrs);
 // The HTTP plan on the same state (rl_http_dev.cuh): as rl_rls_dev_plan, and the one read before the store call also
 // brings the store calls back: *out_runs[0 .. *out_n_runs) (pinned host memory owned by *st, valid until the next plan).
 int rl_http_dev_plan(rl_rls_dev** st, rl_engine* e, rl_matcher* m, int endpoint, uint64_t n, const uint8_t* buf,

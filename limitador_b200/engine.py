@@ -43,6 +43,9 @@ LIMIT_DESC_DTYPE = np.dtype(
 
 # every symbol include/rl_engine.h declares (tests check the library exports them all)
 ABI_SYMBOLS = [
+    "rl_shard_batch_create", "rl_shard_batch_destroy", "rl_shard_batch_slab", "rl_shard_batch_engine", "rl_shard_batch_ipc_handle",
+    "rl_shard_batch_connect_ipc", "rl_shard_batch_connect_ptrs", "rl_shard_batch_send", "rl_shard_batch_decide",
+    "rl_shard_batch_collect", "rl_shard_batch_step",
     "rl_engine_create", "rl_engine_destroy", "rl_last_error", "rl_engine_set_stream", "rl_engine_stream",
     "rl_engine_max_counters_per_request",
     "rl_sync", "rl_get_stats", "rl_limits_set", "rl_limits_delete", "rl_check_and_update_records",
@@ -170,6 +173,20 @@ def load_library(path: str | None = None):
     L.rl_shard_fence.argtypes = [vp]
     L.rl_shard_debug.argtypes = [vp, vp]
     L.rl_trace_dump.argtypes = [vp, u32, vp, vp, vp, vp]
+    L.rl_shard_batch_create.argtypes = [vp, u32, u32, u32, u32, C.POINTER(vp)]
+    L.rl_shard_batch_destroy.argtypes = [vp]
+    L.rl_shard_batch_destroy.restype = None
+    L.rl_shard_batch_slab.argtypes = [vp]
+    L.rl_shard_batch_slab.restype = vp
+    L.rl_shard_batch_engine.argtypes = [vp]
+    L.rl_shard_batch_engine.restype = vp
+    L.rl_shard_batch_ipc_handle.argtypes = [vp, vp]
+    L.rl_shard_batch_connect_ipc.argtypes = [vp, vp]
+    L.rl_shard_batch_connect_ptrs.argtypes = [vp, vp]
+    L.rl_shard_batch_send.argtypes = [vp, u64, u64, vp, vp, vp, vp, i32, vp, i32]
+    L.rl_shard_batch_decide.argtypes = [vp]
+    L.rl_shard_batch_collect.argtypes = [vp, vp, vp, vp, vp]
+    L.rl_shard_batch_step.argtypes = [vp, u64, u64, vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, vp]
     L.rl_check_and_update_compact.argtypes = [vp, u64, vp, u64, i32, vp, vp]
     if path == _build.LIB_PATH:
         _lib = L
@@ -683,3 +700,71 @@ class Shard:
         self._lib.rl_shard_debug(self._h, _p(out))
         ctl = out[:-3].reshape(depth, self.world, 4)[:, :, :3].tolist()
         return {"ctl": ctl, "sent": int(out[-3]), "decided": int(out[-2]), "collected": int(out[-1])}
+
+
+class ShardBatch:
+    """The general (CSR) form of the namespace-sharded peer exchange of one rank (include/rl_engine.h: rl_shard_batch_*):
+    served requests travel to the GPU that owns their namespace, outputs come back, one step at a time.  Attach it to an
+    RlsService (RlsService.attach_shard) to serve RLS and HTTP batches on a sharded store; send / decide / collect take
+    device pointers (ints) for drivers of their own."""
+
+    CHECK_AND_UPDATE, IS_WITHIN, UPDATE = 0, 1, 2
+
+    def __init__(self, engine: "Engine", rank: int, world: int, cap_requests: int, cap_counters: int):
+        self._lib = engine._lib
+        self._eng = engine
+        self._h = C.c_void_p()
+        engine._check(self._lib.rl_shard_batch_create(engine._h, rank, world, cap_requests, cap_counters, C.byref(self._h)))
+        self.rank, self.world, self.cap_requests, self.cap_counters = rank, world, cap_requests, cap_counters
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.rl_shard_batch_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def slab(self) -> int:
+        return int(self._lib.rl_shard_batch_slab(self._h) or 0)
+
+    def ipc_handle(self) -> bytes:
+        buf = C.create_string_buffer(64)
+        self._eng._check(self._lib.rl_shard_batch_ipc_handle(self._h, buf))
+        return buf.raw
+
+    def connect_ipc(self, handles: bytes):
+        assert len(handles) == 64 * self.world
+        self._eng._check(self._lib.rl_shard_batch_connect_ipc(self._h, C.c_char_p(handles)))
+
+    def connect_ptrs(self, slabs):
+        arr = (C.c_void_p * self.world)(*[C.c_void_p(int(p)) for p in slabs])
+        self._eng._check(self._lib.rl_shard_batch_connect_ptrs(self._h, arr))
+
+    def send(self, n: int, n_ctr: int, off_ptr: int, ctrs_ptr: int, delta_ptr: int, now_ptr: int, op: int,
+             load_ptr: int = 0, load_all: bool = False):
+        v = C.c_void_p
+        self._eng._check(self._lib.rl_shard_batch_send(self._h, n, n_ctr, v(off_ptr), v(ctrs_ptr), v(delta_ptr), v(now_ptr), op,
+                                                       v(load_ptr or 0), int(load_all)))
+
+    def decide(self):
+        """Decide this rank's inbox.  Raises on a source with other limits (after the outputs went back) and on a failed
+        engine call (its requests were answered with error verdicts)."""
+        self._eng._check(self._lib.rl_shard_batch_decide(self._h))
+
+    def step(self, n: int, n_ctr: int, off_ptr: int, ctrs_ptr: int, delta_ptr: int, now_ptr: int, op: int, limited_ptr: int,
+             first_ptr: int = 0, remaining_ptr: int = 0, ttl_ptr: int = 0, load_ptr: int = 0, load_all: bool = False):
+        """send + decide + collect: the one call of a one-process-per-GPU deployment."""
+        v = C.c_void_p
+        self._eng._check(self._lib.rl_shard_batch_step(self._h, n, n_ctr, v(off_ptr), v(ctrs_ptr), v(delta_ptr), v(now_ptr), op,
+                                                       v(load_ptr or 0), int(load_all), v(limited_ptr), v(first_ptr or 0),
+                                                       v(remaining_ptr or 0), v(ttl_ptr or 0)))
+
+    def collect(self, limited_ptr: int, first_ptr: int = 0, remaining_ptr: int = 0, ttl_ptr: int = 0):
+        v = C.c_void_p
+        self._eng._check(self._lib.rl_shard_batch_collect(self._h, v(limited_ptr), v(first_ptr or 0), v(remaining_ptr or 0),
+                                                          v(ttl_ptr or 0)))

@@ -25,6 +25,7 @@ HEADERS_NONE, HEADERS_DRAFT_VERSION_03, HEADERS_OTHER = 0, 1, 2
 HEADER_NAMES = ("X-RateLimit-Limit", "X-RateLimit-Remaining", "X-RateLimit-Reset")
 
 HTTP_SYMBOLS = (
+    "rl_http_serve_sharded", "rl_http_send", "rl_http_decide", "rl_http_collect",
     "rl_http_decode_body", "rl_http_create", "rl_http_destroy", "rl_http_last_error", "rl_http_plan", "rl_http_plan_device",
     "rl_http_plan_view", "rl_http_finish", "rl_http_responses", "rl_http_serve", "rl_http_last_timings", "rl_http_get_limits",
     "rl_http_get_counters", "rl_http_render_counters", "rl_http_get_response",
@@ -58,6 +59,10 @@ def _lib():
     L.rl_http_finish.argtypes = [vp, vp, vp, vp, vp, vp]
     L.rl_http_responses.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.rl_http_serve.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_serve_sharded.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_send.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_http_decide.argtypes = [vp]
+    L.rl_http_collect.argtypes = [vp]
     L.rl_http_last_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(u32)]
     L.rl_http_get_limits.argtypes = [vp, C.c_char_p, u32]
     L.rl_http_get_counters.argtypes = [vp, C.c_char_p, u32, u64]
@@ -172,6 +177,19 @@ class HttpApi:
         """plan_device -> the engine (one call per run) -> finish.  Needs an engine."""
         self._n = len(off) - 1
         _rls._batch_call(self, self._lib.rl_http_serve, endpoint, buf, off, now_us)
+
+    def send(self, endpoint: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """Sharded step (the RLS service has a ShardBatch attached), phase 1: plan and send; then decide and collect, as
+        RlsService.send / decide / collect."""
+        self._n = len(off) - 1
+        _rls._batch_call(self, self._lib.rl_http_send, endpoint, buf, off, now_us)
+
+    def decide(self):
+        self._check(self._lib.rl_http_decide(self._h))
+
+    def collect(self):
+        self._check(self._lib.rl_http_collect(self._h))
+        return self.responses()
 
     def timings(self) -> Dict[str, float]:
         a, b, c, k = C.c_double(), C.c_double(), C.c_double(), C.c_uint32()

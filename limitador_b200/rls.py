@@ -25,6 +25,7 @@ GRPC_OK, GRPC_INTERNAL, GRPC_UNAVAILABLE = 0, 13, 14
 NO_STORE = 0xFFFFFFFF
 
 RLS_SYMBOLS = (
+    "rl_rls_attach_shard", "rl_rls_serve_sharded", "rl_rls_send", "rl_rls_decide", "rl_rls_collect",
     "rl_rls_decode_request", "rl_rls_encode_response", "rl_rls_create", "rl_rls_destroy", "rl_rls_last_error",
     "rl_rls_plan", "rl_rls_plan_view", "rl_rls_finish", "rl_rls_responses", "rl_rls_serve", "rl_rls_metrics_render",
     "rl_rls_last_timings", "rl_rls_plan_device", "rl_rls_keep_counter_vars", "rl_rls_counter_vars_stats",
@@ -98,6 +99,11 @@ def _lib():
     L.rl_rls_counter_vars_drain.argtypes = [vp, u64, u64, vp, vp, vp, vp, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(i32)]
     L.rl_rls_configure.argtypes = [vp, C.POINTER(LimitSpec), u32, i32, C.POINTER(ConfigureReport)]
     L.rl_rls_config_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+    L.rl_rls_attach_shard.argtypes = [vp, vp]
+    L.rl_rls_serve_sharded.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_rls_send.argtypes = [vp, i32, u64, vp, vp, u64]
+    L.rl_rls_decide.argtypes = [vp]
+    L.rl_rls_collect.argtypes = [vp]
     L._rl_rls_ready = True
     return L
 
@@ -303,6 +309,27 @@ class RlsService:
         self._check(self._lib.rl_rls_finish(self._h, store_status, _ptr(limited, np.uint8, keep),
                                             _ptr(first_limited, np.uint32, keep), _ptr(remaining, np.uint64, keep),
                                             _ptr(ttl_us, np.uint64, keep)))
+        return self.responses()
+
+    def attach_shard(self, shard: Optional[_eng.ShardBatch]):
+        """Serve on a namespace-sharded store: from now on `serve` ships every store request to the rank that owns its
+        namespace (every rank runs its own service with the same limits and issues the same serve calls).  None
+        detaches."""
+        self._check(self._lib.rl_rls_attach_shard(self._h, shard._h if shard is not None else None))
+        self._shard = shard  # keep it alive
+
+    def send(self, method: int, buf: np.ndarray, off: np.ndarray, now_us: int = 0):
+        """Sharded step, phase 1: plan on the device and send the store requests to their owners.  A one-process driver of
+        several ranks calls every rank's send, then every decide, then every collect."""
+        _batch_call(self, self._lib.rl_rls_send, method, buf, off, now_us)
+
+    def decide(self):
+        """Sharded step, phase 2: decide this rank's inbox."""
+        self._check(self._lib.rl_rls_decide(self._h))
+
+    def collect(self):
+        """Sharded step, phase 3: collect this rank's outputs and finish its responses -> responses()."""
+        self._check(self._lib.rl_rls_collect(self._h))
         return self.responses()
 
     def responses(self) -> List[Tuple[int, bytes]]:
